@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- streaming Whisper on B200 behind WhisperLiveKit's AlignAtt seam.
+"""bench.py -- streaming Whisper on H100 behind WhisperLiveKit's AlignAtt seam.
 
 Headline config (`--config alignatt-large-v3`, the default; BASELINE.json's metric): Whisper large-v3, 0.5 s
 chunks, 30 s rolling window fully re-encoded per chunk (the reference's parity mode), B concurrent streams per GPU.
@@ -27,6 +27,12 @@ Numbers in the one JSON line:
               AlignAtt hooks) on the host cores, same per-chunk workload (oracle/ref_driver.py).
 
     python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--config C] [--streams B] [--no-extras]
+                    [--dump-outputs DIR]
+--dump-outputs DIR (headline config): what the last timed tick returned to its caller, as DIR/<name>.npy -- tokens, logprobs
+and frames [decode iteration][stream] of every select call, no_speech_prob [stream], and logits [stream][vocab] as left by
+the last decode step (suppressed entries, -inf, stored as the lowest finite float32; above 60 MB a fixed sample of the
+streams, listed in logits_streams.npy).  Inputs are seeded: two builds run
+with the same arguments can be compared array by array.
 Multi-GPU: python -m torch.distributed.run --nproc-per-node N bench.py --gpus N ...  (one rank per GPU; sessions are
 sharded, NCCL is used once to broadcast the packed weights; weak scaling, no data-path collective).
 """
@@ -51,21 +57,17 @@ WINDOW = 480000
 PREFIX = int(os.environ.get("WLK_BENCH_PREFIX", "48"))            # the headline workload: 48 + 8 (overrides are for experiments)
 STEPS_PER_CHUNK = int(os.environ.get("WLK_BENCH_STEPS", "8"))
 UNIT = "concurrent real-time streams (audio-s per wall-s)"
+DUMP_LOGITS_BYTES = 60 << 20          # --dump-outputs writes at most 64 MB: the other arrays are a few KB per stream
 CONFIGS = ["alignatt-large-v3", "alignatt-base-en-1stream", "localagreement-large-v3-64", "alignatt-large-v3-sortformer-64",
            "qwen-tower-128", "alignatt-large-v3-incremental"]
 
 
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(bf16_tflops=d.get("bf16_tflops_sustained") or d.get("bf16_tflops"), hbm_gbs=d.get("hbm_gbs"),
-                    source="measured (MEASURED_PEAKS.json, sustained)")
-    return dict(bf16_tflops=1400.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(bf16_tflops=989.0, hbm_gbs=3350.0, source="NVIDIA H100 SXM data sheet (dense BF16, HBM3 at 700 W): a bound, not a measured rate")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -113,7 +115,7 @@ def cpu_baseline_leg(dims, sd, heads, n_chunks=2):
         model = rd.build_model(dims, sd, heads)
         per, threads = rd.time_single_stream(model, dims, PREFIX, STEPS_PER_CHUNK, n_chunks, cores, warmup=0)
         kind, what = "reference", "staged unmodified reference (oracle/_ref): its AlignAtt hooks over its vendored torch Whisper, fp32"
-    else:                                                     # the recipe could not run (no /root/reference at build time)
+    else:                                                     # the reference was not available when build() ran
         import torch
         torch.set_num_threads(cores)
         per, threads = oracle_port_chunks(dims, sd, heads, n_chunks), torch.get_num_threads()
@@ -148,7 +150,7 @@ def oracle_port_chunks(dims, sd, heads, n_chunks):
 
 
 def reference_arm(args, dims, heads, metric, workload):
-    """bench.py --impl reference: rank 0 only.  Two figures (BASELINE.md section 4): (ii) `cores` single-thread
+    """bench.py --impl reference: rank 0 only.  Two figures (BASELINE.md section 3): (ii) `cores` single-thread
     streams in parallel, then (i) one stream on all cores; `value` is the better of the two (CPU throughput)."""
     from oracle import ref_driver as rd
     from whisperlivekit_b200.weights import synthetic_state_dict
@@ -187,7 +189,7 @@ def reference_arm(args, dims, heads, metric, workload):
                 data="synthetic", impl="reference",
                 config=dict(workload=workload.replace(f"{args.streams} streams/GPU", "host CPU"), model=args.model,
                             note="staged unmodified reference (oracle/_ref), `--backend whisper` path: its own AlignAtt hooks over "
-                                 "its vendored torch Whisper, fp32, scripted to the same per-chunk work as the B200 arm"),
+                                 "its vendored torch Whisper, fp32, scripted to the same per-chunk work as the GPU arm"),
                 cpu_baseline=dict(value=value, unit=UNIT, cores=cores, kind=fig_i.get("kind", "reference"),
                                   cpu_model=rd.cpu_model(), nproc=os.cpu_count(), cpu_quota=rd.cpu_quota(),
                                   omp_env=os.environ.get("OMP_NUM_THREADS"),
@@ -747,7 +749,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="alignatt-large-v3", choices=CONFIGS)
-    ap.add_argument("--streams", type=int, default=int(os.environ.get("WLK_BENCH_STREAMS", "96")), help="streams per GPU")
+    ap.add_argument("--streams", type=int, default=int(os.environ.get("WLK_BENCH_STREAMS", "48")),
+                    help="streams per GPU (default 48: sessions for 80 streams -- 48 + the seam probes' headroom -- hold ~26 GB of K/V of the 80 GB)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed tick returned (tokens, logprobs, frames, no_speech_prob, logits) as DIR/<name>.npy")
     ap.add_argument("--model", default="large-v3")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "bf16x3"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -755,12 +760,14 @@ def main():
     ap.add_argument("--no-seam", action="store_true", help="skip the real-time paced run through the seam")
     ap.add_argument("--seam-ticks", type=int, default=16)
     ap.add_argument("--seam-mode", default="cohort", choices=["cohort", "continuous", "threads"],
-                    help="cohort: closed cohorts (best p95 capacity); continuous: arrivals join between rounds (measured: p50 0.20 s "
-                         "instead of 0.34 s at 64 streams, same p95, but the small encoder batches cost capacity: 80 streams run away)")
+                    help="cohort: closed cohorts (best p95 capacity); continuous: arrivals join between rounds (lower median latency, "
+                         "but the small encoder batches cost capacity)")
     ap.add_argument("--seam-streams", type=int, default=0, help="first stream count probed through the seam (default: 2/3 of --streams)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
+    if args.dump_outputs and (args.impl != "b200" or args.config != "alignatt-large-v3"):
+        ap.error("--dump-outputs covers the headline config (--config alignatt-large-v3) of the GPU arm")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -811,7 +818,7 @@ def main():
                               clocks=clocks, detail=r)))
         return
 
-    # ---------------------------------------------------------------- B200 arm, headline config
+    # ---------------------------------------------------------------- GPU arm, headline config
     import torch
     import torch.distributed as dist
     from whisperlivekit_b200.engine import WhisperEngine
@@ -843,7 +850,7 @@ def main():
     rng = np.random.default_rng(1000 + rank)
     base = synthetic_audio(36.0, seed=7)
 
-    def scripted(eng, B, steps, warmup, profile_pass=True, io_only=False):
+    def scripted(eng, B, steps, warmup, profile_pass=True, io_only=False, dump_dir=None):
         """The scripted tick (module docstring).  -> (ms device-resident, ms with per-chunk IO, profile, host enqueue)"""
         sp = eng.specials
         sids = [eng.open_session() for _ in range(B)]
@@ -854,6 +861,7 @@ def main():
         sup = sp.alignatt_suppress_tokens()
         chunk_host = torch.empty(B, CHUNK, dtype=torch.float32).pin_memory()
         host = dict(encode=0.0, prefill=0.0, prefill_synced=0.0, step=0.0, n=0, ns=0)
+        last = dict(nsp=None, sel=None)                      # what the most recent tick returned to its caller
 
         def step(with_io, sync_before_prefill=False):
             if with_io:
@@ -874,9 +882,10 @@ def main():
                 host["prefill_synced"] += t2 - t1; host["ns"] += 1
             else:
                 host["encode"] += t1 - t0; host["prefill"] += t2 - t1; host["n"] += 1
-            eng.no_speech_prob(sids)
+            last["nsp"], last["sel"] = eng.no_speech_prob(sids), []
             for _ in range(STEPS_PER_CHUNK):
                 r = eng.select(sids, sup)                    # suppress -> greedy token/logprob -> alignment reduce -> frame
+                last["sel"].append(r)
                 t3 = time.perf_counter()
                 eng.decode(sids, [[t[0]] for t in r])
                 if not sync_before_prefill:
@@ -929,6 +938,21 @@ def main():
             sampler.start()
         ms_dev, _ = timed(False, steps, warmup, False)
         clocks = sampler.summary() if sampler else None
+        if dump_dir and rank == 0:                           # after the timed window, before anything else touches the sessions
+            os.makedirs(dump_dir, exist_ok=True)
+            sel = np.asarray(last["sel"], np.float64)        # [iteration][stream][token, logprob, frame]
+            logits = np.stack([eng.read_logits(s) for s in sids])
+            np.save(os.path.join(dump_dir, "tokens.npy"), sel[:, :, 0])
+            np.save(os.path.join(dump_dir, "logprobs.npy"), sel[:, :, 1].astype(np.float32))
+            np.save(os.path.join(dump_dir, "frames.npy"), sel[:, :, 2])
+            np.save(os.path.join(dump_dir, "no_speech_prob.npy"), np.asarray(last["nsp"], np.float32))
+            # only -inf (a suppressed token) is replaced: a NaN or +inf from a broken build must stay visible
+            logits = np.where(np.isneginf(logits), np.finfo(np.float32).min, logits).astype(np.float32)
+            if logits.nbytes > DUMP_LOGITS_BYTES:            # many streams: a fixed, seeded sample of the streams
+                keep = np.sort(np.random.default_rng(0).choice(len(sids), DUMP_LOGITS_BYTES // logits[0].nbytes, replace=False))
+                np.save(os.path.join(dump_dir, "logits_streams.npy"), keep.astype(np.float64))
+                logits = logits[keep]
+            np.save(os.path.join(dump_dir, "logits.npy"), logits)
         ms_io, prof, ms_prof = None, None, None
         if profile_pass:
             ms_io, _ = timed(True, steps, max(1, warmup // 3), False)
@@ -971,7 +995,7 @@ def main():
         return
 
     eng = make_engine(args.precision, max(B, seam_bmax), max(B, seam_bmax))
-    r = scripted(eng, B, args.steps, args.warmup)
+    r = scripted(eng, B, args.steps, args.warmup, dump_dir=args.dump_outputs)
     note(f"scripted tick: {r['ms_dev'] / args.steps:.1f} ms device-resident, {r['ms_io'] / args.steps:.1f} ms with host chunks")
     seam_best, seam_probes = None, []
     if not args.no_seam:
@@ -1006,8 +1030,8 @@ def main():
         engx.close()
         msx = rx["ms_dev"] / 2
         note(f"bf16x3 tick at {Bx} streams: {msx:.1f} ms")
-        exact = dict(mode="bf16x3 (WLK_PREC_BF16X3: split operands, 3 tcgen05 MMAs per product; fp32 activations, softmax, K/V)",
-                     parity="|dlogits| 2.4e-4 vs the reference at large-v3, tokens and frames identical (tests/test_gpu_large_v3.py)",
+        exact = dict(mode="bf16x3 (WLK_PREC_BF16X3: split operands, 3 wgmma MMAs per product; fp32 activations, softmax, K/V)",
+                     parity="|dlogits| <= 1e-3 vs the reference at large-v3, tokens and frames identical (asserted by tests/test_gpu_large_v3.py)",
                      value=Bx * world * CHUNK_S / (msx / 1e3), unit=UNIT, streams_per_gpu=Bx, ms_per_step=msx)
         if rank == 0 and world == 1:
             reuse = {"localagreement-large-v3-64": la64, "alignatt-large-v3-sortformer-64": diar64}
@@ -1020,15 +1044,7 @@ def main():
         ms_dev, ms_io, prof, host = r["ms_dev"], r["ms_io"], r["prof"], r["host"]
         value = total_streams * CHUNK_S * args.steps / (ms_dev / 1e3)
         g = prof["gemm_enc"]
-        traffic, tnote = None, "no ncu capture for this configuration"
-        for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(tpath) and B == 96 and args.model == "large-v3":
-                tj = json.load(open(tpath))
-                traffic = tj["mean_dram_bytes_per_launch"]
-                tnote = (f"dram__bytes_read+write per launch, mean of one encoder layer's GEMMs, ncu --set full at 96 streams "
-                         f"(profiles/{name}); algorithmic {tj.get('algorithmic_bytes_per_launch', 2.04e9) / 1e9:.2f} GB")
-                break
+        traffic, tnote = None, "DRAM traffic of the encoder GEMMs: not measured"
         ach = g["flops"] / (g["ms"] / 1e3) / 1e12 if g["ms"] else 0.0
         mult = dict(mel=2, align=3)
         launches = int(sum(v["launches"] * mult.get(k, 1) for k, v in prof.items()))
@@ -1064,16 +1080,16 @@ def main():
             dtype="bf16" if args.precision == "bf16" else "bf16x3",
             data="synthetic (seeded random weights at true large-v3 dims, synthetic speech-like audio)",
             config=dict(workload=workload, model=args.model, streams_per_gpu=B, parallelism=f"sessions sharded x{world}",
-                        chunk_s=CHUNK_S, l2="working set (3.4 GB weights + per-stream KV) exceeds the 126 MB L2",
+                        chunk_s=CHUNK_S, l2="working set (3.4 GB weights + per-stream KV) exceeds the 50 MB L2",
                         rtf_per_stream=(ms_dev / args.steps / 1e3) / CHUNK_S,
                         frac_of_encoder_gemm_stream_ceiling=value / world / (peaks["bf16_tflops"] / 5.18),
-                        parity="bf16 mode: tokens identical to the reference wherever its top-2 logit gap exceeds the test's epsilon (63-64 of 64 "
-                               "teacher-forced steps on two large-v3 streams; the one flip seen has a reference gap of 0.006), max |dlogits| 0.05-0.075 "
-                               "(tests/test_gpu_large_v3.py, profiles/r02_parity_large_v3_bf16.json); fp32 and bf16x3 modes: 1e-3 on logits, identical"),
+                        parity="bf16 mode: tokens identical to the reference wherever its top-2 logit gap exceeds the test's epsilon on "
+                               "teacher-forced steps of two large-v3 streams (tests/test_gpu_large_v3.py); fp32 and bf16x3 modes: 1e-3 on logits, "
+                               "identical tokens and frames"),
             e2e=e2e,
             gpu_launches=launches,
             clocks=r["clocks"],
-            roofline=dict(bound="tensor", kernel="gemm_tc2_kernel (cta_group::2 pair GEMM; encoder GEMMs, class gemm_enc)", achieved=ach,
+            roofline=dict(bound="tensor", kernel="gemm_tc_kernel (wgmma GEMM; encoder GEMMs, class gemm_enc)", achieved=ach,
                           peak=peaks["bf16_tflops"], unit="TFLOP/s", frac=ach / peaks["bf16_tflops"], traffic=traffic,
                           traffic_note=tnote, peak_source=peaks["source"],
                           flops_per_launch=g["flops"] / max(1, g["launches"]), ms_per_launch=g["ms"] / max(1, g["launches"])),

@@ -1,5 +1,5 @@
 /*
- * wlk_b200.h -- C ABI of the B200-native streaming-Whisper engine.
+ * wlk_b200.h -- C ABI of the H100-native streaming-Whisper engine.
  *
  * The reference (QuentinFuxa/WhisperLiveKit) has no FFI: its plugin surface for
  * this path is Python duck-typing (SURVEY.md §8b).  This header is the boundary a
@@ -35,7 +35,7 @@ typedef struct wlk_dims {
 
 enum { WLK_PREC_FP32 = 0,     /* SIMT fp32 kernels end to end: the 1e-3-on-logits parity mode                    */
        WLK_PREC_BF16 = 1,     /* bf16 operands / fp32 accumulate + fp32 residual: the serving mode                */
-       WLK_PREC_BF16X3 = 2 }; /* tcgen05 with split operands (x = hi + lo, both bf16; A_hi W_hi + A_lo W_hi +    *
+       WLK_PREC_BF16X3 = 2 }; /* wgmma with split operands (x = hi + lo, both bf16; A_hi W_hi + A_lo W_hi +    *
                                * A_hi W_lo into one fp32 accumulator): 1e-3 on logits at tensor-core speed / 3;   *
                                * activations, softmax, LayerNorm and K/V caches stay fp32                         */
 enum { WLK_BACKEND_AUTO = 0, WLK_BACKEND_SIMT = 1, WLK_BACKEND_TCGEN05 = 2 };
@@ -45,7 +45,7 @@ typedef struct wlk_config {
     int32_t precision;       /* WLK_PREC_* */
     int32_t max_sessions;    /* device state is pooled for this many sessions */
     int32_t max_batch;       /* sessions per encode/decode call */
-    int32_t gemm_backend;    /* WLK_BACKEND_* (AUTO: tcgen05 in bf16 mode, SIMT in fp32 mode) */
+    int32_t gemm_backend;    /* WLK_BACKEND_* (AUTO: wgmma in bf16 mode, SIMT in fp32 mode) */
     int32_t attn_backend;    /* WLK_BACKEND_* for the encoder self-attention */
     int32_t max_align_heads; /* capacity of the alignment-head export */
     int32_t reserved;
@@ -112,7 +112,7 @@ int wlk_encode(wlk_engine* e, const int32_t* sids, int n, int32_t* content_mel_l
  *   rolling window, simul_whisper.py:224-236) -- runs through the conv stem and the layers, attending to the retained
  *   K/V of every other position.  The first call of a stream takes the whole window as its block and equals wlk_encode;
  *   buffers are ring-addressed after a slide (nothing is moved).  Not bit- or 1e-3-comparable with the reference by
- *   construction: graded by token / attended-frame agreement with the parity mode.  bf16 tcgen05 mode only.
+ *   construction: graded by token / attended-frame agreement with the parity mode.  bf16 wgmma mode only.
  *   block_rows_out[i] (may be NULL) = positions that went through the encoder for session i.                          */
 int wlk_encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* content_mel_len_out, int32_t* block_rows_out);
 /* forget the retained encoder K/V of a session: its next wlk_encode_incremental takes the whole window as its block
@@ -169,8 +169,8 @@ int wlk_read_logits(wlk_engine* e, int32_t sid, int32_t which /* 0 last, 1 sot r
 int wlk_read_align_attn(wlk_engine* e, int32_t sid, float* out, int64_t capacity, int32_t* rows, int32_t* cols);
 
 /* ---- op-level entry points (kernel tests, roofline benches). Device pointers.
- *      backend: WLK_BACKEND_SIMT, WLK_BACKEND_TCGEN05 (auto tile choice), 3 = force the one-CTA tcgen05 kernel,
- *      4 = force the CTA-pair (cta_group::2) kernel.
+ *      backend: WLK_BACKEND_SIMT, WLK_BACKEND_TCGEN05 (auto tile choice), 3 = force the 64-wide-tile wgmma kernel,
+ *      4 = force the 128-wide-tile one.
  *      a_type/w_type/c_type: 0 = fp32, 1 = bf16.  C[M,N] = act(A[M,K] W[N,K]^T + bias); `gelu` is a flag
  *      word: bit 0 = erf-GELU, bit 1 = accumulate into the fp32 C in place (C += A W^T + bias).           */
 int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t lda,
@@ -182,9 +182,6 @@ int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int ty
  *      median_kernel / dtw_kernel (whisper/triton_ops.py:13-103) with the semantics of its CPU path
  *      (whisper/timing.py:19-54 median_filter; :57-105 dtw_cpu + backtrace).  x is device fp32.
  *      wlk_op_dtw: x[N tokens, M frames] -> alignment path (text_idx[i], time_idx[i]), i < *len <= N+M.   */
-/* diagnostic: the tcgen05 encoder attention with one CTA stamping clock64() at its pipeline hand-offs, [12 key tiles][8]:
- * MMA warp before S_j / before P_j V, softmax warp after S ready / exponentials done / arrive (tools/attn_trace.py)      */
-int wlk_op_encoder_attention_trace(wlk_engine* e, const void* qkv_dev, int batch, void* out_dev, int64_t* stamps_host);
 int wlk_op_median_filter(wlk_engine* e, const float* x_dev, float* out_dev, int rows, int cols, int width);
 int wlk_op_dtw(wlk_engine* e, const float* x_dev, int N, int M, int32_t* text_idx_host, int32_t* time_idx_host,
                int32_t* len_out);

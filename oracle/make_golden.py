@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the REAL reference on CPU.
 
-Run in the build container only (needs /root/reference):
+Needs the staged reference (oracle/_ref, see oracle/stage_reference.py):
 
     python oracle/make_golden.py
 
@@ -26,7 +26,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")   # the staged reference (oracle/stage_reference.py)
 
 
 def import_reference():

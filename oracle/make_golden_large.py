@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generate tests/golden/large_v3_forced.npz by running the REAL reference on CPU at the true large-v3
-geometry (the geometry bench.py times).  Build container only (needs /root/reference):
+geometry (the geometry bench.py times).  Needs the staged reference (oracle/_ref):
 
     python oracle/make_golden_large.py
 

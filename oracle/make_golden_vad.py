@@ -11,7 +11,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-JIT = "/root/reference/whisperlivekit/silero_vad_models/silero_vad.jit"
+JIT = os.path.join(ROOT, "oracle", "_ref", "whisperlivekit", "silero_vad_models", "silero_vad.jit")
 
 
 def main():

@@ -1,5 +1,5 @@
 """Drive the STAGED, unmodified reference (oracle/_ref, see oracle/stage_reference.py) through the same per-chunk
-workload bench.py times on the B200 engine, on the host cores: the reference arm (`bench.py --impl reference`)
+workload bench.py times on the H100 engine, on the host cores: the reference arm (`bench.py --impl reference`)
 and the `cpu_baseline` leg.  Benchmark infrastructure only -- nothing in whisperlivekit_b200/ imports this.
 
 What is timed is the reference's own code: ``AlignAtt.insert_audio`` (rolling 30 s window, simul_whisper.py:219-237),
@@ -145,7 +145,7 @@ class RefStream:
                 if new_segment:
                     a._check_no_speech(logits)                       # computed; the scripted workload does not stop on it
                 if it == self.steps:
-                    break                                            # the B200 arm's last call is a decode as well
+                    break                                            # the H100 arm's last call is a decode as well
                 logits = logits[:, -1, :]
                 if new_segment:
                     logits = a._suppress_blank_tokens(logits)
@@ -175,7 +175,7 @@ def time_single_stream(model, dims, prefix_len, steps, n_chunks, threads, warmup
 
 
 def time_parallel_single_thread(model, dims, prefix_len, steps, procs, timeout_s=300.0):
-    """`procs` single-thread streams in parallel (BASELINE.md section 4, figure ii): fork one process per stream (the
+    """`procs` single-thread streams in parallel (BASELINE.md section 3, figure ii): fork one process per stream (the
     model's weights are shared copy-on-write), each runs ONE stream-chunk; returns (wall seconds, finished).
     Must be called before this process has run any multi-threaded torch op (OpenMP pools do not survive fork)."""
     import select

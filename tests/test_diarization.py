@@ -1,6 +1,6 @@
 """Diarization post-processing (SURVEY.md 8f-4, reference sortformer_backend.py:313-363).
 CPU: oracle/diar_oracle.py against the known answers of the reference's own tests
-(/root/reference/tests/test_sortformer_max_speakers.py:78-125, 183-215) and -- in the build container -- against the
+(its tests/test_sortformer_max_speakers.py:78-125, 183-215) and -- where the reference is staged under oracle/_ref -- against the
 reference's method itself on random predictions.  GPU: the device run-length kernel (wlk_diar_segments, through the
 C ABI) against the oracle, bit-exact (integer work)."""
 import sys
@@ -46,12 +46,8 @@ def _reference_online(preds, max_speakers, len_prediction, chunk_index, gto):
     """The reference's own method on a bare instance, NeMo stubbed out like its tests do (:18-52)."""
     import importlib
     import torch
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    if "soundfile" not in sys.modules:
-        m = types.ModuleType("soundfile")
-        m.__spec__ = __import__("importlib.machinery").machinery.ModuleSpec("soundfile", loader=None)
-        sys.modules["soundfile"] = m
+    from oracle import stage_reference
+    stage_reference.import_staged_reference()
     for name in ("nemo", "nemo.collections", "nemo.collections.asr", "nemo.collections.asr.models", "nemo.collections.asr.modules"):
         sys.modules.setdefault(name, types.ModuleType(name))
     sys.modules["nemo.collections.asr.models"].SortformerEncLabelModel = object

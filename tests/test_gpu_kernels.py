@@ -58,7 +58,7 @@ SHAPES_TC = [(128, 256, 64), (256, 256, 128), (1500, 1280, 1280), (3000, 384, 24
 
 @pytest.mark.parametrize("M,N,K", SHAPES_TC)
 def test_gemm_tcgen05_bf16(eng, M, N, K):
-    """tcgen05 GEMM vs fp32 reference on the same bf16-rounded operands: only the fp32
+    """Tensor-core (wgmma) GEMM vs fp32 reference on the same bf16-rounded operands: only the fp32
     accumulation order differs, so the bound is tight (1e-3 relative to the output scale)."""
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     A = torch.randn(M, K, device="cuda", generator=g).bfloat16()
@@ -105,7 +105,7 @@ def test_encoder_attention_simt(eng, dtype):
 
 @pytest.mark.parametrize("d,H,B", [(128, 2, 1), (384, 6, 2), (1280, 20, 1)])
 def test_encoder_attention_tcgen05(eng, d, H, B):
-    """Fused tcgen05 attention vs fp32 softmax(QK^T)V on the same bf16 inputs.  P is rounded to
+    """Fused tensor-core attention vs fp32 softmax(QK^T)V on the same bf16 inputs.  P is rounded to
     bf16 before the PV product (8 mantissa bits): tolerance 2e-2 on outputs of O(1)."""
     from whisperlivekit_b200.dims import ModelDimensions
     from whisperlivekit_b200.engine import WhisperEngine
@@ -126,9 +126,9 @@ def test_encoder_attention_tcgen05(eng, d, H, B):
 
 
 def test_encoder_attention_tcgen05_moving_reference():
-    """The one-pass softmax keeps a reference maximum per row and only moves it (rescaling O and l in TMEM and redoing the
-    tile) when a key tile exceeds it by more than 2^8.  Random inputs almost never take that path: here the keys of later
-    tiles are scaled up so that most rows move their reference several times, at different tiles."""
+    """The online softmax keeps a running maximum per row and rescales O and l in registers whenever a key tile raises it.
+    With random inputs the maximum settles in the first tiles: here the keys of later tiles are scaled up so that most rows
+    move it by large factors several times, at different tiles."""
     from whisperlivekit_b200.dims import ModelDimensions
     from whisperlivekit_b200.engine import WhisperEngine
     d, H, B = 256, 4, 2
@@ -159,7 +159,7 @@ def test_encoder_attention_tcgen05_moving_reference():
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (512, 512, 256), (1500, 1280, 1280), (3000, 384, 240),
                                    (257, 300, 72), (24000, 1280, 1280), (4500, 5120, 1280)])
 def test_gemm_tcgen05_cta_pair(eng, M, N, K):
-    """cta_group::2 kernel (256x256 tiles over 2-CTA clusters) vs fp32 reference and vs the 1-CTA kernel."""
+    """The 128-wide-tile instantiation (backend "tcgen05_pair") vs fp32 reference and vs the 64-wide one ("tcgen05_1cta")."""
     g = torch.Generator(device="cuda").manual_seed(M + 3 * N + K)
     A = torch.randn(M, K, device="cuda", generator=g).bfloat16()
     W = (torch.randn(N, K, device="cuda", generator=g) / K ** 0.5).bfloat16()

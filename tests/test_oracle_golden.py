@@ -1,6 +1,8 @@
 """CPU: the oracle restatement against fixtures recorded from the real reference
 (oracle/make_golden.py), plus host-logic checks.  Tolerances: fp32 CPU vs fp32
 CPU of the same algorithm -> 2e-4 abs on O(1..10) tensors; integer traces exact."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -83,7 +85,8 @@ def test_alignment_heads_table_shape():
 @pytest.mark.reference
 def test_alignment_heads_match_reference():
     import base64, gzip, re, ast
-    src = open("/root/reference/whisperlivekit/whisper/__init__.py").read()
+    from oracle import stage_reference
+    src = open(os.path.join(stage_reference.TARGET, "whisperlivekit", "whisper", "__init__.py")).read()
     dumps = ast.literal_eval(re.search(r"_ALIGNMENT_HEADS = (\{.*?\n\})", src, re.S).group(1))
     for k, heads in ALIGNMENT_HEADS.items():
         d = DIMS[k]

@@ -1,5 +1,5 @@
 """CPU: the Silero VAD oracle against probabilities recorded from the reference's scripted model
-(oracle/make_golden_vad.py): seeded weights everywhere; with the trained weights only where /root/reference exists."""
+(oracle/make_golden_vad.py): seeded weights everywhere; with the trained weights only where the reference is staged (oracle/_ref)."""
 import os
 
 import numpy as np
@@ -29,7 +29,8 @@ def test_vad_oracle_matches_reference_model_with_trained_weights():
     import torch
     from oracle.vad_oracle import VadOracle
     g = dict(np.load(os.path.join(HERE, "golden", "vad.npz")))
-    m = torch.jit.load("/root/reference/whisperlivekit/silero_vad_models/silero_vad.jit", map_location="cpu")
+    from oracle import stage_reference
+    m = torch.jit.load(os.path.join(stage_reference.TARGET, "whisperlivekit", "silero_vad_models", "silero_vad.jit"), map_location="cpu")
     o = VadOracle({k: v.numpy() for k, v in m.state_dict().items()})
     audio, n = _audio(), int(g["n_windows"])
     a, b = o.open_session(), o.open_session()

@@ -1,4 +1,4 @@
-"""Build container only (needs /root/reference): ``plugin.install()`` executed against the reference's own
+"""Needs the staged reference (oracle/_ref): ``plugin.install()`` executed against the reference's own
 ``SimulStreamingASR`` / ``SimulStreamingOnlineProcessor`` (simul_whisper/backend.py:61-71, 530-553), and the two hooks
 no other test reaches -- ``lang_id`` (simul_whisper.py:266-292) and the CIF end-of-word test
 (eow_detection.py:37-77).  The CUDA engine is replaced by the CPU oracle through ``install(engine_factory=...)``:
@@ -17,14 +17,8 @@ pytestmark = pytest.mark.reference
 
 
 def _import_reference():
-    if "soundfile" not in sys.modules:
-        m = types.ModuleType("soundfile")
-        m.__spec__ = __import__("importlib.machinery").machinery.ModuleSpec("soundfile", loader=None)
-        m.read = m.write = m.info = lambda *a, **k: (_ for _ in ()).throw(RuntimeError("stub"))
-        sys.modules["soundfile"] = m
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    import whisperlivekit  # noqa: F401
+    from oracle import stage_reference
+    stage_reference.import_staged_reference()
 
 
 ASR_KW = dict(decoder_type="greedy", beams=1, model_size=None, model_path=None, decoder_model_path=None,

@@ -1,4 +1,4 @@
-"""Build container only (needs /root/reference): the drop-in seam.  The reference's own
+"""Needs the staged reference (oracle/_ref): the drop-in seam.  The reference's own
 AlignAttBase.infer() drives our hooks (AlignAttHooks); with the CPU oracle standing in for the
 CUDA engine behind the same session API, the emitted tokens / attended frames must equal what the
 reference's AlignAtt produced (the golden fixtures)."""
@@ -15,14 +15,8 @@ pytestmark = pytest.mark.reference
 
 
 def _import_reference():
-    if "soundfile" not in sys.modules:
-        m = types.ModuleType("soundfile")
-        m.__spec__ = __import__("importlib.machinery").machinery.ModuleSpec("soundfile", loader=None)   # find_spec() must not choke on the stub
-        m.read = m.write = m.info = lambda *a, **k: (_ for _ in ()).throw(RuntimeError("stub"))
-        sys.modules["soundfile"] = m
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    import whisperlivekit  # noqa: F401
+    from oracle import stage_reference
+    stage_reference.import_staged_reference()
 
 
 @pytest.mark.parametrize("name", ["micro", "microml"])

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Diagnose the tcgen05 attention kernel against fp32 torch: where (rows / dims) do errors sit?"""
+"""Diagnose the wgmma attention kernel against fp32 torch: where (rows / dims) do errors sit?"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

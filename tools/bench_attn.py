@@ -21,4 +21,4 @@ e.timer_record(1)
 e.sync()
 ms = e.timer_elapsed_ms(0, 1) / iters
 exps = B * H * 1500 * 1536
-print(f"attn B={B}: {ms*1e3:.1f} us  {4.0*B*H*1500*1500*64/ms/1e9:.0f} TFLOP/s  {exps/ms/1e6/148:.2f} Gexp/s/SM  pad={os.environ.get('WLK_ATTN_SMEM_PAD','0')}")
+print(f"attn B={B}: {ms*1e3:.1f} us  {4.0*B*H*1500*1500*64/ms/1e9:.0f} TFLOP/s  {exps/ms/1e6/132:.2f} Gexp/s/SM  pad={os.environ.get('WLK_ATTN_SMEM_PAD','0')}")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Micro-benchmark of the tcgen05 GEMM (for ncu captures): python tools/bench_gemm.py M N K [iters]"""
+"""Micro-benchmark of the wgmma GEMM (for ncu captures): python tools/bench_gemm.py M N K [iters]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,4 +1,4 @@
-"""B200-native streaming Whisper engine behind WhisperLiveKit's backend surface.
+"""H100-native streaming Whisper engine behind WhisperLiveKit's backend surface.
 
 Importing the package does not load CUDA; ``whisperlivekit_b200.engine`` loads
 the in-tree C-ABI library (``csrc/libwlk_b200.so``) and raises if it is missing.

@@ -1,7 +1,7 @@
 """ctypes binding of include/wlk_b200.h (the C-ABI boundary).
 
 There is no CPU fallback: if the in-tree library is missing this raises, and
-``wlk_engine_create`` itself fails when no sm_100 device is present.
+``wlk_engine_create`` itself fails when no sm_90 device is present.
 """
 from __future__ import annotations
 
@@ -125,7 +125,6 @@ SIGNATURES = {
     "wlk_op_gemm": (C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_int64, _vp, C.c_int, C.c_int64, _vp,
                               _vp, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]),
     "wlk_op_encoder_attention": (C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_int, _vp]),
-    "wlk_op_encoder_attention_trace": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "wlk_op_median_filter": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
     "wlk_op_dtw": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _i32p]),
     "wlk_timer_record": (C.c_int, [_vp, C.c_int]),
@@ -152,7 +151,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise WlkError(
             f"{LIB_PATH} is missing: build it with `python -m whisperlivekit_b200.build` "
-            "(nvcc, sm_100a). The B200 engine has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). The H100 engine has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported

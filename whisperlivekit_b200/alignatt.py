@@ -7,7 +7,7 @@ Two things live here:
   against the engine session API (``engine.WhisperEngine``).  With
   WhisperLiveKit importable, ``plugin.make_b200_alignatt_class()`` mixes these
   into the reference's own ``AlignAttBase`` so its ``infer()`` and the
-  SimulStreaming processor run unchanged on the B200 engine.
+  SimulStreaming processor run unchanged on the H100 engine.
 * ``StreamingAlignAtt`` -- a self-contained mirror of the control flow of
   ``AlignAttBase.infer`` (align_att_base.py:174-322) and ``AlignAtt.insert_audio``
   (simul_whisper.py:219-237) on token ids only (no tokenizer/text), for hosts

@@ -3,7 +3,7 @@
 WhisperLiveKit drives every session from its own worker thread (reference audio_processor.py:543-551:
 ``await asyncio.to_thread(self.transcription.process_iter)``) and each thread issues single-session model
 calls (``_encode``, ``_get_logits_and_cross_attn``, ... -- simul_whisper/align_att_base.py:174-322).  On the
-B200 engine the unit of efficiency is a *batched* call: one ``wlk_encode`` over 96 sessions costs about as
+H100 engine the unit of efficiency is a *batched* call: one ``wlk_encode`` over 96 sessions costs about as
 much GPU time as 96 back-to-back single-session calls cost in launch latency alone.
 
 ``BatchingEngine`` keeps the per-session call surface (it duck-types ``WhisperEngine``) and coalesces

@@ -1,7 +1,4 @@
-"""In-tree build of the C-ABI library (csrc/libwlk_b200.so) with nvcc for sm_100a.
-
-The .so is git-ignored but travels to the GPU box with the repo snapshot.
-"""
+"""In-tree build of the C-ABI library (csrc/libwlk_b200.so) with nvcc for sm_90a."""
 from __future__ import annotations
 
 import os
@@ -12,8 +9,8 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libwlk_b200.so")
-SOURCES = ["engine.cu", "kernels.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_tc2.cu", "attn_tc.cu", "attn_tc2.cu", "qwen.cu", "diar.cu", "vad.cu", "sortformer.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["engine.cu", "kernels.cu", "gemm_simt.cu", "gemm_tc.cu", "attn_tc.cu", "qwen.cu", "diar.cu", "vad.cu", "sortformer.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wno-subobject-linkage", "--expt-relaxed-constexpr"]
 
 

@@ -1,4 +1,4 @@
-// Shared declarations for the B200 streaming-Whisper engine (sm_100a only).
+// Shared declarations for the streaming-Whisper engine (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -43,7 +43,7 @@ struct Error {
 
 // ---------------------------------------------------------------------------------
 // Programmatic dependent launch for the decoder's chains of short kernels: the next kernel's CTAs become
-// resident (and run their prologue -- barrier init, TMEM allocation, weight-panel TMA) while the previous
+// resident (and run their prologue -- barrier init, weight-panel TMA) while the previous
 // kernel drains.  Contract: a kernel launched through launch_pdl() executes ptx::griddep_wait() before it
 // touches anything an earlier kernel produced (or still reads), so completion stays transitive along the
 // chain; WLK_PDL=0 turns the attribute off (plain stream order).
@@ -85,7 +85,7 @@ enum DType { DT_F32 = 0, DT_BF16 = 1, DT_BF16X2 = 2 };
 inline size_t dtype_size(int t) { return t == DT_BF16 ? 2 : 4; }
 
 // ---------------------------------------------------------------------------------
-// GEMM epilogue description shared by the SIMT and the tcgen05 GEMM kernels.
+// GEMM epilogue description shared by the SIMT and the tensor-core GEMM kernels.
 //   v = acc + bias[n];  v = act(v) (gelu: 1 erf-GELU, 2 ReLU, 3 SiLU);  if n < scale_cols: v *= col_scale;
 //   if residual: v += residual[m, n];   then stored according to `mode`.
 // ---------------------------------------------------------------------------------
@@ -137,8 +137,7 @@ constexpr size_t SK_SCRATCH_FLOATS = (size_t)8 << 20;     // 32 MB per engine
 constexpr int SK_MAX_TILES = 4096;
 
 void gemm_simt(const GemmArgs& g, cudaStream_t st);
-void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant = 0);   // 0 auto, 1 one-CTA, 2 CTA pair
-void gemm_tcgen05_pair(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms);
+void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant = 0);   // 0 auto, 1 64-wide tiles, 2 128-wide tiles
 bool gemm_tcgen05_supported(const GemmArgs& g, std::string* why);
 
 // ---------------------------------------------------------------------------------
@@ -267,8 +266,8 @@ __device__ __forceinline__ void epi_store8(const Epilogue& e, int m, int n0, con
 }
 
 // ---------------------------------------------------------------------------------
-// Factored destination addressing for the tcgen05 GEMM epilogue:
-//   address(m, n) = rowptr(m, variant) + colterm(n) * elem_size,  variant chosen per 32-column chunk.
+// Factored destination addressing for the tensor-core GEMM epilogue:
+//   address(m, n) = rowptr(m, variant) + colterm(n) * elem_size,  variant chosen per 8-column chunk.
 // rowptr is computed once per tile and row (it hides the per-batch base pointer and every div/mod on m),
 // colterm once per chunk and lane, so the per-element work is an add.
 // ---------------------------------------------------------------------------------

@@ -99,7 +99,7 @@ struct wlk_engine {
     int wt = DT_F32;                  // weight-matrix type: = act, or DT_BF16X2 (hi + lo bf16 planes) in WLK_PREC_BF16X3
     void* a_split = nullptr; size_t a_split_elems = 0;   // BF16X3: (hi, lo) planes of a GEMM's fp32 activation operand
     int gemm_backend = WLK_BACKEND_SIMT, attn_backend = WLK_BACKEND_SIMT;
-    int num_sms = 148;
+    int num_sms = 132;
     cudaStream_t st = nullptr;
     std::mutex mu;
     // token-step CUDA graphs: the ~390 launches of one decoder step depend only on the batch size (every per-session
@@ -600,7 +600,7 @@ void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev) {
                 split_f32_planes_async(reinterpret_cast<const float*>(e->qkv), hi, lo, (int64_t)M * 3 * d, e->st);
                 enc_attention_tcgen05_x3(hi, lo, n, D.n_audio_head, d, reinterpret_cast<float*>(e->att), e->st);
             } else if (e->attn_backend == WLK_BACKEND_TCGEN05)
-                enc_attention_tcgen05(e->qkv, n, D.n_audio_head, d, e->att, e->st, e->num_sms);
+                enc_attention_tcgen05(e->qkv, n, D.n_audio_head, d, e->att, e->st);
             else
                 enc_attention_simt(e->qkv, e->act, n, D.n_audio_head, d, e->att, e->st); }
         {   GemmArgs g;
@@ -698,7 +698,7 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
     const int d = D.n_audio_state, dt = D.n_text_state, nm = D.n_mels, H = D.n_audio_head;
     const size_t es = e->es();
     WLK_CHECK(e->act == DT_BF16 && e->wt == DT_BF16 && e->attn_backend == WLK_BACKEND_TCGEN05 && e->gemm_backend == WLK_BACKEND_TCGEN05,
-              "the incremental encoder runs in the bf16 tcgen05 mode only");
+              "the incremental encoder runs in the bf16 wgmma mode only");
     WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
     for (int i = 0; i < n; ++i) {
         Session& s = get_root_session(e, sids[i], "encode");
@@ -1095,13 +1095,13 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the B200 engine has no CPU fallback",
+    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the engine has no CPU fallback",
               cudaGetErrorString(ce));
     WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
     CUDA_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 10, "this library contains sm_100a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
 
     auto* e = new wlk_engine();
     e->dims = *dims; e->cfg = *cfg;
@@ -1804,24 +1804,10 @@ int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int ty
     ProfScope ps(e, WLK_KC_MISC, 4.0 * batch * e->dims.n_audio_head * (double)N_CTX * N_CTX * 64, 0);
     if (backend == WLK_BACKEND_TCGEN05) {
         WLK_CHECK(type == DT_BF16, "tcgen05 attention needs bf16");
-        enc_attention_tcgen05(qkv, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st, e->num_sms);
+        enc_attention_tcgen05(qkv, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st);
     } else {
         enc_attention_simt(qkv, type, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st);
     }
-    WLK_API_END
-}
-
-int wlk_op_encoder_attention_trace(wlk_engine* e, const void* qkv, int batch, void* out, int64_t* stamps_host /*[12][8]*/) {
-    WLK_API_BEGIN
-    LOCK(e);
-    WLK_CHECK(qkv && out && stamps_host, "null argument");
-    long long* dev = nullptr;
-    CUDA_CHECK(cudaMalloc(&dev, 96 * 8));
-    CUDA_CHECK(cudaMemsetAsync(dev, 0, 96 * 8, e->st));
-    enc_attention_tcgen05(qkv, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st, e->num_sms, dev);
-    CUDA_CHECK(cudaMemcpyAsync(stamps_host, dev, 96 * 8, cudaMemcpyDeviceToHost, e->st));
-    CUDA_CHECK(cudaStreamSynchronize(e->st));
-    cudaFree(dev);
     WLK_API_END
 }
 

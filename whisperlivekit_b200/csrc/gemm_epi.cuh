@@ -1,15 +1,13 @@
-// Shared epilogue of the tcgen05 GEMM kernels (1-CTA and CTA-pair variants).
+// Epilogue and tile rasterisation of the wgmma GEMM kernel.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace wlk {
 
-constexpr int EPI_BIAS_FLOATS = 128;   // per-warp smem scratch: the bias of the warp's 128 columns
-
 // erf-GELU for the tensor-core epilogue.  erf by Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below
 // the bf16 rounding of everything this epilogue feeds): 5 FMAs, one MUFU.RCP and one MUFU.EX2 instead of
-// the ~35-instruction erff() -- the epilogue has to drain a 128x256 tile in the ~10k cycles its MMAs take.
+// the ~35-instruction erff(): the warpgroup's tensor pipe idles while its epilogue runs.
 __device__ __forceinline__ float gelu_erf_fast(float x) {
     const float z = fabsf(x) * 0.70710678118654752440f;
     const float t = __fdividef(1.0f, fmaf(0.3275911f, z, 1.0f));
@@ -27,120 +25,52 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// One epilogue warp drains `n_chunks` 16-column chunks of its 32 accumulator rows.  tcgen05.ld hands a
-// thread one accumulator ROW, and the row stays in that thread: 16 independent values give the math its
-// instruction-level parallelism, the thread's output (and fp32 residual) is a contiguous 32-64 byte run of
-// its own row (whole sectors, 128-bit accesses), the row's destination pointer -- including every div/mod of
-// the scatter modes -- was computed once per tile (`row`), and the column part once per chunk (epi_col).
-__device__ __forceinline__ void epilogue_warp_tile(const Epilogue& epi, float* sbias, const EpiRow& row,
-                                                   uint32_t tmem_row_addr, int n_tile_base, int col_begin, int n_chunks,
-                                                   int N, int lane, const float* partials = nullptr, int splits = 1,
-                                                   int own_split = 0, int64_t split_stride = 0, int tile_ld = 0) {
+// Fused epilogue of one warpgroup's 64 x BN accumulator, straight from the wgmma fragment: a thread owns, for every
+// 8-column chunk, two adjacent columns of rows g and g + 8 (ptx.cuh), so the four lanes of a quad write one 32-byte
+// (fp32) or 16-byte (bf16) run of a row.  The rows' destination pointers -- including every div/mod of the scatter
+// modes -- are computed once per tile (`row`), the column part once per chunk (epi_col; a chunk never straddles a head).
+template <int BN>
+__device__ __forceinline__ void epilogue_fragment_tile(const Epilogue& epi, const EpiRow (&row)[2], float (&acc)[BN / 2],
+                                                       int n_tile_base, int N, int lane) {
     const int es = (epi.c_type == DT_F32) ? 4 : 2;
-    // bias of this warp's columns -> smem (each lane 4 floats), read back as broadcasts
-    if (epi.bias) {
+    const int t2 = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < EPI_BIAS_FLOATS / 32; ++j) {
-            const int n = n_tile_base + col_begin + lane + 32 * j;
-            sbias[lane + 32 * j] = (n < N && lane + 32 * j < n_chunks * 16) ? __ldg(epi.bias + n) : 0.f;
-        }
-        __syncwarp();
-    }
-#pragma unroll 1
-    for (int c = 0; c < n_chunks; ++c) {
-        const int c0 = col_begin + c * 16;
-        const int n0 = n_tile_base + c0;
-        uint32_t r[16];
-        __syncwarp();                                       // tcgen05.ld is warp-collective (.sync.aligned)
-        ptx::tmem_ld_32x16(tmem_row_addr + c0, r);
-        ptx::tmem_ld_wait();
-        if (n0 >= N) continue;
+    for (int c = 0; c < BN / 8; ++c) {
+        const int n0 = n_tile_base + c * 8;
+        if (n0 >= N) break;
         int variant;
-        const int64_t coff = epi_col(epi, n0, &variant) * es;
-        char* p = variant ? row.ptr1 : row.ptr0;
-        if (p == nullptr) continue;
-        p += coff;
-        float v[16];
+        const int64_t coff = (epi_col(epi, n0, &variant) + t2) * es;
+        const int n = n0 + t2;
+        const bool ok0 = n < N, ok1 = n + 1 < N;
+        float b0 = 0.f, b1 = 0.f;
+        if (epi.bias) { if (ok0) b0 = __ldg(epi.bias + n); if (ok1) b1 = __ldg(epi.bias + n + 1); }
+        const bool scaled = (epi.scale_period ? (n0 % epi.scale_period) : n0) < epi.scale_cols;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (partials) {
-            // split-K fix-up: this CTA arrived last at the tile; fold in the other K ranges' partial sums
-            // (fp32, [split][128 rows][tile_ld cols] in global scratch; `partials` already points at this row)
-            for (int sp = 0; sp < splits; ++sp) {
-                if (sp == own_split) continue;
-                const float4* pp = reinterpret_cast<const float4*>(partials + sp * split_stride + c0);
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                    const float4 b = __ldcg(pp + j4);
-                    v[4 * j4] += b.x; v[4 * j4 + 1] += b.y; v[4 * j4 + 2] += b.z; v[4 * j4 + 3] += b.w;
-                }
+        for (int h = 0; h < 2; ++h) {
+            char* p = variant ? row[h].ptr1 : row[h].ptr0;
+            if (p == nullptr || !ok0) continue;
+            p += coff;
+            float v0 = acc[4 * c + 2 * h] + b0, v1 = acc[4 * c + 2 * h + 1] + b1;
+            if (epi.gelu == 1) { v0 = gelu_erf_fast(v0); v1 = gelu_erf_fast(v1); }
+            else if (epi.gelu == 2) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            else if (epi.gelu == 3) { v0 = __fdividef(v0, 1.0f + __expf(-v0)); v1 = __fdividef(v1, 1.0f + __expf(-v1)); }
+            if (scaled) { v0 *= epi.col_scale; v1 *= epi.col_scale; }
+            if (row[h].res) {
+                v0 += row[h].res[n];
+                if (ok1) v1 += row[h].res[n + 1];
             }
-        }
-        if (epi.bias) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-                const float4 b = *reinterpret_cast<const float4*>(sbias + c * 16 + 4 * j4);
-                v[4 * j4] += b.x; v[4 * j4 + 1] += b.y; v[4 * j4 + 2] += b.z; v[4 * j4 + 3] += b.w;
-            }
-        }
-        if (epi.gelu == 1) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = gelu_erf_fast(v[j]);
-        } else if (epi.gelu == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (epi.gelu == 3) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __fdividef(v[j], 1.0f + __expf(-v[j]));
-        }
-        if ((epi.scale_period ? (n0 % epi.scale_period) : n0) < epi.scale_cols) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] *= epi.col_scale;
-        }
-        const bool full = (n0 + 16 <= N) && ((reinterpret_cast<uintptr_t>(p) & 15) == 0);
-        if (row.res) {
-            const float* rp = row.res + n0;
-            if (full && (reinterpret_cast<uintptr_t>(rp) & 15) == 0) {
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                    const float4 b = *reinterpret_cast<const float4*>(rp + 4 * j4);
-                    v[4 * j4] += b.x; v[4 * j4 + 1] += b.y; v[4 * j4 + 2] += b.z; v[4 * j4 + 3] += b.w;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) if (n0 + j < N) v[j] += rp[j];
-            }
-        }
-        if (full) {
             if (es == 4) {
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4)
-                    reinterpret_cast<float4*>(p)[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
+                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 7) == 0) *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+                else { reinterpret_cast<float*>(p)[0] = v0; if (ok1) reinterpret_cast<float*>(p)[1] = v1; }
             } else {
-#pragma unroll
-                for (int j8 = 0; j8 < 2; ++j8) {
-                    uint4 u;
-                    u.x = pack_bf16x2(v[8 * j8], v[8 * j8 + 1]);
-                    u.y = pack_bf16x2(v[8 * j8 + 2], v[8 * j8 + 3]);
-                    u.z = pack_bf16x2(v[8 * j8 + 4], v[8 * j8 + 5]);
-                    u.w = pack_bf16x2(v[8 * j8 + 6], v[8 * j8 + 7]);
-                    reinterpret_cast<uint4*>(p)[j8] = u;
-                }
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                if (n0 + j < N) {
-                    if (es == 4) reinterpret_cast<float*>(p)[j] = v[j];
-                    else reinterpret_cast<bf16*>(p)[j] = __float2bfloat16_rn(v[j]);
-                }
+                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 3) == 0) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(v0, v1);
+                else { reinterpret_cast<bf16*>(p)[0] = __float2bfloat16_rn(v0); if (ok1) reinterpret_cast<bf16*>(p)[1] = __float2bfloat16_rn(v1); }
             }
         }
     }
-    __syncwarp();
 }
 
-// Tile rasterisation shared by the three warp roles.  Work item t -> (m block, n block): tiles are walked
+// Tile rasterisation shared by the producer and the consumer warps.  Work item t -> (m block, n block): tiles are walked
 // in bands of `band` m-blocks, n-blocks fastest-but-one inside a band, so the ~num_sms tiles in flight at
 // any time cover one band x a few n-blocks: the band's A rows are fetched from HBM once and then served
 // from L2 for the whole sweep over n, and the few W panels in flight are shared by every CTA.
@@ -153,8 +83,8 @@ __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int ban
     *m_blk = b * band + (r - (*n_blk) * h);
 }
 
-// Pull the fp32 residual values this thread will add (its own row, `n_cols` columns from n_begin) into L2 while
-// the tile's MMAs are still running, so the epilogue's residual loads are L2 hits instead of HBM round trips.
+// Pull the fp32 residual values a row's epilogue will add (`n_cols` columns from n_begin) into L2 while the tile's
+// MMAs are still running, so the epilogue's residual loads are L2 hits instead of HBM round trips.
 __device__ __forceinline__ void epilogue_prefetch_residual(const EpiRow& row, int n_begin, int n_cols, int N) {
     if (row.res == nullptr) return;
     const char* p = reinterpret_cast<const char*>(row.res + n_begin);
@@ -162,25 +92,26 @@ __device__ __forceinline__ void epilogue_prefetch_residual(const EpiRow& row, in
     for (int off = 0; off < bytes; off += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + off));
 }
 
-// split-K, phase 1: dump this K range's raw accumulators of the warp's rows/columns to the global scratch
-__device__ __forceinline__ void epilogue_store_partials(float* dst_row /* scratch row of this thread */, bool row_valid,
-                                                        uint32_t tmem_row_addr, int col_begin, int n_chunks) {
-#pragma unroll 1
-    for (int c = 0; c < n_chunks; ++c) {
-        const int c0 = col_begin + c * 16;
-        uint32_t r[16];
-        __syncwarp();
-        ptx::tmem_ld_32x16(tmem_row_addr + c0, r);
-        ptx::tmem_ld_wait();
-        if (row_valid) {
+// split-K: this K range's raw accumulators to / from a [BM][BN] fp32 tile of the global scratch (`tile_row0` points at
+// the warpgroup's first row of that tile); same fragment positions both ways
+template <int BN>
+__device__ __forceinline__ void partials_store(float* tile_row0, const float (&acc)[BN / 2], int warp_in_wg, int lane) {
+    float* r0 = tile_row0 + (int64_t)(warp_in_wg * 16 + (lane >> 2)) * BN + 2 * (lane & 3);
 #pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4)
-                __stcg(reinterpret_cast<float4*>(dst_row + c0) + j4,
-                       make_float4(__uint_as_float(r[4 * j4]), __uint_as_float(r[4 * j4 + 1]), __uint_as_float(r[4 * j4 + 2]),
-                                   __uint_as_float(r[4 * j4 + 3])));
-        }
+    for (int c = 0; c < BN / 8; ++c) {
+        __stcg(reinterpret_cast<float2*>(r0 + c * 8), make_float2(acc[4 * c], acc[4 * c + 1]));
+        __stcg(reinterpret_cast<float2*>(r0 + 8 * BN + c * 8), make_float2(acc[4 * c + 2], acc[4 * c + 3]));
     }
-    __syncwarp();
+}
+template <int BN>
+__device__ __forceinline__ void partials_add(const float* tile_row0, float (&acc)[BN / 2], int warp_in_wg, int lane) {
+    const float* r0 = tile_row0 + (int64_t)(warp_in_wg * 16 + (lane >> 2)) * BN + 2 * (lane & 3);
+#pragma unroll
+    for (int c = 0; c < BN / 8; ++c) {
+        const float2 a = __ldcg(reinterpret_cast<const float2*>(r0 + c * 8));
+        const float2 b = __ldcg(reinterpret_cast<const float2*>(r0 + 8 * BN + c * 8));
+        acc[4 * c] += a.x; acc[4 * c + 1] += a.y; acc[4 * c + 2] += b.x; acc[4 * c + 3] += b.y;
+    }
 }
 
 bool make_tmap_bf16_2d(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,

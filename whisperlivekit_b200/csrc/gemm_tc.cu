@@ -1,13 +1,14 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = epilogue(A[M,K] * W[N,K]^T), bf16 operands, fp32 accumulate.
+// wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] * W[N,K]^T), bf16 operands, fp32 accumulate.
 //
 // Persistent, warp-specialised, one CTA per SM:
-//   warp 0      TMA producer  : cp.async.bulk.tensor 2D loads of the A (128x64) and W (BNx64) k-slabs,
-//                               128B-swizzled, into a STAGES-deep shared-memory ring (mbarrier full/empty)
-//   warp 1      MMA issuer    : one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN,
-//                               K=16) x4 per slab; accumulators live in TMEM, double-buffered (2 x BN cols)
-//   warps 2..9  epilogue      : tcgen05.ld the finished accumulator (lane = row), fused bias / GELU /
-//                               column scale / fp32 residual, then bf16 or fp32 stores (plain or scattered
-//                               into the head-major KV layouts), overlapping the next tile's MMAs.
+//   warps 0..7  MMA + epilogue: two warpgroups, each owning 64 rows of the 128 x BN tile.  Per k-slab four
+//                               wgmma.mma_async (M=64, N=BN, K=16) read both operands from shared memory and
+//                               accumulate in registers, one slab in flight while the next is issued; then the
+//                               fused bias / GELU / column scale / fp32 residual epilogue and bf16 or fp32
+//                               stores (plain or scattered into the head-major KV layouts) from the fragment.
+//   warp 8      TMA producer  : cp.async.bulk.tensor 2D loads of the A (128x64) and W (BNx64) k-slabs,
+//                               128B-swizzled, into a STAGES-deep shared-memory ring (mbarrier full/empty);
+//                               it keeps filling the ring with the next tile while the epilogue runs.
 // Tiles are walked m-fastest so the CTAs of a wave share one W panel (L2-resident) while A streams.
 #include <cudaTypedefs.h>
 
@@ -81,9 +82,8 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int UMMA_K = 16;
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;   // TMA warp, MMA warp, 8 epilogue warps
+constexpr int NUM_MMA_WARPS = 8;                        // two warpgroups, 64 rows of the tile each
+constexpr int NUM_THREADS = 32 * NUM_MMA_WARPS + 32;    // + the TMA warp (last, so the warpgroups start at warp 0 and 4)
 
 
 // X3 (WLK_PREC_BF16X3): every operand arrives as two bf16 planes, hi = bf16(x) and lo = bf16(x - hi); a k-slab stages
@@ -95,10 +95,8 @@ struct SmemLayout {
     static constexpr uint32_t PLANES = X3 ? 2 : 1;
     static constexpr uint32_t A_BYTES = BM * BK * 2;
     static constexpr uint32_t B_BYTES = BN * BK * 2;
-    static constexpr uint32_t STG_OFF = STAGES * PLANES * (A_BYTES + B_BYTES);     // epilogue bias staging
-    static constexpr uint32_t STG_BYTES = NUM_EPI_WARPS * EPI_BIAS_FLOATS * 4;   // per-warp bias scratch
-    static constexpr uint32_t BAR_OFF = STG_OFF + STG_BYTES;
-    static constexpr uint32_t TOTAL = BAR_OFF + (2 * STAGES + 4) * 8 + 16;
+    static constexpr uint32_t BAR_OFF = STAGES * PLANES * (A_BYTES + B_BYTES);
+    static constexpr uint32_t TOTAL = BAR_OFF + 2 * STAGES * 8 + 16;
     static constexpr uint32_t DYN = TOTAL + 1024;   // slack for manual 1024-byte alignment
 };
 
@@ -109,7 +107,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                int splits, float* __restrict__ sk_scratch, int* __restrict__ sk_counters, Epilogue epi) {
     using L = SmemLayout<BN, STAGES, X3>;
     constexpr uint32_t STAGE_TX = L::PLANES * (L::A_BYTES + L::B_BYTES);
-    constexpr uint32_t TMEM_COLS = 2 * BN;           // 128 / 256 / 512: powers of two >= 32
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
@@ -119,10 +116,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t sBlo = sAlo + STAGES * L::A_BYTES;              // X3 only
     const uint32_t bar_full = smem_base + L::BAR_OFF;              // [STAGES]
     const uint32_t bar_empty = bar_full + STAGES * 8;              // [STAGES]
-    const uint32_t bar_tfull = bar_empty + STAGES * 8;             // [2]
-    const uint32_t bar_tempty = bar_tfull + 16;                    // [2]
-    const uint32_t tmem_slot = bar_tempty + 16;
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -134,30 +127,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int band = max(1, (int)gridDim.x / 2);
 
     ptx::griddep_launch();
-    if (warp == 0 && lane == 0) {
+    if (warp == NUM_MMA_WARPS && lane == 0) {
         ptx::prefetch_tensormap(&tmA);
         ptx::prefetch_tensormap(&tmW);
         if (X3) { ptx::prefetch_tensormap(&tmAlo); ptx::prefetch_tensormap(&tmWlo); }
         for (int i = 0; i < STAGES; ++i) {
             ptx::mbar_init(bar_full + 8 * i, 1);
-            ptx::mbar_init(bar_empty + 8 * i, 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(bar_tfull + 8 * i, 1);
-            ptx::mbar_init(bar_tempty + 8 * i, 32 * NUM_EPI_WARPS);
+            ptx::mbar_init(bar_empty + 8 * i, NUM_MMA_WARPS);      // lane 0 of every MMA warp releases a slot
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc(tmem_slot, TMEM_COLS);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
 
-    if (warp == 0) {
+    if (warp == NUM_MMA_WARPS) {
         // ===================== TMA producer =====================
         if (lane == 0) {
             // The weight panels never depend on the previous kernel: the first ring-full of them is requested
@@ -198,97 +180,77 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = ptx::umma_idesc_bf16(BM, BN, 0, 0);
-        uint32_t stage = 0, phase = 0, it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-            const uint32_t as = it & 1, ap = (it >> 1) & 1;
-            ptx::mbar_wait(bar_tempty + 8 * as, ap ^ 1);
-            ptx::tc_fence_after();
-            const int sp = tile / num_mn;
-            const int kb_begin = sp * kb_per_split, kb_end = min(num_k_total, (sp + 1) * kb_per_split);
-            for (int kb = kb_begin; kb < kb_end; ++kb) {
-                ptx::mbar_wait(bar_full + 8 * stage, phase);
-                ptx::tc_fence_after();
-                if (lane == 0) {
-                    const uint64_t da = ptx::umma_desc_kmajor_sw128(sA + stage * L::A_BYTES);
-                    const uint64_t db = ptx::umma_desc_kmajor_sw128(sB + stage * L::B_BYTES);
-                    const uint64_t dal = ptx::umma_desc_kmajor_sw128(sAlo + stage * L::A_BYTES);
-                    const uint64_t dbl = ptx::umma_desc_kmajor_sw128(sBlo + stage * L::B_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        // advancing K by 16 bf16 = 32 bytes = +2 in the (addr >> 4) field
-                        ptx::umma_bf16_ss(tmem_base + as * BN, da + 2 * k, db + 2 * k, idesc,
-                                          (kb > kb_begin || k > 0) ? 1u : 0u);
-                        if (X3) {
-                            ptx::umma_bf16_ss(tmem_base + as * BN, dal + 2 * k, db + 2 * k, idesc, 1u);
-                            ptx::umma_bf16_ss(tmem_base + as * BN, da + 2 * k, dbl + 2 * k, idesc, 1u);
-                        }
-                    }
-                    ptx::umma_commit(bar_empty + 8 * stage);              // frees the smem slot when MMAs retire
-                    if (kb == kb_end - 1) ptx::umma_commit(bar_tfull + 8 * as);  // accumulator ready
-                }
-                __syncwarp();
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
     } else {
-        // ===================== epilogue (warps 2..9) =====================
-        // Two warps per TMEM lane quadrant, each owning half of the tile's columns (see gemm_epi.cuh).
-        const int ew = warp - 2;
-        const int q = warp & 3;                       // TMEM lane quadrant this warp may access
-        const int hc = ew >> 2;                       // which half of the tile's columns
-        float* sbias = reinterpret_cast<float*>(smem_gen + L::STG_OFF) + ew * EPI_BIAS_FLOATS;
-        volatile int* sk_flag = reinterpret_cast<volatile int*>(smem_gen + (tmem_slot - smem_base) + 8);
-        uint32_t it = 0;
+        // ===================== MMA + epilogue (warps 0..7) =====================
+        // The producer runs ahead through the ring, so the next tile's first k-slabs land while this one's epilogue runs.
+        const int wg = warp >> 2, wq = warp & 3;
+        constexpr uint32_t WG_A_OFF = 64 * BK * 2;          // the warpgroup's 64 rows of the 128-row A tile
+        volatile int* sk_flag = reinterpret_cast<volatile int*>(smem_gen + L::BAR_OFF + 2 * STAGES * 8);
+        uint32_t stage = 0, phase = 0;
         ptx::griddep_wait();                          // residual, split-K scratch and C belong to the stream's past
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int sp = tile / num_mn, mn = tile - sp * num_mn;
             int m_blk, n_blk;
             tile_coords(mn, num_m, num_n, band, &m_blk, &n_blk);
-            const uint32_t as = it & 1, ap = (it >> 1) & 1;
-            const EpiRow row = epi_row(epi, m_blk * BM + q * 32 + lane, M);
-            epilogue_prefetch_residual(row, n_blk * BN + hc * (BN / 2), BN / 2, N);
-            ptx::mbar_wait(bar_tfull + 8 * as, ap);
-            ptx::tc_fence_after();
-            const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
+            const int row0 = m_blk * BM + wg * 64 + wq * 16 + (lane >> 2);
+            const EpiRow rows[2] = {epi_row(epi, row0, M), epi_row(epi, row0 + 8, M)};
+            epilogue_prefetch_residual(rows[0], n_blk * BN, BN, N);
+            epilogue_prefetch_residual(rows[1], n_blk * BN, BN, N);
+            const int kb_begin = sp * kb_per_split, kb_end = min(num_k_total, (sp + 1) * kb_per_split);
+            float acc[BN / 2];
+            int prev = -1;                            // slot whose MMAs are still in flight
+            for (int kb = kb_begin; kb < kb_end; ++kb) {
+                ptx::mbar_wait(bar_full + 8 * stage, phase);
+                const uint64_t da = ptx::wgmma_desc_sw128(sA + stage * L::A_BYTES + wg * WG_A_OFF);
+                const uint64_t db = ptx::wgmma_desc_sw128(sB + stage * L::B_BYTES);
+                const uint64_t dal = ptx::wgmma_desc_sw128(sAlo + stage * L::A_BYTES + wg * WG_A_OFF);
+                const uint64_t dbl = ptx::wgmma_desc_sw128(sBlo + stage * L::B_BYTES);
+                ptx::wgmma_fence_regs(acc);
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    // advancing K by 16 bf16 = 32 bytes = +2 in the (addr >> 4) field
+                    ptx::WgmmaSS<BN>::mma(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1u : 0u);
+                    if (X3) {
+                        ptx::WgmmaSS<BN>::mma(acc, dal + 2 * k, db + 2 * k, 1u);
+                        ptx::WgmmaSS<BN>::mma(acc, da + 2 * k, dbl + 2 * k, 1u);
+                    }
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_wait<1>();                 // the previous slab's MMAs have retired: its slot is free
+                if (prev >= 0 && lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            ptx::wgmma_wait<0>();
+            ptx::wgmma_fence_regs(acc);
+            if (prev >= 0 && lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
             if (splits > 1) {
                 // Split-K with a serial fix-up: every CTA of a tile parks its raw partial sums in global scratch;
                 // the one that arrives last (atomic ticket) adds the others to its own accumulators and runs the
                 // normal fused epilogue, so any output type / scatter mode works.
                 const int64_t split_stride = (int64_t)num_mn * BM * BN;
-                float* my_row = sk_scratch + ((int64_t)sp * num_mn + mn) * BM * BN + (int64_t)(q * 32 + lane) * BN;
-                const bool row_valid = (m_blk * BM + q * 32 + lane) < M;
-                epilogue_store_partials(my_row, row_valid, tacc, hc * (BN / 2), BN / 32);
+                float* tile0 = sk_scratch + (int64_t)mn * BM * BN + (int64_t)wg * 64 * BN;
+                partials_store<BN>(tile0 + sp * split_stride, acc, wq, lane);
                 __threadfence();
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_EPI_WARPS) : "memory");
-                if (ew == 0 && lane == 0) {
+                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_MMA_WARPS) : "memory");
+                if (warp == 0 && lane == 0) {
                     const int old = atomicAdd(sk_counters + mn, 1);
                     const int last = (old == splits - 1);
                     if (last) sk_counters[mn] = 0;                    // every split has arrived: re-arm for the next launch
                     *sk_flag = last;
                 }
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_EPI_WARPS) : "memory");
+                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_MMA_WARPS) : "memory");
                 const int last = *sk_flag;
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_EPI_WARPS) : "memory");   // flag may be rewritten next tile
-                if (last) {
-                    __threadfence();
-                    const float* base_row = sk_scratch + (int64_t)mn * BM * BN + (int64_t)(q * 32 + lane) * BN;
-                    epilogue_warp_tile(epi, sbias, row, tacc, n_blk * BN, hc * (BN / 2), BN / 32, N, lane,
-                                       base_row, splits, sp, split_stride, BN);
-                }
-            } else {
-                epilogue_warp_tile(epi, sbias, row, tacc, n_blk * BN, hc * (BN / 2), BN / 32, N, lane);
+                asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_MMA_WARPS) : "memory");   // flag may be rewritten next tile
+                if (!last) continue;
+                __threadfence();
+                for (int s2 = 0; s2 < splits; ++s2)
+                    if (s2 != sp) partials_add<BN>(tile0 + s2 * split_stride, acc, wq, lane);
             }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(bar_tempty + 8 * as);
+            epilogue_fragment_tile<BN>(epi, rows, acc, n_blk * BN, N, lane);
         }
     }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 
@@ -356,7 +318,7 @@ void launch(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t 
 }  // namespace
 
 void split_f32_planes_async(const float* src, bf16* hi, bf16* lo, int64_t n, cudaStream_t st) {
-    int grid = (int)std::min<int64_t>((n / 4 + 255) / 256, 148 * 8);
+    int grid = (int)std::min<int64_t>((n / 4 + 255) / 256, 132 * 8);
     if (grid < 1) grid = 1;
     CUDA_CHECK(launch_pdl(split_f32_kernel, dim3(grid), dim3(256), 0, st, src, hi, lo, n));
 }
@@ -395,25 +357,21 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         split_f32_planes_async(reinterpret_cast<const float*>(g.A), hi, lo, n, st);
         A_hi = hi; A_lo = lo;
     }
-    // Large problems go to the CTA-pair kernel (256x256 tiles, half the operand traffic per MAC); the
-    // one-CTA kernel serves narrow or short problems with smaller tiles so the grid still covers the SMs.
-    const int tiles_pair = ((g.M + 255) / 256) * ((g.N + 255) / 256);
-    if (variant == 2 || (variant == 0 && g.N >= 256 && g.M >= 256 && tiles_pair >= num_sms / 2)) {
-        gemm_tcgen05_pair(g, A_hi, A_lo, st, num_sms);
-        return;
-    }
-    // tuning hooks (WLK_GEMM_VARIANT): 3 = <64,8>, 4 = <32,10>, 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4
-    if (variant >= 3 && variant <= 8) {
+    // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = <128,6>, 4 = <32,10>,
+    // 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4
+    if (variant == 2) { launch<128, 6, 3>(g, A_hi, A_lo, st, num_sms); return; }
+    if (variant == 1 || (variant >= 4 && variant <= 8)) {
         const int num_k = (g.K + BK - 1) / BK;
         int sp = (variant == 5 || variant == 7) ? 2 : (variant == 6 || variant == 8) ? 4 : 1;
         if (sp > num_k / 2) sp = 1;
-        if (variant == 3 || variant == 5 || variant == 6) launch<64, 8, 4>(g, A_hi, A_lo, st, num_sms, sp);
+        const int kbps = (num_k + sp - 1) / sp;
+        sp = (num_k + kbps - 1) / kbps;                       // no empty K range
+        if (variant == 1 || variant == 5 || variant == 6) launch<64, 8, 4>(g, A_hi, A_lo, st, num_sms, sp);
         else launch<32, 10, 5>(g, A_hi, A_lo, st, num_sms, sp);
         return;
     }
-    const int tiles256 = ((g.M + BM - 1) / BM) * ((g.N + 255) / 256);
-    if (g.N >= 256 && tiles256 >= num_sms) launch<256, 4, 2>(g, A_hi, A_lo, st, num_sms);
-    else if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) launch<128, 6, 3>(g, A_hi, A_lo, st, num_sms);
+    // 128-wide tiles while they still cover half the SMs, else 64-wide ones
+    if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) launch<128, 6, 3>(g, A_hi, A_lo, st, num_sms);
     else {
         // Short, narrow problems (the decoder's per-token GEMMs) cannot fill the GPU with output tiles alone and
         // a CTA walking all of K pays one TMA round trip per ring refill.  The K range is split across CTAs
@@ -421,7 +379,7 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         const int tiles64 = ((g.M + BM - 1) / BM) * ((g.N + 63) / 64);
         const int num_k = (g.K + BK - 1) / BK;
         int splits = 1;
-        // (measured: the fix-up costs ~6 us, a ring refill ~2.4 us -- it pays from ~40 k-slabs, i.e. K = 5120)
+        // (the fix-up is a round trip through global memory: it only pays for long K, from ~40 k-slabs, i.e. K = 5120)
         if (tiles64 < num_sms && num_k >= 40) {
             splits = num_sms / tiles64;
             if (splits > num_k / 8) splits = num_k / 8;       // at least one full ring (8 k-slabs) per split

@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the streaming-Whisper hot path (sm_100a).  Everything here is
+// Non-GEMM kernels of the streaming-Whisper hot path (sm_90a).  Everything here is
 // bandwidth- or latency-bound SIMT code; the tensor-core kernels live in gemm_tc.cu / attn_tc.cu.
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -103,13 +103,15 @@ mel_power_kernel(const MelJob* __restrict__ jobs, int n_mels, const float* __res
         ptx::mbar_wait(bar, 0);
     }
     for (int i = tid; i < N_FFT; i += 224) tw[i] = twiddle[i];
+    // __fmul_rn: the product is rounded on its own in both branches (never contracted into the sums below), so a frame has
+    // the same bits whether its CTA staged or gathered -- the incremental front end keeps rows across that difference
     auto sample = [&](int fr, int j) -> float {         // windowed sample j of frame fr
-        if (staged) return stage[fr * HOP + j] * window[j];
+        if (staged) return __fmul_rn(stage[fr * HOP + j], window[j]);
         int s = (f0 + fr) * HOP - HALF + j;             // torch.stft(center=True): reflect pad n_fft/2
         if (s < 0) s = -s;
         if (job.pad && s >= job.n) s = 2 * (job.n - 1) - s;  // streaming window: reflect at the right edge too
         const float x = (s >= 0 && s < job.n) ? job.audio[s] : 0.f;   // right of the audio: the appended zeros
-        return x * window[j];
+        return __fmul_rn(x, window[j]);
     };
     for (int i = tid; i < FR * HALF; i += 224) {
         const int fr = i / HALF, j = i - fr * HALF;

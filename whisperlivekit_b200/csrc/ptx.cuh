@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the
-// tcgen05 kernels: mbarrier, TMA (cp.async.bulk.tensor), TMEM alloc/ld, tcgen05.mma/commit.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the tensor-core
+// kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors / mma_async / commit / wait.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -91,90 +91,97 @@ __device__ __forceinline__ void tma_load_1d(uint32_t smem_dst, const void* gsrc,
         : "memory");
 }
 
-// ---- TMEM -----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_result), "r"(ncols)
-                 : "memory");
+// ---- wgmma (bf16 x bf16 -> fp32; one warpgroup = 4 warps computes 64 rows) ---------------------
+// Accumulator fragment of m64nN: thread (g = lane / 4, t = lane % 4) of warp w holds, for every 8-column chunk c,
+// d[4c + 0..1] = (row 16w + g, cols 8c + 2t, +1) and d[4c + 2..3] = (row 16w + g + 8, same cols).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING> __device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp gets lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+// keeps the compiler from moving reads or writes of accumulator registers across an asynchronous wgmma boundary
+template <int N> __device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-// ---- tcgen05.mma (bf16 x bf16 -> fp32, operands in shared memory) ---------------------------
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart).
-// Field layout: cute::UMMA::SmemDescriptor (cute/arch/mma_sm100_desc.hpp).
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
+// 128-byte-swizzled operand tile as TMA writes it: rows of 64 bf16 (128 B), 8-row groups 1024 B apart.  The same
+// descriptor serves a K-major operand (rows are M or N) and, with the instruction's transpose bit, an MN-major one
+// (rows are K, one 64-wide atom along MN).  Field layout: cute::GmmaDescriptor (cute/arch/mma_sm90_desc.hpp).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);        // start address, bits [0,14)
-    d |= static_cast<uint64_t>(0) << 16;                             // leading byte offset (unused: 1 atom in K)
+    d |= static_cast<uint64_t>(1) << 16;                             // leading byte offset (unused: one swizzle atom)
     d |= static_cast<uint64_t>(1024u >> 4) << 32;                    // stride byte offset between 8-row groups
-    d |= static_cast<uint64_t>(1) << 46;                             // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(2) << 61;                             // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;                             // SWIZZLE_128B
     return d;
 }
-// MN-major, 128-byte-swizzled operand tile: rows are K, each row 64 bf16 (128 B) along MN.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;   // between 64-wide MN atoms
-    d |= static_cast<uint64_t>(1024u >> 4) << 32;                    // between 8-row K groups
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory
+template <int N> struct WgmmaSS;
+template <> struct WgmmaSS<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+            "%16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+    }
+};
+template <> struct WgmmaSS<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+    }
+};
+template <> struct WgmmaSS<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+    }
+};
+// D[64 x 64] += A * B with A (64 x 16 bf16) in registers -- the accumulator fragment of a previous wgmma, packed to bf16 --
+// and B MN-major in shared memory (rows are K): the P V product of the attention kernels.
+__device__ __forceinline__ void wgmma_rs_n64_bt(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+      "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+      "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+      "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1u));
 }
-// cute::UMMA::InstrDescriptor: bf16 A/B, fp32 accumulate, dense.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4)                       // c_format = F32
-           | (1u << 7)                     // a_format = BF16
-           | (1u << 10)                    // b_format = BF16
-           | (static_cast<uint32_t>(a_mn_major) << 15) | (static_cast<uint32_t>(b_mn_major) << 16)
-           | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
+
 
 }  // namespace ptx
 }  // namespace wlk

@@ -204,7 +204,7 @@ using namespace wlk;
 struct wlk_qwen {
     wlk_qwen_dims dims{};
     wlk_config cfg{};
-    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 148;
+    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
     int ring = 0, max_rows = 0;
     cudaStream_t st = nullptr;
     std::mutex mu;
@@ -396,12 +396,12 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the B200 engine has no CPU fallback", cudaGetErrorString(ce));
+    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the H100 engine has no CPU fallback", cudaGetErrorString(ce));
     WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
     CUDA_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 10, "this library contains sm_100a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
 
     auto* q = new wlk_qwen();
     q->dims = D; q->cfg = *cfg;

@@ -16,7 +16,7 @@
 //   update      SortformerModules.streaming_update_async + _compress_spkcache for every stream (one CTA per stream)
 // Streams are batched by packing their ragged sequences (<= spkcache + fifo + 25 rows each) into one row buffer: every
 // GEMM of a step sees all streams of the call; attention, the conv module and the cache update run per stream.
-// GEMMs go through the engine's tcgen05 / SIMT GEMM kernels (bf16 mode / fp32 parity mode); everything else is here.
+// GEMMs go through the engine's wgmma / SIMT GEMM kernels (bf16 mode / fp32 parity mode); everything else is here.
 #include <math.h>
 
 #include <map>
@@ -279,7 +279,7 @@ sf_attention_kernel(const T* __restrict__ qkv, const SfJob* __restrict__ jobs, i
 // bf16 mode: the same attention on warp-level tensor-core MMAs (mma.sync m16n8k16, bf16 operands, fp32 accumulate).
 // The diarizer is ~2 % of a config-4 stream's FLOPs, its sequences are <= 401 rows and the relative-position term needs
 // a per-row shift of the score tile, so a 16-query CTA with the scores staged in shared memory is the shape that fits;
-// the tcgen05 pipeline of attn_tc.cu is reserved for the 1500-position Whisper encoder.
+// the wgmma pipeline of attn_tc.cu is reserved for the 1500-position Whisper encoder.
 //   block = 16 queries of one (stream, head), 4 warps:
 //     S[i][j]  = (q_i + u) . k_j                     warps split the 8-key column tiles          -> smem fp32
 //     S[i][j] += (q_i + v) . p[c - (i - j)]          computed as a dense 16 x (T + 15) tile over the positions the block
@@ -701,7 +701,7 @@ using namespace wlk;
 struct wlk_sf {
     wlk_sf_dims dims{};
     wlk_config cfg{};
-    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 148;
+    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
     int F1 = 0, F2 = 0, F3 = 0, frames_per_chunk = 0, prev_keep = 99, chunk_samples = 0, n_freq = 0;
     int max_T = 0, max_T3 = 0, max_feat = 0, max_pop = 0, max_chunk_cap = 0;
     cudaStream_t st = nullptr;
@@ -976,12 +976,12 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the B200 engine has no CPU fallback", cudaGetErrorString(ce));
+    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the engine has no CPU fallback", cudaGetErrorString(ce));
     WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
     CUDA_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 10, "this library contains sm_100a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
 
     auto* q = new wlk_sf();
     q->dims = D; q->cfg = *cfg;

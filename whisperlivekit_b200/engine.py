@@ -2,10 +2,10 @@
 
 ``WhisperEngine`` exposes the session API the AlignAtt host code drives
 (``alignatt.StreamingAlignAtt`` / ``AlignAttHooks``); every method is one C call
-into hand-written sm_100a CUDA.  Inputs are host numpy arrays (the reference's
+into hand-written sm_90a CUDA.  Inputs are host numpy arrays (the reference's
 callers hand CPU float32 PCM, SURVEY.md §8b); device memory is owned by the
 engine.  There is no fallback path: construction raises without the library or
-without a B200.
+without a H100.
 """
 from __future__ import annotations
 

@@ -4,7 +4,7 @@ The LocalAgreement policy (reference local_agreement/online_asr.py:219-261) call
 ``asr.transcribe(audio, init_prompt)`` -> ``whisper.transcribe(model, audio, ...)``
 (local_agreement/backends.py:62-77), whose host logic (30 s seek loop, temperature fallback,
 timestamp rules, DecodingTask, add_word_timestamps/find_alignment, DTW) stays the reference's.  This
-module supplies the *model*: every tensor operation it is asked for goes to the B200 engine through
+module supplies the *model*: every tensor operation it is asked for goes to the H100 engine through
 the C ABI.  Needs WhisperLiveKit importable (it reuses the reference's decode/transcribe functions).
 
 What the reference touches on ``model`` (whisper/decoding.py:144-160,636-704; whisper/timing.py:163-215;
@@ -161,7 +161,7 @@ class B200TranscribeModel:
         m = mel.detach().cpu().float().numpy()
         if m.ndim == 3:
             if m.shape[0] != 1:
-                raise NotImplementedError("B200 LocalAgreement model: one audio segment per call")
+                raise NotImplementedError("H100 LocalAgreement model: one audio segment per call")
             m = m[0]
         # The word-timestamp pass (timing.py:197) asks for model(mel, tokens) on the very segment that
         # DecodingTask just encoded: the session still holds that encoder output and its cross-K/V, so a

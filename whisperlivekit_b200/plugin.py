@@ -1,4 +1,4 @@
-"""Registration of the B200 engine behind WhisperLiveKit's SimulStreaming/AlignAtt seam.
+"""Registration of the H100 engine behind WhisperLiveKit's SimulStreaming/AlignAtt seam.
 
 Needs WhisperLiveKit importable (it is not a dependency of the engine itself).  Nothing in
 WhisperLiveKit is modified on disk: ``install()`` swaps the ``AlignAtt`` symbol that
@@ -62,7 +62,7 @@ def make_b200_alignatt_class():
 
 def install(precision: str = "bf16", device: int = 0, max_sessions: int = 64, max_batch: int = 64,
             batching: bool = True, max_wait_s: float = 0.002, engine_factory=None, incremental_encoder: bool = False):
-    """Route WhisperLiveKit's SimulStreaming backend through the B200 engine (call once, before
+    """Route WhisperLiveKit's SimulStreaming backend through the H100 engine (call once, before
     TranscriptionEngine is constructed).  With ``batching`` the per-session calls of the worker threads
     (audio_processor.py:543-551) are coalesced into batched C-ABI calls by batching.BatchingEngine.
 
@@ -131,10 +131,10 @@ def sortformer_state_dict_from_nemo(path: str):
 
 def install_sortformer(state_dict=None, dims=None, precision: str = "bf16", device: int = 0, max_sessions: int = 64,
                        max_batch: int = 64):
-    """Route ``--diarization-backend sortformer`` through the B200 engine without editing WhisperLiveKit: core.py imports
+    """Route ``--diarization-backend sortformer`` through the H100 engine without editing WhisperLiveKit: core.py imports
     ``SortformerDiarization`` / ``SortformerDiarizationOnline`` from ``whisperlivekit.diarization.sortformer_backend``
     (core.py:297-299, 472-477), a module that exits at import when NeMo is missing (sortformer_backend.py:14-22).  This
-    puts a module of that name in ``sys.modules`` whose two classes are the B200 drop-ins, with the reference's constructor
+    puts a module of that name in ``sys.modules`` whose two classes are the H100 drop-ins, with the reference's constructor
     signatures (``SortformerDiarization(model_name=..., model_path=...)``, ``SortformerDiarizationOnline(shared_model,
     sample_rate, max_speakers)``).  Weights: ``state_dict`` (NeMo names), else ``model_path`` must point at a ``.nemo``."""
     import sys

@@ -3,7 +3,7 @@
 Mirrors how the reference drives QwenAudioCausalKVEncoder (third_party/qwen3-asr-causal/src/qwen3_asr_causal/
 causal.py:713-782): ``forward_chunk(mels, state) -> (hidden, state)`` becomes ``forward_chunk(sids, mels)`` over
 device-resident per-session state, batched over sessions.  No CPU fallback: construction fails without the CUDA
-library or a B200."""
+library or a H100."""
 from __future__ import annotations
 
 import ctypes as C

@@ -1,5 +1,5 @@
 """Drop-in for the reference's ``QwenAudioCausalKVEncoder`` (third_party/qwen3-asr-causal/src/qwen3_asr_causal/
-causal.py:60-782) over the B200 tower engine.
+causal.py:60-782) over the H100 tower engine.
 
 The realtime model owns one encoder object and threads a per-stream state through it
 (``audio_hidden, state.audio = self.audio_encoder.forward_chunk(mels, state.audio)``, causal.py:841;

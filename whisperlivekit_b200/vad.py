@@ -86,7 +86,7 @@ class B200VadModel:
     def __call__(self, x, sr: int = 16000):
         import torch
         if sr != 16000:
-            raise ValueError("the B200 VAD engine implements the 16 kHz branch")
+            raise ValueError("the H100 VAD engine implements the 16 kHz branch")
         a = x.detach().cpu().float().numpy() if hasattr(x, "detach") else np.asarray(x, np.float32)
         a = a.reshape(-1)
         if a.shape[0] != WINDOW:

@@ -1,4 +1,4 @@
-"""Weight containers for the B200 streaming-Whisper engine.
+"""Weight containers for the H100 streaming-Whisper engine.
 
 * ``synthetic_state_dict`` – seeded "trained-like" random weights with the
   reference's parameter names (reference whisperlivekit/whisper/model.py:224-332;
