@@ -254,6 +254,54 @@ int wlk_qwen_flush_pending(wlk_qwen* q, const int32_t* sids, int n, float* out_h
                            int32_t* out_row_offsets);
 
 /* =====================================================================================
+ * Qwen3-ASR text decoder (HF Qwen3Model + lm_head, reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/
+ * model.py:1498-1507) with a croppable per-session KV cache [L][2][n_kv_head][max_ctx][head_dim].  Tensor names are
+ * Qwen3Model's (embed_tokens.weight, layers.N.self_attn.{q,k,v,o}_proj.weight, layers.N.self_attn.{q,k}_norm.weight,
+ * layers.N.mlp.{gate,up,down}_proj.weight, layers.N.{input,post_attention}_layernorm.weight, norm.weight) plus
+ * lm_head.weight when the head is not tied; fp32 on the host.  max_batch bounds the sessions of one call, and one forward
+ * keeps at most max_batch * 288 logit rows (a full batch of verify blocks: drafts of up to 287 tokens per session).
+ * A forward and the pick / logits call that reads its rows form one phase: the engine keeps only the last forward's rows,
+ * so one engine serves one driving thread at a time.
+ * ===================================================================================== */
+typedef struct wlk_qtext wlk_qtext;
+typedef struct {
+    int32_t vocab, d_model, n_layer, n_head, n_kv_head;
+    int32_t head_dim;            /* 128 */
+    int32_t ffn_dim;
+    int32_t tied;                /* 1: lm_head is embed_tokens */
+    int32_t max_ctx;             /* positions per session */
+    float rope_theta, rms_eps;
+} wlk_qtext_dims;
+
+int wlk_qtext_create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out);
+int wlk_qtext_destroy(wlk_qtext* t);
+int wlk_qtext_load_tensor(wlk_qtext* t, const char* name, const float* host, const int64_t* shape, int ndim);
+int wlk_qtext_finalize_weights(wlk_qtext* t);
+int wlk_qtext_memory(wlk_qtext* t, size_t* weights, size_t* sessions, size_t* workspace);
+int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid);
+int wlk_qtext_session_close(wlk_qtext* t, int32_t sid);
+int wlk_qtext_session_reset(wlk_qtext* t, int32_t sid);
+int wlk_qtext_session_len(wlk_qtext* t, int32_t sid, int32_t* len);
+/* DynamicCache.crop: keep the first len positions (len <= current length) */
+int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len);
+/* One forward over n sessions.  Session i appends rows row_offsets[i] .. row_offsets[i+1] at its positions len .. ;
+ * row r is token row_src[r] (>= 0, gathered from embed_tokens) or host embedding row embeds_host[-1 - row_src[r]]
+ * ([k][d_model] fp32).  The final norm of the last logit_rows[i] rows of each session is kept, in session order, for
+ * wlk_qtext_pick / wlk_qtext_logits.  A forward that would pass max_ctx fails ("context full") and changes nothing. */
+int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
+                      const float* embeds_host, int32_t n_embeds, const int32_t* logit_rows);
+/* The greedy decode controls of _GreedyControlSession.controlled_logits + argmax (model.py:335-418) over every logit row
+ * of the last forward: suppress -> repetition penalty on the unique in-vocab history -> n-gram ban -> max-consecutive
+ * -> argmax (lowest index on ties).  Row j's history is hist_tokens[hist_off[j] .. hist_off[j] + hist_len[j]).
+ * wait_token_id < 0, or a wait token that is also in `suppress`, disarms max-consecutive (model.py:1067-1072).  picks_out[j] (int32) and the controlled value of the pick (value_out, may be null). */
+int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_tokens, const int32_t* hist_off,
+                   const int32_t* hist_len, const int32_t* suppress, int32_t n_suppress, float repetition_penalty,
+                   int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id, int32_t* picks_out,
+                   float* value_out);
+/* raw lm_head outputs [n_rows][vocab] fp32 of logit rows row0 .. row0 + n_rows of the last forward */
+int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host);
+
+/* =====================================================================================
  * Step after the diarization forward (SURVEY.md section 8f item 4).  Replaces SortformerDiarizationOnline.
  * _process_predictions (reference whisperlivekit/diarization/sortformer_backend.py:313-363): for every stream the last
  * len_prediction[i] frames of its device-resident predictions preds_dev[i] = [n_frames_total[i]][n_spk] fp32 are reduced

@@ -24,6 +24,12 @@ class wlk_qwen_dims(C.Structure):
         "chunk_frames", "block_frames", "left_context_steps", "block_bidirectional", "conv_out_bias", "mutable_tail_steps")]
 
 
+class wlk_qtext_dims(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in (
+        "vocab", "d_model", "n_layer", "n_head", "n_kv_head", "head_dim", "ffn_dim", "tied", "max_ctx")] + [
+        (n, C.c_float) for n in ("rope_theta", "rms_eps")]
+
+
 class wlk_sf_dims(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "n_mels", "n_fft", "win_length", "hop", "conv_channels", "d_model", "n_head", "n_layer", "ff_mult", "conv_kernel",
@@ -83,6 +89,20 @@ SIGNATURES = {
     "wlk_qwen_forward_chunk": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp]),
     "wlk_qwen_append_audio": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp, C.c_int32]),
     "wlk_qwen_flush_pending": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int64, _vp]),
+    "wlk_qtext_create": (C.c_int, [_vp, _vp, _vp]),
+    "wlk_qtext_destroy": (C.c_int, [_vp]),
+    "wlk_qtext_load_tensor": (C.c_int, [_vp, C.c_char_p, _vp, _vp, C.c_int]),
+    "wlk_qtext_finalize_weights": (C.c_int, [_vp]),
+    "wlk_qtext_memory": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "wlk_qtext_session_open": (C.c_int, [_vp, _vp]),
+    "wlk_qtext_session_close": (C.c_int, [_vp, C.c_int32]),
+    "wlk_qtext_session_reset": (C.c_int, [_vp, C.c_int32]),
+    "wlk_qtext_session_len": (C.c_int, [_vp, C.c_int32, _vp]),
+    "wlk_qtext_crop": (C.c_int, [_vp, C.c_int32, C.c_int32]),
+    "wlk_qtext_forward": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int32, _vp]),
+    "wlk_qtext_pick": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32,
+                                 C.c_int32, _vp, _vp]),
+    "wlk_qtext_logits": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp]),
     "wlk_select": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp]),
     "wlk_vad_create": (C.c_int, [C.c_int, C.c_int, _vp]),
     "wlk_vad_destroy": (C.c_int, [_vp]),

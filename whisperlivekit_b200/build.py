@@ -9,7 +9,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libwlk_b200.so")
-SOURCES = ["engine.cu", "kernels.cu", "gemm_simt.cu", "gemm_tc.cu", "attn_tc.cu", "qwen.cu", "diar.cu", "vad.cu", "sortformer.cu"]
+SOURCES = ["engine.cu", "kernels.cu", "gemm_simt.cu", "gemm_tc.cu", "attn_tc.cu", "qwen.cu", "qwen_text.cu", "diar.cu", "vad.cu", "sortformer.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wno-subobject-linkage", "--expt-relaxed-constexpr"]
 

@@ -1,0 +1,930 @@
+// Qwen3-ASR text decoder (HF Qwen3Model + lm_head) behind the C ABI (wlk_qtext_* in include/wlk_b200.h).
+//   reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/model.py:
+//     text model wiring :1498-1507, generate_full_hypothesis_rolling :991-1250,
+//     generate_full_hypothesis_from_cached_audio :839-989, _GreedyControlSession :254-438
+// The host drives the generate logic (whisperlivekit_b200/qwen_text_engine.py); this file owns the forward over a
+// croppable per-session KV cache and the decode controls + argmax over the logit rows.
+//
+// Data layout (per round, R <= QT_ROUND_ROWS rows packed over the sessions of the call, each session's rows in position
+// order, so a row always finds the keys of its predecessors either in earlier rounds or in this round's scatter):
+//   residual x   fp32 [R][d];  xn act [R][d];  qkv fp32 [R][(H + 2 KV) * 128];  q act [R][H * 128];
+//   K/V per session act [L][K|V][KV][max_ctx][128] (written by the QK-norm + RoPE kernel);  gate|up fp32 [R][2F]
+//   hlog act [logit rows][d]: final-normed rows the lm_head runs on, in groups of logit_group rows (256 MB of fp32 logits)
+#include <map>
+#include <mutex>
+#include <set>
+#include <string>
+#include <vector>
+
+#include "../../include/wlk_b200.h"
+#include "kernels.cuh"
+
+namespace wlk {
+namespace {
+
+constexpr int QT_HD = 128;              // head_dim the kernels specialise on
+constexpr int QT_ROUND_ROWS = 1024;     // rows of one forward round (workspace bound)
+constexpr size_t QT_LOGIT_BYTES = (size_t)256 << 20;   // logits workspace: lm_head + pick run in groups of rows that fit
+constexpr int QT_PICK_THREADS = 512;
+
+__device__ __forceinline__ float block_reduce_sum(float v, float* red) {
+    v = warp_sum(v);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (l == 0) red[w] = v;
+    __syncthreads();
+    float r = 0.f;
+    for (int i = 0; i < nw; ++i) r += red[i];
+    return r;
+}
+
+// x[r] = embed_tokens[src] (src >= 0) or the uploaded host row up[-1 - src]
+__global__ void qt_embed_kernel(const int32_t* __restrict__ src, const float* __restrict__ emb, const float* __restrict__ up,
+                                float* __restrict__ x, int d) {
+    const int r = blockIdx.x;
+    const int s = src[r];
+    const float* from = s >= 0 ? emb + (int64_t)s * d : up + (int64_t)(-1 - s) * d;
+    for (int i = threadIdx.x; i < d; i += blockDim.x) x[(int64_t)r * d + i] = from[i];
+}
+
+// Qwen3RMSNorm: w * (x * rsqrt(mean(x^2) + eps)), fp32 statistics; out row = out_row ? out_row[r] : r (skip when < 0)
+template <typename T>
+__global__ void qt_rmsnorm_kernel(const float* __restrict__ x, const float* __restrict__ w, T* __restrict__ out,
+                                  const int32_t* __restrict__ out_row, int d, float eps) {
+    __shared__ float red[32];
+    const int r = blockIdx.x;
+    const int o = out_row ? out_row[r] : r;
+    if (o < 0) return;
+    const float* xr = x + (int64_t)r * d;
+    float s = 0.f;
+    for (int i = threadIdx.x; i < d; i += blockDim.x) s += xr[i] * xr[i];
+    s = block_reduce_sum(s, red);
+    const float inv = rsqrtf(s / (float)d + eps);
+    for (int i = threadIdx.x; i < d; i += blockDim.x) out[(int64_t)o * d + i] = from_f32<T>(w[i] * (xr[i] * inv));
+}
+
+// After the fused QKV GEMM: per-head RMSNorm (q_norm / k_norm over 128 dims), HF rotate-half RoPE at the row's position,
+// q -> qout [R][H*128], k / v -> the session cache.  grid (R, H + 2 KV), 128 threads (one per dim).
+template <typename T>
+__global__ void __launch_bounds__(QT_HD)
+qt_qk_rope_kernel(const float* __restrict__ qkv, const float* __restrict__ qn, const float* __restrict__ kn,
+                  const float* __restrict__ inv_freq, const int32_t* __restrict__ row_pos, const int32_t* __restrict__ row_slot,
+                  void* const* __restrict__ kv_ptrs, T* __restrict__ qout, int layer, int H, int KV, int max_ctx, float eps) {
+    __shared__ float red[4];
+    __shared__ float vals[QT_HD];
+    const int r = blockIdx.x, hh = blockIdx.y, i = threadIdx.x;
+    const int W = (H + 2 * KV) * QT_HD;
+    float v = qkv[(int64_t)r * W + hh * QT_HD + i];
+    const int pos = row_pos[r];
+    T* kvbase = reinterpret_cast<T*>(kv_ptrs[row_slot[r]]);
+    if (hh >= H + KV) {                                            // v head: straight to the cache
+        const int kh = hh - H - KV;
+        kvbase[((((int64_t)layer * 2 + 1) * KV + kh) * max_ctx + pos) * QT_HD + i] = from_f32<T>(v);
+        return;
+    }
+    const float s = block_reduce_sum(v * v, red);
+    v = (hh < H ? qn[i] : kn[i]) * (v * rsqrtf(s / (float)QT_HD + eps));
+    vals[i] = v;
+    __syncthreads();
+    const int j = i & (QT_HD / 2 - 1);
+    const float ang = (float)pos * inv_freq[j];
+    const float c = cosf(ang), sn = sinf(ang);
+    const float rot = i < QT_HD / 2 ? -vals[i + QT_HD / 2] : vals[i - QT_HD / 2];
+    const float o = v * c + rot * sn;
+    if (hh < H) qout[(int64_t)r * H * QT_HD + hh * QT_HD + i] = from_f32<T>(o);
+    else kvbase[((((int64_t)layer * 2 + 0) * KV + (hh - H)) * max_ctx + pos) * QT_HD + i] = from_f32<T>(o);
+}
+
+// fp32 mode: causal GQA attention over the session cache: the query at position p attends to cache positions 0 .. p (its own
+// block's keys were scattered before this kernel).  grid (R, KV); one warp per query head of the KV group, so the
+// group's heads stream the same K/V rows (L1-shared) instead of one pass per head.  Online fp32 softmax, scale 128^-0.5.
+template <typename T>
+__global__ void __launch_bounds__(256)
+qt_attention_kernel(const T* __restrict__ q, const int32_t* __restrict__ row_pos, const int32_t* __restrict__ row_slot,
+                    void* const* __restrict__ kv_ptrs, T* __restrict__ out, int layer, int H, int KV, int max_ctx) {
+    __shared__ float qs[8][QT_HD];
+    const int r = blockIdx.x, kh = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int G = H / KV;
+    if (warp >= G) return;
+    const int h = kh * G + warp;
+    const int pos = row_pos[r];
+    const T* kv = reinterpret_cast<const T*>(kv_ptrs[row_slot[r]]);
+    const T* kb = kv + (((int64_t)layer * 2 + 0) * KV + kh) * max_ctx * QT_HD;
+    const T* vb = kv + (((int64_t)layer * 2 + 1) * KV + kh) * max_ctx * QT_HD;
+    const float scale = 0.08838834764831845f;                      // 128^-0.5
+#pragma unroll
+    for (int e = 0; e < 4; ++e) qs[warp][lane + 32 * e] = to_f32(q[(int64_t)r * H * QT_HD + h * QT_HD + lane + 32 * e]) * scale;
+    __syncwarp();
+    float m = -INFINITY, l = 0.f, acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int k0 = 0; k0 <= pos; k0 += 32) {
+        const int k = k0 + lane;
+        float sc = -INFINITY;
+        if (k <= pos) {
+            const T* kr = kb + (int64_t)k * QT_HD;
+            float a = 0.f;
+#pragma unroll 16
+            for (int e = 0; e < QT_HD; ++e) a = fmaf(qs[warp][e], to_f32(kr[e]), a);
+            sc = a;
+        }
+        const float mt = warp_max(sc);
+        const float mn = fmaxf(m, mt);
+        const float corr = expf(m - mn);                           // m = -inf on the first tile: corr = 0
+        const float p = k <= pos ? expf(sc - mn) : 0.f;
+        l = l * corr + warp_sum(p);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[e] *= corr;
+        const int nk = min(32, pos + 1 - k0);
+        for (int j = 0; j < nk; ++j) {
+            const float pj = __shfl_sync(0xffffffffu, p, j);
+            const T* vr = vb + (int64_t)(k0 + j) * QT_HD;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) acc[e] = fmaf(pj, to_f32(vr[lane + 32 * e]), acc[e]);
+        }
+        m = mn;
+    }
+    const float inv = 1.0f / l;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) out[(int64_t)r * H * QT_HD + h * QT_HD + lane + 32 * e] = from_f32<T>(acc[e] * inv);
+}
+
+// bf16 mode: the same attention on warp-level tensor cores (mma.sync m16n8k16, bf16 operands, fp32 accumulate).
+// One CTA per (tile of <= 16 consecutive query rows of one session, KV head), one warp per query head of the group:
+// the CTA stages 64-key K and V tiles in shared memory once and every head of the group runs its 16 x 64 score MMA,
+// the online fp32 softmax and the P V MMA on them, so a tile's K/V leave HBM once per KV group.  Rows past n_rows of a
+// tile carry zero queries and are not stored; row r attends to keys 0 .. pos0 + r.
+struct QTAttnTile { int32_t row0, n_rows, slot, pos0; };
+constexpr int QT_KT = 64;                         // keys per shared-memory tile
+constexpr int QT_KPAD = QT_HD + 8;                // padded row: the fragment loads of a quad hit distinct banks
+
+__device__ __forceinline__ void qt_mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ uint32_t qt_pack(float lo, float hi) {
+    __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ uint32_t qt_pack_bf(bf16 lo, bf16 hi) {
+    return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
+}
+
+__global__ void __launch_bounds__(256)
+qt_attention_mma_kernel(const bf16* __restrict__ q, const QTAttnTile* __restrict__ tiles, void* const* __restrict__ kv_ptrs,
+                        bf16* __restrict__ out, int layer, int H, int KV, int max_ctx) {
+    __shared__ __align__(16) bf16 ks[QT_KT][QT_KPAD];
+    __shared__ __align__(16) bf16 vs[QT_KT][QT_KPAD];
+    const QTAttnTile tl = tiles[blockIdx.x];
+    const int kh = blockIdx.y, G = H / KV, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int h = kh * G + warp;
+    const bf16* kv = reinterpret_cast<const bf16*>(kv_ptrs[tl.slot]);
+    const bf16* kb = kv + (((int64_t)layer * 2 + 0) * KV + kh) * max_ctx * QT_HD;
+    const bf16* vb = kv + (((int64_t)layer * 2 + 1) * KV + kh) * max_ctx * QT_HD;
+    const int kend = tl.pos0 + tl.n_rows;
+    const bool ok0 = g < tl.n_rows, ok1 = g + 8 < tl.n_rows;
+    const bf16* q0 = q + (int64_t)(tl.row0 + g) * H * QT_HD + h * QT_HD;
+    const bf16* q1 = q + (int64_t)(tl.row0 + g + 8) * H * QT_HD + h * QT_HD;
+    uint32_t qa[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+        const int c = kk * 16 + 2 * t;
+        qa[kk][0] = ok0 ? *reinterpret_cast<const uint32_t*>(q0 + c) : 0u;
+        qa[kk][1] = ok1 ? *reinterpret_cast<const uint32_t*>(q1 + c) : 0u;
+        qa[kk][2] = ok0 ? *reinterpret_cast<const uint32_t*>(q0 + c + 8) : 0u;
+        qa[kk][3] = ok1 ? *reinterpret_cast<const uint32_t*>(q1 + c + 8) : 0u;
+    }
+    const int lim0 = min(tl.pos0 + g, kend - 1), lim1 = min(tl.pos0 + g + 8, kend - 1);
+    const float scale = 0.08838834764831845f;                      // 128^-0.5
+    float o[16][4];
+#pragma unroll
+    for (int n = 0; n < 16; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    for (int k0 = 0; k0 < kend; k0 += QT_KT) {
+        __syncthreads();                                           // the previous tile is consumed
+        for (int i = threadIdx.x; i < QT_KT * (QT_HD / 8); i += blockDim.x) {
+            const int r = i / (QT_HD / 8), c = (i % (QT_HD / 8)) * 8;
+            uint4 kz = make_uint4(0, 0, 0, 0), vz = kz;
+            if (k0 + r < kend) {
+                kz = *reinterpret_cast<const uint4*>(kb + (int64_t)(k0 + r) * QT_HD + c);
+                vz = *reinterpret_cast<const uint4*>(vb + (int64_t)(k0 + r) * QT_HD + c);
+            }
+            *reinterpret_cast<uint4*>(&ks[r][c]) = kz;
+            *reinterpret_cast<uint4*>(&vs[r][c]) = vz;
+        }
+        __syncthreads();
+        float s[8][4];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+                const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&ks[8 * j + g][kk * 16 + 2 * t]);
+                const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&ks[8 * j + g][kk * 16 + 2 * t + 8]);
+                qt_mma16816(s[j], qa[kk], b0, b1);
+            }
+        }
+        float mx0 = m0, mx1 = m1;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = k0 + 8 * j + 2 * t + (e & 1);
+                const bool ok = key <= (e < 2 ? lim0 : lim1);
+                s[j][e] = ok ? s[j][e] * scale : -INFINITY;
+                if (e < 2) mx0 = fmaxf(mx0, s[j][e]); else mx1 = fmaxf(mx1, s[j][e]);
+            }
+#pragma unroll
+        for (int off = 1; off <= 2; off <<= 1) {
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
+        }
+        const float c0 = expf(m0 - mx0), c1 = expf(m1 - mx1);     // the first tile always holds key 0: mx is finite
+        float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            s[j][0] = expf(s[j][0] - mx0); s[j][1] = expf(s[j][1] - mx0);
+            s[j][2] = expf(s[j][2] - mx1); s[j][3] = expf(s[j][3] - mx1);
+            sum0 += s[j][0] + s[j][1];
+            sum1 += s[j][2] + s[j][3];
+        }
+#pragma unroll
+        for (int off = 1; off <= 2; off <<= 1) {
+            sum0 += __shfl_xor_sync(0xffffffffu, sum0, off);
+            sum1 += __shfl_xor_sync(0xffffffffu, sum1, off);
+        }
+        l0 = l0 * c0 + sum0;
+        l1 = l1 * c1 + sum1;
+#pragma unroll
+        for (int n = 0; n < 16; ++n) { o[n][0] *= c0; o[n][1] *= c0; o[n][2] *= c1; o[n][3] *= c1; }
+#pragma unroll
+        for (int kk = 0; kk < QT_KT / 16; ++kk) {
+            const uint32_t pa[4] = {qt_pack(s[2 * kk][0], s[2 * kk][1]), qt_pack(s[2 * kk][2], s[2 * kk][3]),
+                                    qt_pack(s[2 * kk + 1][0], s[2 * kk + 1][1]), qt_pack(s[2 * kk + 1][2], s[2 * kk + 1][3])};
+            const int kr = 16 * kk + 2 * t;
+#pragma unroll
+            for (int n = 0; n < 16; ++n) {
+                const int c = 8 * n + g;
+                const uint32_t b0 = qt_pack_bf(vs[kr][c], vs[kr + 1][c]);
+                const uint32_t b1 = qt_pack_bf(vs[kr + 8][c], vs[kr + 9][c]);
+                qt_mma16816(o[n], pa, b0, b1);
+            }
+        }
+        m0 = mx0; m1 = mx1;
+    }
+    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+#pragma unroll
+    for (int n = 0; n < 16; ++n) {
+        const int c = h * QT_HD + 8 * n + 2 * t;
+        if (ok0) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g) * H * QT_HD + c) = qt_pack(o[n][0] * i0, o[n][1] * i0);
+        if (ok1) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g + 8) * H * QT_HD + c) = qt_pack(o[n][2] * i1, o[n][3] * i1);
+    }
+}
+
+// SwiGLU: hid[r][j] = silu(gate[r][j]) * up[r][j], gate|up = gu[r][0:F] | gu[r][F:2F] (fp32, down_proj(act(gate) * up))
+template <typename T>
+__global__ void qt_swiglu_kernel(const float* __restrict__ gu, T* __restrict__ hid, int rows, int F) {
+    const int64_t total = (int64_t)rows * F;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / F, j = i % F;
+        const float g = gu[r * 2 * F + j], u = gu[r * 2 * F + F + j];
+        hid[i] = from_f32<T>(g / (1.0f + expf(-g)) * u);
+    }
+}
+
+struct PickArgs {
+    float* logits; int64_t ld; int vocab;
+    const int32_t* hist; const int32_t* hist_off; const int32_t* hist_len;
+    const int32_t* suppress; int n_suppress;
+    float penalty; int penalize; int ngram; int max_consec; int wait_id;
+    int32_t* picks; float* values;
+};
+
+// _GreedyControlSession.controlled_logits + argmax (model.py:335-418), one CTA per logit row, in place on the row:
+// suppress (-inf) -> repetition penalty on the unique in-vocab history (first occurrence claims the token in a shared
+// vocab bitmap) -> n-gram ban (finfo(float32).min) -> max-consecutive (only the wait score stays) -> argmax, lowest index on
+// ties.  The modified set is a few hundred ids; the argmax then reads each logit once.
+__global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
+    extern __shared__ uint32_t seen[];
+    __shared__ float bv[QT_PICK_THREADS / 32];
+    __shared__ int bi[QT_PICK_THREADS / 32];
+    const int row = blockIdx.x, tid = threadIdx.x;
+    float* lg = a.logits + (int64_t)row * a.ld;
+    const int32_t* h = a.hist + a.hist_off[row];
+    const int n = a.hist_len[row];
+    const int words = (a.vocab + 31) / 32;
+    const float fmin = -3.4028234663852886e38f;
+    for (int i = tid; i < a.n_suppress; i += blockDim.x) lg[a.suppress[i]] = -INFINITY;
+    for (int i = tid; i < words; i += blockDim.x) seen[i] = 0u;
+    __syncthreads();
+    if (a.penalize) {
+        for (int i = tid; i < n; i += blockDim.x) {
+            const int t = h[i];
+            if (t < 0 || t >= a.vocab) continue;
+            const uint32_t bit = 1u << (t & 31);
+            if (atomicOr(&seen[t >> 5], bit) & bit) continue;          // not the first occurrence
+            const float x = lg[t];
+            lg[t] = x < 0.f ? x * a.penalty : x / a.penalty;
+        }
+    }
+    __syncthreads();
+    if (a.ngram > 0) {
+        const int pre = a.ngram - 1;
+        for (int s = tid; s <= n - a.ngram; s += blockDim.x) {
+            bool match = true;
+            for (int k = 0; k < pre && match; ++k) match = h[s + k] == h[n - pre + k];
+            const int t = h[s + pre];
+            if (match && t >= 0 && t < a.vocab) lg[t] = fmin;
+        }
+    }
+    __syncthreads();
+    if (a.max_consec > 0 && a.wait_id >= 0 && a.wait_id < a.vocab && n >= a.max_consec) {
+        if (tid == 0) {                                               // every other entry is finfo.min
+            const float w = lg[a.wait_id];
+            const int pick = (w > fmin || a.wait_id == 0) ? a.wait_id : 0;
+            a.picks[row] = pick;
+            if (a.values) a.values[row] = pick == a.wait_id ? w : fmin;
+        }
+        return;
+    }
+    float best = -INFINITY;
+    int besti = 0x7fffffff;
+    for (int v = tid; v < a.vocab; v += blockDim.x) {
+        const float x = lg[v];
+        if (x > best || (x == best && v < besti)) { best = x; besti = v; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+        if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
+    }
+    if ((tid & 31) == 0) { bv[tid >> 5] = best; bi[tid >> 5] = besti; }
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+            if (bv[w] > best || (bv[w] == best && bi[w] < besti)) { best = bv[w]; besti = bi[w]; }
+        if (besti == 0x7fffffff) besti = 0;                            // NaN row: torch.argmax would say 0 too
+        a.picks[row] = besti;
+        if (a.values) a.values[row] = best;
+    }
+}
+
+struct QTLayerW {
+    void *Wqkv = nullptr, *Wo = nullptr, *Wgu = nullptr, *Wd = nullptr;
+    float *qn = nullptr, *kn = nullptr, *ln1 = nullptr, *ln2 = nullptr;
+};
+
+struct QTSession {
+    bool open = false;
+    int len = 0;
+    void* kv = nullptr;
+};
+
+}  // namespace
+}  // namespace wlk
+
+using namespace wlk;
+
+struct wlk_qtext {
+    wlk_qtext_dims dims{};
+    wlk_config cfg{};
+    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
+    cudaStream_t st = nullptr;
+    std::mutex mu;
+    std::vector<void*> allocs;
+    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0, kv_bytes = 0;
+    float *emb = nullptr, *normw = nullptr, *inv_freq = nullptr;
+    void* head = nullptr;                               // lm_head [V][d] act type (the embedding table when tied)
+    std::vector<QTLayerW> L;
+    std::set<std::string> loaded;
+    bool finalized = false;
+    float* stage_f32 = nullptr; size_t stage_cap = 0;
+    std::vector<QTSession> sess;
+    float *x = nullptr, *qkv = nullptr, *gu = nullptr, *up = nullptr, *logits = nullptr, *values_d = nullptr;
+    void *xn = nullptr, *qb = nullptr, *att = nullptr, *hid = nullptr, *hlog = nullptr;
+    int32_t* picks_d = nullptr;
+    float* up_h = nullptr;                               // pinned: the round's host embedding rows, one H2D copy per round
+    cudaEvent_t stg_ev = nullptr;                        // recorded after the last H2D copy out of stg_h / up_h
+    int32_t* pick_d = nullptr; size_t pick_cap = 0;      // device copy of a pick call's histories, suppress list, offsets
+    int logit_group = 0;
+    int up_rows = 0;                                     // rows of `up` (uploaded embedding rows)
+    int logit_cap = 0, n_logit = 0;                      // rows of hlog; rows the last forward kept
+    float* sk_scratch = nullptr; int* sk_counters = nullptr;
+    uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
+    size_t es() const { return dtype_size(act); }
+};
+
+namespace {
+
+void* talloc(wlk_qtext* t, size_t bytes, size_t* acct) {
+    void* p = nullptr;
+    if (bytes == 0) bytes = 16;
+    CUDA_CHECK(cudaMalloc(&p, bytes));
+    t->allocs.push_back(p);
+    if (acct) *acct += bytes;
+    return p;
+}
+
+void tgemm(wlk_qtext* t, GemmArgs& g) {
+    if (g.M <= 0) return;
+    g.sk_scratch = t->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
+    g.sk_counters = t->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
+    if (t->gemm_backend == WLK_BACKEND_TCGEN05) {
+        std::string why;
+        WLK_CHECK(gemm_tcgen05_supported(g, &why), "text decoder GEMM %dx%dx%d has no wgmma kernel: %s", g.M, g.N, g.K, why.c_str());
+        gemm_tcgen05(g, t->st, t->num_sms);
+    } else {
+        gemm_simt(g, t->st);
+    }
+}
+
+void put(wlk_qtext* t, const float* host, size_t n, void* dst, int dst_type) {
+    if (n > t->stage_cap) {
+        if (t->stage_f32) { CUDA_CHECK(cudaStreamSynchronize(t->st)); CUDA_CHECK(cudaFree(t->stage_f32)); }
+        CUDA_CHECK(cudaMalloc(&t->stage_f32, n * 4));
+        t->stage_cap = n;
+    }
+    CUDA_CHECK(cudaMemcpyAsync(t->stage_f32, host, n * 4, cudaMemcpyHostToDevice, t->st));
+    if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, t->stage_f32, n * 4, cudaMemcpyDeviceToDevice, t->st));
+    else convert_f32_to(t->stage_f32, dst, dst_type, (int64_t)n, t->st);
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
+}
+
+void expect(const char* name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
+    bool ok = (int)want.size() == ndim;
+    int i = 0;
+    for (int64_t w : want) { if (ok && shape[i] != w) ok = false; ++i; }
+    WLK_CHECK(ok, "tensor %s has the wrong shape for this text-decoder geometry", name);
+}
+
+void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const int64_t* shape, int ndim) {
+    const wlk_qtext_dims& D = t->dims;
+    const int d = D.d_model, F = D.ffn_dim, qd = D.n_head * QT_HD, kvd = D.n_kv_head * QT_HD;
+    int64_t n = 1;
+    for (int i = 0; i < ndim; ++i) n *= shape[i];
+    const size_t es = t->es();
+    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name.c_str(), shape, ndim, {rows, cols}); put(t, host, n, dst, t->act); };
+    auto vec = [&](float* dst, int64_t len) { expect(name.c_str(), shape, ndim, {len}); put(t, host, n, dst, DT_F32); };
+    if (name == "embed_tokens.weight") {
+        expect(name.c_str(), shape, ndim, {D.vocab, d});
+        put(t, host, n, t->emb, DT_F32);
+        if (D.tied) put(t, host, n, t->head, t->act);
+    }
+    else if (name == "lm_head.weight") { WLK_CHECK(!D.tied, "this geometry ties lm_head to embed_tokens"); mat(t->head, D.vocab, d); }
+    else if (name == "norm.weight") vec(t->normw, d);
+    else if (name.rfind("layers.", 0) == 0) {
+        const size_t dot = name.find('.', 7);
+        WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
+        const int li = atoi(name.substr(7, dot - 7).c_str());
+        WLK_CHECK(li >= 0 && li < D.n_layer, "layer index out of range in %s", name.c_str());
+        const std::string rest = name.substr(dot + 1);
+        QTLayerW& Lw = t->L[li];
+        if (rest == "self_attn.q_proj.weight") { expect(name.c_str(), shape, ndim, {qd, d}); put(t, host, n, Lw.Wqkv, t->act); }
+        else if (rest == "self_attn.k_proj.weight") { expect(name.c_str(), shape, ndim, {kvd, d}); put(t, host, n, (char*)Lw.Wqkv + (size_t)qd * d * es, t->act); }
+        else if (rest == "self_attn.v_proj.weight") { expect(name.c_str(), shape, ndim, {kvd, d}); put(t, host, n, (char*)Lw.Wqkv + (size_t)(qd + kvd) * d * es, t->act); }
+        else if (rest == "self_attn.o_proj.weight") mat(Lw.Wo, d, qd);
+        else if (rest == "self_attn.q_norm.weight") vec(Lw.qn, QT_HD);
+        else if (rest == "self_attn.k_norm.weight") vec(Lw.kn, QT_HD);
+        else if (rest == "mlp.gate_proj.weight") { expect(name.c_str(), shape, ndim, {F, d}); put(t, host, n, Lw.Wgu, t->act); }
+        else if (rest == "mlp.up_proj.weight") { expect(name.c_str(), shape, ndim, {F, d}); put(t, host, n, (char*)Lw.Wgu + (size_t)F * d * es, t->act); }
+        else if (rest == "mlp.down_proj.weight") mat(Lw.Wd, d, F);
+        else if (rest == "input_layernorm.weight") vec(Lw.ln1, d);
+        else if (rest == "post_attention_layernorm.weight") vec(Lw.ln2, d);
+        else WLK_CHECK(false, "unknown tensor %s", name.c_str());
+    }
+    else WLK_CHECK(false, "unknown tensor %s", name.c_str());
+    t->loaded.insert(name);
+}
+
+std::vector<std::string> required(const wlk_qtext_dims& D) {
+    std::vector<std::string> r = {"embed_tokens.weight", "norm.weight"};
+    if (!D.tied) r.push_back("lm_head.weight");
+    for (int i = 0; i < D.n_layer; ++i) {
+        const std::string p = "layers." + std::to_string(i) + ".";
+        for (const char* s : {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "self_attn.q_norm",
+                              "self_attn.k_norm", "mlp.gate_proj", "mlp.up_proj", "mlp.down_proj", "input_layernorm",
+                              "post_attention_layernorm"})
+            r.push_back(p + s + ".weight");
+    }
+    return r;
+}
+
+void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) {
+    WLK_CHECK(dims && cfg && out, "null argument");
+    const wlk_qtext_dims& D = *dims;
+    WLK_CHECK(D.head_dim == QT_HD, "head_dim must be %d", QT_HD);
+    WLK_CHECK(D.n_kv_head >= 1 && D.n_head % D.n_kv_head == 0 && D.n_head / D.n_kv_head <= 8, "n_head must be a multiple (<= 8x) of n_kv_head");
+    WLK_CHECK(D.d_model % 8 == 0 && D.ffn_dim % 8 == 0 && D.vocab >= 1, "d_model and ffn_dim must be multiples of 8");
+    WLK_CHECK(D.max_ctx >= 1 && D.max_ctx <= 32768, "max_ctx must be in [1, 32768]");
+    WLK_CHECK((size_t)(D.vocab + 31) / 32 * 4 <= 200 * 1024, "vocab too large for the pick kernel's bitmap");
+    WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
+    int ndev = 0;
+    cudaError_t ce = cudaGetDeviceCount(&ndev);
+    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the H100 engine has no CPU fallback", cudaGetErrorString(ce));
+    WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
+    CUDA_CHECK(cudaSetDevice(cfg->device));
+    cudaDeviceProp prop;
+    CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
+    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+
+    auto* t = new wlk_qtext();
+    t->dims = D; t->cfg = *cfg;
+    t->num_sms = prop.multiProcessorCount;
+    t->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
+    t->gemm_backend = t->act == DT_BF16 ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&t->st, cudaStreamNonBlocking));
+    const size_t es = t->es();
+    const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
+    const size_t W = (size_t)(H + 2 * KV) * QT_HD;
+    size_t* aw = &t->bytes_weights;
+    t->emb = (float*)talloc(t, (size_t)D.vocab * d * 4, aw);
+    t->head = talloc(t, (size_t)D.vocab * d * es, aw);
+    t->normw = (float*)talloc(t, (size_t)d * 4, aw);
+    t->inv_freq = (float*)talloc(t, QT_HD / 2 * 4, aw);
+    t->L.resize(D.n_layer);
+    for (auto& Lw : t->L) {
+        Lw.Wqkv = talloc(t, W * d * es, aw);
+        Lw.Wo = talloc(t, (size_t)d * H * QT_HD * es, aw);
+        Lw.Wgu = talloc(t, (size_t)2 * F * d * es, aw);
+        Lw.Wd = talloc(t, (size_t)d * F * es, aw);
+        Lw.qn = (float*)talloc(t, QT_HD * 4, aw); Lw.kn = (float*)talloc(t, QT_HD * 4, aw);
+        Lw.ln1 = (float*)talloc(t, (size_t)d * 4, aw); Lw.ln2 = (float*)talloc(t, (size_t)d * 4, aw);
+    }
+    {   // inv_freq = 1 / theta^(2i / 128), as HF's default rope init computes it (fp32 arange / dim, then pow)
+        std::vector<float> f(QT_HD / 2);
+        for (int i = 0; i < QT_HD / 2; ++i) f[i] = (float)(1.0 / pow((double)D.rope_theta, (double)(float)(2 * i) / (double)QT_HD));
+        CUDA_CHECK(cudaMemcpy(t->inv_freq, f.data(), f.size() * 4, cudaMemcpyHostToDevice));
+    }
+    const size_t R = QT_ROUND_ROWS;
+    size_t* ws = &t->bytes_workspace;
+    t->x = (float*)talloc(t, R * d * 4, ws);
+    t->xn = talloc(t, R * d * es, ws);
+    t->qkv = (float*)talloc(t, R * W * 4, ws);
+    t->qb = talloc(t, R * H * QT_HD * es, ws);
+    t->att = talloc(t, R * H * QT_HD * es, ws);
+    t->gu = (float*)talloc(t, R * 2 * F * 4, ws);
+    t->hid = talloc(t, R * F * es, ws);
+    t->up_rows = (int)R;
+    t->up = (float*)talloc(t, R * d * 4, ws);
+    t->logit_cap = cfg->max_batch * 288;
+    t->hlog = talloc(t, (size_t)t->logit_cap * d * es, ws);
+    t->logit_group = (int)std::max<size_t>(1, std::min<size_t>((size_t)t->logit_cap, QT_LOGIT_BYTES / ((size_t)D.vocab * 4)));
+    t->logits = (float*)talloc(t, (size_t)t->logit_group * D.vocab * 4, ws);
+    t->picks_d = (int32_t*)talloc(t, (size_t)t->logit_cap * 4, ws);
+    t->values_d = (float*)talloc(t, (size_t)t->logit_cap * 4, ws);
+    if (t->gemm_backend == WLK_BACKEND_TCGEN05) {
+        t->sk_scratch = (float*)talloc(t, SK_SCRATCH_FLOATS * 4, ws);
+        t->sk_counters = (int*)talloc(t, SK_MAX_TILES * 4, ws);
+        CUDA_CHECK(cudaMemset(t->sk_counters, 0, SK_MAX_TILES * 4));
+    }
+    t->stg_bytes = R * 32 + (size_t)cfg->max_batch * 16 + 8192;
+    CUDA_CHECK(cudaMallocHost(&t->stg_h, t->stg_bytes));
+    CUDA_CHECK(cudaMallocHost(&t->up_h, R * d * 4));
+    CUDA_CHECK(cudaEventCreateWithFlags(&t->stg_ev, cudaEventDisableTiming));
+    t->stg_d = (uint8_t*)talloc(t, t->stg_bytes, ws);
+    t->kv_bytes = (size_t)D.n_layer * 2 * KV * D.max_ctx * QT_HD * es;
+    t->sess.resize(cfg->max_sessions);
+    CUDA_CHECK(cudaFuncSetAttribute(qt_pick_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    *out = t;
+}
+
+void destroy(wlk_qtext* t) {
+    cudaStreamSynchronize(t->st);
+    for (auto& s : t->sess) if (s.kv) cudaFree(s.kv);
+    for (void* p : t->allocs) cudaFree(p);
+    if (t->stage_f32) cudaFree(t->stage_f32);
+    if (t->stg_h) cudaFreeHost(t->stg_h);
+    if (t->up_h) cudaFreeHost(t->up_h);
+    if (t->pick_d) cudaFree(t->pick_d);
+    if (t->stg_ev) cudaEventDestroy(t->stg_ev);
+    cudaStreamDestroy(t->st);
+    delete t;
+}
+
+QTSession& tsession(wlk_qtext* t, int32_t sid) {
+    WLK_CHECK(sid >= 0 && sid < (int)t->sess.size() && t->sess[sid].open, "invalid session id %d", sid);
+    return t->sess[sid];
+}
+
+template <typename T>
+void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, const int32_t* slot_d, void* const* kv_d,
+               const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles) {
+    const wlk_qtext_dims& D = t->dims;
+    const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
+    const int W = (H + 2 * KV) * QT_HD;
+    qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, t->emb, t->up, t->x, d);
+    for (int li = 0; li < D.n_layer; ++li) {
+        QTLayerW& Lw = t->L[li];
+        qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, Lw.ln1, (T*)t->xn, nullptr, d, D.rms_eps);
+        {   GemmArgs g;
+            g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wqkv; g.w_type = t->act; g.ldw = d;
+            g.M = R; g.N = W; g.K = d;
+            g.epi.C = t->qkv; g.epi.c_type = DT_F32; g.epi.ldc = W;
+            tgemm(t, g); }
+        qt_qk_rope_kernel<T><<<dim3(R, H + 2 * KV), QT_HD, 0, t->st>>>(t->qkv, Lw.qn, Lw.kn, t->inv_freq, pos_d, slot_d, kv_d,
+                                                                     (T*)t->qb, li, H, KV, D.max_ctx, D.rms_eps);
+        if (t->act == DT_BF16)
+            qt_attention_mma_kernel<<<dim3(n_tiles, KV), 32 * (H / KV), 0, t->st>>>((const bf16*)t->qb, tiles_d, kv_d, (bf16*)t->att,
+                                                                                  li, H, KV, D.max_ctx);
+        else
+            qt_attention_kernel<T><<<dim3(R, KV), 32 * (H / KV), 0, t->st>>>((const T*)t->qb, pos_d, slot_d, kv_d, (T*)t->att, li,
+                                                                            H, KV, D.max_ctx);
+        {   GemmArgs g;
+            g.A = t->att; g.a_type = t->act; g.lda = H * QT_HD; g.W = Lw.Wo; g.w_type = t->act; g.ldw = H * QT_HD;
+            g.M = R; g.N = d; g.K = H * QT_HD;
+            g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
+            tgemm(t, g); }
+        qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, Lw.ln2, (T*)t->xn, nullptr, d, D.rms_eps);
+        {   GemmArgs g;
+            g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wgu; g.w_type = t->act; g.ldw = d;
+            g.M = R; g.N = 2 * F; g.K = d;
+            g.epi.C = t->gu; g.epi.c_type = DT_F32; g.epi.ldc = 2 * F;
+            tgemm(t, g); }
+        {   const int64_t total = (int64_t)R * F;
+            const int blocks = (int)std::min<int64_t>((total + 255) / 256, 65535);
+            qt_swiglu_kernel<T><<<blocks, 256, 0, t->st>>>(t->gu, (T*)t->hid, R, F); }
+        {   GemmArgs g;
+            g.A = t->hid; g.a_type = t->act; g.lda = F; g.W = Lw.Wd; g.w_type = t->act; g.ldw = F;
+            g.M = R; g.N = d; g.K = F;
+            g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
+            tgemm(t, g); }
+    }
+    qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, t->normw, (T*)t->hlog, logit_row_d, d, D.rms_eps);
+    CUDA_CHECK(cudaGetLastError());
+}
+
+void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_off, const float* embeds,
+             int n_embeds, const int32_t* logit_rows) {
+    const wlk_qtext_dims& D = t->dims;
+    WLK_CHECK(t->finalized, "weights not finalized");
+    WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
+    int n_logit = 0;
+    for (int i = 0; i < n; ++i) {
+        QTSession& s = tsession(t, sids[i]);
+        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        const int r = row_off[i + 1] - row_off[i];
+        WLK_CHECK(r >= 1, "session %d has no rows", sids[i]);
+        WLK_CHECK(s.len + r <= D.max_ctx, "context full: session %d holds %d positions, %d more exceed max_ctx %d", sids[i], s.len, r, D.max_ctx);
+        WLK_CHECK(logit_rows[i] >= 0 && logit_rows[i] <= r, "logit_rows[%d] = %d outside [0, %d]", i, logit_rows[i], r);
+        n_logit += logit_rows[i];
+    }
+    WLK_CHECK(n_logit <= t->logit_cap, "%d logit rows exceed the engine's %d", n_logit, t->logit_cap);
+    const int total = row_off[n] - row_off[0];
+    for (int r = 0; r < total; ++r) {
+        const int s = row_src[row_off[0] + r];
+        WLK_CHECK(s < D.vocab && (s >= 0 || -1 - s < n_embeds), "row %d: source %d is neither a token id nor an embedding row", r, s);
+    }
+    // the packed row list: (session index, position, logit row or -1)
+    std::vector<int> r_sess(total), r_pos(total), r_log(total);
+    {   int r = 0, lg = 0;
+        for (int i = 0; i < n; ++i) {
+            const int cnt = row_off[i + 1] - row_off[i];
+            for (int k = 0; k < cnt; ++k, ++r) {
+                r_sess[r] = i; r_pos[r] = t->sess[sids[i]].len + k;
+                r_log[r] = k >= cnt - logit_rows[i] ? lg++ : -1;
+            }
+        }
+    }
+    for (int r0 = 0; r0 < total; r0 += QT_ROUND_ROWS) {
+        const int R = std::min(QT_ROUND_ROWS, total - r0);
+        size_t off = 0;
+        auto carve = [&](size_t bytes) { size_t o = (off + 255) / 256 * 256; off = o + bytes; WLK_CHECK(off <= t->stg_bytes, "staging overflow"); return o; };
+        const size_t o_src = carve((size_t)R * 4), o_pos = carve((size_t)R * 4), o_slot = carve((size_t)R * 4),
+                     o_log = carve((size_t)R * 4), o_kv = carve((size_t)n * sizeof(void*)),
+                     o_tile = carve((size_t)R * sizeof(QTAttnTile));
+        CUDA_CHECK(cudaEventSynchronize(t->stg_ev));     // the previous H2D copy out of stg_h / up_h has been consumed
+        int32_t* src = reinterpret_cast<int32_t*>(t->stg_h + o_src);
+        int32_t* pos = reinterpret_cast<int32_t*>(t->stg_h + o_pos);
+        int32_t* slot = reinterpret_cast<int32_t*>(t->stg_h + o_slot);
+        int32_t* lrow = reinterpret_cast<int32_t*>(t->stg_h + o_log);
+        void** kvp = reinterpret_cast<void**>(t->stg_h + o_kv);
+        for (int i = 0; i < n; ++i) kvp[i] = t->sess[sids[i]].kv;
+        // embedding rows of this round go to `up` in the order they appear: packed into pinned memory, one copy
+        int n_up = 0;
+        QTAttnTile* tiles = reinterpret_cast<QTAttnTile*>(t->stg_h + o_tile);
+        int n_tiles = 0;
+        for (int k = 0; k < R; ++k) {
+            const int r = r0 + k;
+            int s = row_src[row_off[0] + r];
+            if (s < 0) {
+                memcpy(t->up_h + (size_t)n_up * D.d_model, embeds + (size_t)(-1 - s) * D.d_model, (size_t)D.d_model * 4);
+                s = -1 - n_up++;
+            }
+            src[k] = s; pos[k] = r_pos[r]; slot[k] = r_sess[r]; lrow[k] = r_log[r];
+            // attention tiles: <= 16 consecutive rows of one session
+            if (n_tiles == 0 || tiles[n_tiles - 1].slot != r_sess[r] || tiles[n_tiles - 1].n_rows == 16)
+                tiles[n_tiles++] = QTAttnTile{k, 0, r_sess[r], r_pos[r]};
+            tiles[n_tiles - 1].n_rows++;
+        }
+        if (n_up) CUDA_CHECK(cudaMemcpyAsync(t->up, t->up_h, (size_t)n_up * D.d_model * 4, cudaMemcpyHostToDevice, t->st));
+        CUDA_CHECK(cudaMemcpyAsync(t->stg_d, t->stg_h, off, cudaMemcpyHostToDevice, t->st));
+        CUDA_CHECK(cudaEventRecord(t->stg_ev, t->st));
+        const int32_t* src_d = reinterpret_cast<const int32_t*>(t->stg_d + o_src);
+        const int32_t* pos_d = reinterpret_cast<const int32_t*>(t->stg_d + o_pos);
+        const int32_t* slot_d = reinterpret_cast<const int32_t*>(t->stg_d + o_slot);
+        const int32_t* log_d = reinterpret_cast<const int32_t*>(t->stg_d + o_log);
+        void* const* kv_d = reinterpret_cast<void* const*>(t->stg_d + o_kv);
+        const QTAttnTile* tiles_d = reinterpret_cast<const QTAttnTile*>(t->stg_d + o_tile);
+        if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles);
+        else run_round<bf16>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles);
+    }
+    // no host sync here: the pick (or logits) call that follows synchronizes once for the whole phase
+    for (int i = 0; i < n; ++i) t->sess[sids[i]].len += row_off[i + 1] - row_off[i];
+    t->n_logit = n_logit;
+}
+
+void head_group(wlk_qtext* t, int row0, int rows) {
+    GemmArgs g;
+    g.A = (const char*)t->hlog + (size_t)row0 * t->dims.d_model * t->es(); g.a_type = t->act; g.lda = t->dims.d_model;
+    g.W = t->head; g.w_type = t->act; g.ldw = t->dims.d_model;
+    g.M = rows; g.N = t->dims.vocab; g.K = t->dims.d_model;
+    g.epi.C = t->logits; g.epi.c_type = DT_F32; g.epi.ldc = t->dims.vocab;
+    tgemm(t, g);
+}
+
+void pick(wlk_qtext* t, const int32_t* hist, int n_hist, const int32_t* hist_off, const int32_t* hist_len, const int32_t* suppress,
+          int n_suppress, float penalty, int ngram, int max_consec, int wait_id, int32_t* picks, float* values) {
+    const wlk_qtext_dims& D = t->dims;
+    WLK_CHECK(t->finalized, "weights not finalized");
+    const int N = t->n_logit;
+    if (N == 0) return;
+    for (int j = 0; j < N; ++j)
+        WLK_CHECK(hist_off[j] >= 0 && hist_len[j] >= 0 && hist_off[j] + hist_len[j] <= n_hist, "history of row %d out of range", j);
+    std::vector<int32_t> sup;
+    for (int i = 0; i < n_suppress; ++i) if (suppress[i] >= 0 && suppress[i] < D.vocab) sup.push_back(suppress[i]);
+    // the reference only arms max-consecutive when the wait token is not suppressed (model.py:1067-1072)
+    for (int32_t v : sup) if (v == wait_id) wait_id = -1;
+    // one device buffer, grown on demand: [2N offsets/lengths][suppress][histories]
+    const size_t need = (size_t)2 * N + sup.size() + (size_t)n_hist + 1;
+    if (need > t->pick_cap) {
+        CUDA_CHECK(cudaStreamSynchronize(t->st));
+        if (t->pick_d) CUDA_CHECK(cudaFree(t->pick_d));
+        t->pick_cap = std::max(need, (size_t)1 << 16);
+        CUDA_CHECK(cudaMalloc(&t->pick_d, t->pick_cap * 4));
+    }
+    int32_t* meta_d = t->pick_d;
+    int32_t* hist_d = t->pick_d + 2 * N + sup.size();
+    if (n_hist) CUDA_CHECK(cudaMemcpyAsync(hist_d, hist, (size_t)n_hist * 4, cudaMemcpyHostToDevice, t->st));
+    CUDA_CHECK(cudaMemcpyAsync(meta_d, hist_off, (size_t)N * 4, cudaMemcpyHostToDevice, t->st));
+    CUDA_CHECK(cudaMemcpyAsync(meta_d + N, hist_len, (size_t)N * 4, cudaMemcpyHostToDevice, t->st));
+    if (!sup.empty()) CUDA_CHECK(cudaMemcpyAsync(meta_d + 2 * N, sup.data(), sup.size() * 4, cudaMemcpyHostToDevice, t->st));
+    const size_t smem = (size_t)(D.vocab + 31) / 32 * 4;
+    for (int g0 = 0; g0 < N; g0 += t->logit_group) {
+        const int rows = std::min(t->logit_group, N - g0);
+        head_group(t, g0, rows);
+        PickArgs a;
+        a.logits = t->logits; a.ld = D.vocab; a.vocab = D.vocab;
+        a.hist = hist_d; a.hist_off = meta_d + g0; a.hist_len = meta_d + N + g0;
+        a.suppress = meta_d + 2 * N; a.n_suppress = (int)sup.size();
+        a.penalty = penalty; a.penalize = penalty != 1.0f && penalty > 0.0f; a.ngram = ngram; a.max_consec = max_consec;
+        a.wait_id = wait_id; a.picks = t->picks_d + g0; a.values = t->values_d + g0;
+        qt_pick_kernel<<<rows, QT_PICK_THREADS, smem, t->st>>>(a);
+        CUDA_CHECK(cudaGetLastError());
+    }
+    CUDA_CHECK(cudaMemcpyAsync(picks, t->picks_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
+    if (values) CUDA_CHECK(cudaMemcpyAsync(values, t->values_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
+    CUDA_CHECK(cudaStreamSynchronize(t->st));            // the one host sync of a forward + pick phase
+}
+
+void logits_out(wlk_qtext* t, int row0, int rows, float* out) {
+    WLK_CHECK(t->finalized, "weights not finalized");
+    WLK_CHECK(row0 >= 0 && rows >= 0 && row0 + rows <= t->n_logit, "logit rows [%d, %d) outside the last forward's %d", row0, row0 + rows, t->n_logit);
+    for (int g0 = 0; g0 < rows; g0 += t->logit_group) {
+        const int r = std::min(t->logit_group, rows - g0);
+        head_group(t, row0 + g0, r);
+        CUDA_CHECK(cudaMemcpyAsync(out + (size_t)g0 * t->dims.vocab, t->logits, (size_t)r * t->dims.vocab * 4, cudaMemcpyDeviceToHost, t->st));
+        CUDA_CHECK(cudaStreamSynchronize(t->st));
+    }
+}
+
+}  // namespace
+
+#define WLK_API_BEGIN try {
+#define WLK_API_END                                              \
+    return 0;                                                    \
+    } catch (const wlk::Error& err) {                            \
+        wlk::set_last_error(err.msg);                            \
+        return 1;                                                \
+    } catch (const std::exception& ex) {                         \
+        wlk::set_last_error(std::string("exception: ") + ex.what()); \
+        return 2;                                                \
+    } catch (...) {                                              \
+        wlk::set_last_error("unknown exception");                \
+        return 3;                                                \
+    }
+#define TLOCK(t) WLK_CHECK((t) != nullptr, "null engine"); std::lock_guard<std::mutex> _lk((t)->mu); \
+                 CUDA_CHECK(cudaSetDevice((t)->cfg.device))
+
+extern "C" {
+
+int wlk_qtext_create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) {
+    WLK_API_BEGIN
+    create(dims, cfg, out);
+    WLK_API_END
+}
+int wlk_qtext_destroy(wlk_qtext* t) {
+    WLK_API_BEGIN
+    WLK_CHECK(t != nullptr, "null engine");
+    CUDA_CHECK(cudaSetDevice(t->cfg.device));
+    destroy(t);
+    WLK_API_END
+}
+int wlk_qtext_load_tensor(wlk_qtext* t, const char* name, const float* host, const int64_t* shape, int ndim) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
+    load_tensor(t, name, host, shape, ndim);
+    WLK_API_END
+}
+int wlk_qtext_finalize_weights(wlk_qtext* t) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    std::string missing;
+    int nmiss = 0;
+    for (auto& r : required(t->dims)) if (!t->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
+    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    if (t->stage_f32) { CUDA_CHECK(cudaFree(t->stage_f32)); t->stage_f32 = nullptr; t->stage_cap = 0; }
+    t->finalized = true;
+    WLK_API_END
+}
+int wlk_qtext_memory(wlk_qtext* t, size_t* weights, size_t* sessions, size_t* workspace) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    if (weights) *weights = t->bytes_weights;
+    if (sessions) *sessions = t->bytes_sessions;
+    if (workspace) *workspace = t->bytes_workspace;
+    WLK_API_END
+}
+int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(sid, "null out pointer");
+    int found = -1;
+    for (int i = 0; i < (int)t->sess.size(); ++i) if (!t->sess[i].open) { found = i; break; }
+    WLK_CHECK(found >= 0, "all %d sessions in use", (int)t->sess.size());
+    QTSession& s = t->sess[found];
+    CUDA_CHECK(cudaMalloc(&s.kv, t->kv_bytes));
+    t->bytes_sessions += t->kv_bytes;
+    s.open = true; s.len = 0;
+    *sid = found;
+    WLK_API_END
+}
+int wlk_qtext_session_close(wlk_qtext* t, int32_t sid) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    QTSession& s = tsession(t, sid);
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
+    cudaFree(s.kv);
+    t->bytes_sessions -= t->kv_bytes;
+    s = QTSession{};
+    WLK_API_END
+}
+int wlk_qtext_session_reset(wlk_qtext* t, int32_t sid) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    tsession(t, sid).len = 0;
+    WLK_API_END
+}
+int wlk_qtext_session_len(wlk_qtext* t, int32_t sid, int32_t* len) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(len, "null out pointer");
+    *len = tsession(t, sid).len;
+    WLK_API_END
+}
+int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    QTSession& s = tsession(t, sid);
+    WLK_CHECK(len >= 0 && len <= s.len, "crop to %d outside [0, %d]", len, s.len);
+    s.len = len;
+    WLK_API_END
+}
+int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
+                      const float* embeds_host, int32_t n_embeds, const int32_t* logit_rows) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(sids && row_src && row_offsets && logit_rows && (embeds_host || n_embeds == 0), "null argument");
+    forward(t, sids, n, row_src, row_offsets, embeds_host, n_embeds, logit_rows);
+    WLK_API_END
+}
+int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_tokens, const int32_t* hist_off,
+                   const int32_t* hist_len, const int32_t* suppress, int32_t n_suppress, float repetition_penalty,
+                   int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id, int32_t* picks_out,
+                   float* value_out) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(hist_off && hist_len && picks_out && (hist_tokens || n_hist_tokens == 0) && (suppress || n_suppress == 0), "null argument");
+    pick(t, hist_tokens, n_hist_tokens, hist_off, hist_len, suppress, n_suppress, repetition_penalty, no_repeat_ngram_size,
+         max_consecutive, wait_token_id, picks_out, value_out);
+    WLK_API_END
+}
+int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(out_host || n_rows == 0, "null output buffer");
+    logits_out(t, row0, n_rows, out_host);
+    WLK_API_END
+}
+
+}  // extern "C"

@@ -102,3 +102,72 @@ def synthetic_tower_state_dict(dims: QwenTowerDims, seed: int = 0) -> Dict[str, 
         sd[p + "fc1.weight"] = w(F, d, fan_in=d); sd[p + "fc1.bias"] = b(F)
         sd[p + "fc2.weight"] = w(d, F, fan_in=F); sd[p + "fc2.bias"] = b(d)
     return sd
+
+
+@dataclass(frozen=True)
+class QwenTextDims:
+    """Geometry of the Qwen3 text decoder behind Qwen3-ASR (HF ``Qwen3Model`` + ``lm_head``; reference
+    third_party/qwen3-asr-causal/src/qwen3_asr_causal/model.py:1498-1507).
+
+    Qwen3-ASR's thinker uses MRoPE; with audio rows and text only, its three position streams are equal, so it reduces
+    to plain 1D rotate-half RoPE over ``head_dim`` with ``inv_freq = rope_theta ** (-2i / head_dim)``.  The engine
+    assumes exactly that."""
+    vocab: int = 151936
+    d_model: int = 1024
+    n_layer: int = 28
+    n_head: int = 16
+    n_kv_head: int = 8
+    head_dim: int = 128               # the kernels specialise on 128
+    ffn_dim: int = 3072
+    rope_theta: float = 1e6
+    rms_eps: float = 1e-6
+    tied: bool = True                 # lm_head shares embed_tokens
+    max_ctx: int = 1024               # positions per session
+
+    def as_tuple(self):
+        return (self.vocab, self.d_model, self.n_layer, self.n_head, self.n_kv_head, self.head_dim, self.ffn_dim,
+                int(self.tied), self.max_ctx, float(self.rope_theta), float(self.rms_eps))
+
+
+QWEN_TEXT_DIMS: Dict[str, QwenTextDims] = {
+    "tnano": QwenTextDims(vocab=2048, d_model=256, n_layer=2, n_head=4, n_kv_head=2, ffn_dim=512, rope_theta=1e6,
+                          tied=False, max_ctx=1024),
+    # Qwen3-ASR-0.6B text model (public Qwen3-0.6B numbers: d 1024, 28 layers, 16 / 8 heads of 128, ffn 3072,
+    # vocab 151936, theta 1e6, tied embeddings); to be confirmed against the checkpoint's thinker_config.text_config
+    "qwen3-asr-0.6b": QwenTextDims(),
+}
+
+
+def synthetic_text_state_dict(dims: QwenTextDims, seed: int = 0) -> Dict[str, np.ndarray]:
+    """Seeded weights with HF ``Qwen3Model`` parameter names (plus ``lm_head.weight`` when untied).  Embedding rows
+    have unit variance (the residual stream's scale); the head is scaled so that logits have sigma ~3.  With tied
+    embeddings the embedding table carries that head scale instead."""
+    rng = np.random.default_rng(seed)
+    d, F, hd = dims.d_model, dims.ffn_dim, dims.head_dim
+    qd, kvd = dims.n_head * hd, dims.n_kv_head * hd
+
+    def w(*shape, fan_in, s=1.0):
+        return (rng.standard_normal(shape) * (s / np.sqrt(fan_in))).astype(np.float32)
+
+    def g(n):
+        return (1.0 + 0.1 * rng.standard_normal(n)).astype(np.float32)
+
+    emb = w(dims.vocab, d, fan_in=d, s=3.0) if dims.tied else rng.standard_normal((dims.vocab, d)).astype(np.float32)
+    sd = {"embed_tokens.weight": emb}
+    for i in range(dims.n_layer):
+        p = f"layers.{i}."
+        sd[p + "self_attn.q_proj.weight"] = w(qd, d, fan_in=d)
+        sd[p + "self_attn.k_proj.weight"] = w(kvd, d, fan_in=d)
+        sd[p + "self_attn.v_proj.weight"] = w(kvd, d, fan_in=d)
+        sd[p + "self_attn.o_proj.weight"] = w(d, qd, fan_in=qd, s=0.5)
+        sd[p + "self_attn.q_norm.weight"] = g(hd)
+        sd[p + "self_attn.k_norm.weight"] = g(hd)
+        sd[p + "mlp.gate_proj.weight"] = w(F, d, fan_in=d)
+        sd[p + "mlp.up_proj.weight"] = w(F, d, fan_in=d)
+        sd[p + "mlp.down_proj.weight"] = w(d, F, fan_in=F, s=0.5)
+        sd[p + "input_layernorm.weight"] = g(d)
+        sd[p + "post_attention_layernorm.weight"] = g(d)
+    sd["norm.weight"] = g(d)
+    if not dims.tied:
+        sd["lm_head.weight"] = w(dims.vocab, d, fan_in=d, s=3.0)
+    return sd

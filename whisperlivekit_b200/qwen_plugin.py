@@ -162,3 +162,160 @@ class B200StreamingMelExtractor:
     def reset(self) -> None:
         self.engine.reset_session(self.sid)
         self._emitted = 0
+
+
+class B200DecoderRollingState:
+    """Stands in for the reference's DecoderRollingState (model.py:53-68) in ``state.decoder``: the KV of
+    [head + audio_steps] lives in an engine session, ``cache`` is that session's handle.  The session closes when the
+    object is collected (segment rollover builds fresh decode states)."""
+
+    disabled = False
+
+    def __init__(self, engine, sid: int):
+        self.engine, self.sid = engine, sid
+        self.head_token_ids: tuple = ()
+        self.head_len = 0
+        self.audio_steps = 0
+
+    @property
+    def cache(self):
+        return self if self.engine is not None else None
+
+    def get_seq_length(self) -> int:
+        return self.engine.session_len(self.sid)
+
+    def close(self):
+        if self.engine is not None:
+            self.engine.close_session(self.sid)
+            self.engine = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class B200QwenTextDecoder:
+    """Drop-in for the text half of the reference's realtime model: ``generate_full_hypothesis_rolling`` (model.py:
+    991-1250) and ``generate_full_hypothesis_from_cached_audio`` (:839-989) rebound on one model instance over the text
+    engine (``wlk_qtext_*``), the rolling prefix KV in a device session per stream::
+
+        B200QwenTextDecoder.install(model, precision="bf16")
+
+    Frame rows cross the seam as the host tensor the reference hands over; only the rows the session has not seen are
+    uploaded.  ``use_decoder_kv_cache=False`` takes the same cached path (the reference documents the two as
+    greedy-equal)."""
+
+    def __init__(self, model, engine, dims):
+        self.model, self.engine, self.dims = model, engine, dims
+
+    @staticmethod
+    def dims_of(model, max_ctx: int = 1024):
+        from .qwen_dims import QwenTextDims
+        c = model.text_model.config
+        rope = getattr(c, "rope_parameters", None) or {}
+        theta = rope.get("rope_theta", getattr(c, "rope_theta", 10000.0))
+        tied = model.lm_head.weight.data_ptr() == model.text_model.embed_tokens.weight.data_ptr()
+        return QwenTextDims(vocab=int(model.lm_head.weight.shape[0]), d_model=int(c.hidden_size),
+                            n_layer=int(c.num_hidden_layers), n_head=int(c.num_attention_heads),
+                            n_kv_head=int(c.num_key_value_heads),
+                            head_dim=int(getattr(c, "head_dim", c.hidden_size // c.num_attention_heads)),
+                            ffn_dim=int(c.intermediate_size), rope_theta=float(theta), rms_eps=float(c.rms_norm_eps),
+                            tied=bool(tied), max_ctx=int(max_ctx))
+
+    @classmethod
+    def install(cls, model, engine_factory=None, precision: str = "bf16", max_ctx: int = 1024, max_sessions: int = 8,
+                **engine_kw):
+        dims = cls.dims_of(model, max_ctx)
+        sd = {k: v.detach().float().cpu().numpy() for k, v in model.text_model.state_dict().items()}
+        if not dims.tied:
+            sd["lm_head.weight"] = model.lm_head.weight.detach().float().cpu().numpy()
+        if engine_factory is None:
+            from .qwen_text_engine import QwenTextEngine
+            engine = QwenTextEngine(dims, sd, precision=precision, max_sessions=max_sessions, **engine_kw)
+        else:
+            engine = engine_factory(dims, sd)
+        dec = cls(model, engine, dims)
+        model.generate_full_hypothesis_rolling = dec.generate_full_hypothesis_rolling
+        model.generate_full_hypothesis_from_cached_audio = dec.generate_full_hypothesis_from_cached_audio
+        model.b200_text_decoder = dec
+        return dec
+
+    def _controls(self, eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                  max_consecutive_text_tokens):
+        return dict(eos_token_id=eos_token_id, stop_token_ids=stop_token_ids, suppress_token_ids=suppress_token_ids,
+                    repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
+                    max_consecutive_text_tokens=max_consecutive_text_tokens, wait_token_id=self.model.wait_token_id)
+
+    def generate_full_hypothesis_from_cached_audio(self, frame_hidden, *, prefix_token_ids=None,
+                                                   audio_placeholder_token_id=None, prompt_token_ids=None,
+                                                   max_new_tokens: int = 128, eos_token_id=None, stop_token_ids=None,
+                                                   suppress_token_ids=None, repetition_penalty: float = 1.0,
+                                                   no_repeat_ngram_size: int = 0, max_consecutive_text_tokens: int = 0,
+                                                   use_decoder_kv_cache: bool = True):
+        import torch
+        if frame_hidden.ndim != 3:
+            raise ValueError("frame_hidden must have shape [batch, steps, hidden]")
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        batch = int(frame_hidden.shape[0])
+        device = frame_hidden.device
+        if max_new_tokens == 0:
+            return torch.empty(batch, 0, dtype=torch.long, device=device)
+        kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                            max_consecutive_text_tokens)
+        ctl = self.engine.make_controls(**kw)
+        fh = frame_hidden.detach().float().cpu().numpy()
+
+        def rows(ids, b):
+            if ids is None:
+                return None
+            t = torch.as_tensor(ids).long()
+            return (t if t.ndim == 1 else t[b]).tolist()
+
+        outs = [self.engine.generate_full(fh[b], prefix_token_ids=rows(prefix_token_ids, b),
+                                          audio_placeholder_token_id=audio_placeholder_token_id,
+                                          prompt_token_ids=rows(prompt_token_ids, b), max_new_tokens=max_new_tokens,
+                                          controls=ctl, bos_token_id=self.model.bos_token_id) for b in range(batch)]
+        # rows that stopped early are filled with the stop-fill id while the others decode (model.py:419-436)
+        width = max(len(o) for o in outs)
+        if ctl.stop_ids:
+            fill = ctl.eos_token_id if ctl.eos_token_id is not None else min(ctl.stop_ids)
+            outs = [o + [fill] * (width - len(o)) for o in outs]
+        return torch.tensor(outs, dtype=torch.long, device=device).reshape(batch, width)
+
+    def generate_full_hypothesis_rolling(self, frame_hidden, *, state, template_token_ids, audio_placeholder_token_id,
+                                         draft_token_ids=None, max_new_tokens: int = 128, eos_token_id=None,
+                                         stop_token_ids=None, suppress_token_ids=None, repetition_penalty: float = 1.0,
+                                         no_repeat_ngram_size: int = 0, max_consecutive_text_tokens: int = 0):
+        import torch
+        from .qwen_text_engine import RollingState, split_template
+        if frame_hidden.ndim != 3:
+            raise ValueError("frame_hidden must have shape [batch, steps, hidden]")
+        head, tail = split_template(template_token_ids, audio_placeholder_token_id)
+        kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                            max_consecutive_text_tokens)
+        audio_steps = int(frame_hidden.shape[1])
+        if int(frame_hidden.shape[0]) != 1 or max_new_tokens <= 0 or audio_steps == 0:
+            expanded = head + [int(audio_placeholder_token_id)] * audio_steps + tail
+            toks = self.generate_full_hypothesis_from_cached_audio(
+                frame_hidden, prefix_token_ids=expanded, audio_placeholder_token_id=audio_placeholder_token_id,
+                max_new_tokens=max_new_tokens, **{k: v for k, v in kw.items() if k != "wait_token_id"})
+            return toks, {"decoder_path": "full"}
+        dec = getattr(state, "decoder", None)
+        if not isinstance(dec, B200DecoderRollingState) or dec.engine is not self.engine:
+            dec = B200DecoderRollingState(self.engine, self.engine.open_session())
+            prev = None
+        else:
+            prev = RollingState(dec.head_token_ids, dec.head_len, dec.audio_steps)
+        fh = frame_hidden[0].detach().float().cpu().numpy()
+        toks, stats, states = self.engine.generate_rolling(
+            [dec.sid], [fh], [prev], template_token_ids, audio_placeholder_token_id,
+            [None if draft_token_ids is None else [int(t) for t in draft_token_ids]], max_new_tokens=max_new_tokens,
+            bos_token_id=self.model.bos_token_id, **kw)
+        st = states[0]
+        if stats[0].get("decoder_path") != "full":
+            dec.head_token_ids, dec.head_len, dec.audio_steps = st.head_token_ids, st.head_len, st.audio_steps
+            state.decoder = dec
+        return torch.tensor([toks[0]], dtype=torch.long, device=frame_hidden.device), stats[0]
