@@ -300,6 +300,33 @@ int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_toke
                    float* value_out);
 /* raw lm_head outputs [n_rows][vocab] fp32 of logit rows row0 .. row0 + n_rows of the last forward */
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host);
+/* RoPE frequencies: the optional tensor "rotary_emb.inv_freq" [head_dim / 2] (HF's non-persistent buffer of that name,
+ * absent from state_dict()) sets them.  Without it the engine computes 1 / rope_theta^(2i / head_dim) in fp32 (powf),
+ * which can be one ulp away from torch's fp32 pow in a few entries, an error that grows with the position: hosts should
+ * load the tensor (QwenTextEngine does).
+ *
+ * ---- op-level entry points of the text decoder (kernel tests): one kernel of a forward round on caller-owned device
+ *      buffers, with the engine's dims and precision, on its stream, synchronised before returning; weights need not be
+ *      loaded.  "act" is the activation type: fp32 in WLK_PREC_FP32 mode, bf16 in WLK_PREC_BF16 mode.  rows in [1, 1024].
+ *      A KV cache is one session's layout [n_layer][2 (K, V)][n_kv_head][max_ctx][head_dim] act; kv_ptrs_host holds
+ *      n_slots device pointers and row r belongs to cache row_slot_host[r] at position row_pos_host[r] < max_ctx.
+ * wlk_qtext_op_rmsnorm:   out[o(r)] = w * x[r] * rsqrt(mean(x[r]^2) + rms_eps) over d_model, x / w fp32, out act;
+ *                         o(r) = out_row_host[r] (-1: the row is skipped), or r when out_row_host is NULL.
+ * wlk_qtext_op_qk_rope:   qkv fp32 [rows][(n_head + 2 n_kv_head) * 128]: per-head RMSNorm (q_norm_w / k_norm_w fp32 [128])
+ *                         and rotate-half RoPE of the q and k heads; q -> q_out act [rows][n_head * 128], k and v (as is)
+ *                         -> the row's cache at (layer, kv head, position).
+ * wlk_qtext_op_attention: causal GQA attention of q act [rows][n_head * 128] over cache positions 0 .. row_pos_host[r]
+ *                         -> out act [rows][n_head * 128], on the kernel the forward uses in this precision (tensor cores
+ *                         in bf16, SIMT in fp32) with the forward's tiling.  The rows must be packed as a forward packs
+ *                         them: each slot's rows contiguous and at consecutive positions.
+ * wlk_qtext_op_swiglu:    hid act [rows][ffn_dim] = silu(gate) * up, gu fp32 [rows][gate (ffn_dim) | up (ffn_dim)].   */
+int wlk_qtext_op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int32_t rows, const int32_t* out_row_host);
+int wlk_qtext_op_qk_rope(wlk_qtext* t, const float* qkv, const float* q_norm_w, const float* k_norm_w, const int32_t* row_pos_host,
+                         const int32_t* row_slot_host, int32_t rows, void* const* kv_ptrs_host, int32_t n_slots, int32_t layer,
+                         void* q_out);
+int wlk_qtext_op_attention(wlk_qtext* t, const void* q, const int32_t* row_pos_host, const int32_t* row_slot_host, int32_t rows,
+                           void* const* kv_ptrs_host, int32_t n_slots, int32_t layer, void* out);
+int wlk_qtext_op_swiglu(wlk_qtext* t, const float* gu, void* hid, int32_t rows);
 
 /* =====================================================================================
  * Step after the diarization forward (SURVEY.md section 8f item 4).  Replaces SortformerDiarizationOnline.

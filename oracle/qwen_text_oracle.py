@@ -61,7 +61,10 @@ class QwenTextOracle(TextDecodeDriver):
         if dims.tied:
             self.w["lm_head.weight"] = self.w["embed_tokens.weight"]
         hd = dims.head_dim
-        self.inv_freq = 1.0 / (dims.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd))
+        if "rotary_emb.inv_freq" in self.w:                 # the model's own buffer, when the host passes it
+            self.inv_freq = self.w["rotary_emb.inv_freq"].clone()
+        else:
+            self.inv_freq = 1.0 / (dims.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd))
         self.sessions: Dict[int, list] = {}
         self._next = 0
         self._last = torch.zeros(0, dims.vocab)

@@ -161,15 +161,47 @@ def _tie_weights(dims, seed):
     return sd
 
 
+def _long_histories(logits, vocab, rng):
+    """Histories of 600 .. 2000 tokens, longer than the pick kernel's 512-thread CTA, so its strided penalty and n-gram
+    loops run several times: the rows' own best ids repeated across thread strides (the first occurrence must claim the
+    penalty, whichever thread meets it), n-gram matches at both ends, ids outside the vocabulary, and a period-512
+    history that puts every repeat on the same thread."""
+    top = [[int(t) for t in torch.topk(logits[j], 6).indices] for j in range(logits.shape[0])]
+    a, b = vocab - 7, vocab - 6                              # the n-gram prefix: nowhere else in these histories
+    h8 = rng.integers(0, 64, 600)
+    for k, i in enumerate([3, 515, 300, 599, 4, 516]):     # same thread (3 / 515, 4 / 516) and other threads
+        h8[i] = top[8][k % 3]
+    n = 1100
+    h9 = rng.integers(100, 1000, n)
+    h9[:3] = [a, b, top[9][0]]                               # matches at the first window ...
+    h9[n - 5:n - 2] = [a, b, top[9][1]]                      # ... and the last windows
+    h9[n - 2:] = [a, b]
+    h10 = rng.integers(-3, vocab + 3, 2000)                  # a few ids outside [0, vocab): skipped by every control
+    h10[0] = h10[1999] = top[10][0]
+    h10[1024] = top[10][1]
+    h11 = np.tile(rng.integers(0, vocab, 512), 4)[:1537]
+    h11[[7, 519, 1031, 1536]] = top[11][0]
+    return [[int(t) for t in h] for h in (h8, h9, h10, h11)]
+
+
 def test_pick_kernel_adversarial_rows():
-    dims = dataclasses.replace(QWEN_TEXT_DIMS["tnano"], max_ctx=64)
+    """The pick kernel against the oracle's controls, at the tnano vocabulary and at Qwen3's 151936 ids (a 19 KB
+    seen-bitmap), on short adversarial rows and on histories up to 4x the 512-thread CTA."""
+    for vocab in (2048, 151936):
+        _pick_adversarial_rows(vocab)
+
+
+def _pick_adversarial_rows(vocab):
+    dims = dataclasses.replace(QWEN_TEXT_DIMS["tnano"], vocab=vocab, max_ctx=64)
     eng = QwenTextEngine(dims, _tie_weights(dims, 5), precision="fp32", max_sessions=1, max_batch=1)
     sid = eng.open_session()
-    eng.forward([sid], [(np.arange(20, 28, dtype=np.int32), None)], [8])
+    n_rows = 12
+    eng.forward([sid], [(np.arange(20, 20 + n_rows, dtype=np.int32), None)], [n_rows])
     logits = torch.as_tensor(eng.logits())
-    top = [int(torch.argmax(logits[j])) for j in range(8)]
+    top = [int(torch.argmax(logits[j])) for j in range(n_rows)]
     hists = [[], [top[1]], [top[2], top[2] + 1, 5, 6, 5], [5, 6, 7, 5, 6], [3] * 6, [1, 2, 1, 2, 1], list(range(40)),
-             [top[7]] * 3]
+             [top[7]] * 3] + _long_histories(logits, dims.vocab, np.random.default_rng(vocab))
+    assert len(hists) == n_rows and min(len(h) for h in hists[8:]) >= 600
     everything = list(range(dims.vocab))
     cases = [
         eng.make_controls(),
@@ -180,17 +212,17 @@ def test_pick_kernel_adversarial_rows():
         eng.make_controls(no_repeat_ngram_size=1, max_consecutive_text_tokens=2, wait_token_id=6),
         eng.make_controls(repetition_penalty=0.5, no_repeat_ngram_size=2, suppress_token_ids=top[:4]),
     ]
-    off = np.zeros(8, np.int32)
+    off = np.zeros(n_rows, np.int32)
     ln = np.asarray([len(h) for h in hists], np.int32)
     off[1:] = np.cumsum(ln[:-1])
     flat = np.asarray([t for h in hists for t in h], np.int32)
     for ci, ctl in enumerate(cases):
         picks, vals = eng.pick(flat, off, ln, ctl, return_values=True)
-        for j in range(8):
+        for j in range(n_rows):
             x = controlled_logits(logits[j], hists[j], ctl, dims.vocab)
             want = int(torch.argmax(x))
-            assert int(picks[j]) == want, (ci, j, int(picks[j]), want)
-            assert vals[j] == pytest.approx(float(x[want]), rel=1e-6), (ci, j, vals[j], float(x[want]))
+            assert int(picks[j]) == want, (vocab, ci, j, int(picks[j]), want)
+            assert vals[j] == pytest.approx(float(x[want]), rel=1e-6), (vocab, ci, j, vals[j], float(x[want]))
     eng.close()
 
 

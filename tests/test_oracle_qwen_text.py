@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from oracle.qwen_text_oracle import QwenTextOracle, banned_ngram_tokens
-from whisperlivekit_b200.qwen_dims import QWEN_TEXT_DIMS, synthetic_text_state_dict
+from whisperlivekit_b200.qwen_dims import QWEN_TEXT_DIMS, rope_inv_freq, synthetic_text_state_dict
 from qwen_text_replay import capture_logits, load_fixture, replay
 
 
@@ -47,6 +47,24 @@ def test_schedule_covers_the_paths():
     assert any(s["draft_all_accepted"] for s in st)
     assert any(s["draft_tokens"] and not s["draft_all_accepted"] for s in st)
     assert any(c.get("draft") and len(c["draft"]) > int(fx["max_new_tokens"]) for c in fx["calls"])
+
+
+@pytest.mark.parametrize("theta", [1e4, 1e6])
+def test_rope_inv_freq_is_transformers_bit_for_bit(theta):
+    """The RoPE frequencies every QwenTextEngine loads are transformers' own buffer, bit for bit.  Rounding a
+    double-precision pow once instead puts 19 (1e4) and 24 (1e6) of the 64 entries one ulp away: 2e-3 rad of angle at
+    position 32767."""
+    pytest.importorskip("transformers")
+    from transformers import Qwen3Config
+    from transformers.models.qwen3.modeling_qwen3 import Qwen3RotaryEmbedding
+    cfg = Qwen3Config(hidden_size=256, num_attention_heads=2, num_key_value_heads=1, head_dim=128,
+                      rope_parameters={"rope_type": "default", "rope_theta": theta})
+    want = Qwen3RotaryEmbedding(cfg).inv_freq.numpy()
+    got = rope_inv_freq(theta, 128)
+    assert got.dtype == np.float32 and got.shape == (64,)
+    assert np.array_equal(got.view(np.uint32), want.view(np.uint32)), np.flatnonzero(got != want)
+    rounded_once = np.asarray([1.0 / theta ** (2 * i / 128) for i in range(64)], np.float64).astype(np.float32)
+    assert (rounded_once != want).sum() >= 19                # what the helper exists to avoid
 
 
 def test_banned_ngrams_match_the_reference_rule():

@@ -30,6 +30,8 @@ def _models():
 
     dec = B200QwenTextDecoder.install(mine, engine_factory=factory)
     assert dec.dims == dims                                  # geometry recovered from the HF config
+    # the engine gets the model's live RoPE buffer (non-persistent: not in state_dict())
+    assert torch.equal(oracles[0].inv_freq, mine.text_model.rotary_emb.inv_freq)
     return ref, mine, oracles[0]
 
 

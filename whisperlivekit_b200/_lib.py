@@ -103,6 +103,10 @@ SIGNATURES = {
     "wlk_qtext_pick": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32,
                                  C.c_int32, _vp, _vp]),
     "wlk_qtext_logits": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp]),
+    "wlk_qtext_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp]),
+    "wlk_qtext_op_qk_rope": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
+    "wlk_qtext_op_attention": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
+    "wlk_qtext_op_swiglu": (C.c_int, [_vp, _vp, _vp, C.c_int32]),
     "wlk_select": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp]),
     "wlk_vad_create": (C.c_int, [C.c_int, C.c_int, _vp]),
     "wlk_vad_destroy": (C.c_int, [_vp]),

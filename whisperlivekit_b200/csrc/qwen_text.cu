@@ -472,6 +472,7 @@ void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const
     }
     else if (name == "lm_head.weight") { WLK_CHECK(!D.tied, "this geometry ties lm_head to embed_tokens"); mat(t->head, D.vocab, d); }
     else if (name == "norm.weight") vec(t->normw, d);
+    else if (name == "rotary_emb.inv_freq") vec(t->inv_freq, QT_HD / 2);     // optional: the host's own RoPE frequencies
     else if (name.rfind("layers.", 0) == 0) {
         const size_t dot = name.find('.', 7);
         WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
@@ -550,9 +551,11 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
         Lw.qn = (float*)talloc(t, QT_HD * 4, aw); Lw.kn = (float*)talloc(t, QT_HD * 4, aw);
         Lw.ln1 = (float*)talloc(t, (size_t)d * 4, aw); Lw.ln2 = (float*)talloc(t, (size_t)d * 4, aw);
     }
-    {   // inv_freq = 1 / theta^(2i / 128), as HF's default rope init computes it (fp32 arange / dim, then pow)
+    {   // default inv_freq = 1 / theta^(2i / 128) in fp32 arithmetic like HF's default rope init (fp32 exponent, pow, then
+        // 1 / x); libm's powf can still land one ulp away from torch's pow in a few entries, so hosts load
+        // "rotary_emb.inv_freq" (whisperlivekit_b200/qwen_text_engine.py always does)
         std::vector<float> f(QT_HD / 2);
-        for (int i = 0; i < QT_HD / 2; ++i) f[i] = (float)(1.0 / pow((double)D.rope_theta, (double)(float)(2 * i) / (double)QT_HD));
+        for (int i = 0; i < QT_HD / 2; ++i) f[i] = 1.0f / powf(D.rope_theta, (float)(2 * i) / (float)QT_HD);
         CUDA_CHECK(cudaMemcpy(t->inv_freq, f.data(), f.size() * 4, cudaMemcpyHostToDevice));
     }
     const size_t R = QT_ROUND_ROWS;
@@ -606,6 +609,51 @@ QTSession& tsession(wlk_qtext* t, int32_t sid) {
     return t->sess[sid];
 }
 
+// Attention tiles of one round (the bf16 kernel's CTAs): <= 16 consecutive rows of one slot, a new tile whenever the
+// slot changes.  Rows of a slot are contiguous and at consecutive positions, so a tile's row k sits at pos0 + k.
+int make_tiles(const int32_t* pos, const int32_t* slot, int R, QTAttnTile* tiles) {
+    int n = 0;
+    for (int k = 0; k < R; ++k) {
+        if (n == 0 || tiles[n - 1].slot != slot[k] || tiles[n - 1].n_rows == 16) tiles[n++] = QTAttnTile{k, 0, slot[k], pos[k]};
+        tiles[n - 1].n_rows++;
+    }
+    return n;
+}
+
+// The per-kernel launches of a round, shared by run_round and the op-level entry points.
+template <typename T>
+void launch_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, const int32_t* out_row_d, int R) {
+    qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(x, w, (T*)out, out_row_d, t->dims.d_model, t->dims.rms_eps);
+}
+
+template <typename T>
+void launch_qk_rope(wlk_qtext* t, const float* qkv, const float* qn, const float* kn, const int32_t* pos_d, const int32_t* slot_d,
+                    void* const* kv_d, int layer, void* qout, int R) {
+    const wlk_qtext_dims& D = t->dims;
+    qt_qk_rope_kernel<T><<<dim3(R, D.n_head + 2 * D.n_kv_head), QT_HD, 0, t->st>>>(qkv, qn, kn, t->inv_freq, pos_d, slot_d, kv_d,
+                                                                                 (T*)qout, layer, D.n_head, D.n_kv_head,
+                                                                                 D.max_ctx, D.rms_eps);
+}
+
+template <typename T>
+void launch_attention(wlk_qtext* t, const void* q, const int32_t* pos_d, const int32_t* slot_d, void* const* kv_d,
+                      const QTAttnTile* tiles_d, int n_tiles, int layer, void* out, int R) {
+    const int H = t->dims.n_head, KV = t->dims.n_kv_head;
+    if (t->act == DT_BF16)
+        qt_attention_mma_kernel<<<dim3(n_tiles, KV), 32 * (H / KV), 0, t->st>>>((const bf16*)q, tiles_d, kv_d, (bf16*)out,
+                                                                              layer, H, KV, t->dims.max_ctx);
+    else
+        qt_attention_kernel<T><<<dim3(R, KV), 32 * (H / KV), 0, t->st>>>((const T*)q, pos_d, slot_d, kv_d, (T*)out, layer,
+                                                                        H, KV, t->dims.max_ctx);
+}
+
+template <typename T>
+void launch_swiglu(wlk_qtext* t, const float* gu, void* hid, int R) {
+    const int64_t total = (int64_t)R * t->dims.ffn_dim;
+    const int blocks = (int)std::min<int64_t>((total + 255) / 256, 65535);
+    qt_swiglu_kernel<T><<<blocks, 256, 0, t->st>>>(gu, (T*)hid, R, t->dims.ffn_dim);
+}
+
 template <typename T>
 void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, const int32_t* slot_d, void* const* kv_d,
                const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles) {
@@ -615,41 +663,33 @@ void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, 
     qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, t->emb, t->up, t->x, d);
     for (int li = 0; li < D.n_layer; ++li) {
         QTLayerW& Lw = t->L[li];
-        qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, Lw.ln1, (T*)t->xn, nullptr, d, D.rms_eps);
+        launch_rmsnorm<T>(t, t->x, Lw.ln1, t->xn, nullptr, R);
         {   GemmArgs g;
             g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wqkv; g.w_type = t->act; g.ldw = d;
             g.M = R; g.N = W; g.K = d;
             g.epi.C = t->qkv; g.epi.c_type = DT_F32; g.epi.ldc = W;
             tgemm(t, g); }
-        qt_qk_rope_kernel<T><<<dim3(R, H + 2 * KV), QT_HD, 0, t->st>>>(t->qkv, Lw.qn, Lw.kn, t->inv_freq, pos_d, slot_d, kv_d,
-                                                                     (T*)t->qb, li, H, KV, D.max_ctx, D.rms_eps);
-        if (t->act == DT_BF16)
-            qt_attention_mma_kernel<<<dim3(n_tiles, KV), 32 * (H / KV), 0, t->st>>>((const bf16*)t->qb, tiles_d, kv_d, (bf16*)t->att,
-                                                                                  li, H, KV, D.max_ctx);
-        else
-            qt_attention_kernel<T><<<dim3(R, KV), 32 * (H / KV), 0, t->st>>>((const T*)t->qb, pos_d, slot_d, kv_d, (T*)t->att, li,
-                                                                            H, KV, D.max_ctx);
+        launch_qk_rope<T>(t, t->qkv, Lw.qn, Lw.kn, pos_d, slot_d, kv_d, li, t->qb, R);
+        launch_attention<T>(t, t->qb, pos_d, slot_d, kv_d, tiles_d, n_tiles, li, t->att, R);
         {   GemmArgs g;
             g.A = t->att; g.a_type = t->act; g.lda = H * QT_HD; g.W = Lw.Wo; g.w_type = t->act; g.ldw = H * QT_HD;
             g.M = R; g.N = d; g.K = H * QT_HD;
             g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
             tgemm(t, g); }
-        qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, Lw.ln2, (T*)t->xn, nullptr, d, D.rms_eps);
+        launch_rmsnorm<T>(t, t->x, Lw.ln2, t->xn, nullptr, R);
         {   GemmArgs g;
             g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wgu; g.w_type = t->act; g.ldw = d;
             g.M = R; g.N = 2 * F; g.K = d;
             g.epi.C = t->gu; g.epi.c_type = DT_F32; g.epi.ldc = 2 * F;
             tgemm(t, g); }
-        {   const int64_t total = (int64_t)R * F;
-            const int blocks = (int)std::min<int64_t>((total + 255) / 256, 65535);
-            qt_swiglu_kernel<T><<<blocks, 256, 0, t->st>>>(t->gu, (T*)t->hid, R, F); }
+        launch_swiglu<T>(t, t->gu, t->hid, R);
         {   GemmArgs g;
             g.A = t->hid; g.a_type = t->act; g.lda = F; g.W = Lw.Wd; g.w_type = t->act; g.ldw = F;
             g.M = R; g.N = d; g.K = F;
             g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
             tgemm(t, g); }
     }
-    qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(t->x, t->normw, (T*)t->hlog, logit_row_d, d, D.rms_eps);
+    launch_rmsnorm<T>(t, t->x, t->normw, t->hlog, logit_row_d, R);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -701,8 +741,6 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
         for (int i = 0; i < n; ++i) kvp[i] = t->sess[sids[i]].kv;
         // embedding rows of this round go to `up` in the order they appear: packed into pinned memory, one copy
         int n_up = 0;
-        QTAttnTile* tiles = reinterpret_cast<QTAttnTile*>(t->stg_h + o_tile);
-        int n_tiles = 0;
         for (int k = 0; k < R; ++k) {
             const int r = r0 + k;
             int s = row_src[row_off[0] + r];
@@ -711,11 +749,9 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
                 s = -1 - n_up++;
             }
             src[k] = s; pos[k] = r_pos[r]; slot[k] = r_sess[r]; lrow[k] = r_log[r];
-            // attention tiles: <= 16 consecutive rows of one session
-            if (n_tiles == 0 || tiles[n_tiles - 1].slot != r_sess[r] || tiles[n_tiles - 1].n_rows == 16)
-                tiles[n_tiles++] = QTAttnTile{k, 0, r_sess[r], r_pos[r]};
-            tiles[n_tiles - 1].n_rows++;
         }
+        QTAttnTile* tiles = reinterpret_cast<QTAttnTile*>(t->stg_h + o_tile);
+        const int n_tiles = make_tiles(pos, slot, R, tiles);
         if (n_up) CUDA_CHECK(cudaMemcpyAsync(t->up, t->up_h, (size_t)n_up * D.d_model * 4, cudaMemcpyHostToDevice, t->st));
         CUDA_CHECK(cudaMemcpyAsync(t->stg_d, t->stg_h, off, cudaMemcpyHostToDevice, t->st));
         CUDA_CHECK(cudaEventRecord(t->stg_ev, t->st));
@@ -795,6 +831,102 @@ void logits_out(wlk_qtext* t, int row0, int rows, float* out) {
         CUDA_CHECK(cudaMemcpyAsync(out + (size_t)g0 * t->dims.vocab, t->logits, (size_t)r * t->dims.vocab * 4, cudaMemcpyDeviceToHost, t->st));
         CUDA_CHECK(cudaStreamSynchronize(t->st));
     }
+}
+
+// ---- op-level entry points: one kernel of a round on caller-owned device buffers ----------------------------------
+// Device copies of an op call's host index arrays, freed once the op's work on the stream is done.
+struct OpUpload {
+    wlk_qtext* t;
+    std::vector<void*> bufs;
+    template <typename X>
+    const X* put(const X* host, size_t n) {
+        void* p = nullptr;
+        CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(X)));
+        bufs.push_back(p);
+        CUDA_CHECK(cudaMemcpyAsync(p, host, n * sizeof(X), cudaMemcpyHostToDevice, t->st));
+        return (const X*)p;
+    }
+    ~OpUpload() {
+        cudaStreamSynchronize(t->st);
+        for (void* p : bufs) cudaFree(p);
+    }
+};
+
+void op_rows(int rows) { WLK_CHECK(rows >= 1 && rows <= QT_ROUND_ROWS, "rows %d outside [1, %d]", rows, QT_ROUND_ROWS); }
+
+// What the qk-rope and attention kernels index with: slot and position of each row, a layer, the slots' caches.
+// `packed`: the rows are laid out as a forward packs them (each slot's rows contiguous, at consecutive positions), which
+// the attention tiles assume.
+void op_check_rows(wlk_qtext* t, const int32_t* pos, const int32_t* slot, int rows, void* const* kv, int n_slots, int layer,
+                   bool packed) {
+    op_rows(rows);
+    WLK_CHECK(layer >= 0 && layer < t->dims.n_layer, "layer %d outside [0, %d)", layer, t->dims.n_layer);
+    WLK_CHECK(n_slots >= 1, "no KV caches");
+    std::vector<char> done(n_slots, 0);
+    for (int r = 0; r < rows; ++r) {
+        WLK_CHECK(slot[r] >= 0 && slot[r] < n_slots, "row %d: slot %d outside [0, %d)", r, slot[r], n_slots);
+        WLK_CHECK(kv[slot[r]] != nullptr, "row %d: slot %d has no KV cache", r, slot[r]);
+        WLK_CHECK(pos[r] >= 0 && pos[r] < t->dims.max_ctx, "row %d: position %d outside [0, %d)", r, pos[r], t->dims.max_ctx);
+        if (!packed) continue;
+        if (r > 0 && slot[r] == slot[r - 1]) {
+            WLK_CHECK(pos[r] == pos[r - 1] + 1, "row %d: position %d does not follow %d of the same slot", r, pos[r], pos[r - 1]);
+        } else {
+            WLK_CHECK(!done[slot[r]], "row %d: the rows of slot %d are not contiguous", r, slot[r]);
+            done[slot[r]] = 1;
+        }
+    }
+}
+
+void op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int rows, const int32_t* out_row) {
+    WLK_CHECK(x && w && out, "null argument");
+    op_rows(rows);
+    if (out_row) for (int r = 0; r < rows; ++r) WLK_CHECK(out_row[r] >= -1, "row %d: output row %d", r, out_row[r]);
+    OpUpload up{t};
+    const int32_t* out_row_d = out_row ? up.put(out_row, rows) : nullptr;
+    if (t->act == DT_F32) launch_rmsnorm<float>(t, x, w, out, out_row_d, rows);
+    else launch_rmsnorm<bf16>(t, x, w, out, out_row_d, rows);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
+}
+
+void op_qk_rope(wlk_qtext* t, const float* qkv, const float* qn, const float* kn, const int32_t* pos, const int32_t* slot, int rows,
+                void* const* kv, int n_slots, int layer, void* qout) {
+    WLK_CHECK(qkv && qn && kn && pos && slot && kv && qout, "null argument");
+    op_check_rows(t, pos, slot, rows, kv, n_slots, layer, false);
+    OpUpload up{t};
+    const int32_t* pos_d = up.put(pos, rows);
+    const int32_t* slot_d = up.put(slot, rows);
+    void* const* kv_d = up.put(kv, n_slots);
+    if (t->act == DT_F32) launch_qk_rope<float>(t, qkv, qn, kn, pos_d, slot_d, kv_d, layer, qout, rows);
+    else launch_qk_rope<bf16>(t, qkv, qn, kn, pos_d, slot_d, kv_d, layer, qout, rows);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
+}
+
+void op_attention(wlk_qtext* t, const void* q, const int32_t* pos, const int32_t* slot, int rows, void* const* kv, int n_slots,
+                  int layer, void* out) {
+    WLK_CHECK(q && pos && slot && kv && out, "null argument");
+    op_check_rows(t, pos, slot, rows, kv, n_slots, layer, true);
+    std::vector<QTAttnTile> tiles(rows);
+    const int n_tiles = make_tiles(pos, slot, rows, tiles.data());
+    OpUpload up{t};
+    const int32_t* pos_d = up.put(pos, rows);
+    const int32_t* slot_d = up.put(slot, rows);
+    void* const* kv_d = up.put(kv, n_slots);
+    const QTAttnTile* tiles_d = up.put(tiles.data(), n_tiles);
+    if (t->act == DT_F32) launch_attention<float>(t, q, pos_d, slot_d, kv_d, tiles_d, n_tiles, layer, out, rows);
+    else launch_attention<bf16>(t, q, pos_d, slot_d, kv_d, tiles_d, n_tiles, layer, out, rows);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
+}
+
+void op_swiglu(wlk_qtext* t, const float* gu, void* hid, int rows) {
+    WLK_CHECK(gu && hid, "null argument");
+    op_rows(rows);
+    if (t->act == DT_F32) launch_swiglu<float>(t, gu, hid, rows);
+    else launch_swiglu<bf16>(t, gu, hid, rows);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(t->st));
 }
 
 }  // namespace
@@ -924,6 +1056,33 @@ int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host
     TLOCK(t);
     WLK_CHECK(out_host || n_rows == 0, "null output buffer");
     logits_out(t, row0, n_rows, out_host);
+    WLK_API_END
+}
+int wlk_qtext_op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int32_t rows, const int32_t* out_row_host) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    op_rmsnorm(t, x, w, out, rows, out_row_host);
+    WLK_API_END
+}
+int wlk_qtext_op_qk_rope(wlk_qtext* t, const float* qkv, const float* q_norm_w, const float* k_norm_w, const int32_t* row_pos_host,
+                         const int32_t* row_slot_host, int32_t rows, void* const* kv_ptrs_host, int32_t n_slots, int32_t layer,
+                         void* q_out) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    op_qk_rope(t, qkv, q_norm_w, k_norm_w, row_pos_host, row_slot_host, rows, kv_ptrs_host, n_slots, layer, q_out);
+    WLK_API_END
+}
+int wlk_qtext_op_attention(wlk_qtext* t, const void* q, const int32_t* row_pos_host, const int32_t* row_slot_host, int32_t rows,
+                           void* const* kv_ptrs_host, int32_t n_slots, int32_t layer, void* out) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    op_attention(t, q, row_pos_host, row_slot_host, rows, kv_ptrs_host, n_slots, layer, out);
+    WLK_API_END
+}
+int wlk_qtext_op_swiglu(wlk_qtext* t, const float* gu, void* hid, int32_t rows) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    op_swiglu(t, gu, hid, rows);
     WLK_API_END
 }
 

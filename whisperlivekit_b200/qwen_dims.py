@@ -110,8 +110,8 @@ class QwenTextDims:
     third_party/qwen3-asr-causal/src/qwen3_asr_causal/model.py:1498-1507).
 
     Qwen3-ASR's thinker uses MRoPE; with audio rows and text only, its three position streams are equal, so it reduces
-    to plain 1D rotate-half RoPE over ``head_dim`` with ``inv_freq = rope_theta ** (-2i / head_dim)``.  The engine
-    assumes exactly that."""
+    to plain 1D rotate-half RoPE over ``head_dim`` with ``inv_freq = rope_theta ** (-2i / head_dim)`` (``rope_inv_freq``,
+    in HF's fp32 arithmetic).  The engine assumes exactly that."""
     vocab: int = 151936
     d_model: int = 1024
     n_layer: int = 28
@@ -136,6 +136,17 @@ QWEN_TEXT_DIMS: Dict[str, QwenTextDims] = {
     # vocab 151936, theta 1e6, tied embeddings); to be confirmed against the checkpoint's thinker_config.text_config
     "qwen3-asr-0.6b": QwenTextDims(),
 }
+
+
+def rope_inv_freq(rope_theta: float, head_dim: int = 128) -> np.ndarray:
+    """RoPE frequencies [head_dim / 2] exactly as HF's default rope init computes them (transformers'
+    ``Qwen3RotaryEmbedding``, and the reference's ``_qwen3_asr_default_rope_init``): fp32 torch arithmetic,
+    ``1 / base ** (arange(0, dim, 2).float() / dim)``.  Rounded once from a double-precision pow, or by a C ``powf``, some
+    entries land one ulp away, and the angle error grows with the position."""
+    import torch
+    base = float(rope_theta)
+    inv = 1.0 / (base ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(dtype=torch.float) / head_dim))
+    return inv.numpy().astype(np.float32)
 
 
 def synthetic_text_state_dict(dims: QwenTextDims, seed: int = 0) -> Dict[str, np.ndarray]:

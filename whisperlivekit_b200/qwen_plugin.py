@@ -229,6 +229,10 @@ class B200QwenTextDecoder:
                 **engine_kw):
         dims = cls.dims_of(model, max_ctx)
         sd = {k: v.detach().float().cpu().numpy() for k, v in model.text_model.state_dict().items()}
+        rotary = getattr(model.text_model, "rotary_emb", None)
+        if rotary is not None and getattr(rotary, "inv_freq", None) is not None:
+            # the live buffer the model rotates with (non-persistent, so not in state_dict())
+            sd["rotary_emb.inv_freq"] = rotary.inv_freq.detach().float().cpu().numpy()
         if not dims.tied:
             sd["lm_head.weight"] = model.lm_head.weight.detach().float().cpu().numpy()
         if engine_factory is None:

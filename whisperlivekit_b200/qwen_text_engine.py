@@ -21,7 +21,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib as L
-from .qwen_dims import QwenTextDims
+from .qwen_dims import QwenTextDims, rope_inv_freq
 
 
 def _ptr(a: np.ndarray):
@@ -296,6 +296,8 @@ class QwenTextEngine(TextDecodeDriver):
         self.h = h
         self._closed = False
         self._n_logit = 0
+        # HF's fp32 RoPE frequencies; a state dict that carries the model's own buffer overrides them
+        self.load_tensor("rotary_emb.inv_freq", rope_inv_freq(dims.rope_theta, dims.head_dim))
         if state_dict is not None:
             self.load_state_dict(state_dict)
 
@@ -376,6 +378,32 @@ class QwenTextEngine(TextDecodeDriver):
         out = np.zeros((max(n_rows, 1), self.vocab), np.float32)
         L.check(self.lib.wlk_qtext_logits(self.h, int(row0), int(n_rows), _ptr(out)))
         return out[:n_rows]
+
+    # -- op-level (device pointers, e.g. torch tensors' data_ptr(); activations are fp32 or bf16 as the precision) ----
+    def op_rmsnorm(self, x_ptr, w_ptr, out_ptr, rows: int, out_row: Optional[Sequence[int]] = None) -> None:
+        orow = None if out_row is None else np.ascontiguousarray(out_row, np.int32)
+        L.check(self.lib.wlk_qtext_op_rmsnorm(self.h, x_ptr, w_ptr, out_ptr, int(rows), None if orow is None else _ptr(orow)))
+
+    @staticmethod
+    def _rows(row_pos, row_slot, kv_ptrs):
+        pos = np.ascontiguousarray(row_pos, np.int32)
+        slot = np.ascontiguousarray(row_slot, np.int32)
+        kv = (C.c_void_p * len(kv_ptrs))(*[int(p) for p in kv_ptrs])
+        return pos, slot, kv
+
+    def op_qk_rope(self, qkv_ptr, q_norm_ptr, k_norm_ptr, row_pos, row_slot, kv_ptrs: Sequence[int], layer: int,
+                   q_out_ptr) -> None:
+        pos, slot, kv = self._rows(row_pos, row_slot, kv_ptrs)
+        L.check(self.lib.wlk_qtext_op_qk_rope(self.h, qkv_ptr, q_norm_ptr, k_norm_ptr, _ptr(pos), _ptr(slot), len(pos), kv,
+                                              len(kv_ptrs), int(layer), q_out_ptr))
+
+    def op_attention(self, q_ptr, row_pos, row_slot, kv_ptrs: Sequence[int], layer: int, out_ptr) -> None:
+        pos, slot, kv = self._rows(row_pos, row_slot, kv_ptrs)
+        L.check(self.lib.wlk_qtext_op_attention(self.h, q_ptr, _ptr(pos), _ptr(slot), len(pos), kv, len(kv_ptrs), int(layer),
+                                                out_ptr))
+
+    def op_swiglu(self, gu_ptr, hid_ptr, rows: int) -> None:
+        L.check(self.lib.wlk_qtext_op_swiglu(self.h, gu_ptr, hid_ptr, int(rows)))
 
     def close(self) -> None:
         if not self._closed:
