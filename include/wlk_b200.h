@@ -252,6 +252,17 @@ int wlk_qwen_append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* 
  * one piece (whatever the block size), a sub-chunk remainder is dropped.                                          */
 int wlk_qwen_flush_pending(wlk_qwen* q, const int32_t* sids, int n, float* out_host, int64_t out_capacity_rows,
                            int32_t* out_row_offsets);
+/* The same two calls with the output rows in device memory (out_dev, fp32 [rows][out_dim]): the rows are copied device to
+ * device and are complete when the call returns.                                                                 */
+int wlk_qwen_forward_chunk_device(wlk_qwen* q, const int32_t* sids, int n, const float* mels_host, const int32_t* frame_offsets,
+                                  float* out_dev, int64_t out_capacity_rows, int32_t* out_row_offsets);
+int wlk_qwen_flush_pending_device(wlk_qwen* q, const int32_t* sids, int n, float* out_dev, int64_t out_capacity_rows,
+                                  int32_t* out_row_offsets);
+/* QwenAudioCausalKVState.mel_buffer: the mel frames a session holds until a whole block (or chunk) is ready, [frames][n_mels]
+ * fp32 on the host.  get copies them out (*n_frames = their count; fails when it exceeds capacity_frames); set replaces
+ * them, e.g. to carry a stream's pending frames into a fresh session.                                              */
+int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int64_t capacity_frames, int32_t* n_frames);
+int wlk_qwen_session_set_pending(wlk_qwen* q, int32_t sid, const float* mels_host, int32_t n_frames);
 
 /* =====================================================================================
  * Qwen3-ASR text decoder (HF Qwen3Model + lm_head, reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/
@@ -290,6 +301,22 @@ int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len);
  * wlk_qtext_pick / wlk_qtext_logits.  A forward that would pass max_ctx fails ("context full") and changes nothing. */
 int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
                       const float* embeds_host, int32_t n_embeds, const int32_t* logit_rows);
+/* wlk_qtext_forward with the embedding rows in device memory: row j of embeds_dev (fp32, embeds_ld >= d_model floats
+ * apart) is gathered in place, with no host copy.  The rows must be complete when the call starts: the engine runs on
+ * its own stream and does not order itself after the producer's. */
+int wlk_qtext_forward_device(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
+                             const float* embeds_dev, int64_t embeds_ld, int32_t n_embeds, const int32_t* logit_rows);
+/* The frame adapter of the realtime model (QwenAudioSurgeryFrameAdapter, reference model.py:631-691), loaded as optional
+ * tensors under the module's names before finalize: adapter.proj.weight [d_model][in_dim] (no bias), and per block i
+ * adapter.blocks.i.norm.weight [d_model], adapter.blocks.i.mlp.{gate,up}.weight [hidden][d_model],
+ * adapter.blocks.i.mlp.down.weight [d_model][hidden], plus adapter.residual_scale [1] when there are blocks.  finalize
+ * derives in_dim, the block count and the hidden width from the shapes.
+ * wlk_qtext_adapt: out_dev[r] (fp32 [rows][d_model], row pitch out_ld) = the adapter of in_dev[r] (fp32 [rows][in_dim], row
+ * pitch in_ld): x = proj(in); per block x = x + residual_scale * down(silu(gate(n)) * up(n)), n = RMSNorm(x) with eps
+ * 1e-6.  GEMMs in the engine's precision; complete when the call returns.  Fails without adapter tensors.
+ * wlk_qtext_adapter_dims: in_dim (0 without an adapter), block count and hidden width.                              */
+int wlk_qtext_adapt(wlk_qtext* t, const float* in_dev, int32_t rows, int64_t in_ld, float* out_dev, int64_t out_ld);
+int wlk_qtext_adapter_dims(wlk_qtext* t, int32_t* in_dim, int32_t* n_blocks, int32_t* hidden);
 /* The greedy decode controls of _GreedyControlSession.controlled_logits + argmax (model.py:335-418) over every logit row
  * of the last forward: suppress -> repetition penalty on the unique in-vocab history -> n-gram ban -> max-consecutive
  * -> argmax (lowest index on ties).  Row j's history is hist_tokens[hist_off[j] .. hist_off[j] + hist_len[j]).

@@ -89,6 +89,10 @@ SIGNATURES = {
     "wlk_qwen_forward_chunk": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp]),
     "wlk_qwen_append_audio": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp, C.c_int32]),
     "wlk_qwen_flush_pending": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int64, _vp]),
+    "wlk_qwen_forward_chunk_device": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp]),
+    "wlk_qwen_flush_pending_device": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int64, _vp]),
+    "wlk_qwen_session_get_pending": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, _vp]),
+    "wlk_qwen_session_set_pending": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32]),
     "wlk_qtext_create": (C.c_int, [_vp, _vp, _vp]),
     "wlk_qtext_destroy": (C.c_int, [_vp]),
     "wlk_qtext_load_tensor": (C.c_int, [_vp, C.c_char_p, _vp, _vp, C.c_int]),
@@ -100,6 +104,9 @@ SIGNATURES = {
     "wlk_qtext_session_len": (C.c_int, [_vp, C.c_int32, _vp]),
     "wlk_qtext_crop": (C.c_int, [_vp, C.c_int32, C.c_int32]),
     "wlk_qtext_forward": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int32, _vp]),
+    "wlk_qtext_forward_device": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, C.c_int64, C.c_int32, _vp]),
+    "wlk_qtext_adapt": (C.c_int, [_vp, _vp, C.c_int32, C.c_int64, _vp, C.c_int64]),
+    "wlk_qtext_adapter_dims": (C.c_int, [_vp, _vp, _vp, _vp]),
     "wlk_qtext_pick": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32,
                                  C.c_int32, _vp, _vp]),
     "wlk_qtext_logits": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp]),

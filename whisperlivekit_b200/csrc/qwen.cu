@@ -566,8 +566,9 @@ void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, void*
 
 // flush = false: forward_chunk (causal.py:713-782).  flush = true: flush_pending (causal.py:687-711) -- no new frames,
 // the buffered whole 8-frame chunks are encoded as one piece regardless of the block size, the remainder is dropped.
+// out_dev: `out` is device memory (the rows never leave the GPU).
 void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, const int32_t* frame_off, float* out,
-                   int64_t cap_rows, int32_t* out_row_off, bool flush) {
+                   int64_t cap_rows, int32_t* out_row_off, bool flush, bool out_dev = false) {
     const wlk_qwen_dims& D = q->dims;
     WLK_CHECK(q->finalized, "weights not finalized");
     WLK_CHECK(n >= 1 && n <= q->cfg.max_batch, "batch %d outside [1, %d]", n, q->cfg.max_batch);
@@ -666,7 +667,8 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
         for (int k = 0; k < nj; ++k) {
             const int i = who[k];
             CUDA_CHECK(cudaMemcpyAsync(out + ((size_t)out_row_off[i] + done_steps[i]) * D.out_dim, q->outbuf + (size_t)r * D.out_dim,
-                                       (size_t)steps[k] * D.out_dim * 4, cudaMemcpyDeviceToHost, q->st));
+                                       (size_t)steps[k] * D.out_dim * 4, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                                       q->st));
             r += steps[k];
             done_steps[i] += steps[k];
             q->sess[sids[i]].emitted += M > 0 ? freeze[i] : steps[k];    // a mutable tail: only the frozen steps count (:638)
@@ -895,6 +897,44 @@ int wlk_qwen_flush_pending(wlk_qwen* q, const int32_t* sids, int n, float* out_h
     WLK_CHECK(sids && out_row_offsets, "null argument");
     WLK_CHECK(out_host || out_capacity_rows == 0, "null output buffer");
     forward_chunk(q, sids, n, nullptr, nullptr, out_host, out_capacity_rows, out_row_offsets, true);
+    WLK_API_END
+}
+int wlk_qwen_forward_chunk_device(wlk_qwen* q, const int32_t* sids, int n, const float* mels_host, const int32_t* frame_offsets,
+                                  float* out_dev, int64_t out_capacity_rows, int32_t* out_row_offsets) {
+    WLK_API_BEGIN
+    QLOCK(q);
+    WLK_CHECK(sids && frame_offsets && out_row_offsets && (mels_host || frame_offsets[n] == frame_offsets[0]), "null argument");
+    WLK_CHECK(out_dev || out_capacity_rows == 0, "null output buffer");
+    forward_chunk(q, sids, n, mels_host, frame_offsets, out_dev, out_capacity_rows, out_row_offsets, false, true);
+    WLK_API_END
+}
+int wlk_qwen_flush_pending_device(wlk_qwen* q, const int32_t* sids, int n, float* out_dev, int64_t out_capacity_rows,
+                                  int32_t* out_row_offsets) {
+    WLK_API_BEGIN
+    QLOCK(q);
+    WLK_CHECK(sids && out_row_offsets, "null argument");
+    WLK_CHECK(out_dev || out_capacity_rows == 0, "null output buffer");
+    forward_chunk(q, sids, n, nullptr, nullptr, out_dev, out_capacity_rows, out_row_offsets, true, true);
+    WLK_API_END
+}
+int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int64_t capacity_frames, int32_t* n_frames) {
+    WLK_API_BEGIN
+    QLOCK(q);
+    QSession& s = qsession(q, sid);
+    WLK_CHECK(n_frames, "null argument");
+    const int64_t have = (int64_t)(s.pending.size() / q->dims.n_mels);
+    WLK_CHECK(have <= capacity_frames, "%lld pending frames exceed the buffer's %lld", (long long)have, (long long)capacity_frames);
+    WLK_CHECK(mels_host || have == 0, "null output buffer");
+    if (have) memcpy(mels_host, s.pending.data(), s.pending.size() * 4);
+    *n_frames = (int32_t)have;
+    WLK_API_END
+}
+int wlk_qwen_session_set_pending(wlk_qwen* q, int32_t sid, const float* mels_host, int32_t n_frames) {
+    WLK_API_BEGIN
+    QLOCK(q);
+    QSession& s = qsession(q, sid);
+    WLK_CHECK(n_frames >= 0 && (mels_host || n_frames == 0), "bad arguments");
+    s.pending.assign(mels_host, mels_host + (size_t)n_frames * q->dims.n_mels);
     WLK_API_END
 }
 int wlk_qwen_append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm_host, const int64_t* sample_offsets,

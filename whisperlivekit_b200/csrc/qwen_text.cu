@@ -38,13 +38,21 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
     return r;
 }
 
-// x[r] = embed_tokens[src] (src >= 0) or the uploaded host row up[-1 - src]
+// x[r] = embed_tokens[src] (src >= 0) or the embedding row up[-1 - src] (rows up_ld floats apart: the uploaded host rows,
+// or the caller's device rows)
 __global__ void qt_embed_kernel(const int32_t* __restrict__ src, const float* __restrict__ emb, const float* __restrict__ up,
-                                float* __restrict__ x, int d) {
+                                int64_t up_ld, float* __restrict__ x, int d) {
     const int r = blockIdx.x;
     const int s = src[r];
-    const float* from = s >= 0 ? emb + (int64_t)s * d : up + (int64_t)(-1 - s) * d;
+    const float* from = s >= 0 ? emb + (int64_t)s * d : up + (int64_t)(-1 - s) * up_ld;
     for (int i = threadIdx.x; i < d; i += blockDim.x) x[(int64_t)r * d + i] = from[i];
+}
+
+// fp32 rows [R][cols] with row pitch ld -> act [R][cols] (the frame adapter's GEMM operand)
+template <typename T>
+__global__ void qt_rows_to_act_kernel(const float* __restrict__ in, int64_t ld, T* __restrict__ out, int cols) {
+    const int r = blockIdx.x;
+    for (int i = threadIdx.x; i < cols; i += blockDim.x) out[(int64_t)r * cols + i] = from_f32<T>(in[(int64_t)r * ld + i]);
 }
 
 // Qwen3RMSNorm: w * (x * rsqrt(mean(x^2) + eps)), fp32 statistics; out row = out_row ? out_row[r] : r (skip when < 0)
@@ -380,6 +388,21 @@ struct QTSession {
     void* kv = nullptr;
 };
 
+// QwenAudioSurgeryFrameAdapter (reference model.py:631-691): proj [d][in_dim] without bias, then `nb` blocks of
+// x + scale * down(silu(gate(n)) * up(n)), n = RMSNorm(x) with eps 1e-6 (the reference's own RMSNorm, model.py:83-91).
+// Tensors are stashed on load and packed by finalize, which derives in_dim, nb and the hidden width from their shapes.
+struct QTAdapter {
+    int in_dim = 0, hidden = 0, nb = 0;
+    float scale = 0.f;
+    void* Wp = nullptr;                              // act [d][in_dim]
+    std::vector<float*> norm;                        // fp32 [d]
+    std::vector<void*> Wgu, Wd;                      // act [2 hidden][d] (gate | up), [d][hidden]
+    void* a_in = nullptr;                            // act [QT_ROUND_ROWS][in_dim]
+    float* a_gu = nullptr;                           // fp32 [QT_ROUND_ROWS][2 hidden]
+    void* a_hid = nullptr;                           // act [QT_ROUND_ROWS][hidden]
+};
+constexpr float QT_ADAPTER_EPS = 1e-6f;
+
 }  // namespace
 }  // namespace wlk
 
@@ -411,6 +434,9 @@ struct wlk_qtext {
     int logit_cap = 0, n_logit = 0;                      // rows of hlog; rows the last forward kept
     float* sk_scratch = nullptr; int* sk_counters = nullptr;
     uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
+    std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> adapter_stash;   // until finalize
+    bool has_adapter = false;
+    QTAdapter ad;
     size_t es() const { return dtype_size(act); }
 };
 
@@ -473,6 +499,10 @@ void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const
     else if (name == "lm_head.weight") { WLK_CHECK(!D.tied, "this geometry ties lm_head to embed_tokens"); mat(t->head, D.vocab, d); }
     else if (name == "norm.weight") vec(t->normw, d);
     else if (name == "rotary_emb.inv_freq") vec(t->inv_freq, QT_HD / 2);     // optional: the host's own RoPE frequencies
+    else if (name.rfind("adapter.", 0) == 0) {                                   // optional: the frame adapter, packed by finalize
+        WLK_CHECK(!t->finalized, "adapter tensor %s loaded after finalize", name.c_str());
+        t->adapter_stash[name] = {std::vector<int64_t>(shape, shape + ndim), std::vector<float>(host, host + n)};
+    }
     else if (name.rfind("layers.", 0) == 0) {
         const size_t dot = name.find('.', 7);
         WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
@@ -508,6 +538,71 @@ std::vector<std::string> required(const wlk_qtext_dims& D) {
             r.push_back(p + s + ".weight");
     }
     return r;
+}
+
+// Pack the stashed adapter tensors (no-op when none were loaded).
+void build_adapter(wlk_qtext* t) {
+    auto& st = t->adapter_stash;
+    if (st.empty()) return;
+    const int d = t->dims.d_model;
+    auto get = [&](const std::string& name) -> std::pair<std::vector<int64_t>, std::vector<float>>& {
+        auto it = st.find(name);
+        WLK_CHECK(it != st.end(), "adapter tensor %s missing", name.c_str());
+        return it->second;
+    };
+    auto& proj = get("adapter.proj.weight");
+    WLK_CHECK(proj.first.size() == 2 && proj.first[0] == d && proj.first[1] >= 8 && proj.first[1] % 8 == 0,
+              "adapter.proj.weight must be [d_model][in_dim] with in_dim a multiple of 8");
+    QTAdapter& A = t->ad;
+    A.in_dim = (int)proj.first[1];
+    int nb = 0;
+    while (st.count("adapter.blocks." + std::to_string(nb) + ".norm.weight")) ++nb;
+    A.nb = nb;
+    size_t used = 1;
+    if (nb > 0) {
+        auto& rs = get("adapter.residual_scale");
+        WLK_CHECK(rs.second.size() == 1, "adapter.residual_scale must hold one value");
+        A.scale = rs.second[0];
+        used++;
+        A.hidden = (int)get("adapter.blocks.0.mlp.gate.weight").first[0];
+        WLK_CHECK(A.hidden >= 8 && A.hidden % 8 == 0, "adapter hidden width %d must be a positive multiple of 8", A.hidden);
+    } else if (st.count("adapter.residual_scale")) {
+        used++;
+    }
+    const size_t es = t->es();
+    size_t* aw = &t->bytes_weights;
+    A.Wp = talloc(t, (size_t)d * A.in_dim * es, aw);
+    put(t, proj.second.data(), proj.second.size(), A.Wp, t->act);
+    const int64_t H = A.hidden;
+    for (int i = 0; i < nb; ++i) {
+        const std::string p = "adapter.blocks." + std::to_string(i) + ".";
+        auto& nw = get(p + "norm.weight");
+        auto& g = get(p + "mlp.gate.weight");
+        auto& u = get(p + "mlp.up.weight");
+        auto& dn = get(p + "mlp.down.weight");
+        WLK_CHECK(nw.first == std::vector<int64_t>{d}, "%snorm.weight must be [d_model]", p.c_str());
+        WLK_CHECK(g.first == (std::vector<int64_t>{H, d}) && u.first == (std::vector<int64_t>{H, d}),
+                  "%smlp.gate / mlp.up must be [hidden][d_model] with the hidden width of block 0", p.c_str());
+        WLK_CHECK(dn.first == (std::vector<int64_t>{d, H}), "%smlp.down.weight must be [d_model][hidden]", p.c_str());
+        float* nd = (float*)talloc(t, (size_t)d * 4, aw);
+        put(t, nw.second.data(), nw.second.size(), nd, DT_F32);
+        void* gu = talloc(t, (size_t)2 * H * d * es, aw);
+        put(t, g.second.data(), g.second.size(), gu, t->act);
+        put(t, u.second.data(), u.second.size(), (char*)gu + (size_t)H * d * es, t->act);
+        void* wd = talloc(t, (size_t)d * H * es, aw);
+        put(t, dn.second.data(), dn.second.size(), wd, t->act);
+        A.norm.push_back(nd); A.Wgu.push_back(gu); A.Wd.push_back(wd);
+        used += 4;
+    }
+    WLK_CHECK(used == st.size(), "%zu adapter tensors do not belong to an adapter of %d blocks", st.size() - used, nb);
+    size_t* ws = &t->bytes_workspace;
+    A.a_in = talloc(t, (size_t)QT_ROUND_ROWS * A.in_dim * es, ws);
+    if (nb > 0) {
+        A.a_gu = (float*)talloc(t, (size_t)QT_ROUND_ROWS * 2 * H * 4, ws);
+        A.a_hid = talloc(t, (size_t)QT_ROUND_ROWS * H * es, ws);
+    }
+    st.clear();
+    t->has_adapter = true;
 }
 
 void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) {
@@ -622,8 +717,8 @@ int make_tiles(const int32_t* pos, const int32_t* slot, int R, QTAttnTile* tiles
 
 // The per-kernel launches of a round, shared by run_round and the op-level entry points.
 template <typename T>
-void launch_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, const int32_t* out_row_d, int R) {
-    qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(x, w, (T*)out, out_row_d, t->dims.d_model, t->dims.rms_eps);
+void launch_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, const int32_t* out_row_d, int R, float eps) {
+    qt_rmsnorm_kernel<T><<<R, 256, 0, t->st>>>(x, w, (T*)out, out_row_d, t->dims.d_model, eps);
 }
 
 template <typename T>
@@ -648,22 +743,22 @@ void launch_attention(wlk_qtext* t, const void* q, const int32_t* pos_d, const i
 }
 
 template <typename T>
-void launch_swiglu(wlk_qtext* t, const float* gu, void* hid, int R) {
-    const int64_t total = (int64_t)R * t->dims.ffn_dim;
+void launch_swiglu(wlk_qtext* t, const float* gu, void* hid, int R, int F) {
+    const int64_t total = (int64_t)R * F;
     const int blocks = (int)std::min<int64_t>((total + 255) / 256, 65535);
-    qt_swiglu_kernel<T><<<blocks, 256, 0, t->st>>>(gu, (T*)hid, R, t->dims.ffn_dim);
+    qt_swiglu_kernel<T><<<blocks, 256, 0, t->st>>>(gu, (T*)hid, R, F);
 }
 
 template <typename T>
 void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, const int32_t* slot_d, void* const* kv_d,
-               const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles) {
+               const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles, const float* up, int64_t up_ld) {
     const wlk_qtext_dims& D = t->dims;
     const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
     const int W = (H + 2 * KV) * QT_HD;
-    qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, t->emb, t->up, t->x, d);
+    qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, t->emb, up, up_ld, t->x, d);
     for (int li = 0; li < D.n_layer; ++li) {
         QTLayerW& Lw = t->L[li];
-        launch_rmsnorm<T>(t, t->x, Lw.ln1, t->xn, nullptr, R);
+        launch_rmsnorm<T>(t, t->x, Lw.ln1, t->xn, nullptr, R, D.rms_eps);
         {   GemmArgs g;
             g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wqkv; g.w_type = t->act; g.ldw = d;
             g.M = R; g.N = W; g.K = d;
@@ -676,26 +771,29 @@ void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, 
             g.M = R; g.N = d; g.K = H * QT_HD;
             g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
             tgemm(t, g); }
-        launch_rmsnorm<T>(t, t->x, Lw.ln2, t->xn, nullptr, R);
+        launch_rmsnorm<T>(t, t->x, Lw.ln2, t->xn, nullptr, R, D.rms_eps);
         {   GemmArgs g;
             g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = Lw.Wgu; g.w_type = t->act; g.ldw = d;
             g.M = R; g.N = 2 * F; g.K = d;
             g.epi.C = t->gu; g.epi.c_type = DT_F32; g.epi.ldc = 2 * F;
             tgemm(t, g); }
-        launch_swiglu<T>(t, t->gu, t->hid, R);
+        launch_swiglu<T>(t, t->gu, t->hid, R, F);
         {   GemmArgs g;
             g.A = t->hid; g.a_type = t->act; g.lda = F; g.W = Lw.Wd; g.w_type = t->act; g.ldw = F;
             g.M = R; g.N = d; g.K = F;
             g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
             tgemm(t, g); }
     }
-    launch_rmsnorm<T>(t, t->x, t->normw, t->hlog, logit_row_d, R);
+    launch_rmsnorm<T>(t, t->x, t->normw, t->hlog, logit_row_d, R, D.rms_eps);
     CUDA_CHECK(cudaGetLastError());
 }
 
+// embeds: host rows [n_embeds][d_model] (staged through pinned memory), or, when embeds_ld > 0, device rows embeds_ld
+// floats apart that the embedding gather reads in place.
 void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_off, const float* embeds,
-             int n_embeds, const int32_t* logit_rows) {
+             int n_embeds, const int32_t* logit_rows, int64_t embeds_ld = 0) {
     const wlk_qtext_dims& D = t->dims;
+    const bool dev_rows = embeds_ld > 0;
     WLK_CHECK(t->finalized, "weights not finalized");
     WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
     int n_logit = 0;
@@ -744,7 +842,7 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
         for (int k = 0; k < R; ++k) {
             const int r = r0 + k;
             int s = row_src[row_off[0] + r];
-            if (s < 0) {
+            if (s < 0 && !dev_rows) {
                 memcpy(t->up_h + (size_t)n_up * D.d_model, embeds + (size_t)(-1 - s) * D.d_model, (size_t)D.d_model * 4);
                 s = -1 - n_up++;
             }
@@ -761,8 +859,10 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
         const int32_t* log_d = reinterpret_cast<const int32_t*>(t->stg_d + o_log);
         void* const* kv_d = reinterpret_cast<void* const*>(t->stg_d + o_kv);
         const QTAttnTile* tiles_d = reinterpret_cast<const QTAttnTile*>(t->stg_d + o_tile);
-        if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles);
-        else run_round<bf16>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles);
+        const float* up = dev_rows ? embeds : t->up;
+        const int64_t up_ld = dev_rows ? embeds_ld : D.d_model;
+        if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld);
+        else run_round<bf16>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld);
     }
     // no host sync here: the pick (or logits) call that follows synchronizes once for the whole phase
     for (int i = 0; i < n; ++i) t->sess[sids[i]].len += row_off[i + 1] - row_off[i];
@@ -883,8 +983,8 @@ void op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int row
     if (out_row) for (int r = 0; r < rows; ++r) WLK_CHECK(out_row[r] >= -1, "row %d: output row %d", r, out_row[r]);
     OpUpload up{t};
     const int32_t* out_row_d = out_row ? up.put(out_row, rows) : nullptr;
-    if (t->act == DT_F32) launch_rmsnorm<float>(t, x, w, out, out_row_d, rows);
-    else launch_rmsnorm<bf16>(t, x, w, out, out_row_d, rows);
+    if (t->act == DT_F32) launch_rmsnorm<float>(t, x, w, out, out_row_d, rows, t->dims.rms_eps);
+    else launch_rmsnorm<bf16>(t, x, w, out, out_row_d, rows, t->dims.rms_eps);
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaStreamSynchronize(t->st));
 }
@@ -923,10 +1023,55 @@ void op_attention(wlk_qtext* t, const void* q, const int32_t* pos, const int32_t
 void op_swiglu(wlk_qtext* t, const float* gu, void* hid, int rows) {
     WLK_CHECK(gu && hid, "null argument");
     op_rows(rows);
-    if (t->act == DT_F32) launch_swiglu<float>(t, gu, hid, rows);
-    else launch_swiglu<bf16>(t, gu, hid, rows);
+    if (t->act == DT_F32) launch_swiglu<float>(t, gu, hid, rows, t->dims.ffn_dim);
+    else launch_swiglu<bf16>(t, gu, hid, rows, t->dims.ffn_dim);
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaStreamSynchronize(t->st));
+}
+
+// The frame adapter over device rows, in chunks of QT_ROUND_ROWS: the residual stream lives in the forward's x workspace.
+template <typename T>
+void adapt_chunk(wlk_qtext* t, const float* in, int R, int64_t in_ld, float* out, int64_t out_ld) {
+    const QTAdapter& A = t->ad;
+    const int d = t->dims.d_model, H = A.hidden;
+    qt_rows_to_act_kernel<T><<<R, 256, 0, t->st>>>(in, in_ld, (T*)A.a_in, A.in_dim);
+    {   GemmArgs g;
+        g.A = A.a_in; g.a_type = t->act; g.lda = A.in_dim; g.W = A.Wp; g.w_type = t->act; g.ldw = A.in_dim;
+        g.M = R; g.N = d; g.K = A.in_dim;
+        g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
+        tgemm(t, g); }
+    for (int b = 0; b < A.nb; ++b) {
+        launch_rmsnorm<T>(t, t->x, A.norm[b], t->xn, nullptr, R, QT_ADAPTER_EPS);
+        {   GemmArgs g;
+            g.A = t->xn; g.a_type = t->act; g.lda = d; g.W = A.Wgu[b]; g.w_type = t->act; g.ldw = d;
+            g.M = R; g.N = 2 * H; g.K = d;
+            g.epi.C = A.a_gu; g.epi.c_type = DT_F32; g.epi.ldc = 2 * H;
+            tgemm(t, g); }
+        launch_swiglu<T>(t, A.a_gu, A.a_hid, R, H);
+        {   GemmArgs g;                                 // x + scale * down(...): col_scale, then the residual
+            g.A = A.a_hid; g.a_type = t->act; g.lda = H; g.W = A.Wd[b]; g.w_type = t->act; g.ldw = H;
+            g.M = R; g.N = d; g.K = H;
+            g.epi.col_scale = A.scale; g.epi.scale_cols = d;
+            g.epi.residual = t->x; g.epi.ldr = d; g.epi.C = t->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
+            tgemm(t, g); }
+    }
+    CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)out_ld * 4, t->x, (size_t)d * 4, (size_t)d * 4, R, cudaMemcpyDeviceToDevice, t->st));
+    CUDA_CHECK(cudaGetLastError());
+}
+
+void adapt(wlk_qtext* t, const float* in, int rows, int64_t in_ld, float* out, int64_t out_ld) {
+    WLK_CHECK(t->finalized, "weights not finalized");
+    WLK_CHECK(t->has_adapter, "no adapter loaded");
+    WLK_CHECK(rows >= 0, "rows %d < 0", rows);
+    WLK_CHECK(in_ld >= t->ad.in_dim, "in_ld %lld < in_dim %d", (long long)in_ld, t->ad.in_dim);
+    WLK_CHECK(out_ld >= t->dims.d_model, "out_ld %lld < d_model %d", (long long)out_ld, t->dims.d_model);
+    WLK_CHECK(rows == 0 || (in && out), "null argument");
+    for (int r0 = 0; r0 < rows; r0 += QT_ROUND_ROWS) {
+        const int R = std::min(QT_ROUND_ROWS, rows - r0);
+        if (t->act == DT_F32) adapt_chunk<float>(t, in + (int64_t)r0 * in_ld, R, in_ld, out + (int64_t)r0 * out_ld, out_ld);
+        else adapt_chunk<bf16>(t, in + (int64_t)r0 * in_ld, R, in_ld, out + (int64_t)r0 * out_ld, out_ld);
+    }
+    CUDA_CHECK(cudaStreamSynchronize(t->st));          // out is complete when the call returns
 }
 
 }  // namespace
@@ -975,6 +1120,7 @@ int wlk_qtext_finalize_weights(wlk_qtext* t) {
     int nmiss = 0;
     for (auto& r : required(t->dims)) if (!t->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
     WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    build_adapter(t);
     if (t->stage_f32) { CUDA_CHECK(cudaFree(t->stage_f32)); t->stage_f32 = nullptr; t->stage_cap = 0; }
     t->finalized = true;
     WLK_API_END
@@ -1038,6 +1184,29 @@ int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* r
     TLOCK(t);
     WLK_CHECK(sids && row_src && row_offsets && logit_rows && (embeds_host || n_embeds == 0), "null argument");
     forward(t, sids, n, row_src, row_offsets, embeds_host, n_embeds, logit_rows);
+    WLK_API_END
+}
+int wlk_qtext_forward_device(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
+                             const float* embeds_dev, int64_t embeds_ld, int32_t n_embeds, const int32_t* logit_rows) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    WLK_CHECK(sids && row_src && row_offsets && logit_rows && (embeds_dev || n_embeds == 0), "null argument");
+    WLK_CHECK(embeds_ld >= t->dims.d_model, "embeds_ld %lld < d_model %d", (long long)embeds_ld, t->dims.d_model);
+    forward(t, sids, n, row_src, row_offsets, embeds_dev, n_embeds, logit_rows, embeds_ld);
+    WLK_API_END
+}
+int wlk_qtext_adapt(wlk_qtext* t, const float* in_dev, int32_t rows, int64_t in_ld, float* out_dev, int64_t out_ld) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    adapt(t, in_dev, rows, in_ld, out_dev, out_ld);
+    WLK_API_END
+}
+int wlk_qtext_adapter_dims(wlk_qtext* t, int32_t* in_dim, int32_t* n_blocks, int32_t* hidden) {
+    WLK_API_BEGIN
+    TLOCK(t);
+    if (in_dim) *in_dim = t->has_adapter ? t->ad.in_dim : 0;
+    if (n_blocks) *n_blocks = t->ad.nb;
+    if (hidden) *hidden = t->ad.hidden;
     WLK_API_END
 }
 int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_tokens, const int32_t* hist_off,

@@ -182,3 +182,24 @@ def synthetic_text_state_dict(dims: QwenTextDims, seed: int = 0) -> Dict[str, np
     if not dims.tied:
         sd["lm_head.weight"] = w(dims.vocab, d, fan_in=d, s=3.0)
     return sd
+
+
+def synthetic_adapter_state_dict(in_dim: int, d_model: int, hidden: int = 0, layers: int = 0, residual_scale: float = 0.1,
+                                 seed: int = 0) -> Dict[str, np.ndarray]:
+    """Seeded frame-adapter weights (QwenAudioSurgeryFrameAdapter) under the text engine's "adapter.*" names.  proj is
+    not the identity (trained checkpoints move it away from the reference's init): a near-orthogonal [d_model][in_dim]
+    matrix plus noise, so rows keep their scale."""
+    rng = np.random.default_rng(seed)
+    proj = rng.standard_normal((d_model, in_dim)) / np.sqrt(in_dim)
+    if in_dim == d_model:
+        proj = np.eye(d_model) + 0.5 * proj
+    sd = {"adapter.proj.weight": proj.astype(np.float32)}
+    for i in range(layers):
+        p = f"adapter.blocks.{i}."
+        sd[p + "norm.weight"] = (1.0 + 0.1 * rng.standard_normal(d_model)).astype(np.float32)
+        sd[p + "mlp.gate.weight"] = (rng.standard_normal((hidden, d_model)) / np.sqrt(d_model)).astype(np.float32)
+        sd[p + "mlp.up.weight"] = (rng.standard_normal((hidden, d_model)) / np.sqrt(d_model)).astype(np.float32)
+        sd[p + "mlp.down.weight"] = (rng.standard_normal((d_model, hidden)) / np.sqrt(hidden)).astype(np.float32)
+    if layers:
+        sd["adapter.residual_scale"] = np.asarray([residual_scale], np.float32)
+    return sd

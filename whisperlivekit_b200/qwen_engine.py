@@ -79,8 +79,20 @@ class QwenTowerEngine:
         L.check(self.lib.wlk_qwen_session_mutable_steps(self.h, sid, C.byref(m)))
         return m.value
 
+    def get_pending(self, sid: int) -> np.ndarray:
+        """QwenAudioCausalKVState.mel_buffer: the session's pending mel frames [frames, n_mels]."""
+        out = np.zeros((max(self.pending_frames(sid), 1), self.dims.n_mels), np.float32)
+        n = C.c_int32()
+        L.check(self.lib.wlk_qwen_session_get_pending(self.h, sid, _ptr(out), out.shape[0], C.byref(n)))
+        return out[:n.value]
+
+    def set_pending(self, sid: int, mels: np.ndarray) -> None:
+        m = np.ascontiguousarray(mels, np.float32).reshape(-1, self.dims.n_mels)
+        L.check(self.lib.wlk_qwen_session_set_pending(self.h, sid, _ptr(m if m.shape[0] else np.zeros(1, np.float32)),
+                                                      m.shape[0]))
+
     # -- forward_chunk (causal.py:713-782), batched over sessions -----------------------------
-    def forward_chunk(self, sids: Sequence[int], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
+    def _chunk_args(self, sids, mels):
         n = len(sids)
         if n != len(mels):
             raise ValueError("sids and mels differ in length")
@@ -92,11 +104,29 @@ class QwenTowerEngine:
         consume = D.block_frames if D.block_frames > 0 else D.chunk_frames
         cap = int(sum((self.pending_frames(s) + p.shape[0]) // consume * consume // D.chunk_frames for s, p in zip(sids, parts)))
         cap += D.mutable_tail_steps * n                      # a mutable tail re-emits its steps with every call
-        out = np.zeros((max(cap, 1), D.out_dim), np.float32)
-        rows = np.zeros(n + 1, np.int32)
-        ids = np.asarray(list(sids), np.int32)
-        L.check(self.lib.wlk_qwen_forward_chunk(self.h, _ptr(ids), n, _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+        return np.asarray(list(sids), np.int32), flat, offs, cap
+
+    def forward_chunk(self, sids: Sequence[int], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
+        ids, flat, offs, cap = self._chunk_args(sids, mels)
+        out = np.zeros((max(cap, 1), self.dims.out_dim), np.float32)
+        rows = np.zeros(len(ids) + 1, np.int32)
+        L.check(self.lib.wlk_qwen_forward_chunk(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
+        return [out[rows[i]: rows[i + 1]].copy() for i in range(len(ids))]
+
+    def _device_out(self, cap: int):
+        import torch
+        out = torch.empty(max(cap, 1), self.dims.out_dim, dtype=torch.float32, device=f"cuda:{self.device}")
+        torch.cuda.current_stream(out.device).synchronize()   # the engine's stream does not order itself after torch's
+        return out
+
+    def forward_chunk_device(self, sids: Sequence[int], mels: Sequence[np.ndarray]):
+        """forward_chunk with the rows left on the device: (fp32 CUDA tensor [rows, out_dim], row offsets [n + 1])."""
+        ids, flat, offs, cap = self._chunk_args(sids, mels)
+        out = self._device_out(cap)
+        rows = np.zeros(len(ids) + 1, np.int32)
+        L.check(self.lib.wlk_qwen_forward_chunk_device(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs),
+                                                       C.c_void_p(out.data_ptr()), cap, _ptr(rows)))
+        return out[:int(rows[-1])], rows
 
     # -- incremental log-mel front end (StreamingMelExtractor, features.py:32-112) on the device -------------
     def load_mel_filters(self, filters: Optional[np.ndarray] = None) -> None:
@@ -137,6 +167,15 @@ class QwenTowerEngine:
         ids = np.asarray(list(sids), np.int32)
         L.check(self.lib.wlk_qwen_flush_pending(self.h, _ptr(ids), n, _ptr(out), cap, _ptr(rows)))
         return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+
+    def flush_pending_device(self, sids: Sequence[int]):
+        """flush_pending with the rows left on the device, as forward_chunk_device returns them."""
+        cap = int(sum(self.pending_frames(s) // self.dims.chunk_frames for s in sids))
+        out = self._device_out(cap)
+        rows = np.zeros(len(sids) + 1, np.int32)
+        ids = np.asarray(list(sids), np.int32)
+        L.check(self.lib.wlk_qwen_flush_pending_device(self.h, _ptr(ids), len(ids), C.c_void_p(out.data_ptr()), cap, _ptr(rows)))
+        return out[:int(rows[-1])], rows
 
     def close(self) -> None:
         if not self._closed:

@@ -32,6 +32,28 @@ class B200QwenAudioState:
     pending_frames: int = 0
     mutable_steps: int = 0
 
+    @property
+    def mel_buffer(self):
+        """The session's pending mel frames [1, frames, n_mels] (None when there are none).  Assigning loads frames into
+        the session, which is how the reference's segment rollover carries them into a fresh encoder state."""
+        if self.engine is None:
+            return None
+        m = self.engine.get_pending(self.sid)
+        if m.shape[0] == 0:
+            return None
+        import torch
+        return torch.from_numpy(np.ascontiguousarray(m))[None]
+
+    @mel_buffer.setter
+    def mel_buffer(self, value):
+        if value is None:
+            m = np.zeros((0, 1), np.float32)
+        else:
+            if value.ndim != 3 or value.shape[0] != 1:
+                raise ValueError("mel_buffer must have shape [1, frames, n_mels]")
+            m = value[0].detach().float().cpu().numpy() if hasattr(value, "detach") else np.asarray(value[0], np.float32)
+        self.engine.set_pending(self.sid, m)      # like the reference, pending_frames follows at the next forward_chunk
+
     def close(self):
         if self.engine is not None:
             self.engine.close_session(self.sid)
@@ -93,35 +115,69 @@ class B200QwenAudioCausalKVEncoder:
         state.pending_frames = self.engine.pending_frames(state.sid)
         state.mutable_steps = self.engine.mutable_steps(state.sid) if self.mutable_tail_steps else 0
 
-    def forward_chunk(self, mels, state: Optional[B200QwenAudioState] = None):
-        import torch
-        if state is None:
-            state = self.init_state()
+    def _check_mels(self, mels):
         if mels.ndim != 3:
             raise ValueError("mels must have shape [batch, frames, n_mels]")
         if mels.shape[-1] != self.dims.n_mels:
             raise ValueError(f"expected {self.dims.n_mels} mel bins, got {mels.shape[-1]}")
         if mels.shape[0] != 1:
             raise ValueError("one stream per state: batch sessions through engine.forward_chunk")
-        n = int(mels.shape[1])
-        state.last_input_frames = n
-        state.frames_seen += n
-        before = self.engine.pending_frames(state.sid)
-        tail_frames = state.mutable_steps * self.chunk_frames if n else 0     # causal.py:753-760: tail mels run again
-        h = self.engine.forward_chunk([state.sid], [mels[0].detach().float().cpu().numpy()])[0]
-        self._sync(state)
-        state.last_recomputed_frames = tail_frames + before + n - state.pending_frames if n else 0
-        state.last_recomputed_context_frames = tail_frames
-        return torch.from_numpy(np.ascontiguousarray(h))[None].to(mels.device), state
+
+    def encode_rows(self, states, mels=None, flush: bool = False, device_rows: bool = True):
+        """forward_chunk (flush=False, mels [1, frames, n_mels] per state) or flush_pending (flush=True) for N states in
+        one engine call, with each state's fields updated as those two methods do.  Returns (rows [total, out_dim],
+        row offsets [N + 1]): a CUDA tensor when the engine runs on the device and device_rows is set, else a CPU
+        tensor."""
+        import torch
+        if flush:
+            before = [self.engine.pending_frames(s.sid) for s in states]
+            sids = [s.sid for s in states]
+            dev = device_rows and hasattr(self.engine, "flush_pending_device")
+            if dev:
+                rows, offs = self.engine.flush_pending_device(sids)
+            else:
+                hs = self.engine.flush_pending(sids)
+        else:
+            for m in mels:
+                self._check_mels(m)
+            ns = [int(m.shape[1]) for m in mels]
+            for st, n in zip(states, ns):
+                st.last_input_frames = n
+                st.frames_seen += n
+            before = [self.engine.pending_frames(s.sid) for s in states]
+            tails = [st.mutable_steps * self.chunk_frames if n else 0 for st, n in zip(states, ns)]  # causal.py:753-760
+            sids = [s.sid for s in states]
+            host = [m[0].detach().float().cpu().numpy() for m in mels]
+            dev = device_rows and hasattr(self.engine, "forward_chunk_device")
+            if dev:
+                rows, offs = self.engine.forward_chunk_device(sids, host)
+            else:
+                hs = self.engine.forward_chunk(sids, host)
+        if not dev:
+            offs = np.zeros(len(states) + 1, np.int64)
+            offs[1:] = np.cumsum([h.shape[0] for h in hs])
+            rows = torch.from_numpy(np.ascontiguousarray(np.concatenate(hs) if hs else np.zeros((0, self.dims.out_dim),
+                                                                                              np.float32)))
+        for i, st in enumerate(states):
+            self._sync(st)
+            if flush:
+                st.last_recomputed_frames = before[i] // self.chunk_frames * self.chunk_frames
+                st.last_recomputed_context_frames = 0
+            else:
+                n = ns[i]
+                st.last_recomputed_frames = tails[i] + before[i] + n - st.pending_frames if n else 0
+                st.last_recomputed_context_frames = tails[i]
+        return rows, [int(o) for o in offs]
+
+    def forward_chunk(self, mels, state: Optional[B200QwenAudioState] = None):
+        if state is None:
+            state = self.init_state()
+        rows, _ = self.encode_rows([state], [mels], device_rows=False)
+        return rows[None].to(mels.device), state
 
     def flush_pending(self, state: B200QwenAudioState):
-        import torch
-        before = self.engine.pending_frames(state.sid)
-        h = self.engine.flush_pending([state.sid])[0]
-        self._sync(state)
-        state.last_recomputed_frames = before // self.chunk_frames * self.chunk_frames
-        state.last_recomputed_context_frames = 0
-        return torch.from_numpy(np.ascontiguousarray(h))[None], state
+        rows, _ = self.encode_rows([state], flush=True, device_rows=False)
+        return rows[None], state
 
     def forward_full(self, mels):
         state = self.init_state()
@@ -226,9 +282,11 @@ class B200QwenTextDecoder:
 
     @classmethod
     def install(cls, model, engine_factory=None, precision: str = "bf16", max_ctx: int = 1024, max_sessions: int = 8,
-                **engine_kw):
+                extra_tensors=None, **engine_kw):
+        """extra_tensors: more named tensors for the engine, e.g. the frame adapter's (adapter_tensors)."""
         dims = cls.dims_of(model, max_ctx)
         sd = {k: v.detach().float().cpu().numpy() for k, v in model.text_model.state_dict().items()}
+        sd.update(extra_tensors or {})
         rotary = getattr(model.text_model, "rotary_emb", None)
         if rotary is not None and getattr(rotary, "inv_freq", None) is not None:
             # the live buffer the model rotates with (non-persistent, so not in state_dict())
@@ -270,7 +328,7 @@ class B200QwenTextDecoder:
         kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
                             max_consecutive_text_tokens)
         ctl = self.engine.make_controls(**kw)
-        fh = frame_hidden.detach().float().cpu().numpy()
+        fh = self._rows(frame_hidden)
 
         def rows(ids, b):
             if ids is None:
@@ -289,12 +347,17 @@ class B200QwenTextDecoder:
             outs = [o + [fill] * (width - len(o)) for o in outs]
         return torch.tensor(outs, dtype=torch.long, device=device).reshape(batch, width)
 
+    def _rows(self, frame_hidden):
+        """CUDA frame rows stay on the device when the engine reads device rows; otherwise they go to the host."""
+        fh = frame_hidden.detach().float()
+        return fh if fh.is_cuda and getattr(self.engine, "device_rows", False) else fh.cpu().numpy()
+
     def generate_full_hypothesis_rolling(self, frame_hidden, *, state, template_token_ids, audio_placeholder_token_id,
                                          draft_token_ids=None, max_new_tokens: int = 128, eos_token_id=None,
                                          stop_token_ids=None, suppress_token_ids=None, repetition_penalty: float = 1.0,
                                          no_repeat_ngram_size: int = 0, max_consecutive_text_tokens: int = 0):
         import torch
-        from .qwen_text_engine import RollingState, split_template
+        from .qwen_text_engine import split_template
         if frame_hidden.ndim != 3:
             raise ValueError("frame_hidden must have shape [batch, steps, hidden]")
         head, tail = split_template(template_token_ids, audio_placeholder_token_id)
@@ -307,19 +370,101 @@ class B200QwenTextDecoder:
                 frame_hidden, prefix_token_ids=expanded, audio_placeholder_token_id=audio_placeholder_token_id,
                 max_new_tokens=max_new_tokens, **{k: v for k, v in kw.items() if k != "wait_token_id"})
             return toks, {"decoder_path": "full"}
-        dec = getattr(state, "decoder", None)
-        if not isinstance(dec, B200DecoderRollingState) or dec.engine is not self.engine:
-            dec = B200DecoderRollingState(self.engine, self.engine.open_session())
-            prev = None
-        else:
-            prev = RollingState(dec.head_token_ids, dec.head_len, dec.audio_steps)
-        fh = frame_hidden[0].detach().float().cpu().numpy()
-        toks, stats, states = self.engine.generate_rolling(
-            [dec.sid], [fh], [prev], template_token_ids, audio_placeholder_token_id,
-            [None if draft_token_ids is None else [int(t) for t in draft_token_ids]], max_new_tokens=max_new_tokens,
-            bos_token_id=self.model.bos_token_id, **kw)
-        st = states[0]
-        if stats[0].get("decoder_path") != "full":
-            dec.head_token_ids, dec.head_len, dec.audio_steps = st.head_token_ids, st.head_len, st.audio_steps
-            state.decoder = dec
+        toks, stats = self.generate_rolling_batch(
+            [frame_hidden[0]], [state], [draft_token_ids], template_token_ids=template_token_ids,
+            audio_placeholder_token_id=audio_placeholder_token_id, max_new_tokens=max_new_tokens, **kw)
         return torch.tensor([toks[0]], dtype=torch.long, device=frame_hidden.device), stats[0]
+
+    def generate_rolling_batch(self, frame_rows, states, drafts, *, template_token_ids, audio_placeholder_token_id,
+                               max_new_tokens: int = 128, **controls):
+        """generate_full_hypothesis_rolling for N streams in one lockstep pass: frame_rows[i] [steps_i, d] (the
+        stream's whole frame_hidden; only the rows its decoder session has not seen are forwarded), states[i] the
+        stream's CachedAudioDecodeState (its ``decoder`` is read and set), drafts[i] a token list or None.  controls:
+        the generate method's decode controls plus wait_token_id.  Returns (tokens per stream, stats per stream)."""
+        from .qwen_text_engine import RollingState
+        decs, prevs = [], []
+        for state in states:
+            dec = getattr(state, "decoder", None)
+            if not isinstance(dec, B200DecoderRollingState) or dec.engine is not self.engine:
+                dec = B200DecoderRollingState(self.engine, self.engine.open_session())
+                prevs.append(None)
+            else:
+                prevs.append(RollingState(dec.head_token_ids, dec.head_len, dec.audio_steps))
+            decs.append(dec)
+        controls.setdefault("wait_token_id", self.model.wait_token_id)
+        toks, stats, new = self.engine.generate_rolling(
+            [d.sid for d in decs], [self._rows(f) for f in frame_rows], prevs, template_token_ids,
+            audio_placeholder_token_id, [None if d is None else [int(t) for t in d] for d in drafts],
+            max_new_tokens=max_new_tokens, bos_token_id=self.model.bos_token_id, **controls)
+        for dec, state, st, s in zip(decs, states, new, stats):
+            if s.get("decoder_path") != "full":
+                dec.head_token_ids, dec.head_len, dec.audio_steps = st.head_token_ids, st.head_len, st.audio_steps
+                state.decoder = dec
+        return toks, stats
+
+
+def adapter_tensors(adapter) -> dict:
+    """The reference frame adapter (QwenAudioSurgeryFrameAdapter, model.py:631-691) as the text engine's "adapter.*"
+    tensors.  residual_scale is a plain float on each block, the same for all of them; dropout is off in eval."""
+    sd = {"adapter.proj.weight": adapter.proj.weight.detach().float().cpu().numpy()}
+    scales = {float(b.residual_scale) for b in adapter.blocks}
+    if len(scales) > 1:
+        raise ValueError("the adapter's blocks have different residual scales")
+    for i, b in enumerate(adapter.blocks):
+        p = f"adapter.blocks.{i}."
+        sd[p + "norm.weight"] = b.norm.weight.detach().float().cpu().numpy()
+        for n in ("gate", "up", "down"):
+            sd[p + f"mlp.{n}.weight"] = getattr(b.mlp, n).weight.detach().float().cpu().numpy()
+    if scales:
+        sd["adapter.residual_scale"] = np.asarray([scales.pop()], np.float32)
+    return sd
+
+
+class B200QwenRealtimeModel:
+    """The whole realtime model (``Qwen3ASRRealtimeQwenAudioCausalModel``) on the engines, installed on one instance::
+
+        B200QwenRealtimeModel.install(model, precision="bf16")
+
+    replaces ``model.audio_encoder`` with the tower drop-in, installs the text decoder drop-in with the frame adapter
+    packed into its engine, and rebinds ``append_audio_to_cache`` / ``flush_audio_to_cache`` onto
+    ``qwen_realtime.RealtimeFrames`` (N = 1).  With CUDA engines ``state.frame_hidden`` is a device tensor and the
+    generate methods read it in place: no frame row reaches the host.  The reference streamers
+    (``SegmentedCachedFullHypothesisStreamer``) run over the installed model unchanged."""
+
+    def __init__(self, model, encoder, decoder):
+        from .qwen_realtime import RealtimeFrames
+        self.model, self.encoder, self.decoder = model, encoder, decoder
+        self.frames = RealtimeFrames(encoder, decoder.engine, decoder.dims.d_model)
+
+    @classmethod
+    def install(cls, model, precision: str = "bf16", max_ctx: int = 1024, max_sessions: int = 8, tower_factory=None,
+                text_factory=None):
+        """tower_factory(dims, state_dict) / text_factory(dims, state_dict): engines to use instead of the CUDA ones
+        (the CPU oracles in tests)."""
+        tower_kw = {} if tower_factory else dict(precision=precision, max_sessions=max_sessions)
+        encoder = B200QwenAudioCausalKVEncoder.from_reference(model.audio_encoder, engine_factory=tower_factory, **tower_kw)
+        if encoder.dims.out_dim != model.adapter.proj.weight.shape[1]:
+            raise ValueError(f"tower rows are {encoder.dims.out_dim} wide, the adapter takes "
+                             f"{model.adapter.proj.weight.shape[1]}")
+        decoder = B200QwenTextDecoder.install(model, engine_factory=text_factory, precision=precision, max_ctx=max_ctx,
+                                              max_sessions=max_sessions, extra_tensors=adapter_tensors(model.adapter))
+        rt = cls(model, encoder, decoder)
+        if "audio_encoder" in getattr(model, "_modules", {}):
+            del model._modules["audio_encoder"]        # an nn.Module takes only modules as child attributes
+        model.audio_encoder = encoder
+        model.append_audio_to_cache = rt.append_audio_to_cache
+        model.flush_audio_to_cache = rt.flush_audio_to_cache
+        model.b200_realtime = rt
+        return rt
+
+    def append_audio_to_cache(self, mels, state=None):
+        if state is None:
+            state = self.model.init_cached_audio_decode_state()
+        (cached, delta), = self.frames.append([state], [mels])
+        return cached, delta, state
+
+    def flush_audio_to_cache(self, state=None):
+        if state is None:
+            state = self.model.init_cached_audio_decode_state()
+        (cached, delta), = self.frames.append([state], flush=True)
+        return cached, delta, state

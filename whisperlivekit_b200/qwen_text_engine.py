@@ -28,6 +28,13 @@ def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _frame_rows(x):
+    """Frame rows as an engine takes them: a CUDA tensor stays where it is (fp32), anything else becomes fp32 numpy."""
+    if getattr(x, "is_cuda", False):
+        return x.float()
+    return np.ascontiguousarray(x, np.float32)
+
+
 @dataclass
 class RollingState:
     """The part of the reference's DecoderRollingState (model.py:53-68) the engine needs: the session holds the KV of
@@ -131,7 +138,7 @@ class TextDecodeDriver:
             out_stats[i] = {"decoder_path": "full"}
 
         for i in range(n):
-            fh = np.ascontiguousarray(frame_hidden[i], np.float32)
+            fh = _frame_rows(frame_hidden[i])
             audio_steps = int(fh.shape[0])
             if max_new_tokens <= 0 or audio_steps == 0:
                 fallback(i, fh)
@@ -243,7 +250,7 @@ class TextDecodeDriver:
         if max_new_tokens == 0:
             return []
         ctl = controls if controls is not None else self.make_controls(**control_kwargs)
-        fh = np.ascontiguousarray(frame_hidden, np.float32).reshape(-1, self.dims.d_model)
+        fh = _frame_rows(frame_hidden).reshape(-1, self.dims.d_model)
         if prefix_token_ids is not None:
             if audio_placeholder_token_id is None:
                 raise ValueError("audio_placeholder_token_id is required when prefix_token_ids is set")
@@ -279,7 +286,10 @@ class TextDecodeDriver:
 
 
 class QwenTextEngine(TextDecodeDriver):
-    """The text decoder on the H100.  No CPU fallback: construction fails without the CUDA library or a device."""
+    """The text decoder on the H100.  No CPU fallback: construction fails without the CUDA library or a device.
+    Embedding rows may be host arrays or fp32 CUDA tensors; the latter are read in place by the forward."""
+
+    device_rows = True
 
     def __init__(self, dims: QwenTextDims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8):
@@ -296,6 +306,7 @@ class QwenTextEngine(TextDecodeDriver):
         self.h = h
         self._closed = False
         self._n_logit = 0
+        self._dev_rows = None                    # device rows the last forward reads: alive until its pick synchronizes
         # HF's fp32 RoPE frequencies; a state dict that carries the model's own buffer overrides them
         self.load_tensor("rotary_emb.inv_freq", rope_inv_freq(dims.rope_theta, dims.head_dim))
         if state_dict is not None:
@@ -339,13 +350,16 @@ class QwenTextEngine(TextDecodeDriver):
         L.check(self.lib.wlk_qtext_crop(self.h, int(sid), int(length)))
 
     def forward(self, sids: Sequence[int], blocks, logit_rows: Sequence[int]) -> None:
-        """blocks[i] = (row_src int32 [r], embeds [k][d] or None): row_src >= 0 is a token id, -1 - j is embeds row j."""
+        """blocks[i] = (row_src int32 [r], embeds [k][d] or None): row_src >= 0 is a token id, -1 - j is embeds row j.
+        Embeddings that are CUDA tensors go through wlk_qtext_forward_device without leaving the GPU."""
+        if any(getattr(e, "is_cuda", False) and len(e) for _, e in blocks):
+            return self._forward_device(sids, blocks, logit_rows)
         srcs, embs, offs, base = [], [], [0], 0
         for src, emb in blocks:
             src = np.asarray(src, np.int32).copy()
             if emb is not None and len(emb):
                 src[src < 0] -= base
-                e = np.ascontiguousarray(emb, np.float32).reshape(-1, self.dims.d_model)
+                e = _frame_rows(emb).reshape(-1, self.dims.d_model)
                 embs.append(e)
                 base += e.shape[0]
             srcs.append(src)
@@ -357,6 +371,55 @@ class QwenTextEngine(TextDecodeDriver):
         lr = np.asarray(list(logit_rows), np.int32)
         L.check(self.lib.wlk_qtext_forward(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off), _ptr(emb), base, _ptr(lr)))
         self._n_logit = int(lr.sum())
+
+    def _forward_device(self, sids, blocks, logit_rows) -> None:
+        import torch
+        d = self.dims.d_model
+        srcs, parts, offs, base = [], [], [0], 0
+        for src, emb in blocks:
+            src = np.asarray(src, np.int32).copy()
+            if emb is not None and len(emb):
+                if not getattr(emb, "is_cuda", False):
+                    raise ValueError("a forward takes its embedding rows either all from the host or all from the device")
+                e = emb.reshape(-1, d)
+                src[src < 0] -= base
+                parts.append(e)
+                base += e.shape[0]
+            srcs.append(src)
+            offs.append(offs[-1] + src.shape[0])
+        rows = parts[0] if len(parts) == 1 else torch.cat(parts)       # one session: its rows in place
+        if rows.dtype != torch.float32 or rows.stride(-1) != 1 or (rows.shape[0] > 1 and rows.stride(0) < d):
+            rows = rows.float().contiguous()
+        ld = rows.stride(0) if rows.shape[0] > 1 else d
+        torch.cuda.current_stream(rows.device).synchronize()         # the rows are complete before the engine reads them
+        self._dev_rows = rows
+        flat = np.concatenate(srcs).astype(np.int32)
+        ids = np.asarray(list(sids), np.int32)
+        off = np.asarray(offs, np.int32)
+        lr = np.asarray(list(logit_rows), np.int32)
+        L.check(self.lib.wlk_qtext_forward_device(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off),
+                                                  C.c_void_p(rows.data_ptr()), int(ld), base, _ptr(lr)))
+        self._n_logit = int(lr.sum())
+
+    def adapter_dims(self) -> Tuple[int, int, int]:
+        """(in_dim, blocks, hidden width) of the loaded frame adapter; in_dim 0 without one."""
+        a, b, c = C.c_int32(), C.c_int32(), C.c_int32()
+        L.check(self.lib.wlk_qtext_adapter_dims(self.h, C.byref(a), C.byref(b), C.byref(c)))
+        return a.value, b.value, c.value
+
+    def adapt(self, x, out=None):
+        """The frame adapter (wlk_qtext_adapt) over fp32 CUDA rows x [rows, in_dim] (any row pitch): a new fp32 CUDA tensor
+        [rows, d_model], or `out` (a [rows, >= d_model] row-major view) filled in place."""
+        import torch
+        if x.dim() != 2 or x.dtype != torch.float32 or not x.is_cuda or (x.shape[0] and x.stride(1) != 1):
+            raise ValueError("adapt takes fp32 CUDA rows [rows, in_dim] with unit column stride")
+        rows = int(x.shape[0])
+        if out is None:
+            out = torch.empty(rows, self.dims.d_model, dtype=torch.float32, device=x.device)
+        torch.cuda.current_stream(x.device).synchronize()
+        L.check(self.lib.wlk_qtext_adapt(self.h, C.c_void_p(x.data_ptr()), rows, int(x.stride(0)),
+                                         C.c_void_p(out.data_ptr()), int(out.stride(0))))
+        return out
 
     def pick(self, hist: np.ndarray, hist_off: np.ndarray, hist_len: np.ndarray, ctl: Controls,
              return_values: bool = False):
