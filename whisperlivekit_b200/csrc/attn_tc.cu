@@ -130,7 +130,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ C
             if (X3) ptx::tma_load_2d(sbase + SM_Q + TILE_BYTES, &tm_lo, bar_q, q_col, q_row);
             for (int j = 0; j < NT; ++j) {
                 const uint32_t s = j & 1, ph = (j >> 1) & 1;
-                ptx::mbar_wait(bar_kv_empty + 8 * s, ph ^ 1);
+                ptx::mbar_wait_mma(bar_kv_empty + 8 * s, ph ^ 1);
                 ptx::mbar_arrive_expect_tx(bar_kv_full + 8 * s, 2 * NP * TILE_BYTES);
                 ptx::tma_load_2d(sbase + SM_K + s * NP * TILE_BYTES, tm_kv, bar_kv_full + 8 * s, k_col, k_row + j * BKV);
                 ptx::tma_load_2d(sbase + SM_V + s * NP * TILE_BYTES, tm_kv, bar_kv_full + 8 * s, v_col, v_row + j * BKV);
@@ -152,11 +152,11 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ C
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // running row maximum (log2 domain) and this thread's share of the row sum
-    ptx::mbar_wait(bar_q, 0);
+    ptx::mbar_wait_mma(bar_q, 0);
 #pragma unroll 1
     for (int j = 0; j < NT; ++j) {
         const uint32_t s = j & 1;
-        ptx::mbar_wait(bar_kv_full + 8 * s, (j >> 1) & 1);
+        ptx::mbar_wait_mma(bar_kv_full + 8 * s, (j >> 1) & 1);
         float sc[64];
         {
             const uint64_t dq = ptx::wgmma_desc_sw128(sbase + SM_Q + wg * WG_Q_OFF);
@@ -252,6 +252,8 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ C
         float ls = l[i];
         ls += __shfl_xor_sync(0xffffffffu, ls, 1);
         ls += __shfl_xor_sync(0xffffffffu, ls, 2);
+        // (the IEEE division's slow path is a subroutine call; it is reachable only here, after the last
+        // wgmma_wait<0>, where no wgmma group is in flight, so ptxas keeps the MMAs asynchronous)
         const float inv = 1.0f / ls;
         const int r = r0 + 8 * i;
         if (r >= n_q) continue;

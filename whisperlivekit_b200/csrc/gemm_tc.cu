@@ -169,7 +169,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     if (early > 0) {
                         --early;                       // slot is fresh and its W panel is already in flight
                     } else {
-                        ptx::mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+                        ptx::mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
                         ptx::mbar_arrive_expect_tx(bar_full + 8 * stage, STAGE_TX);
                         ptx::tma_load_2d(sB + stage * L::B_BYTES, &tmW, bar_full + 8 * stage, kb * BK, n_blk * BN);
                         if (X3) ptx::tma_load_2d(sBlo + stage * L::B_BYTES, &tmWlo, bar_full + 8 * stage, kb * BK, n_blk * BN);
@@ -200,7 +200,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             float acc[BN / 2];
             int prev = -1;                            // slot whose MMAs are still in flight
             for (int kb = kb_begin; kb < kb_end; ++kb) {
-                ptx::mbar_wait(bar_full + 8 * stage, phase);
+                ptx::mbar_wait_mma(bar_full + 8 * stage, phase);
                 const uint64_t da = ptx::wgmma_desc_sw128(sA + stage * L::A_BYTES + wg * WG_A_OFF);
                 const uint64_t db = ptx::wgmma_desc_sw128(sB + stage * L::B_BYTES);
                 const uint64_t dal = ptx::wgmma_desc_sw128(sAlo + stage * L::A_BYTES + wg * WG_A_OFF);

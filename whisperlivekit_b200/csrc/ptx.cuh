@@ -63,6 +63,16 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         }
     }
 }
+// The same bounded wait without the message, for every wait in a kernel that issues wgmma: printf is a function call,
+// and a call the MMA warps can reach while a wgmma group is in flight makes ptxas serialize every wgmma of the kernel
+// (C7510: each MMA waits for the previous one to retire).  ptxas does not tell the producer warp's waits from the MMA
+// warps', so the producer uses this form too.
+__device__ __forceinline__ void mbar_wait_mma(uint32_t bar, uint32_t parity) {
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, parity)) {
+        if (++spins > (1u << 26)) __trap();
+    }
+}
 
 // ---- programmatic dependent launch (see launch_pdl in common.cuh) ----------------------
 // wait: blocks until every grid this one depends on has completed and its writes are visible (no-op when the
