@@ -37,6 +37,48 @@ def test_engine_fails_loudly_without_gpu():
         WhisperEngine(DIMS["micro"], None, [(0, 0)])
 
 
+BAD_DEVICE = 99
+
+
+def _qwen():
+    from whisperlivekit_b200.qwen_dims import QWEN_DIMS
+    from whisperlivekit_b200.qwen_engine import QwenTowerEngine
+    QwenTowerEngine(QWEN_DIMS["qnano"], device=BAD_DEVICE)
+
+
+def _qtext():
+    from whisperlivekit_b200.qwen_dims import QWEN_TEXT_DIMS
+    from whisperlivekit_b200.qwen_text_engine import QwenTextEngine
+    QwenTextEngine(QWEN_TEXT_DIMS["tnano"], device=BAD_DEVICE)
+
+
+def _sortformer():
+    from whisperlivekit_b200.sortformer_dims import SORTFORMER_DIMS
+    from whisperlivekit_b200.sortformer_engine import SortformerEngine
+    SortformerEngine(SORTFORMER_DIMS["micro"], device=BAD_DEVICE)
+
+
+def _vad():
+    from whisperlivekit_b200.vad import VadEngine
+    VadEngine({}, device=BAD_DEVICE)
+
+
+def _diar():
+    from whisperlivekit_b200.diarization import diar_segments
+    diar_segments([0], [0], [0], n_spk=1, max_speakers=1, device=BAD_DEVICE)
+
+
+@pytest.mark.parametrize("entry", [_qwen, _qtext, _sortformer, _vad, _diar], ids=["qwen", "qtext", "sortformer", "vad", "diar"])
+def test_entry_point_rejects_unusable_device(entry):
+    """Every C-ABI unit opens its device through the same checks and reports the failure through the same guard:
+    without a GPU there is no CPU fallback, and with one a device index past the last is refused."""
+    import torch
+    from whisperlivekit_b200 import _lib
+    want = f"device {BAD_DEVICE} out of range" if torch.cuda.is_available() else "no CPU fallback"
+    with pytest.raises(_lib.WlkError, match=want):
+        entry()
+
+
 def test_product_does_not_import_oracle():
     pkg = os.path.join(ROOT, "whisperlivekit_b200")
     for fn in os.listdir(pkg):

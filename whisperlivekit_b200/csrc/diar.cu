@@ -8,9 +8,9 @@
 
 #include "../../include/wlk_b200.h"
 #include "common.cuh"
+#include "host.cuh"
 
 namespace wlk {
-void set_last_error(const std::string& msg);
 namespace {
 
 constexpr int DIAR_MAX_FRAMES = 4096;      // frames of one chunk a stream may hand in (the reference: ~12 per 1 s step)
@@ -78,48 +78,37 @@ using namespace wlk;
 extern "C" int wlk_diar_segments(int device, const float* const* preds_dev, const int32_t* n_frames_total,
                                  const int32_t* len_prediction, int n_streams, int n_spk, int max_speakers,
                                  int32_t* seg_out_host, int32_t* seg_count_host, int max_seg) {
-    try {
-        WLK_CHECK(preds_dev && n_frames_total && len_prediction && seg_out_host && seg_count_host, "null argument");
-        WLK_CHECK(n_streams >= 1 && n_streams <= 65535 && max_seg >= 1, "bad stream / segment count");
-        WLK_CHECK(n_spk >= 1 && max_speakers >= 1, "bad speaker count");
-        // sortformer_backend.py:316-319
-        WLK_CHECK(n_spk >= max_speakers, "Sortformer returned fewer speaker channels (%d) than configured (%d).", n_spk, max_speakers);
-        int ndev = 0;
-        cudaError_t ce = cudaGetDeviceCount(&ndev);
-        WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): no CPU fallback", cudaGetErrorString(ce));
-        WLK_CHECK(device >= 0 && device < ndev, "device %d out of range", device);
-        CUDA_CHECK(cudaSetDevice(device));
-        std::vector<DiarJob> jobs(n_streams);
-        for (int i = 0; i < n_streams; ++i) {
-            WLK_CHECK(n_frames_total[i] >= 0 && len_prediction[i] >= 0, "negative frame count for stream %d", i);
-            const int n = std::min(n_frames_total[i], len_prediction[i]);
-            WLK_CHECK(n <= DIAR_MAX_FRAMES, "stream %d: %d frames in one chunk exceed %d", i, n, DIAR_MAX_FRAMES);
-            WLK_CHECK(n == 0 || preds_dev[i] != nullptr, "stream %d: null predictions", i);
-            jobs[i] = DiarJob{preds_dev[i], n_frames_total[i], len_prediction[i], n_spk, max_speakers};
-        }
-        DiarJob* jobs_dev = nullptr; int32_t *seg_dev = nullptr, *cnt_dev = nullptr;
-        cudaStream_t st;
-        CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-        CUDA_CHECK(cudaMallocAsync(&jobs_dev, sizeof(DiarJob) * n_streams, st));
-        CUDA_CHECK(cudaMallocAsync(&seg_dev, sizeof(int32_t) * 3 * (size_t)max_seg * n_streams, st));
-        CUDA_CHECK(cudaMallocAsync(&cnt_dev, sizeof(int32_t) * n_streams, st));
-        CUDA_CHECK(cudaMemcpyAsync(jobs_dev, jobs.data(), sizeof(DiarJob) * n_streams, cudaMemcpyHostToDevice, st));
-        diar_segments_kernel<<<n_streams, 256, 0, st>>>(jobs_dev, seg_dev, cnt_dev, max_seg);
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(seg_count_host, cnt_dev, sizeof(int32_t) * n_streams, cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaMemcpyAsync(seg_out_host, seg_dev, sizeof(int32_t) * 3 * (size_t)max_seg * n_streams, cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        cudaFreeAsync(jobs_dev, st); cudaFreeAsync(seg_dev, st); cudaFreeAsync(cnt_dev, st);
-        cudaStreamSynchronize(st);
-        cudaStreamDestroy(st);
-        for (int i = 0; i < n_streams; ++i)
-            WLK_CHECK(seg_count_host[i] <= max_seg, "stream %d produced %d segments, capacity %d", i, seg_count_host[i], max_seg);
-        return 0;
-    } catch (const wlk::Error& err) {
-        wlk::set_last_error(err.msg);
-        return 1;
-    } catch (const std::exception& ex) {
-        wlk::set_last_error(std::string("exception: ") + ex.what());
-        return 2;
+    WLK_API_BEGIN
+    WLK_CHECK(preds_dev && n_frames_total && len_prediction && seg_out_host && seg_count_host, "null argument");
+    WLK_CHECK(n_streams >= 1 && n_streams <= 65535 && max_seg >= 1, "bad stream / segment count");
+    WLK_CHECK(n_spk >= 1 && max_speakers >= 1, "bad speaker count");
+    // sortformer_backend.py:316-319
+    WLK_CHECK(n_spk >= max_speakers, "Sortformer returned fewer speaker channels (%d) than configured (%d).", n_spk, max_speakers);
+    use_device(device);
+    std::vector<DiarJob> jobs(n_streams);
+    for (int i = 0; i < n_streams; ++i) {
+        WLK_CHECK(n_frames_total[i] >= 0 && len_prediction[i] >= 0, "negative frame count for stream %d", i);
+        const int n = std::min(n_frames_total[i], len_prediction[i]);
+        WLK_CHECK(n <= DIAR_MAX_FRAMES, "stream %d: %d frames in one chunk exceed %d", i, n, DIAR_MAX_FRAMES);
+        WLK_CHECK(n == 0 || preds_dev[i] != nullptr, "stream %d: null predictions", i);
+        jobs[i] = DiarJob{preds_dev[i], n_frames_total[i], len_prediction[i], n_spk, max_speakers};
     }
+    DiarJob* jobs_dev = nullptr; int32_t *seg_dev = nullptr, *cnt_dev = nullptr;
+    cudaStream_t st;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    CUDA_CHECK(cudaMallocAsync(&jobs_dev, sizeof(DiarJob) * n_streams, st));
+    CUDA_CHECK(cudaMallocAsync(&seg_dev, sizeof(int32_t) * 3 * (size_t)max_seg * n_streams, st));
+    CUDA_CHECK(cudaMallocAsync(&cnt_dev, sizeof(int32_t) * n_streams, st));
+    CUDA_CHECK(cudaMemcpyAsync(jobs_dev, jobs.data(), sizeof(DiarJob) * n_streams, cudaMemcpyHostToDevice, st));
+    diar_segments_kernel<<<n_streams, 256, 0, st>>>(jobs_dev, seg_dev, cnt_dev, max_seg);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(seg_count_host, cnt_dev, sizeof(int32_t) * n_streams, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(seg_out_host, seg_dev, sizeof(int32_t) * 3 * (size_t)max_seg * n_streams, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    cudaFreeAsync(jobs_dev, st); cudaFreeAsync(seg_dev, st); cudaFreeAsync(cnt_dev, st);
+    cudaStreamSynchronize(st);
+    cudaStreamDestroy(st);
+    for (int i = 0; i < n_streams; ++i)
+        WLK_CHECK(seg_count_host[i] <= max_seg, "stream %d produced %d segments, capacity %d", i, seg_count_host[i], max_seg);
+    WLK_API_END
 }

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/wlk_b200.h"
+#include "host.cuh"
 #include "kernels.cuh"
 
 namespace wlk {
@@ -102,6 +103,7 @@ struct wlk_engine {
     int num_sms = 132;
     cudaStream_t st = nullptr;
     std::mutex mu;
+    DeviceAllocs allocs;              // buffers kept from create (or first use) until destroy
     // token-step CUDA graphs: the ~390 launches of one decoder step depend only on the batch size (every per-session
     // quantity travels in the staged job arrays), so they are captured once per batch size and replayed
     bool graphs_on = true;
@@ -288,12 +290,6 @@ void put_conv(wlk_engine* e, void* dst, const float* host, int c_out, int c_in) 
         pack_conv_weight(s, dst, e->wt, c_out, c_in, e->st);
         CUDA_CHECK(cudaStreamSynchronize(e->st));
     }
-}
-
-int64_t numel(const int64_t* shape, int ndim) {
-    int64_t n = 1;
-    for (int i = 0; i < ndim; ++i) n *= shape[i];
-    return n;
 }
 
 void load_tensor(wlk_engine* e, const std::string& name, const float* host, const int64_t* shape, int ndim) {
@@ -671,12 +667,12 @@ void ensure_incremental(wlk_engine* e, Session& s, int sid) {
     const wlk_dims& D = e->dims;
     if (!e->enc_maps_dev) {
         size_t* acct = &e->bytes_workspace;
-        e->enc_maps_dev = reinterpret_cast<uint8_t*>(dmalloc_bytes((size_t)e->cfg.max_sessions * 128, acct));
+        e->enc_maps_dev = reinterpret_cast<uint8_t*>(e->allocs.take((size_t)e->cfg.max_sessions * 128, acct));
         std::vector<int32_t> none((size_t)D.n_audio_layer * D.n_audio_head, -1);
-        e->enc_norank_dev = dmalloc<int32_t>(e, none.size(), acct);
+        e->enc_norank_dev = (int32_t*)e->allocs.take(none.size() * sizeof(int32_t), acct);
         CUDA_CHECK(cudaMemcpy(e->enc_norank_dev, none.data(), none.size() * 4, cudaMemcpyHostToDevice));
-        e->inc_row_slot = dmalloc<int32_t>(e, (size_t)e->cfg.max_batch * N_CTX, acct);
-        e->inc_row_pos = dmalloc<int32_t>(e, (size_t)e->cfg.max_batch * N_CTX, acct);
+        e->inc_row_slot = (int32_t*)e->allocs.take((size_t)e->cfg.max_batch * N_CTX * sizeof(int32_t), acct);
+        e->inc_row_pos = (int32_t*)e->allocs.take((size_t)e->cfg.max_batch * N_CTX * sizeof(int32_t), acct);
         const char* v = getenv("WLK_INC_REFRESH");
         e->inc_refresh = v ? atoi(v) : 0;
     }
@@ -1093,19 +1089,11 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     WLK_CHECK(dims->n_text_state % 64 == 0 && dims->n_text_state / dims->n_text_head == 64, "text heads must be 64 wide");
     WLK_CHECK(dims->n_mels % 8 == 0 && dims->n_mels <= 128, "n_mels must be 80 or 128");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    int ndev = 0;
-    cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the engine has no CPU fallback",
-              cudaGetErrorString(ce));
-    WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
-    CUDA_CHECK(cudaSetDevice(cfg->device));
-    cudaDeviceProp prop;
-    CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    const int num_sms = open_sm90_device(cfg->device);
 
     auto* e = new wlk_engine();
     e->dims = *dims; e->cfg = *cfg;
-    e->num_sms = prop.multiProcessorCount;
+    e->num_sms = num_sms;
     WLK_CHECK(cfg->precision == WLK_PREC_FP32 || cfg->precision == WLK_PREC_BF16 || cfg->precision == WLK_PREC_BF16X3,
               "unknown precision %d", cfg->precision);
     e->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
@@ -1132,9 +1120,8 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     layout_weights(e);
     const size_t wbytes = e->arena.used + ALIGN;
     e->arena = Arena{};
-    e->arena.base = reinterpret_cast<uint8_t*>(dmalloc_bytes(wbytes, &e->bytes_weights));
+    e->arena.base = reinterpret_cast<uint8_t*>(e->allocs.take(wbytes, &e->bytes_weights));
     e->arena.cap = wbytes;
-    CUDA_CHECK(cudaMemsetAsync(e->arena.base, 0, wbytes, e->st));
     layout_weights(e);
     {   // DFT twiddles exp(-2 pi i t / 400) in double -> float
         std::vector<float2> tw(N_FFT);
@@ -1150,19 +1137,18 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     const size_t es = e->es();
     const int B = cfg->max_batch, d = D.n_audio_state, dt = D.n_text_state;
     size_t* acct = &e->bytes_workspace;
-    e->mel_t = dmalloc_bytes((size_t)B * MEL_ROWS * D.n_mels * es, acct);
-    e->h1 = dmalloc_bytes(((size_t)B * MEL_ROWS + 2) * d * es, acct);
-    e->x = dmalloc<float>(e, (size_t)B * N_CTX * d, acct);
-    e->xn = dmalloc_bytes((size_t)B * N_CTX * d * es, acct);
-    e->qkv = dmalloc_bytes((size_t)B * N_CTX * 3 * d * es, acct);
-    e->att = dmalloc_bytes((size_t)B * N_CTX * d * es, acct);
-    e->hid = dmalloc_bytes((size_t)B * N_CTX * 4 * d * es, acct);
-    e->audio_scratch = dmalloc<float>(e, AUDIO_CAP, acct);
-    e->mel_scratch = dmalloc<float>(e, (size_t)MEL_STORE_FRAMES * D.n_mels, acct);
+    e->mel_t = e->allocs.take((size_t)B * MEL_ROWS * D.n_mels * es, acct);
+    e->h1 = e->allocs.take(((size_t)B * MEL_ROWS + 2) * d * es, acct);
+    e->x = (float*)e->allocs.take((size_t)B * N_CTX * d * sizeof(float), acct);
+    e->xn = e->allocs.take((size_t)B * N_CTX * d * es, acct);
+    e->qkv = e->allocs.take((size_t)B * N_CTX * 3 * d * es, acct);
+    e->att = e->allocs.take((size_t)B * N_CTX * d * es, acct);
+    e->hid = e->allocs.take((size_t)B * N_CTX * 4 * d * es, acct);
+    e->audio_scratch = (float*)e->allocs.take(AUDIO_CAP * sizeof(float), acct);
+    e->mel_scratch = (float*)e->allocs.take((size_t)MEL_STORE_FRAMES * D.n_mels * sizeof(float), acct);
     if (e->gemm_backend == WLK_BACKEND_TCGEN05) {
-        e->sk_scratch = dmalloc<float>(e, SK_SCRATCH_FLOATS, acct);
-        e->sk_counters = dmalloc<int>(e, SK_MAX_TILES, acct);
-        CUDA_CHECK(cudaMemset(e->sk_counters, 0, SK_MAX_TILES * 4));
+        e->sk_scratch = (float*)e->allocs.take(SK_SCRATCH_FLOATS * sizeof(float), acct);
+        e->sk_counters = (int*)e->allocs.take(SK_MAX_TILES * sizeof(int), acct);
     }
     {
         std::vector<int64_t> rows(2 * B);
@@ -1172,36 +1158,36 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
             rows[2 * b + 1] = (int64_t)b * MEL_ROWS + MEL_ROWS - 1;
             xp[b] = e->x + (size_t)b * N_CTX * d;
         }
-        e->pad_rows_dev = dmalloc<int64_t>(e, 2 * B, acct);
-        e->xptrs_dev = dmalloc<void*>(e, B, acct);
+        e->pad_rows_dev = (int64_t*)e->allocs.take(2 * B * sizeof(int64_t), acct);
+        e->xptrs_dev = (void**)e->allocs.take(B * sizeof(void*), acct);
         CUDA_CHECK(cudaMemcpy(e->pad_rows_dev, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice));
         CUDA_CHECK(cudaMemcpy(e->xptrs_dev, xp.data(), xp.size() * sizeof(void*), cudaMemcpyHostToDevice));
     }
     e->dec_rows_max = B * D.n_text_ctx;
     const size_t R = e->dec_rows_max;
-    e->dx = dmalloc<float>(e, R * dt, acct);
-    e->dxn = dmalloc_bytes(R * dt * es, acct);
-    e->dq = dmalloc_bytes(R * dt * es, acct);
-    e->datt = dmalloc_bytes(R * dt * es, acct);
-    e->dhid = dmalloc_bytes(R * 4 * dt * es, acct);
-    e->dsel = dmalloc_bytes((size_t)2 * B * dt * es, acct);
+    e->dx = (float*)e->allocs.take(R * dt * sizeof(float), acct);
+    e->dxn = e->allocs.take(R * dt * es, acct);
+    e->dq = e->allocs.take(R * dt * es, acct);
+    e->datt = e->allocs.take(R * dt * es, acct);
+    e->dhid = e->allocs.take(R * 4 * dt * es, acct);
+    e->dsel = e->allocs.take((size_t)2 * B * dt * es, acct);
     if (e->wt == DT_BF16X2) {
         size_t m = (size_t)B * N_CTX * 4 * d;                                  // fc2's operand (the MLP hidden)
         m = std::max(m, R * 4 * dt);                                           // decoder MLP hidden
         m = std::max(m, ((size_t)B * MEL_ROWS + 2) * (size_t)std::max(d, D.n_mels) + 3 * (size_t)d);   // conv views
         e->a_split_elems = (m + 7) / 8 * 8;
-        e->a_split = dmalloc_bytes(e->a_split_elems * 2 * 2, acct);
+        e->a_split = e->allocs.take(e->a_split_elems * 2 * 2, acct);
     }
     e->stg_bytes = (size_t)B * 2048 + R * 16 + 65536 + 1024 * 8 * 4;
     CUDA_CHECK(cudaMallocHost(&e->stg_host, e->stg_bytes));
-    e->stg_dev = reinterpret_cast<uint8_t*>(dmalloc_bytes(e->stg_bytes, acct));
-    e->res_dev = dmalloc<StepResult>(e, B, acct);
+    e->stg_dev = reinterpret_cast<uint8_t*>(e->allocs.take(e->stg_bytes, acct));
+    e->res_dev = (StepResult*)e->allocs.take(B * sizeof(StepResult), acct);
     CUDA_CHECK(cudaMallocHost(&e->res_host, sizeof(StepResult) * B));
     e->sess.resize(cfg->max_sessions);
-    e->kv_maps_dev = reinterpret_cast<uint8_t*>(dmalloc_bytes((size_t)cfg->max_sessions * 128, acct));
-    e->self_maps_dev = reinterpret_cast<uint8_t*>(dmalloc_bytes((size_t)cfg->max_sessions * 128, acct));
+    e->kv_maps_dev = reinterpret_cast<uint8_t*>(e->allocs.take((size_t)cfg->max_sessions * 128, acct));
+    e->self_maps_dev = reinterpret_cast<uint8_t*>(e->allocs.take((size_t)cfg->max_sessions * 128, acct));
     e->align_rank_host.assign((size_t)D.n_text_layer * D.n_text_head, -1);
-    e->align_rank_dev = dmalloc<int32_t>(e, e->align_rank_host.size(), acct);
+    e->align_rank_dev = (int32_t*)e->allocs.take(e->align_rank_host.size() * sizeof(int32_t), acct);
     CUDA_CHECK(cudaMemcpy(e->align_rank_dev, e->align_rank_host.data(), e->align_rank_host.size() * 4, cudaMemcpyHostToDevice));
     *out = e;
 }
@@ -1210,10 +1196,8 @@ void destroy_engine(wlk_engine* e) {
     cudaStreamSynchronize(e->st);
     for (auto& s : e->sess) if (s.open && s.parent >= 0) free_session(e, s);     // forks before their parents
     for (auto& s : e->sess) if (s.open) free_session(e, s);
-    void* ptrs[] = {e->arena.base, e->stage_f32, e->mel_t, e->h1, e->x, e->xn, e->qkv, e->att, e->hid, e->audio_scratch, e->mel_scratch, e->beam_scratch, e->sk_scratch, e->sk_counters, e->a_split,
-                    e->pad_rows_dev, e->xptrs_dev, e->dx, e->dxn, e->dq, e->datt, e->dhid, e->dsel, e->stg_dev,
-                    e->res_dev, e->align_rank_dev, e->kv_maps_dev, e->self_maps_dev, e->all_logits_dev};
-    for (void* p : ptrs) if (p) cudaFree(p);
+    for (void* p : {(void*)e->stage_f32, e->beam_scratch, (void*)e->all_logits_dev}) if (p) cudaFree(p);
+    e->allocs.free_all();
     if (e->stg_host) cudaFreeHost(e->stg_host);
     if (e->res_host) cudaFreeHost(e->res_host);
     if (e->tap_host) cudaFreeHost(e->tap_host);
@@ -1241,22 +1225,6 @@ float* tap_buffer(wlk_engine* e, size_t n) {
 // =========================================================================================
 // C ABI
 // =========================================================================================
-#define WLK_API_BEGIN try {
-#define WLK_API_END                                              \
-    return 0;                                                    \
-    } catch (const wlk::Error& err) {                            \
-        wlk::set_last_error(err.msg);                            \
-        return 1;                                                \
-    } catch (const std::exception& ex) {                         \
-        wlk::set_last_error(std::string("exception: ") + ex.what()); \
-        return 2;                                                \
-    } catch (...) {                                              \
-        wlk::set_last_error("unknown exception");                \
-        return 3;                                                \
-    }
-#define LOCK(e) WLK_CHECK((e) != nullptr, "null engine"); std::lock_guard<std::mutex> _lk((e)->mu); \
-                CUDA_CHECK(cudaSetDevice((e)->cfg.device))
-
 extern "C" {
 
 const char* wlk_last_error(void) { return wlk::g_last_error.c_str(); }
@@ -1276,26 +1244,22 @@ int wlk_engine_destroy(wlk_engine* e) {
 }
 int wlk_engine_load_tensor(wlk_engine* e, const char* name, const float* host, const int64_t* shape, int ndim) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
     load_tensor(e, name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_engine_finalize_weights(wlk_engine* e) {
     WLK_API_BEGIN
-    LOCK(e);
-    std::string missing;
-    int nmiss = 0;
-    for (auto& r : required_tensors(e->dims))
-        if (!e->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
-    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    WLK_ENTER(e, e->cfg.device);
+    require_loaded(e->loaded, required_tensors(e->dims));
     if (e->stage_f32) { CUDA_CHECK(cudaFree(e->stage_f32)); e->stage_f32 = nullptr; e->stage_cap = 0; }
     e->finalized = true;
     WLK_API_END
 }
 int wlk_engine_weight_blob(wlk_engine* e, void** dev, size_t* nbytes) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(dev && nbytes, "null out pointer");
     CUDA_CHECK(cudaStreamSynchronize(e->st));
     *dev = e->arena.base; *nbytes = e->arena.cap;
@@ -1303,13 +1267,13 @@ int wlk_engine_weight_blob(wlk_engine* e, void** dev, size_t* nbytes) {
 }
 int wlk_engine_adopt_weights(wlk_engine* e) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     e->finalized = true;
     WLK_API_END
 }
 int wlk_engine_set_alignment_heads(wlk_engine* e, const int32_t* pairs, int n_pairs) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(n_pairs >= 1 && n_pairs <= e->cfg.max_align_heads, "%d alignment heads outside [1, max_align_heads=%d]",
               n_pairs, e->cfg.max_align_heads);
     for (auto& s : e->sess) WLK_CHECK(!s.open, "set alignment heads before opening sessions");
@@ -1334,13 +1298,13 @@ int wlk_engine_stream(wlk_engine* e, void** cuda_stream) {
 }
 int wlk_engine_sync(wlk_engine* e) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     CUDA_CHECK(cudaStreamSynchronize(e->st));
     WLK_API_END
 }
 int wlk_engine_memory(wlk_engine* e, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     if (weights) *weights = e->bytes_weights;
     if (sessions) *sessions = e->bytes_sessions;
     if (workspace) *workspace = e->bytes_workspace;
@@ -1349,7 +1313,7 @@ int wlk_engine_memory(wlk_engine* e, size_t* weights, size_t* sessions, size_t* 
 
 int wlk_session_open(wlk_engine* e, int32_t* sid) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sid, "null out pointer");
     WLK_CHECK(e->finalized, "weights not finalized");
     WLK_CHECK(e->n_align > 0, "alignment heads not set");
@@ -1363,7 +1327,7 @@ int wlk_session_open(wlk_engine* e, int32_t* sid) {
 }
 int wlk_session_close(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     WLK_CHECK(s.n_forks == 0, "session %d still has %d beam fork(s): close them first", sid, s.n_forks);
     CUDA_CHECK(cudaStreamSynchronize(e->st));
@@ -1372,7 +1336,7 @@ int wlk_session_close(wlk_engine* e, int32_t sid) {
 }
 int wlk_session_fork(wlk_engine* e, int32_t parent, int32_t* child) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(child, "null out pointer");
     get_root_session(e, parent, "forking");
     int found = -1;
@@ -1385,7 +1349,7 @@ int wlk_session_fork(wlk_engine* e, int32_t parent, int32_t* child) {
 }
 int wlk_sessions_gather_decoder(wlk_engine* e, const int32_t* sids, const int32_t* src, int n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && src && n >= 1, "bad argument");
     const wlk_dims& D = e->dims;
     const size_t es = e->es();
@@ -1428,7 +1392,7 @@ int wlk_sessions_gather_decoder(wlk_engine* e, const int32_t* sids, const int32_
 }
 int wlk_session_append_audio(wlk_engine* e, int32_t sid, const float* pcm, int64_t n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "the audio ring");
     WLK_CHECK(n >= 0 && (n == 0 || pcm), "bad audio chunk");
     WLK_CHECK(s.audio_len + n <= AUDIO_CAP, "audio buffer overflow: %lld + %lld > %d samples", (long long)s.audio_len, (long long)n, AUDIO_CAP);
@@ -1438,7 +1402,7 @@ int wlk_session_append_audio(wlk_engine* e, int32_t sid, const float* pcm, int64
 }
 int wlk_session_append_pcm16(wlk_engine* e, int32_t sid, const int16_t* pcm, int64_t n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "the audio ring");
     WLK_CHECK(n >= 0 && (n == 0 || pcm), "bad audio chunk");
     WLK_CHECK(s.audio_len + n <= AUDIO_CAP, "audio buffer overflow: %lld + %lld > %d samples", (long long)s.audio_len, (long long)n, AUDIO_CAP);
@@ -1452,7 +1416,7 @@ int wlk_session_append_pcm16(wlk_engine* e, int32_t sid, const int16_t* pcm, int
 }
 int wlk_session_drop_audio(wlk_engine* e, int32_t sid, int64_t n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "the audio ring");
     WLK_CHECK(n >= 0 && n <= s.audio_len, "cannot drop %lld of %lld samples", (long long)n, (long long)s.audio_len);
     const int64_t keep = s.audio_len - n;
@@ -1467,14 +1431,14 @@ int wlk_session_drop_audio(wlk_engine* e, int32_t sid, int64_t n) {
 }
 int wlk_session_clear_audio(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     s.audio_len = 0; s.mel_n = -1; s.mel_dropped = 0; s.inc_valid = false;
     WLK_API_END
 }
 int wlk_session_audio_len(wlk_engine* e, int32_t sid, int64_t* n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(n, "null out pointer");
     *n = get_session(e, sid).audio_len;
     WLK_API_END
@@ -1482,7 +1446,7 @@ int wlk_session_audio_len(wlk_engine* e, int32_t sid, int64_t* n) {
 
 int wlk_session_reset_decoder(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear();
     WLK_API_END
@@ -1490,14 +1454,14 @@ int wlk_session_reset_decoder(wlk_engine* e, int32_t sid) {
 
 int wlk_encode(wlk_engine* e, const int32_t* sids, int n, int32_t* content_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && content_out, "null argument");
     encode_batch(e, sids, n, content_out);
     WLK_API_END
 }
 int wlk_encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* content_out, int32_t* block_rows_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && content_out, "null argument");
     WLK_CHECK(e->finalized, "weights not finalized");
     encode_incremental(e, sids, n, content_out, block_rows_out);
@@ -1505,21 +1469,21 @@ int wlk_encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* c
 }
 int wlk_session_reset_incremental(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "the encoder K/V");
     s.inc_valid = false;                       // the next incremental encode takes the whole window as its block
     WLK_API_END
 }
 int wlk_decode(wlk_engine* e, const int32_t* sids, int n, const int32_t* tokens, const int32_t* offsets, int32_t sot_index) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && tokens && offsets, "null argument");
     decode_batch(e, sids, n, tokens, offsets, sot_index);
     WLK_API_END
 }
 int wlk_encode_mel(wlk_engine* e, int32_t sid, const float* mel_host, int32_t content_mel_len) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "encode");
     WLK_CHECK(mel_host && content_mel_len >= 0, "bad arguments");
     const int nm = e->dims.n_mels;
@@ -1539,7 +1503,7 @@ int wlk_encode_mel(wlk_engine* e, int32_t sid, const float* mel_host, int32_t co
 int wlk_decode_all_logits(wlk_engine* e, int32_t sid, const int32_t* tokens, int n_tokens, int32_t sot_index,
                           float* logits_host) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(tokens && logits_host && n_tokens >= 1 && n_tokens <= e->dims.n_text_ctx, "bad arguments");
     const size_t need = (size_t)n_tokens * e->dims.n_vocab;
     if (need > e->all_logits_cap) {
@@ -1555,7 +1519,7 @@ int wlk_decode_all_logits(wlk_engine* e, int32_t sid, const int32_t* tokens, int
 }
 int wlk_read_align_rows(wlk_engine* e, int32_t sid, float* out, int64_t capacity, int32_t* n_align, int32_t* rows) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     WLK_CHECK(out && n_align && rows, "null argument");
     const int R = s.align_rows, A = e->n_align;
@@ -1570,7 +1534,7 @@ int wlk_read_align_rows(wlk_engine* e, int32_t sid, float* out, int64_t capacity
 
 int wlk_no_speech_prob(wlk_engine* e, const int32_t* sids, int n, float* prob_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && prob_out && n >= 1 && n <= e->cfg.max_batch, "bad arguments");
     Stager sg(e);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
@@ -1590,7 +1554,7 @@ int wlk_no_speech_prob(wlk_engine* e, const int32_t* sids, int n, float* prob_ou
 }
 int wlk_suppress(wlk_engine* e, const int32_t* sids, int n, const int32_t* token_ids, int n_tokens) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && n >= 1 && n <= e->cfg.max_batch && n_tokens >= 0 && n_tokens <= 4096, "bad arguments");
     Stager sg(e);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
@@ -1607,7 +1571,7 @@ int wlk_suppress(wlk_engine* e, const int32_t* sids, int n, const int32_t* token
 }
 int wlk_add_logit_bias(wlk_engine* e, int32_t sid, const int32_t* token_ids, const float* bias, int n) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     WLK_CHECK(n >= 0 && n <= 4096, "bad count");
     if (n) {
@@ -1626,7 +1590,7 @@ int wlk_add_logit_bias(wlk_engine* e, int32_t sid, const int32_t* token_ids, con
 int wlk_greedy_and_align(wlk_engine* e, const int32_t* sids, int n, int32_t window_iters, int32_t* token_out,
                          float* logprob_out, int32_t* frame_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && token_out && logprob_out && frame_out && n >= 1 && n <= e->cfg.max_batch && window_iters >= 1, "bad arguments");
     Stager sg(e);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
@@ -1655,7 +1619,7 @@ int wlk_select(wlk_engine* e, const int32_t* sids, int n, const int32_t* suppres
                const float* bias_values, const int32_t* bias_offsets, int32_t window_iters, int32_t* token_out,
                float* logprob_out, int32_t* frame_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && token_out && logprob_out && frame_out && n >= 1 && n <= e->cfg.max_batch && window_iters >= 1, "bad arguments");
     WLK_CHECK(n_suppress >= 0 && n_suppress <= 4096 && n_first >= 0 && n_first <= 64, "bad suppression lists");
     const int n_bias = bias_offsets ? bias_offsets[n] : 0;
@@ -1710,7 +1674,7 @@ int wlk_select(wlk_engine* e, const int32_t* sids, int n, const int32_t* suppres
 // ---- debug taps ---------------------------------------------------------------------------
 int wlk_read_mel(wlk_engine* e, int32_t sid, float* out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_root_session(e, sid, "the mel");
     WLK_CHECK(out && s.encoded, "session not encoded");
     const int nm = e->dims.n_mels;
@@ -1738,7 +1702,7 @@ int wlk_read_mel(wlk_engine* e, int32_t sid, float* out) {
 }
 int wlk_read_encoder(wlk_engine* e, int32_t sid, float* out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = enc_owner(e, get_session(e, sid));
     WLK_CHECK(out && s.encoded, "session not encoded");
     const size_t n = (size_t)N_CTX * e->dims.n_audio_state;
@@ -1753,7 +1717,7 @@ int wlk_read_encoder(wlk_engine* e, int32_t sid, float* out) {
 }
 int wlk_read_logits(wlk_engine* e, int32_t sid, int32_t which, float* out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     WLK_CHECK(out && !s.iter_row_start.empty(), "no decode call in this epoch");
     CUDA_CHECK(cudaMemcpyAsync(out, which ? s.logits_sot : s.logits_last, (size_t)e->dims.n_vocab * 4, cudaMemcpyDeviceToHost, e->st));
@@ -1762,7 +1726,7 @@ int wlk_read_logits(wlk_engine* e, int32_t sid, int32_t which, float* out) {
 }
 int wlk_read_align_attn(wlk_engine* e, int32_t sid, float* out, int64_t capacity, int32_t* rows, int32_t* cols) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     Session& s = get_session(e, sid);
     WLK_CHECK(out && rows && cols && !s.iter_row_start.empty(), "no decode call in this epoch");
     Stager sg(e);
@@ -1784,7 +1748,7 @@ int wlk_read_align_attn(wlk_engine* e, int32_t sid, float* out, int64_t capacity
 int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t lda, const void* Wm, int w_type, int64_t ldw,
                 const float* bias, void* C, int c_type, int64_t ldc, int M, int N, int K, int gelu) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     GemmArgs g;
     g.A = A; g.a_type = a_type; g.lda = lda; g.W = Wm; g.w_type = w_type; g.ldw = ldw; g.M = M; g.N = N; g.K = K;
     g.epi.bias = bias; g.epi.gelu = gelu & 1; g.epi.C = C; g.epi.c_type = c_type; g.epi.ldc = ldc;
@@ -1800,7 +1764,7 @@ int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t l
 }
 int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int type, int batch, void* out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     ProfScope ps(e, WLK_KC_MISC, 4.0 * batch * e->dims.n_audio_head * (double)N_CTX * N_CTX * 64, 0);
     if (backend == WLK_BACKEND_TCGEN05) {
         WLK_CHECK(type == DT_BF16, "tcgen05 attention needs bf16");
@@ -1813,7 +1777,7 @@ int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int ty
 
 int wlk_op_median_filter(wlk_engine* e, const float* x_dev, float* out_dev, int rows, int cols, int width) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(x_dev && out_dev && rows >= 1 && cols >= 1, "bad arguments");
     ProfScope ps(e, WLK_KC_ALIGN);
     median_filter(x_dev, out_dev, rows, cols, width, e->st);
@@ -1822,7 +1786,7 @@ int wlk_op_median_filter(wlk_engine* e, const float* x_dev, float* out_dev, int 
 int wlk_op_dtw(wlk_engine* e, const float* x_dev, int N, int M, int32_t* text_idx_host, int32_t* time_idx_host,
                int32_t* len_out) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(x_dev && text_idx_host && time_idx_host && len_out, "null argument");
     WLK_CHECK(N >= 1 && N <= 4096 && M >= 1 && M <= 8192, "dtw: shape %d x %d out of range", N, M);
     size_t acct = 0;
@@ -1850,14 +1814,14 @@ int wlk_op_dtw(wlk_engine* e, const float* x_dev, int N, int M, int32_t* text_id
 // ---- timers / profile ------------------------------------------------------------------------
 int wlk_timer_record(wlk_engine* e, int slot) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(slot >= 0 && slot < 16, "timer slot out of range");
     CUDA_CHECK(cudaEventRecord(e->timers[slot], e->st));
     WLK_API_END
 }
 int wlk_timer_elapsed_ms(wlk_engine* e, int from_slot, int to_slot, float* ms) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(from_slot >= 0 && from_slot < 16 && to_slot >= 0 && to_slot < 16 && ms, "bad arguments");
     CUDA_CHECK(cudaEventSynchronize(e->timers[to_slot]));
     CUDA_CHECK(cudaEventElapsedTime(ms, e->timers[from_slot], e->timers[to_slot]));
@@ -1865,13 +1829,13 @@ int wlk_timer_elapsed_ms(wlk_engine* e, int from_slot, int to_slot, float* ms) {
 }
 int wlk_profile_enable(wlk_engine* e, int on) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     e->prof_on = on != 0;
     WLK_API_END
 }
 int wlk_profile_reset(wlk_engine* e) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     CUDA_CHECK(cudaStreamSynchronize(e->st));
     for (auto& p : e->prof) e->ev_pool.push_back({p.a, p.b});
     e->prof.clear();
@@ -1879,7 +1843,7 @@ int wlk_profile_reset(wlk_engine* e) {
 }
 int wlk_profile_read(wlk_engine* e, int cls, double* ms, int64_t* launches, double* flops, double* bytes) {
     WLK_API_BEGIN
-    LOCK(e);
+    WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(cls >= 0 && cls < WLK_KC_COUNT, "class out of range");
     CUDA_CHECK(cudaStreamSynchronize(e->st));
     double t = 0, f = 0, b = 0; int64_t n = 0;

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/wlk_b200.h"
+#include "host.cuh"
 #include "kernels.cuh"
 
 namespace wlk {
@@ -208,7 +209,7 @@ struct wlk_qwen {
     int ring = 0, max_rows = 0;
     cudaStream_t st = nullptr;
     std::mutex mu;
-    std::vector<void*> allocs;
+    DeviceAllocs allocs;
     size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
     // weights
     float *c1w = nullptr, *c1b = nullptr, *c2b = nullptr, *c3b = nullptr, *bout = nullptr, *pos_table = nullptr;
@@ -220,7 +221,7 @@ struct wlk_qwen {
     std::vector<QLayerW> L;
     std::set<std::string> loaded;
     bool finalized = false;
-    float* stage_f32 = nullptr; size_t stage_cap = 0;
+    WeightUpload upload;
     // sessions and workspaces
     std::vector<QSession> sess;
     float *mel = nullptr, *x = nullptr, *posbuf = nullptr, *outbuf = nullptr;
@@ -233,15 +234,6 @@ struct wlk_qwen {
 
 namespace {
 
-void* qalloc(wlk_qwen* q, size_t bytes, size_t* acct) {
-    void* p = nullptr;
-    if (bytes == 0) bytes = 16;
-    CUDA_CHECK(cudaMalloc(&p, bytes));
-    q->allocs.push_back(p);
-    if (acct) *acct += bytes;
-    return p;
-}
-
 void qgemm(wlk_qwen* q, GemmArgs& g) {
     if (g.M <= 0) return;
     g.sk_scratch = q->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
@@ -250,37 +242,15 @@ void qgemm(wlk_qwen* q, GemmArgs& g) {
     else gemm_simt(g, q->st);
 }
 
-// upload a host fp32 tensor into a device matrix of the activation type (weights) or fp32 (biases, LN)
-void put(wlk_qwen* q, const float* host, size_t n, void* dst, int dst_type) {
-    if (n > q->stage_cap) {
-        if (q->stage_f32) { CUDA_CHECK(cudaStreamSynchronize(q->st)); CUDA_CHECK(cudaFree(q->stage_f32)); }
-        CUDA_CHECK(cudaMalloc(&q->stage_f32, n * 4));
-        q->stage_cap = n;
-    }
-    CUDA_CHECK(cudaMemcpyAsync(q->stage_f32, host, n * 4, cudaMemcpyHostToDevice, q->st));
-    if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, q->stage_f32, n * 4, cudaMemcpyDeviceToDevice, q->st));
-    else convert_f32_to(q->stage_f32, dst, dst_type, (int64_t)n, q->st);
-    CUDA_CHECK(cudaStreamSynchronize(q->st));          // `host` (and the staging block) may be reused right away
-}
-
-int64_t numel(const int64_t* shape, int ndim) { int64_t n = 1; for (int i = 0; i < ndim; ++i) n *= shape[i]; return n; }
-
-void expect(const char* name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
-    bool ok = (int)want.size() == ndim;
-    int i = 0;
-    for (int64_t w : want) { if (ok && shape[i] != w) ok = false; ++i; }
-    WLK_CHECK(ok, "tensor %s has the wrong shape for this tower geometry", name);
-}
-
 void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const int64_t* shape, int ndim) {
     const wlk_qwen_dims& D = q->dims;
     const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
     const int64_t n = numel(shape, ndim);
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name.c_str(), shape, ndim, {rows, cols}); put(q, host, n, dst, q->act); };
-    auto vec = [&](float* dst, int64_t len) { expect(name.c_str(), shape, ndim, {len}); put(q, host, n, dst, DT_F32); };
+    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect_shape(name.c_str(), shape, ndim, {rows, cols}); q->upload.put(host, n, dst, q->act, q->st); };
+    auto vec = [&](float* dst, int64_t len) { expect_shape(name.c_str(), shape, ndim, {len}); q->upload.put(host, n, dst, DT_F32, q->st); };
     if (name == "mel_filters") {
         // optional: only wlk_qwen_append_audio needs it.  [n_mels][201] (Slaney filterbank of the feature extractor)
-        expect(name.c_str(), shape, ndim, {D.n_mels, N_FREQ});
+        expect_shape(name.c_str(), shape, ndim, {D.n_mels, N_FREQ});
         std::vector<float> t((size_t)n);
         std::vector<int2> span(D.n_mels);
         for (int m = 0; m < D.n_mels; ++m) {
@@ -292,39 +262,39 @@ void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const 
             if (lo >= hi) { lo = 0; hi = 0; }
             span[m] = make_int2(lo, hi);
         }
-        put(q, t.data(), n, q->filtT, DT_F32);
+        q->upload.put(t.data(), n, q->filtT, DT_F32, q->st);
         CUDA_CHECK(cudaMemcpyAsync(q->filt_span, span.data(), span.size() * 8, cudaMemcpyHostToDevice, q->st));
         CUDA_CHECK(cudaStreamSynchronize(q->st));
         q->have_filters = true;
     }
-    else if (name == "conv2d1.weight") { expect(name.c_str(), shape, ndim, {C, 1, 3, 3}); put(q, host, n, q->c1w, DT_F32); }
+    else if (name == "conv2d1.weight") { expect_shape(name.c_str(), shape, ndim, {C, 1, 3, 3}); q->upload.put(host, n, q->c1w, DT_F32, q->st); }
     else if (name == "conv2d1.bias") vec(q->c1b, C);
     else if (name == "conv2d2.weight" || name == "conv2d3.weight") {
         // [Co][Ci][3][3] -> [Co][tap][Ci]: a tap's input channels are contiguous, like the im2col rows
-        expect(name.c_str(), shape, ndim, {C, C, 3, 3});
+        expect_shape(name.c_str(), shape, ndim, {C, C, 3, 3});
         std::vector<float> packed((size_t)n);
         for (int co = 0; co < C; ++co)
             for (int ci = 0; ci < C; ++ci)
                 for (int tap = 0; tap < 9; ++tap)
                     packed[((size_t)co * 9 + tap) * C + ci] = host[((size_t)co * C + ci) * 9 + tap];
-        put(q, packed.data(), n, name == "conv2d2.weight" ? q->W2c : q->W3c, q->act);
+        q->upload.put(packed.data(), n, name == "conv2d2.weight" ? q->W2c : q->W3c, q->act, q->st);
     }
     else if (name == "conv2d2.bias") vec(q->c2b, C);
     else if (name == "conv2d3.bias") vec(q->c3b, C);
     else if (name == "conv_out.weight") {
         // the reference flattens [C][F] (channel-major, causal.py:240-242); activations here are [F][C]
-        expect(name.c_str(), shape, ndim, {d, (int64_t)C * F});
+        expect_shape(name.c_str(), shape, ndim, {d, (int64_t)C * F});
         std::vector<float> packed((size_t)n);
         for (int o = 0; o < d; ++o)
             for (int c = 0; c < C; ++c)
                 for (int f = 0; f < F; ++f)
                     packed[(size_t)o * C * F + (size_t)f * C + c] = host[(size_t)o * C * F + (size_t)c * F + f];
-        put(q, packed.data(), n, q->Wout, q->act);
+        q->upload.put(packed.data(), n, q->Wout, q->act, q->st);
     }
     else if (name == "conv_out.bias") { WLK_CHECK(D.conv_out_bias, "this geometry has no conv_out bias"); vec(q->bout, d); }
     else if (name == "positional_embedding.positional_embedding") {
-        expect(name.c_str(), shape, ndim, {D.max_positions, d});
-        put(q, host, n, q->pos_table, DT_F32);
+        expect_shape(name.c_str(), shape, ndim, {D.max_positions, d});
+        q->upload.put(host, n, q->pos_table, DT_F32, q->st);
     }
     else if (name == "ln_post.weight") vec(q->lnpw, d);
     else if (name == "ln_post.bias") vec(q->lnpb, d);
@@ -341,8 +311,8 @@ void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const 
         QLayerW& Lw = q->L[li];
         const size_t es = q->es();
         auto part = [&](int which, bool is_weight) {            // q / k / v rows of the fused projection
-            if (is_weight) { expect(name.c_str(), shape, ndim, {d, d}); put(q, host, n, (char*)Lw.Wqkv + (size_t)which * d * d * es, q->act); }
-            else { expect(name.c_str(), shape, ndim, {d}); put(q, host, n, Lw.bqkv + (size_t)which * d, DT_F32); }
+            if (is_weight) { expect_shape(name.c_str(), shape, ndim, {d, d}); q->upload.put(host, n, (char*)Lw.Wqkv + (size_t)which * d * d * es, q->act, q->st); }
+            else { expect_shape(name.c_str(), shape, ndim, {d}); q->upload.put(host, n, Lw.bqkv + (size_t)which * d, DT_F32, q->st); }
         };
         if (rest == "self_attn.q_proj.weight") part(0, true);
         else if (rest == "self_attn.k_proj.weight") part(1, true);
@@ -394,18 +364,11 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
     WLK_CHECK(D.mutable_tail_steps == 0 || D.block_frames == 0, "fixed attention blocks and a mutable tail are exclusive");   // causal.py:127-131
     WLK_CHECK(D.left_context_steps >= 1 && D.left_context_steps + Q_STEPS_CAP <= 512, "left_context_steps must be in [1, %d]", 512 - Q_STEPS_CAP);
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    int ndev = 0;
-    cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the H100 engine has no CPU fallback", cudaGetErrorString(ce));
-    WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
-    CUDA_CHECK(cudaSetDevice(cfg->device));
-    cudaDeviceProp prop;
-    CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    const int num_sms = open_sm90_device(cfg->device);
 
     auto* q = new wlk_qwen();
     q->dims = D; q->cfg = *cfg;
-    q->num_sms = prop.multiProcessorCount;
+    q->num_sms = num_sms;
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     q->ring = D.left_context_steps + Q_STEPS_CAP;
@@ -415,44 +378,43 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
     const size_t es = q->es();
     const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
     size_t* aw = &q->bytes_weights;
-    q->c1w = (float*)qalloc(q, (size_t)C * 9 * 4, aw); q->c1b = (float*)qalloc(q, C * 4, aw);
-    q->c2b = (float*)qalloc(q, C * 4, aw); q->c3b = (float*)qalloc(q, C * 4, aw);
-    q->W2c = qalloc(q, (size_t)C * 9 * C * es, aw); q->W3c = qalloc(q, (size_t)C * 9 * C * es, aw);
-    q->Wout = qalloc(q, (size_t)d * C * F * es, aw); q->bout = (float*)qalloc(q, d * 4, aw);
-    q->pos_table = (float*)qalloc(q, (size_t)D.max_positions * d * 4, aw);
-    q->lnpw = (float*)qalloc(q, d * 4, aw); q->lnpb = (float*)qalloc(q, d * 4, aw);
-    q->Wp1 = qalloc(q, (size_t)d * d * es, aw); q->bp1 = (float*)qalloc(q, d * 4, aw);
-    q->Wp2 = qalloc(q, (size_t)D.out_dim * d * es, aw); q->bp2 = (float*)qalloc(q, D.out_dim * 4, aw);
+    q->c1w = (float*)q->allocs.take((size_t)C * 9 * 4, aw); q->c1b = (float*)q->allocs.take(C * 4, aw);
+    q->c2b = (float*)q->allocs.take(C * 4, aw); q->c3b = (float*)q->allocs.take(C * 4, aw);
+    q->W2c = q->allocs.take((size_t)C * 9 * C * es, aw); q->W3c = q->allocs.take((size_t)C * 9 * C * es, aw);
+    q->Wout = q->allocs.take((size_t)d * C * F * es, aw); q->bout = (float*)q->allocs.take(d * 4, aw);
+    q->pos_table = (float*)q->allocs.take((size_t)D.max_positions * d * 4, aw);
+    q->lnpw = (float*)q->allocs.take(d * 4, aw); q->lnpb = (float*)q->allocs.take(d * 4, aw);
+    q->Wp1 = q->allocs.take((size_t)d * d * es, aw); q->bp1 = (float*)q->allocs.take(d * 4, aw);
+    q->Wp2 = q->allocs.take((size_t)D.out_dim * d * es, aw); q->bp2 = (float*)q->allocs.take(D.out_dim * 4, aw);
     q->L.resize(D.n_layer);
     for (auto& Lw : q->L) {
-        Lw.Wqkv = qalloc(q, (size_t)3 * d * d * es, aw); Lw.bqkv = (float*)qalloc(q, 3 * d * 4, aw);
-        Lw.Wo = qalloc(q, (size_t)d * d * es, aw); Lw.bo = (float*)qalloc(q, d * 4, aw);
-        Lw.W1 = qalloc(q, (size_t)ffn * d * es, aw); Lw.b1 = (float*)qalloc(q, ffn * 4, aw);
-        Lw.W2 = qalloc(q, (size_t)d * ffn * es, aw); Lw.b2 = (float*)qalloc(q, d * 4, aw);
-        Lw.ln1w = (float*)qalloc(q, d * 4, aw); Lw.ln1b = (float*)qalloc(q, d * 4, aw);
-        Lw.ln2w = (float*)qalloc(q, d * 4, aw); Lw.ln2b = (float*)qalloc(q, d * 4, aw);
+        Lw.Wqkv = q->allocs.take((size_t)3 * d * d * es, aw); Lw.bqkv = (float*)q->allocs.take(3 * d * 4, aw);
+        Lw.Wo = q->allocs.take((size_t)d * d * es, aw); Lw.bo = (float*)q->allocs.take(d * 4, aw);
+        Lw.W1 = q->allocs.take((size_t)ffn * d * es, aw); Lw.b1 = (float*)q->allocs.take(ffn * 4, aw);
+        Lw.W2 = q->allocs.take((size_t)d * ffn * es, aw); Lw.b2 = (float*)q->allocs.take(d * 4, aw);
+        Lw.ln1w = (float*)q->allocs.take(d * 4, aw); Lw.ln1b = (float*)q->allocs.take(d * 4, aw);
+        Lw.ln2w = (float*)q->allocs.take(d * 4, aw); Lw.ln2b = (float*)q->allocs.take(d * 4, aw);
     }
     const size_t R = (size_t)q->max_rows;
     size_t* ws = &q->bytes_workspace;
-    q->mel = (float*)qalloc(q, R * 8 * D.n_mels * 4, ws);
-    q->a1 = qalloc(q, R * (D.n_mels / 2) * 4 * C * es, ws);
-    q->col = qalloc(q, R * (D.n_mels / 4) * 2 * 9 * C * es, ws);              // conv2's im2col is the larger one
-    q->a2 = qalloc(q, R * (D.n_mels / 4) * 2 * C * es, ws);
-    q->a3 = qalloc(q, R * F * C * es, ws);
-    q->posbuf = (float*)qalloc(q, R * d * 4, ws);
-    q->x = (float*)qalloc(q, R * d * 4, ws);
-    q->xn = qalloc(q, R * d * es, ws); q->qb = qalloc(q, R * d * es, ws); q->att = qalloc(q, R * d * es, ws);
-    q->hid = qalloc(q, R * (size_t)(ffn > d ? ffn : d) * es, ws);
-    q->outbuf = (float*)qalloc(q, R * D.out_dim * 4, ws);
-    q->filtT = (float*)qalloc(q, (size_t)N_FREQ * D.n_mels * 4, aw);
-    q->window = (float*)qalloc(q, N_FFT * 4, aw);
-    q->twiddle = (float2*)qalloc(q, N_FFT * 8, aw);
-    q->filt_span = (int2*)qalloc(q, (size_t)D.n_mels * 8, aw);
-    q->audio_scratch = (float*)qalloc(q, (size_t)QMEL_AUDIO_CAP * 4, ws);
+    q->mel = (float*)q->allocs.take(R * 8 * D.n_mels * 4, ws);
+    q->a1 = q->allocs.take(R * (D.n_mels / 2) * 4 * C * es, ws);
+    q->col = q->allocs.take(R * (D.n_mels / 4) * 2 * 9 * C * es, ws);              // conv2's im2col is the larger one
+    q->a2 = q->allocs.take(R * (D.n_mels / 4) * 2 * C * es, ws);
+    q->a3 = q->allocs.take(R * F * C * es, ws);
+    q->posbuf = (float*)q->allocs.take(R * d * 4, ws);
+    q->x = (float*)q->allocs.take(R * d * 4, ws);
+    q->xn = q->allocs.take(R * d * es, ws); q->qb = q->allocs.take(R * d * es, ws); q->att = q->allocs.take(R * d * es, ws);
+    q->hid = q->allocs.take(R * (size_t)(ffn > d ? ffn : d) * es, ws);
+    q->outbuf = (float*)q->allocs.take(R * D.out_dim * 4, ws);
+    q->filtT = (float*)q->allocs.take((size_t)N_FREQ * D.n_mels * 4, aw);
+    q->window = (float*)q->allocs.take(N_FFT * 4, aw);
+    q->twiddle = (float2*)q->allocs.take(N_FFT * 8, aw);
+    q->filt_span = (int2*)q->allocs.take((size_t)D.n_mels * 8, aw);
+    q->audio_scratch = (float*)q->allocs.take((size_t)QMEL_AUDIO_CAP * 4, ws);
     if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
-        q->sk_scratch = (float*)qalloc(q, SK_SCRATCH_FLOATS * 4, ws);
-        q->sk_counters = (int*)qalloc(q, SK_MAX_TILES * 4, ws);
-        CUDA_CHECK(cudaMemset(q->sk_counters, 0, SK_MAX_TILES * 4));
+        q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
+        q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
     }
     {   // periodic Hann window and DFT twiddles exp(-2 pi i t / 400), evaluated in double
         std::vector<float> win(N_FFT);
@@ -468,7 +430,7 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
     }
     q->stg_bytes = R * 16 + (size_t)cfg->max_batch * (sizeof(QJob) + sizeof(MelJob) + 64) + 4096;
     CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
-    q->stg_d = (uint8_t*)qalloc(q, q->stg_bytes, ws);
+    q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
     q->sess.resize(cfg->max_sessions);
     *out = q;
 }
@@ -477,8 +439,8 @@ void destroy(wlk_qwen* q) {
     cudaStreamSynchronize(q->st);
     for (auto& s : q->sess) { if (s.kv) cudaFree(s.kv); if (s.audio) cudaFree(s.audio); if (s.mel_raw) cudaFree(s.mel_raw); if (s.mel_blockmax) cudaFree(s.mel_blockmax); }
     if (q->mel_out) cudaFree(q->mel_out);
-    for (void* p : q->allocs) cudaFree(p);
-    if (q->stage_f32) cudaFree(q->stage_f32);
+    q->allocs.free_all();
+    q->upload.release();
     if (q->stg_h) cudaFreeHost(q->stg_h);
     cudaStreamDestroy(q->st);
     delete q;
@@ -780,22 +742,6 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
 
 }  // namespace
 
-#define WLK_API_BEGIN try {
-#define WLK_API_END                                              \
-    return 0;                                                    \
-    } catch (const wlk::Error& err) {                            \
-        wlk::set_last_error(err.msg);                            \
-        return 1;                                                \
-    } catch (const std::exception& ex) {                         \
-        wlk::set_last_error(std::string("exception: ") + ex.what()); \
-        return 2;                                                \
-    } catch (...) {                                              \
-        wlk::set_last_error("unknown exception");                \
-        return 3;                                                \
-    }
-#define QLOCK(q) WLK_CHECK((q) != nullptr, "null engine"); std::lock_guard<std::mutex> _lk((q)->mu); \
-                 CUDA_CHECK(cudaSetDevice((q)->cfg.device))
-
 extern "C" {
 
 int wlk_qwen_create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
@@ -812,25 +758,22 @@ int wlk_qwen_destroy(wlk_qwen* q) {
 }
 int wlk_qwen_load_tensor(wlk_qwen* q, const char* name, const float* host, const int64_t* shape, int ndim) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
     load_tensor(q, name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_qwen_finalize_weights(wlk_qwen* q) {
     WLK_API_BEGIN
-    QLOCK(q);
-    std::string missing;
-    int nmiss = 0;
-    for (auto& r : required(q->dims)) if (!q->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
-    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
-    if (q->stage_f32) { CUDA_CHECK(cudaFree(q->stage_f32)); q->stage_f32 = nullptr; q->stage_cap = 0; }
+    WLK_ENTER(q, q->cfg.device);
+    require_loaded(q->loaded, required(q->dims));
+    q->upload.release();
     q->finalized = true;
     WLK_API_END
 }
 int wlk_qwen_session_open(wlk_qwen* q, int32_t* sid) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sid, "null out pointer");
     int found = -1;
     for (int i = 0; i < (int)q->sess.size(); ++i) if (!q->sess[i].open) { found = i; break; }
@@ -845,7 +788,7 @@ int wlk_qwen_session_open(wlk_qwen* q, int32_t* sid) {
 }
 int wlk_qwen_session_close(wlk_qwen* q, int32_t sid) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     cudaFree(s.kv);
@@ -859,7 +802,7 @@ int wlk_qwen_session_close(wlk_qwen* q, int32_t sid) {
 }
 int wlk_qwen_session_reset(wlk_qwen* q, int32_t sid) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     s.emitted = 0; s.pending.clear(); s.tail.clear();
     s.buf_len = s.buf_start_frame = s.mel_emitted = s.total_samples = 0;       // StreamingMelExtractor.reset, features.py:112
@@ -867,7 +810,7 @@ int wlk_qwen_session_reset(wlk_qwen* q, int32_t sid) {
 }
 int wlk_qwen_session_state(wlk_qwen* q, int32_t sid, int32_t* pending_frames, int64_t* emitted_steps) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     if (pending_frames) *pending_frames = (int32_t)(s.pending.size() / q->dims.n_mels);
     if (emitted_steps) *emitted_steps = s.emitted;
@@ -875,7 +818,7 @@ int wlk_qwen_session_state(wlk_qwen* q, int32_t sid, int32_t* pending_frames, in
 }
 int wlk_qwen_session_mutable_steps(wlk_qwen* q, int32_t sid, int32_t* mutable_steps) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     WLK_CHECK(mutable_steps != nullptr, "null argument");
     *mutable_steps = (int32_t)(s.tail.size() / ((size_t)8 * q->dims.n_mels));
@@ -884,7 +827,7 @@ int wlk_qwen_session_mutable_steps(wlk_qwen* q, int32_t sid, int32_t* mutable_st
 int wlk_qwen_forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels_host, const int32_t* frame_offsets,
                            float* out_host, int64_t out_capacity_rows, int32_t* out_row_offsets) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && frame_offsets && out_row_offsets && (mels_host || frame_offsets[n] == frame_offsets[0]), "null argument");
     WLK_CHECK(out_host || out_capacity_rows == 0, "null output buffer");
     forward_chunk(q, sids, n, mels_host, frame_offsets, out_host, out_capacity_rows, out_row_offsets, false);
@@ -893,7 +836,7 @@ int wlk_qwen_forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float*
 int wlk_qwen_flush_pending(wlk_qwen* q, const int32_t* sids, int n, float* out_host, int64_t out_capacity_rows,
                            int32_t* out_row_offsets) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && out_row_offsets, "null argument");
     WLK_CHECK(out_host || out_capacity_rows == 0, "null output buffer");
     forward_chunk(q, sids, n, nullptr, nullptr, out_host, out_capacity_rows, out_row_offsets, true);
@@ -902,7 +845,7 @@ int wlk_qwen_flush_pending(wlk_qwen* q, const int32_t* sids, int n, float* out_h
 int wlk_qwen_forward_chunk_device(wlk_qwen* q, const int32_t* sids, int n, const float* mels_host, const int32_t* frame_offsets,
                                   float* out_dev, int64_t out_capacity_rows, int32_t* out_row_offsets) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && frame_offsets && out_row_offsets && (mels_host || frame_offsets[n] == frame_offsets[0]), "null argument");
     WLK_CHECK(out_dev || out_capacity_rows == 0, "null output buffer");
     forward_chunk(q, sids, n, mels_host, frame_offsets, out_dev, out_capacity_rows, out_row_offsets, false, true);
@@ -911,7 +854,7 @@ int wlk_qwen_forward_chunk_device(wlk_qwen* q, const int32_t* sids, int n, const
 int wlk_qwen_flush_pending_device(wlk_qwen* q, const int32_t* sids, int n, float* out_dev, int64_t out_capacity_rows,
                                   int32_t* out_row_offsets) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && out_row_offsets, "null argument");
     WLK_CHECK(out_dev || out_capacity_rows == 0, "null output buffer");
     forward_chunk(q, sids, n, nullptr, nullptr, out_dev, out_capacity_rows, out_row_offsets, true, true);
@@ -919,7 +862,7 @@ int wlk_qwen_flush_pending_device(wlk_qwen* q, const int32_t* sids, int n, float
 }
 int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int64_t capacity_frames, int32_t* n_frames) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     WLK_CHECK(n_frames, "null argument");
     const int64_t have = (int64_t)(s.pending.size() / q->dims.n_mels);
@@ -931,7 +874,7 @@ int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int
 }
 int wlk_qwen_session_set_pending(wlk_qwen* q, int32_t sid, const float* mels_host, int32_t n_frames) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     QSession& s = qsession(q, sid);
     WLK_CHECK(n_frames >= 0 && (mels_host || n_frames == 0), "bad arguments");
     s.pending.assign(mels_host, mels_host + (size_t)n_frames * q->dims.n_mels);
@@ -940,7 +883,7 @@ int wlk_qwen_session_set_pending(wlk_qwen* q, int32_t sid, const float* mels_hos
 int wlk_qwen_append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm_host, const int64_t* sample_offsets,
                           float* mel_out_host, int64_t out_capacity_frames, int32_t* frame_offsets_out, int32_t flush) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && frame_offsets_out && (flush || sample_offsets), "null argument");
     WLK_CHECK(flush || pcm_host || sample_offsets[n] == sample_offsets[0], "null audio");
     WLK_CHECK(mel_out_host || out_capacity_frames == 0, "null output buffer");
@@ -949,7 +892,7 @@ int wlk_qwen_append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* 
 }
 int wlk_qwen_memory(wlk_qwen* q, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
-    QLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     if (weights) *weights = q->bytes_weights;
     if (sessions) *sessions = q->bytes_sessions;
     if (workspace) *workspace = q->bytes_workspace;

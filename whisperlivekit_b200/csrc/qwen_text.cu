@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "../../include/wlk_b200.h"
+#include "host.cuh"
 #include "kernels.cuh"
 
 namespace wlk {
@@ -414,14 +415,14 @@ struct wlk_qtext {
     int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
     cudaStream_t st = nullptr;
     std::mutex mu;
-    std::vector<void*> allocs;
+    DeviceAllocs allocs;
     size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0, kv_bytes = 0;
     float *emb = nullptr, *normw = nullptr, *inv_freq = nullptr;
     void* head = nullptr;                               // lm_head [V][d] act type (the embedding table when tied)
     std::vector<QTLayerW> L;
     std::set<std::string> loaded;
     bool finalized = false;
-    float* stage_f32 = nullptr; size_t stage_cap = 0;
+    WeightUpload upload;
     std::vector<QTSession> sess;
     float *x = nullptr, *qkv = nullptr, *gu = nullptr, *up = nullptr, *logits = nullptr, *values_d = nullptr;
     void *xn = nullptr, *qb = nullptr, *att = nullptr, *hid = nullptr, *hlog = nullptr;
@@ -442,15 +443,6 @@ struct wlk_qtext {
 
 namespace {
 
-void* talloc(wlk_qtext* t, size_t bytes, size_t* acct) {
-    void* p = nullptr;
-    if (bytes == 0) bytes = 16;
-    CUDA_CHECK(cudaMalloc(&p, bytes));
-    t->allocs.push_back(p);
-    if (acct) *acct += bytes;
-    return p;
-}
-
 void tgemm(wlk_qtext* t, GemmArgs& g) {
     if (g.M <= 0) return;
     g.sk_scratch = t->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
@@ -464,37 +456,17 @@ void tgemm(wlk_qtext* t, GemmArgs& g) {
     }
 }
 
-void put(wlk_qtext* t, const float* host, size_t n, void* dst, int dst_type) {
-    if (n > t->stage_cap) {
-        if (t->stage_f32) { CUDA_CHECK(cudaStreamSynchronize(t->st)); CUDA_CHECK(cudaFree(t->stage_f32)); }
-        CUDA_CHECK(cudaMalloc(&t->stage_f32, n * 4));
-        t->stage_cap = n;
-    }
-    CUDA_CHECK(cudaMemcpyAsync(t->stage_f32, host, n * 4, cudaMemcpyHostToDevice, t->st));
-    if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, t->stage_f32, n * 4, cudaMemcpyDeviceToDevice, t->st));
-    else convert_f32_to(t->stage_f32, dst, dst_type, (int64_t)n, t->st);
-    CUDA_CHECK(cudaStreamSynchronize(t->st));
-}
-
-void expect(const char* name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
-    bool ok = (int)want.size() == ndim;
-    int i = 0;
-    for (int64_t w : want) { if (ok && shape[i] != w) ok = false; ++i; }
-    WLK_CHECK(ok, "tensor %s has the wrong shape for this text-decoder geometry", name);
-}
-
 void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const int64_t* shape, int ndim) {
     const wlk_qtext_dims& D = t->dims;
     const int d = D.d_model, F = D.ffn_dim, qd = D.n_head * QT_HD, kvd = D.n_kv_head * QT_HD;
-    int64_t n = 1;
-    for (int i = 0; i < ndim; ++i) n *= shape[i];
+    const int64_t n = numel(shape, ndim);
     const size_t es = t->es();
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name.c_str(), shape, ndim, {rows, cols}); put(t, host, n, dst, t->act); };
-    auto vec = [&](float* dst, int64_t len) { expect(name.c_str(), shape, ndim, {len}); put(t, host, n, dst, DT_F32); };
+    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect_shape(name.c_str(), shape, ndim, {rows, cols}); t->upload.put(host, n, dst, t->act, t->st); };
+    auto vec = [&](float* dst, int64_t len) { expect_shape(name.c_str(), shape, ndim, {len}); t->upload.put(host, n, dst, DT_F32, t->st); };
     if (name == "embed_tokens.weight") {
-        expect(name.c_str(), shape, ndim, {D.vocab, d});
-        put(t, host, n, t->emb, DT_F32);
-        if (D.tied) put(t, host, n, t->head, t->act);
+        expect_shape(name.c_str(), shape, ndim, {D.vocab, d});
+        t->upload.put(host, n, t->emb, DT_F32, t->st);
+        if (D.tied) t->upload.put(host, n, t->head, t->act, t->st);
     }
     else if (name == "lm_head.weight") { WLK_CHECK(!D.tied, "this geometry ties lm_head to embed_tokens"); mat(t->head, D.vocab, d); }
     else if (name == "norm.weight") vec(t->normw, d);
@@ -510,14 +482,14 @@ void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const
         WLK_CHECK(li >= 0 && li < D.n_layer, "layer index out of range in %s", name.c_str());
         const std::string rest = name.substr(dot + 1);
         QTLayerW& Lw = t->L[li];
-        if (rest == "self_attn.q_proj.weight") { expect(name.c_str(), shape, ndim, {qd, d}); put(t, host, n, Lw.Wqkv, t->act); }
-        else if (rest == "self_attn.k_proj.weight") { expect(name.c_str(), shape, ndim, {kvd, d}); put(t, host, n, (char*)Lw.Wqkv + (size_t)qd * d * es, t->act); }
-        else if (rest == "self_attn.v_proj.weight") { expect(name.c_str(), shape, ndim, {kvd, d}); put(t, host, n, (char*)Lw.Wqkv + (size_t)(qd + kvd) * d * es, t->act); }
+        if (rest == "self_attn.q_proj.weight") { expect_shape(name.c_str(), shape, ndim, {qd, d}); t->upload.put(host, n, Lw.Wqkv, t->act, t->st); }
+        else if (rest == "self_attn.k_proj.weight") { expect_shape(name.c_str(), shape, ndim, {kvd, d}); t->upload.put(host, n, (char*)Lw.Wqkv + (size_t)qd * d * es, t->act, t->st); }
+        else if (rest == "self_attn.v_proj.weight") { expect_shape(name.c_str(), shape, ndim, {kvd, d}); t->upload.put(host, n, (char*)Lw.Wqkv + (size_t)(qd + kvd) * d * es, t->act, t->st); }
         else if (rest == "self_attn.o_proj.weight") mat(Lw.Wo, d, qd);
         else if (rest == "self_attn.q_norm.weight") vec(Lw.qn, QT_HD);
         else if (rest == "self_attn.k_norm.weight") vec(Lw.kn, QT_HD);
-        else if (rest == "mlp.gate_proj.weight") { expect(name.c_str(), shape, ndim, {F, d}); put(t, host, n, Lw.Wgu, t->act); }
-        else if (rest == "mlp.up_proj.weight") { expect(name.c_str(), shape, ndim, {F, d}); put(t, host, n, (char*)Lw.Wgu + (size_t)F * d * es, t->act); }
+        else if (rest == "mlp.gate_proj.weight") { expect_shape(name.c_str(), shape, ndim, {F, d}); t->upload.put(host, n, Lw.Wgu, t->act, t->st); }
+        else if (rest == "mlp.up_proj.weight") { expect_shape(name.c_str(), shape, ndim, {F, d}); t->upload.put(host, n, (char*)Lw.Wgu + (size_t)F * d * es, t->act, t->st); }
         else if (rest == "mlp.down_proj.weight") mat(Lw.Wd, d, F);
         else if (rest == "input_layernorm.weight") vec(Lw.ln1, d);
         else if (rest == "post_attention_layernorm.weight") vec(Lw.ln2, d);
@@ -571,8 +543,8 @@ void build_adapter(wlk_qtext* t) {
     }
     const size_t es = t->es();
     size_t* aw = &t->bytes_weights;
-    A.Wp = talloc(t, (size_t)d * A.in_dim * es, aw);
-    put(t, proj.second.data(), proj.second.size(), A.Wp, t->act);
+    A.Wp = t->allocs.take((size_t)d * A.in_dim * es, aw);
+    t->upload.put(proj.second.data(), proj.second.size(), A.Wp, t->act, t->st);
     const int64_t H = A.hidden;
     for (int i = 0; i < nb; ++i) {
         const std::string p = "adapter.blocks." + std::to_string(i) + ".";
@@ -584,22 +556,22 @@ void build_adapter(wlk_qtext* t) {
         WLK_CHECK(g.first == (std::vector<int64_t>{H, d}) && u.first == (std::vector<int64_t>{H, d}),
                   "%smlp.gate / mlp.up must be [hidden][d_model] with the hidden width of block 0", p.c_str());
         WLK_CHECK(dn.first == (std::vector<int64_t>{d, H}), "%smlp.down.weight must be [d_model][hidden]", p.c_str());
-        float* nd = (float*)talloc(t, (size_t)d * 4, aw);
-        put(t, nw.second.data(), nw.second.size(), nd, DT_F32);
-        void* gu = talloc(t, (size_t)2 * H * d * es, aw);
-        put(t, g.second.data(), g.second.size(), gu, t->act);
-        put(t, u.second.data(), u.second.size(), (char*)gu + (size_t)H * d * es, t->act);
-        void* wd = talloc(t, (size_t)d * H * es, aw);
-        put(t, dn.second.data(), dn.second.size(), wd, t->act);
+        float* nd = (float*)t->allocs.take((size_t)d * 4, aw);
+        t->upload.put(nw.second.data(), nw.second.size(), nd, DT_F32, t->st);
+        void* gu = t->allocs.take((size_t)2 * H * d * es, aw);
+        t->upload.put(g.second.data(), g.second.size(), gu, t->act, t->st);
+        t->upload.put(u.second.data(), u.second.size(), (char*)gu + (size_t)H * d * es, t->act, t->st);
+        void* wd = t->allocs.take((size_t)d * H * es, aw);
+        t->upload.put(dn.second.data(), dn.second.size(), wd, t->act, t->st);
         A.norm.push_back(nd); A.Wgu.push_back(gu); A.Wd.push_back(wd);
         used += 4;
     }
     WLK_CHECK(used == st.size(), "%zu adapter tensors do not belong to an adapter of %d blocks", st.size() - used, nb);
     size_t* ws = &t->bytes_workspace;
-    A.a_in = talloc(t, (size_t)QT_ROUND_ROWS * A.in_dim * es, ws);
+    A.a_in = t->allocs.take((size_t)QT_ROUND_ROWS * A.in_dim * es, ws);
     if (nb > 0) {
-        A.a_gu = (float*)talloc(t, (size_t)QT_ROUND_ROWS * 2 * H * 4, ws);
-        A.a_hid = talloc(t, (size_t)QT_ROUND_ROWS * H * es, ws);
+        A.a_gu = (float*)t->allocs.take((size_t)QT_ROUND_ROWS * 2 * H * 4, ws);
+        A.a_hid = t->allocs.take((size_t)QT_ROUND_ROWS * H * es, ws);
     }
     st.clear();
     t->has_adapter = true;
@@ -614,18 +586,11 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     WLK_CHECK(D.max_ctx >= 1 && D.max_ctx <= 32768, "max_ctx must be in [1, 32768]");
     WLK_CHECK((size_t)(D.vocab + 31) / 32 * 4 <= 200 * 1024, "vocab too large for the pick kernel's bitmap");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    int ndev = 0;
-    cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the H100 engine has no CPU fallback", cudaGetErrorString(ce));
-    WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
-    CUDA_CHECK(cudaSetDevice(cfg->device));
-    cudaDeviceProp prop;
-    CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    const int num_sms = open_sm90_device(cfg->device);
 
     auto* t = new wlk_qtext();
     t->dims = D; t->cfg = *cfg;
-    t->num_sms = prop.multiProcessorCount;
+    t->num_sms = num_sms;
     t->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     t->gemm_backend = t->act == DT_BF16 ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     CUDA_CHECK(cudaStreamCreateWithFlags(&t->st, cudaStreamNonBlocking));
@@ -633,18 +598,18 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
     const size_t W = (size_t)(H + 2 * KV) * QT_HD;
     size_t* aw = &t->bytes_weights;
-    t->emb = (float*)talloc(t, (size_t)D.vocab * d * 4, aw);
-    t->head = talloc(t, (size_t)D.vocab * d * es, aw);
-    t->normw = (float*)talloc(t, (size_t)d * 4, aw);
-    t->inv_freq = (float*)talloc(t, QT_HD / 2 * 4, aw);
+    t->emb = (float*)t->allocs.take((size_t)D.vocab * d * 4, aw);
+    t->head = t->allocs.take((size_t)D.vocab * d * es, aw);
+    t->normw = (float*)t->allocs.take((size_t)d * 4, aw);
+    t->inv_freq = (float*)t->allocs.take(QT_HD / 2 * 4, aw);
     t->L.resize(D.n_layer);
     for (auto& Lw : t->L) {
-        Lw.Wqkv = talloc(t, W * d * es, aw);
-        Lw.Wo = talloc(t, (size_t)d * H * QT_HD * es, aw);
-        Lw.Wgu = talloc(t, (size_t)2 * F * d * es, aw);
-        Lw.Wd = talloc(t, (size_t)d * F * es, aw);
-        Lw.qn = (float*)talloc(t, QT_HD * 4, aw); Lw.kn = (float*)talloc(t, QT_HD * 4, aw);
-        Lw.ln1 = (float*)talloc(t, (size_t)d * 4, aw); Lw.ln2 = (float*)talloc(t, (size_t)d * 4, aw);
+        Lw.Wqkv = t->allocs.take(W * d * es, aw);
+        Lw.Wo = t->allocs.take((size_t)d * H * QT_HD * es, aw);
+        Lw.Wgu = t->allocs.take((size_t)2 * F * d * es, aw);
+        Lw.Wd = t->allocs.take((size_t)d * F * es, aw);
+        Lw.qn = (float*)t->allocs.take(QT_HD * 4, aw); Lw.kn = (float*)t->allocs.take(QT_HD * 4, aw);
+        Lw.ln1 = (float*)t->allocs.take((size_t)d * 4, aw); Lw.ln2 = (float*)t->allocs.take((size_t)d * 4, aw);
     }
     {   // default inv_freq = 1 / theta^(2i / 128) in fp32 arithmetic like HF's default rope init (fp32 exponent, pow, then
         // 1 / x); libm's powf can still land one ulp away from torch's pow in a few entries, so hosts load
@@ -655,31 +620,30 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     }
     const size_t R = QT_ROUND_ROWS;
     size_t* ws = &t->bytes_workspace;
-    t->x = (float*)talloc(t, R * d * 4, ws);
-    t->xn = talloc(t, R * d * es, ws);
-    t->qkv = (float*)talloc(t, R * W * 4, ws);
-    t->qb = talloc(t, R * H * QT_HD * es, ws);
-    t->att = talloc(t, R * H * QT_HD * es, ws);
-    t->gu = (float*)talloc(t, R * 2 * F * 4, ws);
-    t->hid = talloc(t, R * F * es, ws);
+    t->x = (float*)t->allocs.take(R * d * 4, ws);
+    t->xn = t->allocs.take(R * d * es, ws);
+    t->qkv = (float*)t->allocs.take(R * W * 4, ws);
+    t->qb = t->allocs.take(R * H * QT_HD * es, ws);
+    t->att = t->allocs.take(R * H * QT_HD * es, ws);
+    t->gu = (float*)t->allocs.take(R * 2 * F * 4, ws);
+    t->hid = t->allocs.take(R * F * es, ws);
     t->up_rows = (int)R;
-    t->up = (float*)talloc(t, R * d * 4, ws);
+    t->up = (float*)t->allocs.take(R * d * 4, ws);
     t->logit_cap = cfg->max_batch * 288;
-    t->hlog = talloc(t, (size_t)t->logit_cap * d * es, ws);
+    t->hlog = t->allocs.take((size_t)t->logit_cap * d * es, ws);
     t->logit_group = (int)std::max<size_t>(1, std::min<size_t>((size_t)t->logit_cap, QT_LOGIT_BYTES / ((size_t)D.vocab * 4)));
-    t->logits = (float*)talloc(t, (size_t)t->logit_group * D.vocab * 4, ws);
-    t->picks_d = (int32_t*)talloc(t, (size_t)t->logit_cap * 4, ws);
-    t->values_d = (float*)talloc(t, (size_t)t->logit_cap * 4, ws);
+    t->logits = (float*)t->allocs.take((size_t)t->logit_group * D.vocab * 4, ws);
+    t->picks_d = (int32_t*)t->allocs.take((size_t)t->logit_cap * 4, ws);
+    t->values_d = (float*)t->allocs.take((size_t)t->logit_cap * 4, ws);
     if (t->gemm_backend == WLK_BACKEND_TCGEN05) {
-        t->sk_scratch = (float*)talloc(t, SK_SCRATCH_FLOATS * 4, ws);
-        t->sk_counters = (int*)talloc(t, SK_MAX_TILES * 4, ws);
-        CUDA_CHECK(cudaMemset(t->sk_counters, 0, SK_MAX_TILES * 4));
+        t->sk_scratch = (float*)t->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
+        t->sk_counters = (int*)t->allocs.take(SK_MAX_TILES * 4, ws);
     }
     t->stg_bytes = R * 32 + (size_t)cfg->max_batch * 16 + 8192;
     CUDA_CHECK(cudaMallocHost(&t->stg_h, t->stg_bytes));
     CUDA_CHECK(cudaMallocHost(&t->up_h, R * d * 4));
     CUDA_CHECK(cudaEventCreateWithFlags(&t->stg_ev, cudaEventDisableTiming));
-    t->stg_d = (uint8_t*)talloc(t, t->stg_bytes, ws);
+    t->stg_d = (uint8_t*)t->allocs.take(t->stg_bytes, ws);
     t->kv_bytes = (size_t)D.n_layer * 2 * KV * D.max_ctx * QT_HD * es;
     t->sess.resize(cfg->max_sessions);
     CUDA_CHECK(cudaFuncSetAttribute(qt_pick_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -689,8 +653,8 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
 void destroy(wlk_qtext* t) {
     cudaStreamSynchronize(t->st);
     for (auto& s : t->sess) if (s.kv) cudaFree(s.kv);
-    for (void* p : t->allocs) cudaFree(p);
-    if (t->stage_f32) cudaFree(t->stage_f32);
+    t->allocs.free_all();
+    t->upload.release();
     if (t->stg_h) cudaFreeHost(t->stg_h);
     if (t->up_h) cudaFreeHost(t->up_h);
     if (t->pick_d) cudaFree(t->pick_d);
@@ -1076,22 +1040,6 @@ void adapt(wlk_qtext* t, const float* in, int rows, int64_t in_ld, float* out, i
 
 }  // namespace
 
-#define WLK_API_BEGIN try {
-#define WLK_API_END                                              \
-    return 0;                                                    \
-    } catch (const wlk::Error& err) {                            \
-        wlk::set_last_error(err.msg);                            \
-        return 1;                                                \
-    } catch (const std::exception& ex) {                         \
-        wlk::set_last_error(std::string("exception: ") + ex.what()); \
-        return 2;                                                \
-    } catch (...) {                                              \
-        wlk::set_last_error("unknown exception");                \
-        return 3;                                                \
-    }
-#define TLOCK(t) WLK_CHECK((t) != nullptr, "null engine"); std::lock_guard<std::mutex> _lk((t)->mu); \
-                 CUDA_CHECK(cudaSetDevice((t)->cfg.device))
-
 extern "C" {
 
 int wlk_qtext_create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) {
@@ -1108,26 +1056,23 @@ int wlk_qtext_destroy(wlk_qtext* t) {
 }
 int wlk_qtext_load_tensor(wlk_qtext* t, const char* name, const float* host, const int64_t* shape, int ndim) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
     load_tensor(t, name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_qtext_finalize_weights(wlk_qtext* t) {
     WLK_API_BEGIN
-    TLOCK(t);
-    std::string missing;
-    int nmiss = 0;
-    for (auto& r : required(t->dims)) if (!t->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
-    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    WLK_ENTER(t, t->cfg.device);
+    require_loaded(t->loaded, required(t->dims));
     build_adapter(t);
-    if (t->stage_f32) { CUDA_CHECK(cudaFree(t->stage_f32)); t->stage_f32 = nullptr; t->stage_cap = 0; }
+    t->upload.release();
     t->finalized = true;
     WLK_API_END
 }
 int wlk_qtext_memory(wlk_qtext* t, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     if (weights) *weights = t->bytes_weights;
     if (sessions) *sessions = t->bytes_sessions;
     if (workspace) *workspace = t->bytes_workspace;
@@ -1135,7 +1080,7 @@ int wlk_qtext_memory(wlk_qtext* t, size_t* weights, size_t* sessions, size_t* wo
 }
 int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(sid, "null out pointer");
     int found = -1;
     for (int i = 0; i < (int)t->sess.size(); ++i) if (!t->sess[i].open) { found = i; break; }
@@ -1149,7 +1094,7 @@ int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid) {
 }
 int wlk_qtext_session_close(wlk_qtext* t, int32_t sid) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     QTSession& s = tsession(t, sid);
     CUDA_CHECK(cudaStreamSynchronize(t->st));
     cudaFree(s.kv);
@@ -1159,20 +1104,20 @@ int wlk_qtext_session_close(wlk_qtext* t, int32_t sid) {
 }
 int wlk_qtext_session_reset(wlk_qtext* t, int32_t sid) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     tsession(t, sid).len = 0;
     WLK_API_END
 }
 int wlk_qtext_session_len(wlk_qtext* t, int32_t sid, int32_t* len) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(len, "null out pointer");
     *len = tsession(t, sid).len;
     WLK_API_END
 }
 int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     QTSession& s = tsession(t, sid);
     WLK_CHECK(len >= 0 && len <= s.len, "crop to %d outside [0, %d]", len, s.len);
     s.len = len;
@@ -1181,7 +1126,7 @@ int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len) {
 int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
                       const float* embeds_host, int32_t n_embeds, const int32_t* logit_rows) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(sids && row_src && row_offsets && logit_rows && (embeds_host || n_embeds == 0), "null argument");
     forward(t, sids, n, row_src, row_offsets, embeds_host, n_embeds, logit_rows);
     WLK_API_END
@@ -1189,7 +1134,7 @@ int wlk_qtext_forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* r
 int wlk_qtext_forward_device(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_offsets,
                              const float* embeds_dev, int64_t embeds_ld, int32_t n_embeds, const int32_t* logit_rows) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(sids && row_src && row_offsets && logit_rows && (embeds_dev || n_embeds == 0), "null argument");
     WLK_CHECK(embeds_ld >= t->dims.d_model, "embeds_ld %lld < d_model %d", (long long)embeds_ld, t->dims.d_model);
     forward(t, sids, n, row_src, row_offsets, embeds_dev, n_embeds, logit_rows, embeds_ld);
@@ -1197,13 +1142,13 @@ int wlk_qtext_forward_device(wlk_qtext* t, const int32_t* sids, int n, const int
 }
 int wlk_qtext_adapt(wlk_qtext* t, const float* in_dev, int32_t rows, int64_t in_ld, float* out_dev, int64_t out_ld) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     adapt(t, in_dev, rows, in_ld, out_dev, out_ld);
     WLK_API_END
 }
 int wlk_qtext_adapter_dims(wlk_qtext* t, int32_t* in_dim, int32_t* n_blocks, int32_t* hidden) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     if (in_dim) *in_dim = t->has_adapter ? t->ad.in_dim : 0;
     if (n_blocks) *n_blocks = t->ad.nb;
     if (hidden) *hidden = t->ad.hidden;
@@ -1214,7 +1159,7 @@ int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_toke
                    int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id, int32_t* picks_out,
                    float* value_out) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(hist_off && hist_len && picks_out && (hist_tokens || n_hist_tokens == 0) && (suppress || n_suppress == 0), "null argument");
     pick(t, hist_tokens, n_hist_tokens, hist_off, hist_len, suppress, n_suppress, repetition_penalty, no_repeat_ngram_size,
          max_consecutive, wait_token_id, picks_out, value_out);
@@ -1222,14 +1167,14 @@ int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_toke
 }
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(out_host || n_rows == 0, "null output buffer");
     logits_out(t, row0, n_rows, out_host);
     WLK_API_END
 }
 int wlk_qtext_op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int32_t rows, const int32_t* out_row_host) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     op_rmsnorm(t, x, w, out, rows, out_row_host);
     WLK_API_END
 }
@@ -1237,20 +1182,20 @@ int wlk_qtext_op_qk_rope(wlk_qtext* t, const float* qkv, const float* q_norm_w, 
                          const int32_t* row_slot_host, int32_t rows, void* const* kv_ptrs_host, int32_t n_slots, int32_t layer,
                          void* q_out) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     op_qk_rope(t, qkv, q_norm_w, k_norm_w, row_pos_host, row_slot_host, rows, kv_ptrs_host, n_slots, layer, q_out);
     WLK_API_END
 }
 int wlk_qtext_op_attention(wlk_qtext* t, const void* q, const int32_t* row_pos_host, const int32_t* row_slot_host, int32_t rows,
                            void* const* kv_ptrs_host, int32_t n_slots, int32_t layer, void* out) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     op_attention(t, q, row_pos_host, row_slot_host, rows, kv_ptrs_host, n_slots, layer, out);
     WLK_API_END
 }
 int wlk_qtext_op_swiglu(wlk_qtext* t, const float* gu, void* hid, int32_t rows) {
     WLK_API_BEGIN
-    TLOCK(t);
+    WLK_ENTER(t, t->cfg.device);
     op_swiglu(t, gu, hid, rows);
     WLK_API_END
 }

@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "../../include/wlk_b200.h"
+#include "host.cuh"
 #include "kernels.cuh"
 
 namespace wlk {
@@ -706,7 +707,7 @@ struct wlk_sf {
     int max_T = 0, max_T3 = 0, max_feat = 0, max_pop = 0, max_chunk_cap = 0;
     cudaStream_t st = nullptr;
     std::mutex mu;
-    std::vector<void*> allocs;
+    DeviceAllocs allocs;
     size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
     // front end + conv stem
     float *window = nullptr, *fbT = nullptr; float2* twiddle = nullptr; int2* span = nullptr;
@@ -718,7 +719,7 @@ struct wlk_sf {
     float* pe_table = nullptr;          // [2 SF_MAX_T - 1][D] RelPositionalEncoding rows, fp32 (input of the per-layer tables)
     std::set<std::string> loaded;
     bool finalized = false;
-    float* stage_f32 = nullptr; size_t stage_cap = 0;
+    WeightUpload upload;
     std::vector<SfSession> sess;
     // workspaces
     float *pcm = nullptr, *feats = nullptr, *chunk = nullptr, *x = nullptr, *y = nullptr, *preds = nullptr, *out_preds = nullptr;
@@ -730,16 +731,6 @@ struct wlk_sf {
 };
 
 namespace {
-
-void* sfalloc(wlk_sf* q, size_t bytes, size_t* acct) {
-    void* p = nullptr;
-    if (bytes == 0) bytes = 16;
-    CUDA_CHECK(cudaMalloc(&p, bytes));
-    CUDA_CHECK(cudaMemset(p, 0, bytes));
-    q->allocs.push_back(p);
-    if (acct) *acct += bytes;
-    return p;
-}
 
 void sfgemm(wlk_sf* q, GemmArgs& g) {
     if (g.M <= 0) return;
@@ -759,20 +750,6 @@ void gemm(wlk_sf* q, const void* A, int64_t lda, const void* W, int64_t ldw, int
     sfgemm(q, g);
 }
 
-void put(wlk_sf* q, const float* host, size_t n, void* dst, int dst_type) {
-    if (n > q->stage_cap) {
-        if (q->stage_f32) { CUDA_CHECK(cudaStreamSynchronize(q->st)); CUDA_CHECK(cudaFree(q->stage_f32)); }
-        CUDA_CHECK(cudaMalloc(&q->stage_f32, n * 4));
-        q->stage_cap = n;
-    }
-    CUDA_CHECK(cudaMemcpyAsync(q->stage_f32, host, n * 4, cudaMemcpyHostToDevice, q->st));
-    if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, q->stage_f32, n * 4, cudaMemcpyDeviceToDevice, q->st));
-    else convert_f32_to(q->stage_f32, dst, dst_type, (int64_t)n, q->st);
-    CUDA_CHECK(cudaStreamSynchronize(q->st));
-}
-
-int64_t numel(const int64_t* shape, int ndim) { int64_t n = 1; for (int i = 0; i < ndim; ++i) n *= shape[i]; return n; }
-
 void expect(const std::string& name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
     int64_t nw = 1, ns = numel(shape, ndim);
     for (int64_t w : want) nw *= w;
@@ -787,8 +764,8 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
     const wlk_sf_dims& D = q->dims;
     const int C = D.conv_channels, d = D.d_model, t = D.tf_d_model, ff = D.ff_mult * D.d_model, K = D.conv_kernel;
     const int64_t n = numel(shape, ndim);
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name, shape, ndim, {rows, cols}); put(q, host, n, dst, q->act); };
-    auto vec = [&](float* dst, int64_t len) { expect(name, shape, ndim, {len}); put(q, host, n, dst, DT_F32); };
+    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name, shape, ndim, {rows, cols}); q->upload.put(host, n, dst, q->act, q->st); };
+    auto vec = [&](float* dst, int64_t len) { expect(name, shape, ndim, {len}); q->upload.put(host, n, dst, DT_F32, q->st); };
     const std::string pe = "encoder.pre_encode.";
     if (name == "mel_filters") {                    // [n_mels][n_freq] Slaney bank (librosa.filters.mel, as NeMo builds it)
         expect(name, shape, ndim, {D.n_mels, q->n_freq});
@@ -804,17 +781,17 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
             if (lo >= hi) { lo = 0; hi = 0; }
             span[m] = make_int2(lo, hi);
         }
-        put(q, tr.data(), n, q->fbT, DT_F32);
+        q->upload.put(tr.data(), n, q->fbT, DT_F32, q->st);
         CUDA_CHECK(cudaMemcpyAsync(q->span, span.data(), span.size() * 8, cudaMemcpyHostToDevice, q->st));
         CUDA_CHECK(cudaStreamSynchronize(q->st));
     }
-    else if (name == pe + "conv.0.weight") { expect(name, shape, ndim, {C, 9}); put(q, host, n, q->c0w, DT_F32); }
+    else if (name == pe + "conv.0.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->c0w, DT_F32, q->st); }
     else if (name == pe + "conv.0.bias") vec(q->c0b, C);
-    else if (name == pe + "conv.2.weight") { expect(name, shape, ndim, {C, 9}); put(q, host, n, q->dw1w, DT_F32); }
+    else if (name == pe + "conv.2.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->dw1w, DT_F32, q->st); }
     else if (name == pe + "conv.2.bias") vec(q->dw1b, C);
     else if (name == pe + "conv.3.weight") mat(q->Wpw1, C, C);
     else if (name == pe + "conv.3.bias") vec(q->pw1b, C);
-    else if (name == pe + "conv.5.weight") { expect(name, shape, ndim, {C, 9}); put(q, host, n, q->dw2w, DT_F32); }
+    else if (name == pe + "conv.5.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->dw2w, DT_F32, q->st); }
     else if (name == pe + "conv.5.bias") vec(q->dw2b, C);
     else if (name == pe + "conv.6.weight") mat(q->Wpw2, C, C);
     else if (name == pe + "conv.6.bias") vec(q->pw2b, C);
@@ -827,7 +804,7 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
             for (int c = 0; c < C; ++c)
                 for (int f = 0; f < F; ++f)
                     packed[(size_t)o * C * F + (size_t)f * C + c] = host[(size_t)o * C * F + (size_t)c * F + f];
-        put(q, packed.data(), n, q->Wout, q->act);
+        q->upload.put(packed.data(), n, q->Wout, q->act, q->st);
     }
     else if (name == pe + "out.bias") vec(q->outb, d);
     else if (name.rfind("encoder.layers.", 0) == 0) {
@@ -839,8 +816,8 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
         SfLayerW& L = q->L[li];
         const size_t es = q->es();
         auto part = [&](int which, bool w) {
-            if (w) { expect(name, shape, ndim, {d, d}); put(q, host, n, (char*)L.Wqkv + (size_t)which * d * d * es, q->act); }
-            else { expect(name, shape, ndim, {d}); put(q, host, n, L.bqkv + (size_t)which * d, DT_F32); }
+            if (w) { expect(name, shape, ndim, {d, d}); q->upload.put(host, n, (char*)L.Wqkv + (size_t)which * d * d * es, q->act, q->st); }
+            else { expect(name, shape, ndim, {d}); q->upload.put(host, n, L.bqkv + (size_t)which * d, DT_F32, q->st); }
         };
         if (r == "norm_feed_forward1.weight") vec(L.ln_ff1w, d); else if (r == "norm_feed_forward1.bias") vec(L.ln_ff1b, d);
         else if (r == "feed_forward1.linear1.weight") mat(L.W_ff1a, ff, d); else if (r == "feed_forward1.linear1.bias") vec(L.b_ff1a, ff);
@@ -851,11 +828,11 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
         else if (r == "self_attn.linear_v.weight") part(2, true); else if (r == "self_attn.linear_v.bias") part(2, false);
         else if (r == "self_attn.linear_out.weight") mat(L.Wo, d, d); else if (r == "self_attn.linear_out.bias") vec(L.bo, d);
         else if (r == "self_attn.linear_pos.weight") mat(L.Wpos, d, d);
-        else if (r == "self_attn.pos_bias_u") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); put(q, host, n, L.bias_u, DT_F32); }
-        else if (r == "self_attn.pos_bias_v") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); put(q, host, n, L.bias_v, DT_F32); }
+        else if (r == "self_attn.pos_bias_u") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); q->upload.put(host, n, L.bias_u, DT_F32, q->st); }
+        else if (r == "self_attn.pos_bias_v") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); q->upload.put(host, n, L.bias_v, DT_F32, q->st); }
         else if (r == "norm_conv.weight") vec(L.ln_convw, d); else if (r == "norm_conv.bias") vec(L.ln_convb, d);
         else if (r == "conv.pointwise_conv1.weight") mat(L.Wpw1, 2 * d, d); else if (r == "conv.pointwise_conv1.bias") vec(L.bpw1, 2 * d);
-        else if (r == "conv.depthwise_conv.weight") { expect(name, shape, ndim, {d, K}); put(q, host, n, L.dw_w, DT_F32); }
+        else if (r == "conv.depthwise_conv.weight") { expect(name, shape, ndim, {d, K}); q->upload.put(host, n, L.dw_w, DT_F32, q->st); }
         else if (r == "conv.depthwise_conv.bias") vec(L.dw_b, d);
         else if (r == "conv.batch_norm.weight") vec(L.bn_w, d); else if (r == "conv.batch_norm.bias") vec(L.bn_b, d);
         else if (r == "conv.batch_norm.running_mean") vec(L.bn_mean, d); else if (r == "conv.batch_norm.running_var") vec(L.bn_var, d);
@@ -876,8 +853,8 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
         SfTLayerW& L = q->TL[li];
         const size_t es = q->es();
         auto part = [&](int which, bool w) {
-            if (w) { expect(name, shape, ndim, {t, t}); put(q, host, n, (char*)L.Wqkv + (size_t)which * t * t * es, q->act); }
-            else { expect(name, shape, ndim, {t}); put(q, host, n, L.bqkv + (size_t)which * t, DT_F32); }
+            if (w) { expect(name, shape, ndim, {t, t}); q->upload.put(host, n, (char*)L.Wqkv + (size_t)which * t * t * es, q->act, q->st); }
+            else { expect(name, shape, ndim, {t}); q->upload.put(host, n, L.bqkv + (size_t)which * t, DT_F32, q->st); }
         };
         if (r == "first_sub_layer.query_net.weight") part(0, true); else if (r == "first_sub_layer.query_net.bias") part(0, false);
         else if (r == "first_sub_layer.key_net.weight") part(1, true); else if (r == "first_sub_layer.key_net.bias") part(1, false);
@@ -893,7 +870,7 @@ void load_tensor(wlk_sf* q, const std::string& name, const float* host, const in
     else if (name == "sortformer_modules.encoder_proj.bias") vec(q->bproj, t);
     else if (name == "sortformer_modules.first_hidden_to_hidden.weight") mat(q->Wh, t, t);
     else if (name == "sortformer_modules.first_hidden_to_hidden.bias") vec(q->bh, t);
-    else if (name == "sortformer_modules.single_hidden_to_spks.weight") { expect(name, shape, ndim, {D.n_spk, t}); put(q, host, n, q->Wspk, DT_F32); }
+    else if (name == "sortformer_modules.single_hidden_to_spks.weight") { expect(name, shape, ndim, {D.n_spk, t}); q->upload.put(host, n, q->Wspk, DT_F32, q->st); }
     else if (name == "sortformer_modules.single_hidden_to_spks.bias") vec(q->bspk, D.n_spk);
     else WLK_CHECK(false, "unknown tensor %s", name.c_str());
     q->loaded.insert(name);
@@ -925,10 +902,7 @@ std::vector<std::string> required(const wlk_sf_dims& D) {
 
 void finalize(wlk_sf* q) {
     const wlk_sf_dims& D = q->dims;
-    std::string missing;
-    int nmiss = 0;
-    for (auto& r : required(D)) if (!q->loaded.count(r)) { if (nmiss++ < 5) missing += r + " "; }
-    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    require_loaded(q->loaded, required(D));
     const int d = D.d_model, P = 2 * SF_MAX_T - 1;
     // RelPositionalEncoding rows for relative positions SF_MAX_T-1 ... -(SF_MAX_T-1); a row depends on its relative
     // position only, so one table serves every sequence length.  linear_pos of it is a constant per layer.
@@ -941,7 +915,7 @@ void finalize(wlk_sf* q) {
             pe[(size_t)r * d + i + 1] = (float)cos(pos * div);
         }
     }
-    put(q, pe.data(), pe.size(), q->pe_table, DT_F32);
+    q->upload.put(pe.data(), pe.size(), q->pe_table, DT_F32, q->st);
     void* pe_act = q->pe_table;
     void* tmp = nullptr;
     if (q->act != DT_F32) {
@@ -956,7 +930,7 @@ void finalize(wlk_sf* q) {
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     if (tmp) cudaFree(tmp);
-    if (q->stage_f32) { CUDA_CHECK(cudaFree(q->stage_f32)); q->stage_f32 = nullptr; q->stage_cap = 0; }
+    q->upload.release();
     q->finalized = true;
 }
 
@@ -974,18 +948,11 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     WLK_CHECK(D.n_spk >= 1 && D.n_spk <= 8, "n_spk must be in [1, 8]");
     WLK_CHECK(D.spkcache_len >= D.n_spk * (1 + D.spkcache_sil_frames_per_spk), "speaker cache too short for n_spk");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    int ndev = 0;
-    cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the engine has no CPU fallback", cudaGetErrorString(ce));
-    WLK_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d devices)", cfg->device, ndev);
-    CUDA_CHECK(cudaSetDevice(cfg->device));
-    cudaDeviceProp prop;
-    CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    WLK_CHECK(prop.major == 9 && prop.minor == 0, "this library contains sm_90a code only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    const int num_sms = open_sm90_device(cfg->device);
 
     auto* q = new wlk_sf();
     q->dims = D; q->cfg = *cfg;
-    q->num_sms = prop.multiProcessorCount;
+    q->num_sms = num_sms;
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     q->n_freq = D.n_fft / 2 + 1;
@@ -1008,35 +975,35 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     const size_t es = q->es();
     const int C = D.conv_channels, d = D.d_model, t = D.tf_d_model, ff = D.ff_mult * d, K = D.conv_kernel, S = D.n_spk;
     size_t* aw = &q->bytes_weights;
-    auto fv = [&](size_t n) { return (float*)sfalloc(q, n * 4, aw); };
-    q->window = fv(D.win_length); q->twiddle = (float2*)sfalloc(q, (size_t)D.n_fft * 8, aw);
-    q->fbT = fv((size_t)q->n_freq * D.n_mels); q->span = (int2*)sfalloc(q, (size_t)D.n_mels * 8, aw);
+    auto fv = [&](size_t n) { return (float*)q->allocs.take(n * 4, aw); };
+    q->window = fv(D.win_length); q->twiddle = (float2*)q->allocs.take((size_t)D.n_fft * 8, aw);
+    q->fbT = fv((size_t)q->n_freq * D.n_mels); q->span = (int2*)q->allocs.take((size_t)D.n_mels * 8, aw);
     q->c0w = fv((size_t)C * 9); q->c0b = fv(C); q->dw1w = fv((size_t)C * 9); q->dw1b = fv(C); q->dw2w = fv((size_t)C * 9); q->dw2b = fv(C);
     q->pw1b = fv(C); q->pw2b = fv(C); q->outb = fv(d);
-    q->Wpw1 = sfalloc(q, (size_t)C * C * es, aw); q->Wpw2 = sfalloc(q, (size_t)C * C * es, aw);
-    q->Wout = sfalloc(q, (size_t)d * C * q->F3 * es, aw);
+    q->Wpw1 = q->allocs.take((size_t)C * C * es, aw); q->Wpw2 = q->allocs.take((size_t)C * C * es, aw);
+    q->Wout = q->allocs.take((size_t)d * C * q->F3 * es, aw);
     q->pe_table = fv((size_t)(2 * SF_MAX_T - 1) * d);
     q->L.resize(D.n_layer);
     for (auto& L : q->L) {
-        L.W_ff1a = sfalloc(q, (size_t)ff * d * es, aw); L.W_ff1b = sfalloc(q, (size_t)ff * d * es, aw);
-        L.W_ff2a = sfalloc(q, (size_t)ff * d * es, aw); L.W_ff2b = sfalloc(q, (size_t)ff * d * es, aw);
-        L.Wqkv = sfalloc(q, (size_t)3 * d * d * es, aw); L.Wo = sfalloc(q, (size_t)d * d * es, aw); L.Wpos = sfalloc(q, (size_t)d * d * es, aw);
-        L.Wpw1 = sfalloc(q, (size_t)2 * d * d * es, aw); L.Wpw2 = sfalloc(q, (size_t)d * d * es, aw);
+        L.W_ff1a = q->allocs.take((size_t)ff * d * es, aw); L.W_ff1b = q->allocs.take((size_t)ff * d * es, aw);
+        L.W_ff2a = q->allocs.take((size_t)ff * d * es, aw); L.W_ff2b = q->allocs.take((size_t)ff * d * es, aw);
+        L.Wqkv = q->allocs.take((size_t)3 * d * d * es, aw); L.Wo = q->allocs.take((size_t)d * d * es, aw); L.Wpos = q->allocs.take((size_t)d * d * es, aw);
+        L.Wpw1 = q->allocs.take((size_t)2 * d * d * es, aw); L.Wpw2 = q->allocs.take((size_t)d * d * es, aw);
         L.b_ff1a = fv(ff); L.b_ff1b = fv(d); L.b_ff2a = fv(ff); L.b_ff2b = fv(d); L.bqkv = fv(3 * d); L.bo = fv(d); L.bpw1 = fv(2 * d); L.bpw2 = fv(d);
         L.ln_ff1w = fv(d); L.ln_ff1b = fv(d); L.ln_attw = fv(d); L.ln_attb = fv(d); L.ln_convw = fv(d); L.ln_convb = fv(d);
         L.ln_ff2w = fv(d); L.ln_ff2b = fv(d); L.ln_outw = fv(d); L.ln_outb = fv(d);
         L.bias_u = fv(d); L.bias_v = fv(d); L.dw_w = fv((size_t)d * K); L.dw_b = fv(d);
         L.bn_w = fv(d); L.bn_b = fv(d); L.bn_mean = fv(d); L.bn_var = fv(d); L.bnA = fv(d); L.bnB = fv(d);
-        L.ptab = sfalloc(q, (size_t)(2 * SF_MAX_T - 1) * d * es, aw);
+        L.ptab = q->allocs.take((size_t)(2 * SF_MAX_T - 1) * d * es, aw);
     }
     q->TL.resize(D.tf_n_layer);
     for (auto& L : q->TL) {
-        L.Wqkv = sfalloc(q, (size_t)3 * t * t * es, aw); L.Wo = sfalloc(q, (size_t)t * t * es, aw);
-        L.W1 = sfalloc(q, (size_t)D.tf_inner * t * es, aw); L.W2 = sfalloc(q, (size_t)D.tf_inner * t * es, aw);
+        L.Wqkv = q->allocs.take((size_t)3 * t * t * es, aw); L.Wo = q->allocs.take((size_t)t * t * es, aw);
+        L.W1 = q->allocs.take((size_t)D.tf_inner * t * es, aw); L.W2 = q->allocs.take((size_t)D.tf_inner * t * es, aw);
         L.bqkv = fv(3 * t); L.bo = fv(t); L.b1 = fv(D.tf_inner); L.b2 = fv(t); L.ln1w = fv(t); L.ln1b = fv(t); L.ln2w = fv(t); L.ln2b = fv(t);
     }
-    q->Wproj = sfalloc(q, (size_t)t * d * es, aw); q->bproj = fv(t);
-    q->Wh = sfalloc(q, (size_t)t * t * es, aw); q->bh = fv(t);
+    q->Wproj = q->allocs.take((size_t)t * d * es, aw); q->bproj = fv(t);
+    q->Wh = q->allocs.take((size_t)t * t * es, aw); q->bh = fv(t);
     q->Wspk = fv((size_t)S * t); q->bspk = fv(S);
     {   // symmetric Hann window (torch.hann_window(periodic=False), as NeMo builds it) and exp(-2 pi i k / n_fft)
         std::vector<float> win(D.win_length);
@@ -1052,29 +1019,29 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     size_t* ws = &q->bytes_workspace;
     const size_t T1 = (q->max_feat - 1) / 2 + 1, T2 = (T1 - 1) / 2 + 1, T3 = (T2 - 1) / 2 + 1;
     const size_t R = B * q->max_T;
-    q->pcm = (float*)sfalloc(q, B * q->chunk_samples * 4, ws);
-    q->feats = (float*)sfalloc(q, B * q->max_feat * D.n_mels * 4, ws);
-    q->a1 = sfalloc(q, B * T1 * q->F1 * C * es, ws);
-    q->a2 = sfalloc(q, B * T2 * q->F2 * C * es, ws); q->a2p = sfalloc(q, B * T2 * q->F2 * C * es, ws);
-    q->a3 = sfalloc(q, B * T3 * q->F3 * C * es, ws); q->a3p = sfalloc(q, B * T3 * q->F3 * C * es, ws);
-    q->chunk = (float*)sfalloc(q, B * T3 * d * 4, ws);
-    q->x = (float*)sfalloc(q, R * d * 4, ws);
-    q->xn = sfalloc(q, R * d * es, ws);
-    q->qkv = sfalloc(q, R * 3 * d * es, ws);
-    q->att = sfalloc(q, R * d * es, ws);
-    q->hid = sfalloc(q, R * (size_t)ff * es, ws);
-    q->cv = sfalloc(q, R * d * es, ws);
-    q->y = (float*)sfalloc(q, R * t * 4, ws);
-    q->preds = (float*)sfalloc(q, R * S * 4, ws);
-    q->out_preds = (float*)sfalloc(q, B * q->max_chunk_cap * S * 4, ws);
+    q->pcm = (float*)q->allocs.take(B * q->chunk_samples * 4, ws);
+    q->feats = (float*)q->allocs.take(B * q->max_feat * D.n_mels * 4, ws);
+    q->a1 = q->allocs.take(B * T1 * q->F1 * C * es, ws);
+    q->a2 = q->allocs.take(B * T2 * q->F2 * C * es, ws); q->a2p = q->allocs.take(B * T2 * q->F2 * C * es, ws);
+    q->a3 = q->allocs.take(B * T3 * q->F3 * C * es, ws); q->a3p = q->allocs.take(B * T3 * q->F3 * C * es, ws);
+    q->chunk = (float*)q->allocs.take(B * T3 * d * 4, ws);
+    q->x = (float*)q->allocs.take(R * d * 4, ws);
+    q->xn = q->allocs.take(R * d * es, ws);
+    q->qkv = q->allocs.take(R * 3 * d * es, ws);
+    q->att = q->allocs.take(R * d * es, ws);
+    q->hid = q->allocs.take(R * (size_t)ff * es, ws);
+    q->cv = q->allocs.take(R * d * es, ws);
+    q->y = (float*)q->allocs.take(R * t * 4, ws);
+    q->preds = (float*)q->allocs.take(R * S * 4, ws);
+    q->out_preds = (float*)q->allocs.take(B * q->max_chunk_cap * S * 4, ws);
     CUDA_CHECK(cudaMallocHost(&q->out_h, B * q->max_chunk_cap * S * 4));
     if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
-        q->sk_scratch = (float*)sfalloc(q, SK_SCRATCH_FLOATS * 4, ws);
-        q->sk_counters = (int*)sfalloc(q, SK_MAX_TILES * 4, ws);
+        q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
+        q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
     }
     q->stg_bytes = B * sizeof(SfJob) + 4096;
     CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
-    q->stg_d = (uint8_t*)sfalloc(q, q->stg_bytes, ws);
+    q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
     q->sess.resize(cfg->max_sessions);
     *out = q;
 }
@@ -1092,8 +1059,8 @@ void free_session(SfSession& s) {
 void destroy(wlk_sf* q) {
     cudaStreamSynchronize(q->st);
     for (auto& s : q->sess) free_session(s);
-    for (void* p : q->allocs) cudaFree(p);
-    if (q->stage_f32) cudaFree(q->stage_f32);
+    q->allocs.free_all();
+    q->upload.release();
     if (q->stg_h) cudaFreeHost(q->stg_h);
     if (q->out_h) cudaFreeHost(q->out_h);
     cudaStreamDestroy(q->st);
@@ -1310,22 +1277,6 @@ void step(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const in
 
 }  // namespace
 
-#define WLK_API_BEGIN try {
-#define WLK_API_END                                              \
-    return 0;                                                    \
-    } catch (const wlk::Error& err) {                            \
-        wlk::set_last_error(err.msg);                            \
-        return 1;                                                \
-    } catch (const std::exception& ex) {                         \
-        wlk::set_last_error(std::string("exception: ") + ex.what()); \
-        return 2;                                                \
-    } catch (...) {                                              \
-        wlk::set_last_error("unknown exception");                \
-        return 3;                                                \
-    }
-#define SFLOCK(q) WLK_CHECK((q) != nullptr, "null engine"); std::lock_guard<std::mutex> _lk((q)->mu); \
-                  CUDA_CHECK(cudaSetDevice((q)->cfg.device))
-
 extern "C" {
 
 int wlk_sf_create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
@@ -1342,20 +1293,20 @@ int wlk_sf_destroy(wlk_sf* q) {
 }
 int wlk_sf_load_tensor(wlk_sf* q, const char* name, const float* host, const int64_t* shape, int ndim) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
     load_tensor(q, name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_sf_finalize_weights(wlk_sf* q) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     finalize(q);
     WLK_API_END
 }
 int wlk_sf_session_open(wlk_sf* q, int32_t* sid) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sid != nullptr, "null argument");
     const wlk_sf_dims& D = q->dims;
     for (size_t i = 0; i < q->sess.size(); ++i) {
@@ -1384,7 +1335,7 @@ int wlk_sf_session_open(wlk_sf* q, int32_t* sid) {
 }
 int wlk_sf_session_close(wlk_sf* q, int32_t sid) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     SfSession& s = session(q, sid);
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     free_session(s);
@@ -1392,7 +1343,7 @@ int wlk_sf_session_close(wlk_sf* q, int32_t sid) {
 }
 int wlk_sf_session_reset(wlk_sf* q, int32_t sid) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     reset_session(q, session(q, sid));
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     WLK_API_END
@@ -1400,7 +1351,7 @@ int wlk_sf_session_reset(wlk_sf* q, int32_t sid) {
 int wlk_sf_step_audio(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const int64_t* sample_offsets,
                       float* chunk_preds_host, int32_t* row_offsets_out) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && pcm_host && sample_offsets, "null argument");
     step(q, sids, n, pcm_host, sample_offsets, nullptr, nullptr, 0, 0, chunk_preds_host, row_offsets_out);
     WLK_API_END
@@ -1408,7 +1359,7 @@ int wlk_sf_step_audio(wlk_sf* q, const int32_t* sids, int n, const float* pcm_ho
 int wlk_sf_step_features(wlk_sf* q, const int32_t* sids, int n, const float* feats_host, const int32_t* frame_offsets,
                          int32_t left_offset, int32_t right_offset, float* chunk_preds_host, int32_t* row_offsets_out) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sids && feats_host && frame_offsets, "null argument");
     WLK_CHECK(left_offset >= 0 && right_offset >= 0, "negative context offset");
     step(q, sids, n, nullptr, nullptr, feats_host, frame_offsets, left_offset, right_offset, chunk_preds_host, row_offsets_out);
@@ -1416,7 +1367,7 @@ int wlk_sf_step_features(wlk_sf* q, const int32_t* sids, int n, const float* fea
 }
 int wlk_sf_total_preds(wlk_sf* q, int32_t sid, const float** preds_dev, int32_t* n_rows) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     SfSession& s = session(q, sid);
     if (preds_dev) *preds_dev = s.total_preds;
     if (n_rows) *n_rows = s.tp_rows;
@@ -1425,7 +1376,7 @@ int wlk_sf_total_preds(wlk_sf* q, int32_t sid, const float** preds_dev, int32_t*
 int wlk_sf_read_state(wlk_sf* q, int32_t sid, int32_t* lengths /*[4]: spkcache, fifo, n_sil, chunk_index*/, float* spkcache_host,
                       float* spkcache_preds_host, float* fifo_host, float* mean_sil_host) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     SfSession& s = session(q, sid);
     const wlk_sf_dims& D = q->dims;
     CUDA_CHECK(cudaStreamSynchronize(q->st));
@@ -1442,7 +1393,7 @@ int wlk_sf_read_state(wlk_sf* q, int32_t sid, int32_t* lengths /*[4]: spkcache, 
 }
 int wlk_sf_memory(wlk_sf* q, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
-    SFLOCK(q);
+    WLK_ENTER(q, q->cfg.device);
     if (weights) *weights = q->bytes_weights;
     if (sessions) *sessions = q->bytes_sessions;
     if (workspace) *workspace = q->bytes_workspace;

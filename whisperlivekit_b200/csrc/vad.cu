@@ -13,9 +13,9 @@
 
 #include "../../include/wlk_b200.h"
 #include "common.cuh"
+#include "host.cuh"
 
 namespace wlk {
-void set_last_error(const std::string& msg);
 namespace {
 
 constexpr int VW = 512, VCTX = 64, VX = VCTX + VW, VPAD = VX + 64;    // 576 samples in, 640 after the reflect pad
@@ -156,7 +156,7 @@ struct wlk_vad {
     cudaStream_t st = nullptr;
     std::mutex mu;
     VadWeights w{};
-    std::vector<void*> allocs;
+    DeviceAllocs allocs;
     std::set<std::string> loaded;
     float* states = nullptr;                 // [max_sessions][VSTATE]
     std::vector<char> open;
@@ -164,13 +164,6 @@ struct wlk_vad {
 };
 
 namespace {
-float* valloc(wlk_vad* v, size_t n) {
-    void* p = nullptr;
-    CUDA_CHECK(cudaMalloc(&p, n * 4));
-    CUDA_CHECK(cudaMemset(p, 0, n * 4));
-    v->allocs.push_back(p);
-    return reinterpret_cast<float*>(p);
-}
 // host [rows][cols] -> device [cols][rows]
 void put_T(wlk_vad* v, float* dst, const float* host, int rows, int cols) {
     std::vector<float> t((size_t)rows * cols);
@@ -192,52 +185,44 @@ const char* kVadTensors[] = {"stft.forward_basis_buffer", "encoder.0.reparam_con
                              "decoder.decoder.2.weight", "decoder.decoder.2.bias"};
 }  // namespace
 
-#define VAD_BEGIN try {
-#define VAD_END return 0; } catch (const wlk::Error& err) { wlk::set_last_error(err.msg); return 1; } \
-    catch (const std::exception& ex) { wlk::set_last_error(std::string("exception: ") + ex.what()); return 2; }
-#define VLOCK(v) WLK_CHECK((v) != nullptr, "null vad"); std::lock_guard<std::mutex> _lk((v)->mu); CUDA_CHECK(cudaSetDevice((v)->device))
-
 extern "C" {
 
 int wlk_vad_create(int device, int max_sessions, wlk_vad** out) {
-    VAD_BEGIN
+    WLK_API_BEGIN
     WLK_CHECK(out && max_sessions >= 1, "bad arguments");
-    int ndev = 0;
-    cudaError_t ce = cudaGetDeviceCount(&ndev);
-    WLK_CHECK(ce == cudaSuccess && ndev > 0, "no CUDA device available (%s): the VAD engine has no CPU fallback", cudaGetErrorString(ce));
-    WLK_CHECK(device >= 0 && device < ndev, "device %d out of range", device);
-    CUDA_CHECK(cudaSetDevice(device));
+    use_device(device);
     auto* v = new wlk_vad();
     v->device = device; v->max_sessions = max_sessions;
     CUDA_CHECK(cudaStreamCreateWithFlags(&v->st, cudaStreamNonBlocking));
     VadWeights& W = v->w;
-    W.basisT = valloc(v, 256 * 258);
-    W.w0T = valloc(v, NB * 3 * 128); W.b0 = valloc(v, 128);
-    W.w1T = valloc(v, 128 * 3 * 64); W.b1 = valloc(v, 64);
-    W.w2T = valloc(v, 64 * 3 * 64); W.b2 = valloc(v, 64);
-    W.w3T = valloc(v, 64 * 3 * 128); W.b3 = valloc(v, 128);
-    W.wihT = valloc(v, 128 * 512); W.whhT = valloc(v, 128 * 512);
-    W.bih = valloc(v, 512); W.bhh = valloc(v, 512);
-    W.wdec = valloc(v, 128); W.bdec = valloc(v, 1);
-    v->states = valloc(v, (size_t)max_sessions * VSTATE);
+    auto fv = [&](size_t n) { return (float*)v->allocs.take(n * 4, nullptr); };
+    W.basisT = fv(256 * 258);
+    W.w0T = fv(NB * 3 * 128); W.b0 = fv(128);
+    W.w1T = fv(128 * 3 * 64); W.b1 = fv(64);
+    W.w2T = fv(64 * 3 * 64); W.b2 = fv(64);
+    W.w3T = fv(64 * 3 * 128); W.b3 = fv(128);
+    W.wihT = fv(128 * 512); W.whhT = fv(128 * 512);
+    W.bih = fv(512); W.bhh = fv(512);
+    W.wdec = fv(128); W.bdec = fv(1);
+    v->states = fv((size_t)max_sessions * VSTATE);
     v->open.assign(max_sessions, 0);
     *out = v;
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_destroy(wlk_vad* v) {
-    VAD_BEGIN
-    WLK_CHECK(v != nullptr, "null vad");
+    WLK_API_BEGIN
+    WLK_CHECK(v != nullptr, "null engine");
     CUDA_CHECK(cudaSetDevice(v->device));
     cudaStreamSynchronize(v->st);
-    for (void* p : v->allocs) cudaFree(p);
+    v->allocs.free_all();
     if (v->stg_h) { cudaFreeHost(v->stg_h); cudaFree(v->stg_d); }
     cudaStreamDestroy(v->st);
     delete v;
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_load_tensor(wlk_vad* v, const char* name, const float* host, int64_t n) {
-    VAD_BEGIN
-    VLOCK(v);
+    WLK_API_BEGIN
+    WLK_ENTER(v, v->device);
     WLK_CHECK(name && host, "null argument");
     std::string s(name);
     if (s.rfind("_model.", 0) == 0) s = s.substr(7);
@@ -261,11 +246,11 @@ int wlk_vad_load_tensor(wlk_vad* v, const char* name, const float* host, int64_t
     else if (s == "decoder.decoder.2.bias") plain(W.bdec, 1);
     else WLK_CHECK(false, "unknown VAD tensor %s", name);
     v->loaded.insert(s);
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_session_open(wlk_vad* v, int32_t* sid) {
-    VAD_BEGIN
-    VLOCK(v);
+    WLK_API_BEGIN
+    WLK_ENTER(v, v->device);
     WLK_CHECK(sid, "null out pointer");
     for (auto t : kVadTensors) WLK_CHECK(v->loaded.count(t), "VAD tensor %s not loaded", t);
     int found = -1;
@@ -274,26 +259,26 @@ int wlk_vad_session_open(wlk_vad* v, int32_t* sid) {
     CUDA_CHECK(cudaMemsetAsync(v->states + (size_t)found * VSTATE, 0, VSTATE * 4, v->st));
     v->open[found] = 1;
     *sid = found;
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_session_reset(wlk_vad* v, int32_t sid) {           /* reset_states(): context, h, c <- 0 */
-    VAD_BEGIN
-    VLOCK(v);
+    WLK_API_BEGIN
+    WLK_ENTER(v, v->device);
     WLK_CHECK(sid >= 0 && sid < v->max_sessions && v->open[sid], "invalid VAD session %d", sid);
     CUDA_CHECK(cudaMemsetAsync(v->states + (size_t)sid * VSTATE, 0, VSTATE * 4, v->st));
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_session_close(wlk_vad* v, int32_t sid) {
-    VAD_BEGIN
-    VLOCK(v);
+    WLK_API_BEGIN
+    WLK_ENTER(v, v->device);
     WLK_CHECK(sid >= 0 && sid < v->max_sessions && v->open[sid], "invalid VAD session %d", sid);
     v->open[sid] = 0;
-    VAD_END
+    WLK_API_END
 }
 int wlk_vad_forward(wlk_vad* v, const int32_t* sids, int n, const float* pcm_host, const int32_t* window_offsets,
                     float* probs_host) {
-    VAD_BEGIN
-    VLOCK(v);
+    WLK_API_BEGIN
+    WLK_ENTER(v, v->device);
     WLK_CHECK(sids && pcm_host && window_offsets && probs_host && n >= 1, "bad arguments");
     WLK_CHECK(window_offsets[0] == 0, "window_offsets must start at 0");
     const int total = window_offsets[n];
@@ -316,7 +301,7 @@ int wlk_vad_forward(wlk_vad* v, const int32_t* sids, int n, const float* pcm_hos
     CUDA_CHECK(cudaMemcpyAsync(v->stg_h + o_prob, v->stg_d + o_prob, (size_t)total * 4, cudaMemcpyDeviceToHost, v->st));
     CUDA_CHECK(cudaStreamSynchronize(v->st));
     memcpy(probs_host, v->stg_h + o_prob, (size_t)total * 4);
-    VAD_END
+    WLK_API_END
 }
 
 }  // extern "C"
