@@ -361,6 +361,20 @@ int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_toke
                    const int32_t* hist_len, const int32_t* suppress, int32_t n_suppress, float repetition_penalty,
                    int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id, int32_t* picks_out,
                    float* value_out);
+/* generate_full_hypothesis_from_cached_audio's cached path (model.py:839-989) for n caller-owned sessions in one call:
+ * each session is reset, forwards its prefix (row_src / row_offsets as wlk_qtext_forward; embeds on the host when
+ * embeds_ld is 0, else device rows embeds_ld floats apart, as wlk_qtext_forward_device) with one logit row, then
+ * decodes greedily with the controls of wlk_qtext_pick over its own generated tokens.  Every step forwards one row per
+ * session still decoding, in session order; a session stops on a stop id or after max_new_tokens picks.  The histories
+ * stay on the device; each step downloads only its picks.  tokens_out [n][max_new_tokens] (row i's first
+ * n_tokens_out[i] entries are set).  Fails before any work on n outside [1, max_batch], a repeated or invalid session, a
+ * row source out of range, max_new_tokens < 0 or a prefix + max_new_tokens past max_ctx.  Every session is reset on
+ * return, whether the call succeeds or fails: its KV is scratch.  No logit rows are kept for wlk_qtext_pick / logits. */
+int wlk_qtext_generate_full(wlk_qtext* t, const int32_t* sids, int32_t n, const int32_t* row_src, const int32_t* row_offsets,
+                            const float* embeds, int64_t embeds_ld, int32_t n_embeds, int32_t max_new_tokens,
+                            const int32_t* stop_ids, int32_t n_stop, const int32_t* suppress, int32_t n_suppress,
+                            float repetition_penalty, int32_t no_repeat_ngram_size, int32_t max_consecutive,
+                            int32_t wait_token_id, int32_t* tokens_out, int32_t* n_tokens_out);
 /* raw lm_head outputs [n_rows][vocab] fp32 of logit rows row0 .. row0 + n_rows of the last forward */
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host);
 /* RoPE frequencies: the optional tensor "rotary_emb.inv_freq" [head_dim / 2] (HF's non-persistent buffer of that name,

@@ -120,6 +120,8 @@ SIGNATURES = {
     "wlk_qtext_adapter_dims": (C.c_int, [_vp, _vp, _vp, _vp]),
     "wlk_qtext_pick": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32,
                                  C.c_int32, _vp, _vp]),
+    "wlk_qtext_generate_full": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp,
+                                          C.c_int32, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "wlk_qtext_logits": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp]),
     "wlk_qtext_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp]),
     "wlk_qtext_op_qk_rope": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),

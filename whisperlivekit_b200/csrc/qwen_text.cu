@@ -40,11 +40,11 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
 }
 
 // x[r] = embed_tokens[src] (src >= 0) or the embedding row up[-1 - src] (rows up_ld floats apart: the uploaded host rows,
-// or the caller's device rows)
-__global__ void qt_embed_kernel(const int32_t* __restrict__ src, const float* __restrict__ emb, const float* __restrict__ up,
-                                int64_t up_ld, float* __restrict__ x, int d) {
+// or the caller's device rows).  With tok set, src[r] indexes it instead: the token a pick left on the device.
+__global__ void qt_embed_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ tok, const float* __restrict__ emb,
+                                const float* __restrict__ up, int64_t up_ld, float* __restrict__ x, int d) {
     const int r = blockIdx.x;
-    const int s = src[r];
+    const int s = tok ? tok[src[r]] : src[r];
     const float* from = s >= 0 ? emb + (int64_t)s * d : up + (int64_t)(-1 - s) * up_ld;
     for (int i = threadIdx.x; i < d; i += blockDim.x) x[(int64_t)r * d + i] = from[i];
 }
@@ -306,6 +306,9 @@ struct PickArgs {
     const int32_t* suppress; int n_suppress;
     float penalty; int penalize; int ngram; int max_consec; int wait_id;
     int32_t* picks; float* values;
+    // device-resident histories (gen != null): row j picks for session row_sess[j], whose history is its first `step`
+    // tokens gen[row_sess[j]][0 .. step); the pick is appended there and left in next[row_sess[j]] for the next forward
+    int32_t* gen; int gen_ld; const int32_t* row_sess; int step; int32_t* next;
 };
 
 // _GreedyControlSession.controlled_logits + argmax (model.py:335-418), one CTA per logit row, in place on the row:
@@ -318,8 +321,15 @@ __global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
     __shared__ int bi[QT_PICK_THREADS / 32];
     const int row = blockIdx.x, tid = threadIdx.x;
     float* lg = a.logits + (int64_t)row * a.ld;
-    const int32_t* h = a.hist + a.hist_off[row];
-    const int n = a.hist_len[row];
+    const int sess = a.gen ? a.row_sess[row] : 0;
+    int32_t* gh = a.gen ? a.gen + (int64_t)sess * a.gen_ld : nullptr;
+    const int32_t* h = a.gen ? gh : a.hist + a.hist_off[row];
+    const int n = a.gen ? a.step : a.hist_len[row];
+    auto emit = [&](int pick, float value) {                          // thread 0, after every read of the history
+        a.picks[row] = pick;
+        if (a.values) a.values[row] = value;
+        if (gh) { gh[a.step] = pick; a.next[sess] = pick; }
+    };
     const int words = (a.vocab + 31) / 32;
     const float fmin = -3.4028234663852886e38f;
     for (int i = tid; i < a.n_suppress; i += blockDim.x) lg[a.suppress[i]] = -INFINITY;
@@ -350,8 +360,7 @@ __global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
         if (tid == 0) {                                               // every other entry is finfo.min
             const float w = lg[a.wait_id];
             const int pick = (w > fmin || a.wait_id == 0) ? a.wait_id : 0;
-            a.picks[row] = pick;
-            if (a.values) a.values[row] = pick == a.wait_id ? w : fmin;
+            emit(pick, pick == a.wait_id ? w : fmin);
         }
         return;
     }
@@ -373,8 +382,7 @@ __global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
         for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
             if (bv[w] > best || (bv[w] == best && bi[w] < besti)) { best = bv[w]; besti = bi[w]; }
         if (besti == 0x7fffffff) besti = 0;                            // NaN row: torch.argmax would say 0 too
-        a.picks[row] = besti;
-        if (a.values) a.values[row] = best;
+        emit(besti, best);
     }
 }
 
@@ -430,6 +438,7 @@ struct wlk_qtext {
     float* up_h = nullptr;                               // pinned: the round's host embedding rows, one H2D copy per round
     cudaEvent_t stg_ev = nullptr;                        // recorded after the last H2D copy out of stg_h / up_h
     int32_t* pick_d = nullptr; size_t pick_cap = 0;      // device copy of a pick call's histories, suppress list, offsets
+    int32_t* gen_d = nullptr; size_t gen_cap = 0;        // generate_full: per-session token histories + next tokens
     int logit_group = 0;
     int up_rows = 0;                                     // rows of `up` (uploaded embedding rows)
     int logit_cap = 0, n_logit = 0;                      // rows of hlog; rows the last forward kept
@@ -658,6 +667,7 @@ void destroy(wlk_qtext* t) {
     if (t->stg_h) cudaFreeHost(t->stg_h);
     if (t->up_h) cudaFreeHost(t->up_h);
     if (t->pick_d) cudaFree(t->pick_d);
+    if (t->gen_d) cudaFree(t->gen_d);
     if (t->stg_ev) cudaEventDestroy(t->stg_ev);
     cudaStreamDestroy(t->st);
     delete t;
@@ -715,11 +725,12 @@ void launch_swiglu(wlk_qtext* t, const float* gu, void* hid, int R, int F) {
 
 template <typename T>
 void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, const int32_t* slot_d, void* const* kv_d,
-               const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles, const float* up, int64_t up_ld) {
+               const int32_t* logit_row_d, const QTAttnTile* tiles_d, int n_tiles, const float* up, int64_t up_ld,
+               const int32_t* tok_d) {
     const wlk_qtext_dims& D = t->dims;
     const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
     const int W = (H + 2 * KV) * QT_HD;
-    qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, t->emb, up, up_ld, t->x, d);
+    qt_embed_kernel<<<R, 256, 0, t->st>>>(src_d, tok_d, t->emb, up, up_ld, t->x, d);
     for (int li = 0; li < D.n_layer; ++li) {
         QTLayerW& Lw = t->L[li];
         launch_rmsnorm<T>(t, t->x, Lw.ln1, t->xn, nullptr, R, D.rms_eps);
@@ -753,9 +764,10 @@ void run_round(wlk_qtext* t, int R, const int32_t* src_d, const int32_t* pos_d, 
 }
 
 // embeds: host rows [n_embeds][d_model] (staged through pinned memory), or, when embeds_ld > 0, device rows embeds_ld
-// floats apart that the embedding gather reads in place.
+// floats apart that the embedding gather reads in place.  With tok_d set, every row_src entry is an index into the
+// device tokens tok_d [n_tok] instead (generate_full's decode steps: the picks never visit the host).
 void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_off, const float* embeds,
-             int n_embeds, const int32_t* logit_rows, int64_t embeds_ld = 0) {
+             int n_embeds, const int32_t* logit_rows, int64_t embeds_ld = 0, const int32_t* tok_d = nullptr, int n_tok = 0) {
     const wlk_qtext_dims& D = t->dims;
     const bool dev_rows = embeds_ld > 0;
     WLK_CHECK(t->finalized, "weights not finalized");
@@ -774,7 +786,8 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
     const int total = row_off[n] - row_off[0];
     for (int r = 0; r < total; ++r) {
         const int s = row_src[row_off[0] + r];
-        WLK_CHECK(s < D.vocab && (s >= 0 || -1 - s < n_embeds), "row %d: source %d is neither a token id nor an embedding row", r, s);
+        if (tok_d) WLK_CHECK(s >= 0 && s < n_tok, "row %d: token index %d outside [0, %d)", r, s, n_tok);
+        else WLK_CHECK(s < D.vocab && (s >= 0 || -1 - s < n_embeds), "row %d: source %d is neither a token id nor an embedding row", r, s);
     }
     // the packed row list: (session index, position, logit row or -1)
     std::vector<int> r_sess(total), r_pos(total), r_log(total);
@@ -806,7 +819,7 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
         for (int k = 0; k < R; ++k) {
             const int r = r0 + k;
             int s = row_src[row_off[0] + r];
-            if (s < 0 && !dev_rows) {
+            if (s < 0 && !dev_rows && !tok_d) {
                 memcpy(t->up_h + (size_t)n_up * D.d_model, embeds + (size_t)(-1 - s) * D.d_model, (size_t)D.d_model * 4);
                 s = -1 - n_up++;
             }
@@ -825,8 +838,8 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
         const QTAttnTile* tiles_d = reinterpret_cast<const QTAttnTile*>(t->stg_d + o_tile);
         const float* up = dev_rows ? embeds : t->up;
         const int64_t up_ld = dev_rows ? embeds_ld : D.d_model;
-        if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld);
-        else run_round<bf16>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld);
+        if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld, tok_d);
+        else run_round<bf16>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld, tok_d);
     }
     // no host sync here: the pick (or logits) call that follows synchronizes once for the whole phase
     for (int i = 0; i < n; ++i) t->sess[sids[i]].len += row_off[i + 1] - row_off[i];
@@ -842,48 +855,157 @@ void head_group(wlk_qtext* t, int row0, int rows) {
     tgemm(t, g);
 }
 
+// The in-vocab part of a suppress list; the reference only arms max-consecutive when the wait token is not suppressed
+// (model.py:1067-1072), so a suppressed wait id becomes -1.
+std::vector<int32_t> pick_suppress(wlk_qtext* t, const int32_t* suppress, int n_suppress, int* wait_id) {
+    std::vector<int32_t> sup;
+    for (int i = 0; i < n_suppress; ++i) if (suppress[i] >= 0 && suppress[i] < t->dims.vocab) sup.push_back(suppress[i]);
+    for (int32_t v : sup) if (v == *wait_id) *wait_id = -1;
+    return sup;
+}
+
+// The pick call's device buffer, grown on demand to `need` int32
+int32_t* pick_buffer(wlk_qtext* t, size_t need) {
+    if (need > t->pick_cap) {
+        CUDA_CHECK(cudaStreamSynchronize(t->st));
+        if (t->pick_d) CUDA_CHECK(cudaFree(t->pick_d));
+        t->pick_d = nullptr;
+        t->pick_cap = std::max(need, (size_t)1 << 16);
+        CUDA_CHECK(cudaMalloc(&t->pick_d, t->pick_cap * 4));
+    }
+    return t->pick_d;
+}
+
+// lm_head + qt_pick_kernel over the N logit rows of the last forward, in groups of rows the logits workspace holds.
+// a: everything but the logits; its per-row arrays (hist_off / hist_len or row_sess, picks, values) start at row 0.
+void launch_picks(wlk_qtext* t, int N, const PickArgs& a) {
+    const wlk_qtext_dims& D = t->dims;
+    const size_t smem = (size_t)(D.vocab + 31) / 32 * 4;
+    for (int g0 = 0; g0 < N; g0 += t->logit_group) {
+        const int rows = std::min(t->logit_group, N - g0);
+        head_group(t, g0, rows);
+        PickArgs b = a;
+        b.logits = t->logits; b.ld = D.vocab; b.vocab = D.vocab;
+        if (b.gen) b.row_sess += g0;
+        else { b.hist_off += g0; b.hist_len += g0; }
+        b.picks += g0;
+        if (b.values) b.values += g0;
+        qt_pick_kernel<<<rows, QT_PICK_THREADS, smem, t->st>>>(b);
+        CUDA_CHECK(cudaGetLastError());
+    }
+}
+
 void pick(wlk_qtext* t, const int32_t* hist, int n_hist, const int32_t* hist_off, const int32_t* hist_len, const int32_t* suppress,
           int n_suppress, float penalty, int ngram, int max_consec, int wait_id, int32_t* picks, float* values) {
-    const wlk_qtext_dims& D = t->dims;
     WLK_CHECK(t->finalized, "weights not finalized");
     const int N = t->n_logit;
     if (N == 0) return;
     for (int j = 0; j < N; ++j)
         WLK_CHECK(hist_off[j] >= 0 && hist_len[j] >= 0 && hist_off[j] + hist_len[j] <= n_hist, "history of row %d out of range", j);
-    std::vector<int32_t> sup;
-    for (int i = 0; i < n_suppress; ++i) if (suppress[i] >= 0 && suppress[i] < D.vocab) sup.push_back(suppress[i]);
-    // the reference only arms max-consecutive when the wait token is not suppressed (model.py:1067-1072)
-    for (int32_t v : sup) if (v == wait_id) wait_id = -1;
-    // one device buffer, grown on demand: [2N offsets/lengths][suppress][histories]
-    const size_t need = (size_t)2 * N + sup.size() + (size_t)n_hist + 1;
-    if (need > t->pick_cap) {
-        CUDA_CHECK(cudaStreamSynchronize(t->st));
-        if (t->pick_d) CUDA_CHECK(cudaFree(t->pick_d));
-        t->pick_cap = std::max(need, (size_t)1 << 16);
-        CUDA_CHECK(cudaMalloc(&t->pick_d, t->pick_cap * 4));
-    }
-    int32_t* meta_d = t->pick_d;
-    int32_t* hist_d = t->pick_d + 2 * N + sup.size();
+    const std::vector<int32_t> sup = pick_suppress(t, suppress, n_suppress, &wait_id);
+    // one device buffer: [2N offsets/lengths][suppress][histories]
+    int32_t* meta_d = pick_buffer(t, (size_t)2 * N + sup.size() + (size_t)n_hist + 1);
+    int32_t* hist_d = meta_d + 2 * N + sup.size();
     if (n_hist) CUDA_CHECK(cudaMemcpyAsync(hist_d, hist, (size_t)n_hist * 4, cudaMemcpyHostToDevice, t->st));
     CUDA_CHECK(cudaMemcpyAsync(meta_d, hist_off, (size_t)N * 4, cudaMemcpyHostToDevice, t->st));
     CUDA_CHECK(cudaMemcpyAsync(meta_d + N, hist_len, (size_t)N * 4, cudaMemcpyHostToDevice, t->st));
     if (!sup.empty()) CUDA_CHECK(cudaMemcpyAsync(meta_d + 2 * N, sup.data(), sup.size() * 4, cudaMemcpyHostToDevice, t->st));
-    const size_t smem = (size_t)(D.vocab + 31) / 32 * 4;
-    for (int g0 = 0; g0 < N; g0 += t->logit_group) {
-        const int rows = std::min(t->logit_group, N - g0);
-        head_group(t, g0, rows);
-        PickArgs a;
-        a.logits = t->logits; a.ld = D.vocab; a.vocab = D.vocab;
-        a.hist = hist_d; a.hist_off = meta_d + g0; a.hist_len = meta_d + N + g0;
-        a.suppress = meta_d + 2 * N; a.n_suppress = (int)sup.size();
-        a.penalty = penalty; a.penalize = penalty != 1.0f && penalty > 0.0f; a.ngram = ngram; a.max_consec = max_consec;
-        a.wait_id = wait_id; a.picks = t->picks_d + g0; a.values = t->values_d + g0;
-        qt_pick_kernel<<<rows, QT_PICK_THREADS, smem, t->st>>>(a);
-        CUDA_CHECK(cudaGetLastError());
-    }
+    PickArgs a{};
+    a.hist = hist_d; a.hist_off = meta_d; a.hist_len = meta_d + N;
+    a.suppress = meta_d + 2 * N; a.n_suppress = (int)sup.size();
+    a.penalty = penalty; a.penalize = penalty != 1.0f && penalty > 0.0f; a.ngram = ngram; a.max_consec = max_consec;
+    a.wait_id = wait_id; a.picks = t->picks_d; a.values = t->values_d;
+    launch_picks(t, N, a);
     CUDA_CHECK(cudaMemcpyAsync(picks, t->picks_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
     if (values) CUDA_CHECK(cudaMemcpyAsync(values, t->values_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
     CUDA_CHECK(cudaStreamSynchronize(t->st));            // the one host sync of a forward + pick phase
+}
+
+// generate_full_hypothesis_from_cached_audio's cached path (model.py:839-989) for n caller-owned sessions at once: each
+// session is reset and forwards its prefix (packed rounds as forward, one logit row per session), then every step
+// forwards one row per session still decoding, in session order, and picks on it.  A session's generated tokens stay in
+// gen_d, where the pick kernel appends each pick and leaves it for the next step's embedding gather, so a step uploads
+// only its round staging and downloads only the picks the stop test needs.  Every session is reset on return.
+void generate_full(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_off,
+                   const float* embeds, int n_embeds, int64_t embeds_ld, int max_new, const int32_t* stop, int n_stop,
+                   const int32_t* suppress, int n_suppress, float penalty, int ngram, int max_consec, int wait_id,
+                   int32_t* tokens_out, int32_t* n_out) {
+    const wlk_qtext_dims& D = t->dims;
+    auto reset = [&] {                                   // every named session that is open, also when the call fails
+        for (int i = 0; i < n; ++i)
+            if (sids[i] >= 0 && sids[i] < (int)t->sess.size() && t->sess[sids[i]].open) t->sess[sids[i]].len = 0;
+        t->n_logit = 0;                                  // no logit rows survive the call
+    };
+    try {
+        WLK_CHECK(t->finalized, "weights not finalized");
+        WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
+        WLK_CHECK(max_new >= 0, "max_new_tokens %d < 0", max_new);
+        for (int i = 0; i < n; ++i) {
+            tsession(t, sids[i]);
+            for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+            const int r = row_off[i + 1] - row_off[i];
+            WLK_CHECK(r >= 1, "session %d has no rows", sids[i]);
+            WLK_CHECK((int64_t)r + max_new <= D.max_ctx, "session %d: prefix %d + max_new_tokens %d exceed max_ctx %d", sids[i], r,
+                      max_new, D.max_ctx);
+        }
+        for (int r = row_off[0]; r < row_off[n]; ++r)
+            WLK_CHECK(row_src[r] < D.vocab && (row_src[r] >= 0 || -1 - row_src[r] < n_embeds),
+                      "row %d: source %d is neither a token id nor an embedding row", r - row_off[0], row_src[r]);
+        reset();
+        for (int i = 0; i < n; ++i) n_out[i] = 0;
+        if (max_new > 0) {
+            const std::vector<int32_t> sup = pick_suppress(t, suppress, n_suppress, &wait_id);
+            const size_t gen_need = (size_t)n * max_new + n;
+            if (gen_need > t->gen_cap) {
+                CUDA_CHECK(cudaStreamSynchronize(t->st));
+                if (t->gen_d) CUDA_CHECK(cudaFree(t->gen_d));
+                t->gen_d = nullptr;
+                t->gen_cap = std::max(gen_need, (size_t)1 << 14);
+                CUDA_CHECK(cudaMalloc(&t->gen_d, t->gen_cap * 4));
+            }
+            int32_t* next_d = t->gen_d + (size_t)n * max_new;
+            // pick buffer: [suppress][row -> session index of the step]
+            int32_t* sup_d = pick_buffer(t, sup.size() + (size_t)n + 1);
+            int32_t* row_sess_d = sup_d + sup.size();
+            if (!sup.empty()) CUDA_CHECK(cudaMemcpyAsync(sup_d, sup.data(), sup.size() * 4, cudaMemcpyHostToDevice, t->st));
+            PickArgs a{};
+            a.suppress = sup_d; a.n_suppress = (int)sup.size();
+            a.penalty = penalty; a.penalize = penalty != 1.0f && penalty > 0.0f; a.ngram = ngram; a.max_consec = max_consec;
+            a.wait_id = wait_id; a.picks = t->picks_d; a.values = nullptr;
+            a.gen = t->gen_d; a.gen_ld = max_new; a.row_sess = row_sess_d; a.next = next_d;
+
+            std::vector<int32_t> live(n), live_sids(n), offs(n + 1), ones(n, 1), picks(n);
+            for (int i = 0; i < n; ++i) { live[i] = i; offs[i] = i; }
+            offs[n] = n;
+            forward(t, sids, n, row_src, row_off, embeds, n_embeds, ones.data(), embeds_ld);
+            for (int step = 0; !live.empty(); ++step) {
+                const int m = (int)live.size();
+                if (step > 0) {
+                    for (int k = 0; k < m; ++k) live_sids[k] = sids[live[k]];
+                    forward(t, live_sids.data(), m, live.data(), offs.data(), nullptr, 0, ones.data(), 0, next_d, n);
+                }
+                CUDA_CHECK(cudaMemcpyAsync(row_sess_d, live.data(), (size_t)m * 4, cudaMemcpyHostToDevice, t->st));
+                a.step = step;
+                launch_picks(t, m, a);
+                CUDA_CHECK(cudaMemcpyAsync(picks.data(), t->picks_d, (size_t)m * 4, cudaMemcpyDeviceToHost, t->st));
+                CUDA_CHECK(cudaStreamSynchronize(t->st));    // the one host sync of a step
+                int kept = 0;
+                for (int k = 0; k < m; ++k) {
+                    const int i = live[k], tok = picks[k];
+                    tokens_out[(size_t)i * max_new + step] = tok;
+                    n_out[i] = step + 1;
+                    bool stopped = step + 1 == max_new;
+                    for (int s = 0; s < n_stop && !stopped; ++s) stopped = stop[s] == tok;
+                    if (!stopped) live[kept++] = i;
+                }
+                live.resize(kept);
+            }
+        }
+    } catch (...) {
+        reset();
+        throw;
+    }
+    reset();
 }
 
 void logits_out(wlk_qtext* t, int row0, int rows, float* out) {
@@ -1163,6 +1285,20 @@ int wlk_qtext_pick(wlk_qtext* t, const int32_t* hist_tokens, int32_t n_hist_toke
     WLK_CHECK(hist_off && hist_len && picks_out && (hist_tokens || n_hist_tokens == 0) && (suppress || n_suppress == 0), "null argument");
     pick(t, hist_tokens, n_hist_tokens, hist_off, hist_len, suppress, n_suppress, repetition_penalty, no_repeat_ngram_size,
          max_consecutive, wait_token_id, picks_out, value_out);
+    WLK_API_END
+}
+int wlk_qtext_generate_full(wlk_qtext* t, const int32_t* sids, int32_t n, const int32_t* row_src, const int32_t* row_offsets,
+                            const float* embeds, int64_t embeds_ld, int32_t n_embeds, int32_t max_new_tokens,
+                            const int32_t* stop_ids, int32_t n_stop, const int32_t* suppress, int32_t n_suppress,
+                            float repetition_penalty, int32_t no_repeat_ngram_size, int32_t max_consecutive,
+                            int32_t wait_token_id, int32_t* tokens_out, int32_t* n_tokens_out) {
+    WLK_API_BEGIN
+    WLK_ENTER(t, t->cfg.device);
+    WLK_CHECK(sids && row_src && row_offsets && (embeds || n_embeds == 0) && (stop_ids || n_stop == 0) &&
+              (suppress || n_suppress == 0) && (tokens_out || max_new_tokens <= 0) && n_tokens_out, "null argument");
+    WLK_CHECK(embeds_ld == 0 || embeds_ld >= t->dims.d_model, "embeds_ld %lld < d_model %d", (long long)embeds_ld, t->dims.d_model);
+    generate_full(t, sids, n, row_src, row_offsets, embeds, n_embeds, embeds_ld, max_new_tokens, stop_ids, n_stop, suppress,
+                  n_suppress, repetition_penalty, no_repeat_ngram_size, max_consecutive, wait_token_id, tokens_out, n_tokens_out);
     WLK_API_END
 }
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host) {

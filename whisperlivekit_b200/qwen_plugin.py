@@ -422,10 +422,12 @@ class B200QwenTextDecoder:
 
     Frame rows cross the seam as the host tensor the reference hands over; only the rows the session has not seen are
     uploaded.  ``use_decoder_kv_cache=False`` takes the same cached path (the reference documents the two as
-    greedy-equal)."""
+    greedy-equal).  The non-rolling generate runs on scratch sessions the decoder keeps open between calls (``close``
+    releases them)."""
 
     def __init__(self, model, engine, dims):
         self.model, self.engine, self.dims = model, engine, dims
+        self._scratch: list = []
 
     @staticmethod
     def dims_of(model, max_ctx: int = 1024):
@@ -497,16 +499,58 @@ class B200QwenTextDecoder:
             t = torch.as_tensor(ids).long()
             return (t if t.ndim == 1 else t[b]).tolist()
 
-        outs = [self.engine.generate_full(fh[b], prefix_token_ids=rows(prefix_token_ids, b),
-                                          audio_placeholder_token_id=audio_placeholder_token_id,
-                                          prompt_token_ids=rows(prompt_token_ids, b), max_new_tokens=max_new_tokens,
-                                          controls=ctl, bos_token_id=self.model.bos_token_id) for b in range(batch)]
+        prefixes = [self.engine.full_prefix(fh[b], prefix_token_ids=rows(prefix_token_ids, b),
+                                            audio_placeholder_token_id=audio_placeholder_token_id,
+                                            prompt_token_ids=rows(prompt_token_ids, b), bos_token_id=self.model.bos_token_id)
+                    for b in range(batch)]
+        live = [b for b in range(batch) if prefixes[b][0].shape[0]]
+        outs = [[] for _ in range(batch)]
+        for b, toks in zip(live, self._generate_full([prefixes[b][1] for b in live], [prefixes[b][0] for b in live],
+                                                     max_new_tokens, ctl)):
+            outs[b] = toks
         # rows that stopped early are filled with the stop-fill id while the others decode (model.py:419-436)
         width = max(len(o) for o in outs)
         if ctl.stop_ids:
             fill = ctl.eos_token_id if ctl.eos_token_id is not None else min(ctl.stop_ids)
             outs = [o + [fill] * (width - len(o)) for o in outs]
         return torch.tensor(outs, dtype=torch.long, device=device).reshape(batch, width)
+
+    def _generate_full(self, frame_rows, srcs, max_new_tokens: int, ctl):
+        """engine.generate_full_batch over the scratch sessions, in waves of the engine's max_batch."""
+        n = len(srcs)
+        if n == 0:
+            return []
+        wave = int(getattr(self.engine, "max_batch", 0) or n)
+        while len(self._scratch) < min(n, wave):
+            self._scratch.append(self.engine.open_session())
+        out = []
+        for a in range(0, n, wave):
+            k = min(wave, n - a)
+            out += self.engine.generate_full_batch(self._scratch[:k], frame_rows[a: a + k], srcs[a: a + k],
+                                                   max_new_tokens=max_new_tokens, controls=ctl)
+        return out
+
+    def generate_full_batch(self, frame_rows, prefix_token_ids, *, audio_placeholder_token_id, max_new_tokens: int = 128,
+                            **controls):
+        """generate_full_hypothesis_from_cached_audio for N streams in one lockstep pass (the windowed tick):
+        frame_rows[i] [steps_i, d] (a CUDA tensor stays on the device), prefix_token_ids[i] the stream's prompt with one
+        audio placeholder per frame row.  controls: the generate method's decode controls plus wait_token_id.  N above
+        the engine's max_batch runs in waves.  Returns the tokens per stream."""
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        controls.setdefault("wait_token_id", self.model.wait_token_id)
+        ctl = self.engine.make_controls(**controls)
+        prefixes = [self.engine.full_prefix(self._rows(f), prefix_token_ids=p,
+                                            audio_placeholder_token_id=audio_placeholder_token_id)
+                    for f, p in zip(frame_rows, prefix_token_ids)]
+        if max_new_tokens == 0:
+            return [[] for _ in prefixes]
+        return self._generate_full([fh for _, fh in prefixes], [src for src, _ in prefixes], max_new_tokens, ctl)
+
+    def close(self) -> None:
+        """Close the scratch sessions of the non-rolling generate."""
+        while self._scratch:
+            self.engine.close_session(self._scratch.pop())
 
     def _rows(self, frame_hidden):
         """CUDA frame rows stay on the device when the engine reads device rows; otherwise they go to the host."""
@@ -581,15 +625,23 @@ def adapter_tensors(adapter) -> dict:
     return sd
 
 
+def _is_window_encoder(encoder) -> bool:
+    """Whether a reference audio encoder is the windowed QwenAudioSurgeryEncoder (model.py:441-608)."""
+    return any(c.__name__ == "QwenAudioSurgeryEncoder" for c in type(encoder).__mro__)
+
+
 class B200QwenRealtimeModel:
-    """The whole realtime model (``Qwen3ASRRealtimeQwenAudioCausalModel``) on the engines, installed on one instance::
+    """The whole realtime model on the engines, installed on one instance::
 
         B200QwenRealtimeModel.install(model, precision="bf16")
 
-    replaces ``model.audio_encoder`` with the tower drop-in, installs the text decoder drop-in with the frame adapter
-    packed into its engine, and rebinds ``append_audio_to_cache`` / ``flush_audio_to_cache`` onto
-    ``qwen_realtime.RealtimeFrames`` (N = 1).  With CUDA engines ``state.frame_hidden`` is a device tensor and the
-    generate methods read it in place: no frame row reaches the host.  The reference streamers
+    Either backend of the reference: the causal ``Qwen3ASRRealtimeQwenAudioCausalModel`` or the windowed
+    ``Qwen3ASRRealtimeQwenAudioSurgeryModel`` (model.py:1421-1509), told apart by ``model.audio_encoder``.  Install
+    replaces ``model.audio_encoder`` with the matching tower drop-in, installs the text decoder drop-in with the frame
+    adapter packed into its engine, and rebinds ``append_audio_to_cache`` onto ``qwen_realtime.RealtimeFrames``
+    (N = 1), plus ``flush_audio_to_cache`` for the causal model only: the windowed model has none, so the streamer's
+    ``flush_pending_audio`` returns None as in the reference.  With CUDA engines ``state.frame_hidden`` is a device
+    tensor and the generate methods read it in place: no frame row reaches the host.  The reference streamers
     (``SegmentedCachedFullHypothesisStreamer``) run over the installed model unchanged."""
 
     def __init__(self, model, encoder, decoder):
@@ -599,11 +651,17 @@ class B200QwenRealtimeModel:
 
     @classmethod
     def install(cls, model, precision: str = "bf16", max_ctx: int = 1024, max_sessions: int = 8, tower_factory=None,
-                text_factory=None):
+                text_factory=None, attention_blocks: Optional[bool] = None):
         """tower_factory(dims, state_dict) / text_factory(dims, state_dict): engines to use instead of the CUDA ones
-        (the CPU oracles in tests)."""
+        (the CPU oracles in tests).  attention_blocks: the windowed tower's, as B200QwenAudioSurgeryEncoder.dims_of."""
         tower_kw = {} if tower_factory else dict(precision=precision, max_sessions=max_sessions)
-        encoder = B200QwenAudioCausalKVEncoder.from_reference(model.audio_encoder, engine_factory=tower_factory, **tower_kw)
+        windowed = _is_window_encoder(model.audio_encoder)
+        if windowed:
+            encoder = B200QwenAudioSurgeryEncoder.from_reference(model.audio_encoder, engine_factory=tower_factory,
+                                                                 attention_blocks=attention_blocks, **tower_kw)
+        else:
+            encoder = B200QwenAudioCausalKVEncoder.from_reference(model.audio_encoder, engine_factory=tower_factory,
+                                                                  **tower_kw)
         if encoder.dims.out_dim != model.adapter.proj.weight.shape[1]:
             raise ValueError(f"tower rows are {encoder.dims.out_dim} wide, the adapter takes "
                              f"{model.adapter.proj.weight.shape[1]}")
@@ -614,7 +672,8 @@ class B200QwenRealtimeModel:
             del model._modules["audio_encoder"]        # an nn.Module takes only modules as child attributes
         model.audio_encoder = encoder
         model.append_audio_to_cache = rt.append_audio_to_cache
-        model.flush_audio_to_cache = rt.flush_audio_to_cache
+        if not windowed:
+            model.flush_audio_to_cache = rt.flush_audio_to_cache
         model.b200_realtime = rt
         return rt
 

@@ -9,6 +9,8 @@ greedy decode controls + argmax (``pick``).  ``TextDecodeDriver`` runs the refer
     first divergence, crop back to the prefix.  N sessions run in lockstep: one forward for every session's block,
     one pick over all verify rows, then one forward + pick per step over the sessions still decoding.
   * ``generate_full``     - generate_full_hypothesis_from_cached_audio (:839-989) on a scratch session.
+  * ``generate_full_batch`` - the same cached path for N caller-owned sessions in lockstep: one forward of every prefix,
+    then one forward + pick per step over the sessions still decoding.  ``generate_full`` is its N = 1 case.
 
 The CPU oracle (oracle/qwen_text_oracle.py) implements the same primitives, so both run the same driver code."""
 from __future__ import annotations
@@ -86,6 +88,10 @@ class TextDecodeDriver:
     def generate_full(self, *args, **kwargs) -> List[int]:
         with self.phase_lock:
             return self._generate_full(*args, **kwargs)
+
+    def generate_full_batch(self, *args, **kwargs) -> List[List[int]]:
+        with self.phase_lock:
+            return self._generate_full_batch(*args, **kwargs)
 
     def make_controls(self, *, eos_token_id=None, stop_token_ids=None, suppress_token_ids=None, repetition_penalty=1.0,
                       no_repeat_ngram_size=0, max_consecutive_text_tokens=0, wait_token_id=None) -> Controls:
@@ -240,16 +246,11 @@ class TextDecodeDriver:
                 "template_tail_tokens")}
         return out_tokens, out_stats, new_states
 
-    # -- generate_full_hypothesis_from_cached_audio (model.py:839-989), cached path, on a scratch session -------------
-    def _generate_full(self, frame_hidden: np.ndarray, *, prefix_token_ids: Optional[Sequence[int]] = None,
-                      audio_placeholder_token_id: Optional[int] = None, prompt_token_ids: Optional[Sequence[int]] = None,
-                      max_new_tokens: int = 128, controls: Optional[Controls] = None, bos_token_id=None,
-                      **control_kwargs) -> List[int]:
-        if max_new_tokens < 0:
-            raise ValueError("max_new_tokens must be >= 0")
-        if max_new_tokens == 0:
-            return []
-        ctl = controls if controls is not None else self.make_controls(**control_kwargs)
+    # -- generate_full_hypothesis_from_cached_audio (model.py:839-989), cached path -----------------------------------
+    def full_prefix(self, frame_hidden, *, prefix_token_ids: Optional[Sequence[int]] = None,
+                    audio_placeholder_token_id: Optional[int] = None, prompt_token_ids: Optional[Sequence[int]] = None,
+                    bos_token_id=None) -> Tuple[np.ndarray, object]:
+        """The cached path's input rows: (row sources int32 — a token id, or -1 - j for frame row j —, the frame rows)."""
         fh = _frame_rows(frame_hidden).reshape(-1, self.dims.d_model)
         if prefix_token_ids is not None:
             if audio_placeholder_token_id is None:
@@ -267,22 +268,70 @@ class TextDecodeDriver:
             prompt = [] if prefix_token_ids is not None else [int(bos_token_id)]
         else:
             prompt = [int(t) for t in prompt_token_ids]
-        src = np.concatenate([src, np.asarray(prompt, np.int32)])
+        return np.concatenate([src, np.asarray(prompt, np.int32)]), fh
+
+    def _generate_full(self, frame_hidden: np.ndarray, *, prefix_token_ids: Optional[Sequence[int]] = None,
+                      audio_placeholder_token_id: Optional[int] = None, prompt_token_ids: Optional[Sequence[int]] = None,
+                      max_new_tokens: int = 128, controls: Optional[Controls] = None, bos_token_id=None,
+                      **control_kwargs) -> List[int]:
+        """One stream on a scratch session: generate_full_batch with N = 1."""
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        if max_new_tokens == 0:
+            return []
+        src, fh = self.full_prefix(frame_hidden, prefix_token_ids=prefix_token_ids,
+                                   audio_placeholder_token_id=audio_placeholder_token_id,
+                                   prompt_token_ids=prompt_token_ids, bos_token_id=bos_token_id)
         if src.shape[0] == 0:
             return []
         sid = self.open_session()
         try:
-            self.forward([sid], [(src, fh)], [1])
-            gen: List[int] = []
-            for step in range(int(max_new_tokens)):
-                tok = int(self._pick_histories([gen], ctl)[0])
-                gen.append(tok)
-                if tok in ctl.stop_ids or step == max_new_tokens - 1:
-                    break
-                self._step([sid], [tok])
-            return gen
+            return self._generate_full_batch([sid], [fh], [src], max_new_tokens=max_new_tokens, controls=controls,
+                                             **control_kwargs)[0]
         finally:
             self.close_session(sid)
+
+    def _generate_full_batch(self, sids: Sequence[int], frame_rows: Sequence, prefixes: Sequence[Sequence[int]], *,
+                             max_new_tokens: int = 128, controls: Optional[Controls] = None,
+                             **control_kwargs) -> List[List[int]]:
+        """The cached path for N caller-owned sessions in lockstep.  Session i is reset and forwards prefixes[i] (row
+        sources: a token id, or -1 - j for row j of frame_rows[i]) with one logit row; each step then forwards one row
+        per session still decoding, in session order, and picks over that session's generated tokens.  A session stops
+        on a stop id or after max_new_tokens picks.  Returns the tokens per session; every session is reset on return."""
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        ctl = controls if controls is not None else self.make_controls(**control_kwargs)
+        n = len(sids)
+        blocks = []
+        for fr, p in zip(frame_rows, prefixes):
+            src = np.asarray(p, np.int32).reshape(-1)
+            if src.shape[0] == 0:
+                raise ValueError("every session needs a non-empty prefix")
+            blocks.append((src, None if fr is None else _frame_rows(fr).reshape(-1, self.dims.d_model)))
+        if len(blocks) != n:
+            raise ValueError("sids, frame_rows and prefixes must have the same length")
+        for sid in sids:
+            self.reset_session(sid)
+        try:
+            gens: List[List[int]] = [[] for _ in range(n)]
+            if max_new_tokens == 0 or n == 0:
+                return gens
+            self.forward(list(sids), blocks, [1] * n)
+            live = list(range(n))
+            while live:
+                picks = self._pick_histories([gens[i] for i in live], ctl)
+                nxt = []
+                for i, tok in zip(live, picks):
+                    gens[i].append(int(tok))
+                    if int(tok) not in ctl.stop_ids and len(gens[i]) < max_new_tokens:
+                        nxt.append(i)
+                live = nxt
+                if live:
+                    self._step([sids[i] for i in live], [gens[i][-1] for i in live])
+            return gens
+        finally:
+            for sid in sids:
+                self.reset_session(sid)
 
 
 class QwenTextEngine(TextDecodeDriver):
@@ -297,6 +346,7 @@ class QwenTextEngine(TextDecodeDriver):
         self.dims = dims
         self.vocab = dims.vocab
         self.precision = precision
+        self.max_batch = max_batch
         cdims = L.wlk_qtext_dims(*dims.as_tuple())
         cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
                            max_sessions=max_sessions, max_batch=max_batch, gemm_backend=L.BACKEND_AUTO,
@@ -349,11 +399,11 @@ class QwenTextEngine(TextDecodeDriver):
     def crop(self, sid: int, length: int) -> None:
         L.check(self.lib.wlk_qtext_crop(self.h, int(sid), int(length)))
 
-    def forward(self, sids: Sequence[int], blocks, logit_rows: Sequence[int]) -> None:
-        """blocks[i] = (row_src int32 [r], embeds [k][d] or None): row_src >= 0 is a token id, -1 - j is embeds row j.
-        Embeddings that are CUDA tensors go through wlk_qtext_forward_device without leaving the GPU."""
+    def _pack(self, blocks):
+        """blocks as forward takes them -> (flat row sources, row offsets, embedding rows, their count, row pitch).
+        Pitch 0: host fp32 rows.  Otherwise one fp32 CUDA tensor the engine reads in place, complete on return."""
         if any(getattr(e, "is_cuda", False) and len(e) for _, e in blocks):
-            return self._forward_device(sids, blocks, logit_rows)
+            return self._pack_device(blocks)
         srcs, embs, offs, base = [], [], [0], 0
         for src, emb in blocks:
             src = np.asarray(src, np.int32).copy()
@@ -364,15 +414,10 @@ class QwenTextEngine(TextDecodeDriver):
                 base += e.shape[0]
             srcs.append(src)
             offs.append(offs[-1] + src.shape[0])
-        flat = np.concatenate(srcs).astype(np.int32)
         emb = np.concatenate(embs) if embs else np.zeros((1, self.dims.d_model), np.float32)
-        ids = np.asarray(list(sids), np.int32)
-        off = np.asarray(offs, np.int32)
-        lr = np.asarray(list(logit_rows), np.int32)
-        L.check(self.lib.wlk_qtext_forward(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off), _ptr(emb), base, _ptr(lr)))
-        self._n_logit = int(lr.sum())
+        return np.concatenate(srcs).astype(np.int32), np.asarray(offs, np.int32), emb, base, 0
 
-    def _forward_device(self, sids, blocks, logit_rows) -> None:
+    def _pack_device(self, blocks):
         import torch
         d = self.dims.d_model
         srcs, parts, offs, base = [], [], [0], 0
@@ -392,14 +437,55 @@ class QwenTextEngine(TextDecodeDriver):
             rows = rows.float().contiguous()
         ld = rows.stride(0) if rows.shape[0] > 1 else d
         torch.cuda.current_stream(rows.device).synchronize()         # the rows are complete before the engine reads them
-        self._dev_rows = rows
-        flat = np.concatenate(srcs).astype(np.int32)
+        return np.concatenate(srcs).astype(np.int32), np.asarray(offs, np.int32), rows, base, int(ld)
+
+    @staticmethod
+    def _rows_ptr(rows, ld):
+        return C.c_void_p(rows.data_ptr()) if ld else _ptr(rows)
+
+    def forward(self, sids: Sequence[int], blocks, logit_rows: Sequence[int]) -> None:
+        """blocks[i] = (row_src int32 [r], embeds [k][d] or None): row_src >= 0 is a token id, -1 - j is embeds row j.
+        Embeddings that are CUDA tensors go through wlk_qtext_forward_device without leaving the GPU."""
+        flat, off, rows, n_rows, ld = self._pack(blocks)
         ids = np.asarray(list(sids), np.int32)
-        off = np.asarray(offs, np.int32)
         lr = np.asarray(list(logit_rows), np.int32)
-        L.check(self.lib.wlk_qtext_forward_device(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off),
-                                                  C.c_void_p(rows.data_ptr()), int(ld), base, _ptr(lr)))
+        if ld:
+            self._dev_rows = rows                    # alive until the pick that follows synchronizes
+            L.check(self.lib.wlk_qtext_forward_device(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off),
+                                                      self._rows_ptr(rows, ld), ld, n_rows, _ptr(lr)))
+        else:
+            L.check(self.lib.wlk_qtext_forward(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(off), _ptr(rows), n_rows,
+                                               _ptr(lr)))
         self._n_logit = int(lr.sum())
+
+    def generate_full_batch(self, sids: Sequence[int], frame_rows: Sequence, prefixes: Sequence[Sequence[int]], *,
+                            max_new_tokens: int = 128, controls: Optional[Controls] = None,
+                            **control_kwargs) -> List[List[int]]:
+        """TextDecodeDriver.generate_full_batch in one engine call (wlk_qtext_generate_full): the decode loop runs in
+        the engine and the generated histories stay on the device.  Same rounds, same tokens.  Invalid input raises
+        WlkError (the engine checks it) and leaves every named session reset."""
+        ctl = controls if controls is not None else self.make_controls(**control_kwargs)
+        n = len(sids)
+        if len(frame_rows) != n or len(prefixes) != n:
+            raise ValueError("sids, frame_rows and prefixes must have the same length")
+        blocks = [(np.asarray(p, np.int32).reshape(-1), fr) for fr, p in zip(frame_rows, prefixes)]
+        for i, (src, fr) in enumerate(blocks):          # the engine sees the rows packed: check each stream's own bound
+            if src.size and int(-1 - src.min()) >= (0 if fr is None else len(fr)):
+                raise ValueError(f"session {i}: frame row {int(-1 - src.min())} past its {0 if fr is None else len(fr)} rows")
+        flat, off, rows, n_rows, ld = (self._pack(blocks) if blocks else       # the engine rejects n = 0
+                                       (np.zeros(1, np.int32), np.zeros(1, np.int32), np.zeros((1, 1), np.float32), 0, 0))
+        ids = np.asarray(list(sids), np.int32)
+        stop = np.asarray(sorted(ctl.stop_ids), np.int32) if ctl.stop_ids else np.zeros(1, np.int32)
+        sup = ctl.suppress if len(ctl.suppress) else np.zeros(1, np.int32)
+        toks = np.zeros((max(n, 1), max(int(max_new_tokens), 1)), np.int32)
+        counts = np.zeros(max(n, 1), np.int32)
+        with self.phase_lock:
+            L.check(self.lib.wlk_qtext_generate_full(
+                self.h, _ptr(ids), n, _ptr(flat), _ptr(off), self._rows_ptr(rows, ld), ld, n_rows, int(max_new_tokens),
+                _ptr(stop), len(ctl.stop_ids), _ptr(sup), len(ctl.suppress), float(ctl.penalty), ctl.ngram,
+                ctl.max_consecutive, ctl.wait_id, _ptr(toks), _ptr(counts)))
+            self._n_logit = 0
+        return [toks[i, :counts[i]].tolist() for i in range(n)]
 
     def adapter_dims(self) -> Tuple[int, int, int]:
         """(in_dim, blocks, hidden width) of the loaded frame adapter; in_dim 0 without one."""
