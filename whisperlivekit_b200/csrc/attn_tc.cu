@@ -45,10 +45,6 @@ __device__ __forceinline__ float fast_exp2(float x) {      // MUFU.EX2, flush-to
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // MODE 0: encoder self-attention, Q/K/V tiles all come out of the fused qkv buffer (tensor map `tm`).
 // MODE 1: decoder cross-attention of a prefill (many query rows per session): Q tiles from the packed
@@ -228,7 +224,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ C
                     const float p0 = sc[8 * k + 2 * e], p1 = sc[8 * k + 2 * e + 1];
                     const __nv_bfloat162 hb = __floats2bfloat162_rn(p0, p1);
                     pa[k][e] = *reinterpret_cast<const uint32_t*>(&hb);
-                    if (X3) pl[k][e] = pack_bf16x2(p0 - __low2float(hb), p1 - __high2float(hb));   // P = hi + lo like every other operand
+                    if (X3) pl[k][e] = ptx::pack_bf16x2(p0 - __low2float(hb), p1 - __high2float(hb));   // P = hi + lo like every other operand
                 }
             }
             ptx::wgmma_fence_regs(o);
@@ -262,7 +258,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ C
         for (int c = 0; c < DH / 8; ++c) {
             const float v0 = o[4 * c + 2 * i] * inv, v1 = o[4 * c + 2 * i + 1] * inv;
             if (X3) *reinterpret_cast<float2*>(reinterpret_cast<float*>(out_ptr) + off + c * 8) = make_float2(v0, v1);
-            else *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(out_ptr) + off + c * 8) = pack_bf16x2(v0, v1);
+            else *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(out_ptr) + off + c * 8) = ptx::pack_bf16x2(v0, v1);
         }
     }
 }

@@ -20,11 +20,6 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
     return 0.5f * x * (1.0f + copysignf(e, x));
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-
 // Fused epilogue of one warpgroup's 64 x BN accumulator, straight from the wgmma fragment: a thread owns, for every
 // 8-column chunk, two adjacent columns of rows g and g + 8 (ptx.cuh), so the four lanes of a quad write one 32-byte
 // (fp32) or 16-byte (bf16) run of a row.  The rows' destination pointers -- including every div/mod of the scatter
@@ -63,7 +58,7 @@ __device__ __forceinline__ void epilogue_fragment_tile(const Epilogue& epi, cons
                 if (ok1 && (reinterpret_cast<uintptr_t>(p) & 7) == 0) *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
                 else { reinterpret_cast<float*>(p)[0] = v0; if (ok1) reinterpret_cast<float*>(p)[1] = v1; }
             } else {
-                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 3) == 0) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(v0, v1);
+                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 3) == 0) *reinterpret_cast<uint32_t*>(p) = ptx::pack_bf16x2(v0, v1);
                 else { reinterpret_cast<bf16*>(p)[0] = __float2bfloat16_rn(v0); if (ok1) reinterpret_cast<bf16*>(p)[1] = __float2bfloat16_rn(v1); }
             }
         }

@@ -1,7 +1,9 @@
 // Thin inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the tensor-core
-// kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors / mma_async / commit / wait.
+// kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors / mma_async / commit / wait; and the warp-level
+// mma.sync m16n8k16 with its bf16 operand packing.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 
 namespace wlk {
@@ -23,6 +25,22 @@ __device__ __forceinline__ bool elect_one() {
         "selp.u32 %0, 1, 0, P;\n\t}"
         : "=r"(pred));
     return pred != 0;
+}
+
+// ---- mma.sync m16n8k16, bf16 inputs, fp32 accumulators (c += a b) -------------------------
+__device__ __forceinline__ void mma_bf16_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// two floats rounded to one bf16x2 register (lo in the low half)
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+// two bf16 values as one bf16x2 register (lo in the low half)
+__device__ __forceinline__ uint32_t pack_bf16_pair(__nv_bfloat16 lo, __nv_bfloat16 hi) {
+    return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
 }
 
 // ---- mbarrier -----------------------------------------------------------------------

@@ -1,18 +1,26 @@
-// Qwen3-ASR causal-KV audio tower (SURVEY.md section 8 row a17) behind the C ABI (wlk_qwen_* in include/wlk_b200.h).
-//   reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/causal.py:
-//     forward_chunk :713-782, _encode_ready_mels :642-681, _conv_one_block :230-248, _position_embedding :204-228,
-//     _attention_chunk :292-376, _layer_chunk :378-421
-// Append-only execution: every mel frame transits the tower exactly once.  Sessions are batched per "round":
-// round r holds the r-th ready block (or run of chunks) of every session in the call, so a block always finds
-// the K/V its predecessor left in the session's ring.
+// Qwen3-ASR audio towers behind the C ABI (wlk_qwen_* in include/wlk_b200.h), in one of two modes per engine:
+//   causal   (wlk_qwen_create, SURVEY.md section 8 row a17): reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/
+//            causal.py: forward_chunk :713-782, _encode_ready_mels :642-681, _conv_one_block :230-248,
+//            _position_embedding :204-228, _attention_chunk :292-376, _layer_chunk :378-421
+//   windowed (wlk_qwen_window_create): QwenAudioSurgeryEncoder, reference model.py:441-608, over the stock tower
+//            (transformers 5.5 modeling_qwen3_omni_moe.py:710-768)
+// Both modes share the weights, the conv stem, the pre-LN layer stack and the head; each keeps its own planning, its
+// conv_out step, its QKV destination and its attention.
 //
-// Data layout (per round, R = encoder steps in the round, one step = one 8-frame mel chunk):
-//   mel chunks   fp32 [R][8 frames][n_mels]                      (H2D from the caller's buffer)
-//   conv stem    NHWC activations [R][F][T][C]; conv2 / conv3 are im2col + GEMM (K = 9C, taps-major so a tap is one
-//                contiguous run of C channels), conv_out is a GEMM over [R][F*C] with its weight columns permuted
-//                from the reference's (c, f) order at load time; the sinusoid rows ride in as the GEMM's residual
-//   residual x   fp32 [R][d];  q [R][d];  K/V rings per session [L][K|V][H][ring][64], ring = left_context + 128
-//                slots addressed by position % ring (written by the QKV GEMM's scatter epilogue)
+// Causal: append-only execution, every mel frame transits the tower exactly once.  Sessions are batched per "round":
+// round r holds the r-th ready block (or run of chunks) of every session in the call, so a block always finds the K/V
+// its predecessor left in the session's ring.
+//
+// Data layout (R = encoder rows of a round or call):
+//   conv stem    chunks of T0 mel frames fp32 [n][T0][n_mels] (causal: T0 = 8, one chunk per step; windowed: T0 = 100,
+//                13 steps), NHWC activations [n][F][T][C]; conv2 / conv3 are im2col + GEMM (K = 9C, taps-major so a tap
+//                is one contiguous run of C channels), conv_out is a GEMM over [steps][F*C] with its weight columns
+//                permuted from the reference's (c, f) order at load time
+//   residual x   fp32 [R][d]
+//   causal       the sinusoid rows ride into conv_out as the GEMM's residual; q [R][d]; K/V rings per session
+//                [L][K|V][H][ring][64], ring = left_context + 128 slots addressed by position % ring (written by the QKV
+//                GEMM's scatter epilogue)
+//   windowed     each chunk's valid steps are compacted into x with positional rows 0..12; qkv [R][3d]
 #include <map>
 #include <mutex>
 #include <set>
@@ -22,6 +30,7 @@
 #include "../../include/wlk_b200.h"
 #include "host.cuh"
 #include "kernels.cuh"
+#include "ptx.cuh"
 
 namespace wlk {
 namespace {
@@ -36,14 +45,24 @@ struct QJob {                           // one per session in a round (device ar
     int32_t pad;
 };
 
+struct WChunk {                         // one conv chunk (device array)
+    const float* src;                   // the chunk's first mel frame [frames][n_mels]
+    int32_t avail;                      // frames of the window inside the chunk; frames beyond are zero
+    int32_t p0;                         // conv input length: T0, or a window's length when it is under T0 frames
+    int32_t dst_row;                    // residual row of the chunk's first valid step
+    int32_t n_valid;                    // valid steps (windowed: mod-100 rule on avail)
+};
+
 // ---------------------------------------------------------------------------------------------------------
-// conv2d1: 1 -> C channels, 3x3, stride 2, pad 1, GELU.  in: chunk [T0 frames][n_mels] (mel index = conv "height").
-// out: NHWC [F1][T1][C] with F1 = n_mels/2, T1 = T0/2.
+// conv2d1 (1 -> C, 3x3, stride 2, pad 1, GELU) over chunks laid out [n][T0][n_mels] (mel index = conv "height");
+// chunk k's input ends at p0 (the conv's zero padding starts there).  out NHWC [n][n_mels / 2][T0 / 2][C]; steps past
+// the chunk's conv length are computed but never read.
 // ---------------------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void qwen_conv1_kernel(const float* __restrict__ mel, const float* __restrict__ w, const float* __restrict__ b,
-                                  T* __restrict__ out, int n_chunks, int n_mels, int t0, int C) {
-    const int F1 = n_mels / 2, T1 = t0 / 2;
+template <typename T, int T0>
+__global__ void qwen_conv1_kernel(const float* __restrict__ mel, const WChunk* __restrict__ jobs, const float* __restrict__ w,
+                                  const float* __restrict__ b, T* __restrict__ out, int n_chunks, int n_mels, int C) {
+    constexpr int T1 = T0 / 2;
+    const int F1 = n_mels / 2;
     const int64_t total = (int64_t)n_chunks * F1 * T1 * C;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c = i % C;
@@ -51,7 +70,8 @@ __global__ void qwen_conv1_kernel(const float* __restrict__ mel, const float* __
         const int t = r % T1; r /= T1;
         const int f = r % F1;
         const int64_t ch = r / F1;
-        const float* x = mel + ch * t0 * n_mels;
+        const int p0 = jobs[ch].p0;
+        const float* x = mel + ch * T0 * n_mels;
         float acc = b[c];
 #pragma unroll
         for (int kf = 0; kf < 3; ++kf) {
@@ -60,7 +80,7 @@ __global__ void qwen_conv1_kernel(const float* __restrict__ mel, const float* __
 #pragma unroll
             for (int kt = 0; kt < 3; ++kt) {
                 const int fr = 2 * t - 1 + kt;
-                if (fr < 0 || fr >= t0) continue;
+                if (fr < 0 || fr >= p0) continue;
                 acc = fmaf(w[c * 9 + kf * 3 + kt], x[fr * n_mels + m], acc);
             }
         }
@@ -68,21 +88,27 @@ __global__ void qwen_conv1_kernel(const float* __restrict__ mel, const float* __
     }
 }
 
-// im2col for a 3x3 / stride 2 / pad 1 conv over NHWC [n][Fi][Ti][C] -> rows (n, fo, to), columns (tap, c)
+// im2col of a 3x3 / stride 2 / pad 1 conv over NHWC [n][Fi][Ti][C]: rows (n, fo, to), or (n, to, fo) when time_major
+// (conv3, so that conv_out reads one step's [F][C] features as one row); columns (tap, c).  Input steps at or past
+// the chunk's conv length at this stage read as zero (the conv's padding of a shorter input).
 template <typename T>
-__global__ void qwen_im2col_kernel(const T* __restrict__ src, T* __restrict__ dst, int n, int Fi, int Ti, int C) {
+__global__ void qwen_im2col_kernel(const T* __restrict__ src, const WChunk* __restrict__ jobs, T* __restrict__ dst, int n,
+                                   int Fi, int Ti, int stage, int C, int time_major) {
     const int Fo = Fi / 2, To = (Ti + 1) / 2;
     const int64_t total = (int64_t)n * Fo * To * 9 * C;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c = i % C;
         int64_t r = i / C;
         const int tap = r % 9; r /= 9;
-        const int to = r % To; r /= To;
-        const int fo = r % Fo;
-        const int64_t ch = r / Fo;
+        int fo, to;
+        if (time_major) { fo = r % Fo; r /= Fo; to = r % To; r /= To; }
+        else { to = r % To; r /= To; fo = r % Fo; r /= Fo; }
+        const int64_t ch = r;
+        int len = jobs[ch].p0;                                   // conv input length at this stage
+        for (int s = 0; s < stage; ++s) len = (len - 1) / 2 + 1;
         const int f = 2 * fo - 1 + tap / 3, t = 2 * to - 1 + tap % 3;
         T v = from_f32<T>(0.f);
-        if (f >= 0 && f < Fi && t >= 0 && t < Ti) v = src[((ch * Fi + f) * Ti + t) * C + c];
+        if (f >= 0 && f < Fi && t >= 0 && t < len) v = src[((ch * Fi + f) * Ti + t) * C + c];
         dst[i] = v;
     }
 }
@@ -227,17 +253,19 @@ struct wlk_qwen {
     WeightUpload upload;
     // sessions and workspaces
     std::vector<QSession> sess;
-    float *mel = nullptr, *x = nullptr, *posbuf = nullptr, *outbuf = nullptr;
-    void *a1 = nullptr, *col = nullptr, *a2 = nullptr, *a3 = nullptr, *xn = nullptr, *qb = nullptr, *att = nullptr, *hid = nullptr;
-    void *qkv_scratch = nullptr;
+    float *mel = nullptr, *x = nullptr, *outbuf = nullptr;                      // conv chunks, residual, head output
+    void *a1 = nullptr, *col = nullptr, *a2 = nullptr, *a3 = nullptr;           // conv stem
+    void *xn = nullptr, *att = nullptr, *hid = nullptr;                         // layer stack and head
     float* sk_scratch = nullptr; int* sk_counters = nullptr;      // this engine's split-K workspace (GemmArgs)
     uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
-    // windowed engine (wlk_qwen_window_create): geometry, rows of a full window, the conv workspace and the window scratch
+    // causal engine: the positional rows of a round, q of a round (k / v go to the session rings)
+    float* posbuf = nullptr; void* qb = nullptr;
+    // windowed engine (wlk_qwen_window_create): geometry, rows of a full window, conv_out's rows, q/k/v, window scratch
     bool windowed = false;
     wlk_qwen_window_dims wd{};
     int win_rows = 0, win_block_chunks = 0;
-    void *qkv = nullptr, *a1w = nullptr, *colw = nullptr, *a2w = nullptr, *a3w = nullptr;
-    float *xc = nullptr, *mel_chunks = nullptr, *win_scratch = nullptr;
+    void* qkv = nullptr;
+    float *xc = nullptr, *win_scratch = nullptr;
     size_t es() const { return dtype_size(act); }
 };
 
@@ -402,17 +430,15 @@ void alloc_weights(wlk_qwen* q) {
     }
 }
 
-void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
-    WLK_CHECK(dims && cfg && out, "null argument");
-    const wlk_qwen_dims& D = *dims;
+// The creation both modes share: the checks on the shared geometry, device, precision and GEMM backend, stream, weights,
+// the conv stem's workspace (conv_chunks chunks of t0 frames at a time), the layer stack's and the head's workspace
+// (max_rows rows), split-K scratch, the staging block and the sessions.  Each mode checks its own geometry before and
+// adds its own buffers after.
+wlk_qwen* create_common(const wlk_qwen_dims& D, const wlk_config* cfg, int max_rows, size_t conv_chunks, int t0,
+                        size_t stg_bytes) {
     WLK_CHECK(D.n_mels % 8 == 0 && D.n_mels >= 8, "n_mels must be a multiple of 8");
-    WLK_CHECK(D.chunk_frames == 8, "the conv stem maps exactly 8 mel frames to one step");
     WLK_CHECK(D.d_model % 64 == 0 && D.d_model / D.n_head == 64 && D.d_model <= 1280, "heads must be 64 wide, d_model <= 1280");
     WLK_CHECK(D.conv_channels % 8 == 0, "conv_channels must be a multiple of 8");
-    WLK_CHECK(D.block_frames % 8 == 0 && D.block_frames / 8 <= Q_STEPS_CAP, "block_frames must be a multiple of 8 and <= %d", 8 * Q_STEPS_CAP);
-    WLK_CHECK(D.mutable_tail_steps >= 0 && D.mutable_tail_steps < Q_STEPS_CAP, "mutable_tail_steps must be in [0, %d)", Q_STEPS_CAP);
-    WLK_CHECK(D.mutable_tail_steps == 0 || D.block_frames == 0, "fixed attention blocks and a mutable tail are exclusive");   // causal.py:127-131
-    WLK_CHECK(D.left_context_steps >= 1 && D.left_context_steps + Q_STEPS_CAP <= 512, "left_context_steps must be in [1, %d]", 512 - Q_STEPS_CAP);
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
     const int num_sms = open_sm90_device(cfg->device);
 
@@ -421,34 +447,53 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
     q->num_sms = num_sms;
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
-    q->ring = D.left_context_steps + Q_STEPS_CAP;
-    const int steps_per_round = D.block_frames > 0 ? D.block_frames / 8 : Q_STEPS_CAP;
-    q->max_rows = cfg->max_batch * steps_per_round;
+    q->max_rows = max_rows;
     CUDA_CHECK(cudaStreamCreateWithFlags(&q->st, cudaStreamNonBlocking));
     alloc_weights(q);
-    const size_t es = q->es();
+    const size_t es = q->es(), R = (size_t)max_rows, CH = conv_chunks;
     const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
-    const size_t R = (size_t)q->max_rows;
+    const int t1 = t0 / 2, t2 = (t1 + 1) / 2, t3 = (t2 + 1) / 2;                 // steps after conv1 / 2 / 3
     size_t* ws = &q->bytes_workspace;
-    q->mel = (float*)q->allocs.take(R * 8 * D.n_mels * 4, ws);
-    q->a1 = q->allocs.take(R * (D.n_mels / 2) * 4 * C * es, ws);
-    q->col = q->allocs.take(R * (D.n_mels / 4) * 2 * 9 * C * es, ws);              // conv2's im2col is the larger one
-    q->a2 = q->allocs.take(R * (D.n_mels / 4) * 2 * C * es, ws);
-    q->a3 = q->allocs.take(R * F * C * es, ws);
-    q->posbuf = (float*)q->allocs.take(R * d * 4, ws);
+    q->mel = (float*)q->allocs.take(CH * t0 * D.n_mels * 4, ws);
+    q->a1 = q->allocs.take(CH * (D.n_mels / 2) * t1 * C * es, ws);
+    q->col = q->allocs.take(CH * (D.n_mels / 4) * t2 * 9 * C * es, ws);         // conv2's im2col is the larger one
+    q->a2 = q->allocs.take(CH * (D.n_mels / 4) * t2 * C * es, ws);
+    q->a3 = q->allocs.take(CH * t3 * F * C * es, ws);
     q->x = (float*)q->allocs.take(R * d * 4, ws);
-    q->xn = q->allocs.take(R * d * es, ws); q->qb = q->allocs.take(R * d * es, ws); q->att = q->allocs.take(R * d * es, ws);
-    q->hid = q->allocs.take(R * (size_t)(ffn > d ? ffn : d) * es, ws);
+    q->xn = q->allocs.take(R * d * es, ws);
+    q->att = q->allocs.take(R * d * es, ws);
+    q->hid = q->allocs.take(R * (size_t)std::max(ffn, d) * es, ws);
     q->outbuf = (float*)q->allocs.take(R * D.out_dim * 4, ws);
     q->audio_scratch = (float*)q->allocs.take((size_t)QMEL_AUDIO_CAP * 4, ws);
     if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
         q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
         q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
     }
-    q->stg_bytes = R * 16 + (size_t)cfg->max_batch * (sizeof(QJob) + sizeof(MelJob) + 64) + 4096;
+    q->stg_bytes = stg_bytes;
     CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
     q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
     q->sess.resize(cfg->max_sessions);
+    return q;
+}
+
+void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
+    WLK_CHECK(dims && cfg && out, "null argument");
+    const wlk_qwen_dims& D = *dims;
+    WLK_CHECK(D.chunk_frames == 8, "the conv stem maps exactly 8 mel frames to one step");
+    WLK_CHECK(D.block_frames % 8 == 0 && D.block_frames / 8 <= Q_STEPS_CAP, "block_frames must be a multiple of 8 and <= %d", 8 * Q_STEPS_CAP);
+    WLK_CHECK(D.mutable_tail_steps >= 0 && D.mutable_tail_steps < Q_STEPS_CAP, "mutable_tail_steps must be in [0, %d)", Q_STEPS_CAP);
+    WLK_CHECK(D.mutable_tail_steps == 0 || D.block_frames == 0, "fixed attention blocks and a mutable tail are exclusive");   // causal.py:127-131
+    WLK_CHECK(D.left_context_steps >= 1 && D.left_context_steps + Q_STEPS_CAP <= 512, "left_context_steps must be in [1, %d]", 512 - Q_STEPS_CAP);
+    const int steps_per_round = D.block_frames > 0 ? D.block_frames / 8 : Q_STEPS_CAP;
+    const int max_rows = cfg->max_batch * steps_per_round;
+    const size_t R = (size_t)max_rows;
+    // a round stages its jobs, K/V pointers, one conv chunk per step and three int32 row maps
+    const size_t stg = R * (16 + sizeof(WChunk)) + (size_t)cfg->max_batch * (sizeof(QJob) + sizeof(MelJob) + 64) + 4096;
+    wlk_qwen* q = create_common(D, cfg, max_rows, R, 8, stg);
+    q->ring = D.left_context_steps + Q_STEPS_CAP;
+    size_t* ws = &q->bytes_workspace;
+    q->posbuf = (float*)q->allocs.take(R * D.d_model * 4, ws);
+    q->qb = q->allocs.take(R * D.d_model * q->es(), ws);
     *out = q;
 }
 
@@ -468,36 +513,40 @@ QSession& qsession(wlk_qwen* q, int32_t sid) {
     return q->sess[sid];
 }
 
-template <typename T>
-void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, void* const* kv_ptrs_dev, const int32_t* slot_dev,
-                     const int32_t* ringpos_dev, const int32_t* abspos_dev) {
+int grid_1d(int64_t total) { const int64_t b = (total + 255) / 256; return (int)(b > 65535 * 16 ? 65535 * 16 : b); }
+
+// conv2d1 -> im2col -> conv2 GEMM -> im2col -> conv3 GEMM over nc chunks of T0 frames in q->mel; out q->a3, rows
+// (chunk, step, f): one step's [F][C] features are one conv_out row
+template <typename T, int T0>
+void conv_stem(wlk_qwen* q, const WChunk* chunks_dev, int nc) {
+    constexpr int T1 = T0 / 2, T2 = (T1 + 1) / 2, T3 = (T2 + 1) / 2;
     const wlk_qwen_dims& D = q->dims;
-    const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim, H = D.n_head;
-    const int F1 = D.n_mels / 2, F2 = D.n_mels / 4;
-    auto blocks = [](int64_t total) { int64_t b = (total + 255) / 256; return (int)(b > 65535 * 16 ? 65535 * 16 : b); };
-    // conv stem
-    qwen_conv1_kernel<T><<<blocks((int64_t)R * F1 * 4 * C), 256, 0, q->st>>>(q->mel, q->c1w, q->c1b, (T*)q->a1, R, D.n_mels, 8, C);
-    qwen_im2col_kernel<T><<<blocks((int64_t)R * F2 * 2 * 9 * C), 256, 0, q->st>>>((const T*)q->a1, (T*)q->col, R, F1, 4, C);
+    const int C = D.conv_channels, F = D.n_mels / 8, F1 = D.n_mels / 2, F2 = D.n_mels / 4;
+    qwen_conv1_kernel<T, T0><<<grid_1d((int64_t)nc * F1 * T1 * C), 256, 0, q->st>>>(q->mel, chunks_dev, q->c1w, q->c1b, (T*)q->a1,
+                                                                                    nc, D.n_mels, C);
+    qwen_im2col_kernel<T><<<grid_1d((int64_t)nc * F2 * T2 * 9 * C), 256, 0, q->st>>>((const T*)q->a1, chunks_dev, (T*)q->col,
+                                                                                     nc, F1, T1, 1, C, 0);
     {   GemmArgs g;
         g.A = q->col; g.a_type = q->act; g.lda = 9 * C; g.W = q->W2c; g.w_type = q->act; g.ldw = 9 * C;
-        g.M = R * F2 * 2; g.N = C; g.K = 9 * C;
+        g.M = nc * F2 * T2; g.N = C; g.K = 9 * C;
         g.epi.bias = q->c2b; g.epi.gelu = 1; g.epi.C = q->a2; g.epi.c_type = q->act; g.epi.ldc = C;
         qgemm(q, g); }
-    qwen_im2col_kernel<T><<<blocks((int64_t)R * F * 1 * 9 * C), 256, 0, q->st>>>((const T*)q->a2, (T*)q->col, R, F2, 2, C);
+    qwen_im2col_kernel<T><<<grid_1d((int64_t)nc * F * T3 * 9 * C), 256, 0, q->st>>>((const T*)q->a2, chunks_dev, (T*)q->col,
+                                                                                    nc, F2, T2, 2, C, 1);
     {   GemmArgs g;
         g.A = q->col; g.a_type = q->act; g.lda = 9 * C; g.W = q->W3c; g.w_type = q->act; g.ldw = 9 * C;
-        g.M = R * F; g.N = C; g.K = 9 * C;
+        g.M = nc * T3 * F; g.N = C; g.K = 9 * C;
         g.epi.bias = q->c3b; g.epi.gelu = 1; g.epi.C = q->a3; g.epi.c_type = q->act; g.epi.ldc = C;
         qgemm(q, g); }
-    qwen_pos_kernel<<<R, 128, 0, q->st>>>(abspos_dev, q->pos_table, D.max_positions, q->posbuf, R, d);
-    {   GemmArgs g;
-        g.A = q->a3; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
-        g.M = R; g.N = d; g.K = F * C;
-        g.epi.bias = D.conv_out_bias ? q->bout : nullptr; g.epi.residual = q->posbuf; g.epi.ldr = d;
-        g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-        qgemm(q, g); }
-    CUDA_CHECK(cudaGetLastError());
-    // transformer layers with the per-session K/V rings
+}
+
+// The n_layer pre-LN layers over rows [0, R) of q->x (causal.py:378-421): LN, QKV, attention, out-proj + residual, LN,
+// fc1 + GELU, fc2 + residual.  qkv_dst(epi, layer) points the QKV GEMM's epilogue at the mode's destination; attend(layer)
+// runs the mode's attention from there into q->att.
+template <typename QkvDst, typename Attend>
+void run_layers(wlk_qwen* q, int R, QkvDst qkv_dst, Attend attend) {
+    const wlk_qwen_dims& D = q->dims;
+    const int d = D.d_model, ffn = D.ffn_dim;
     for (int li = 0; li < D.n_layer; ++li) {
         QLayerW& L = q->L[li];
         layernorm(q->x, d, L.ln1w, L.ln1b, q->xn, q->act, d, R, d, nullptr, q->st);
@@ -505,12 +554,10 @@ void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, void*
             g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = L.Wqkv; g.w_type = q->act; g.ldw = d;
             g.M = R; g.N = 3 * d; g.K = d;
             g.epi.bias = L.bqkv; g.epi.col_scale = 0.125f; g.epi.scale_cols = d;          // head_dim^-0.5 on q (causal.py:343-346)
-            g.epi.mode = EPI_SELF_QKV; g.epi.C = q->qb; g.epi.ldc = d; g.epi.c_type = q->act;
-            g.epi.batch_ptrs = kv_ptrs_dev; g.epi.row_slot = slot_dev; g.epi.row_pos = ringpos_dev;
-            g.epi.layer = li; g.epi.n_head = H; g.epi.d_model = d; g.epi.kv_len = q->ring;
+            g.epi.c_type = q->act;
+            qkv_dst(g.epi, li);
             qgemm(q, g); }
-        qwen_attention_kernel<T><<<dim3(H, n_jobs), 128, 0, q->st>>>((const T*)q->qb, jobs_dev, li, H, d, q->ring,
-                                                                    D.left_context_steps, D.block_bidirectional, (T*)q->att);
+        attend(li);
         {   GemmArgs g;
             g.A = q->att; g.a_type = q->act; g.lda = d; g.W = L.Wo; g.w_type = q->act; g.ldw = d;
             g.M = R; g.N = d; g.K = d;
@@ -528,19 +575,57 @@ void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, void*
             g.epi.bias = L.b2; g.epi.residual = q->x; g.epi.ldr = d; g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
             qgemm(q, g); }
     }
-    // head: ln_post -> proj1 -> GELU -> proj2 (causal.py:672-676)
-    layernorm(q->x, d, q->lnpw, q->lnpb, q->xn, q->act, d, R, d, nullptr, q->st);
+}
+
+// head: ln_post -> proj1 -> GELU -> proj2 (causal.py:672-676) on `rows` rows of q->x into q->outbuf: rows [0, rows) when
+// row_idx is null, else x's rows row_idx[0 .. rows) (row-wise ops: the same values as over every row)
+void run_head(wlk_qwen* q, int rows, const int32_t* row_idx) {
+    const wlk_qwen_dims& D = q->dims;
+    const int d = D.d_model;
+    if (rows > 0) {
+        layernorm(q->x, d, q->lnpw, q->lnpb, q->xn, q->act, d, rows, d, row_idx, q->st);
+        {   GemmArgs g;
+            g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = q->Wp1; g.w_type = q->act; g.ldw = d;
+            g.M = rows; g.N = d; g.K = d;
+            g.epi.bias = q->bp1; g.epi.gelu = 1; g.epi.C = q->hid; g.epi.c_type = q->act; g.epi.ldc = d;
+            qgemm(q, g); }
+        {   GemmArgs g;
+            g.A = q->hid; g.a_type = q->act; g.lda = d; g.W = q->Wp2; g.w_type = q->act; g.ldw = d;
+            g.M = rows; g.N = D.out_dim; g.K = d;
+            g.epi.bias = q->bp2; g.epi.C = q->outbuf; g.epi.c_type = DT_F32; g.epi.ldc = D.out_dim;
+            qgemm(q, g); }
+    }
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// one causal round: R steps, one 8-frame chunk each, staged in q->mel; the sinusoid rows of their absolute positions
+// ride into conv_out as the GEMM's residual; the QKV GEMM scatters k / v into the session rings
+template <typename T>
+void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, const WChunk* chunks_dev, void* const* kv_ptrs_dev,
+                     const int32_t* slot_dev, const int32_t* ringpos_dev, const int32_t* abspos_dev) {
+    const wlk_qwen_dims& D = q->dims;
+    const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, H = D.n_head;
+    conv_stem<T, 8>(q, chunks_dev, R);
+    qwen_pos_kernel<<<R, 128, 0, q->st>>>(abspos_dev, q->pos_table, D.max_positions, q->posbuf, R, d);
     {   GemmArgs g;
-        g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = q->Wp1; g.w_type = q->act; g.ldw = d;
-        g.M = R; g.N = d; g.K = d;
-        g.epi.bias = q->bp1; g.epi.gelu = 1; g.epi.C = q->hid; g.epi.c_type = q->act; g.epi.ldc = d;
-        qgemm(q, g); }
-    {   GemmArgs g;
-        g.A = q->hid; g.a_type = q->act; g.lda = d; g.W = q->Wp2; g.w_type = q->act; g.ldw = d;
-        g.M = R; g.N = D.out_dim; g.K = d;
-        g.epi.bias = q->bp2; g.epi.C = q->outbuf; g.epi.c_type = DT_F32; g.epi.ldc = D.out_dim;
+        g.A = q->a3; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
+        g.M = R; g.N = d; g.K = F * C;
+        g.epi.bias = D.conv_out_bias ? q->bout : nullptr; g.epi.residual = q->posbuf; g.epi.ldr = d;
+        g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
         qgemm(q, g); }
     CUDA_CHECK(cudaGetLastError());
+    run_layers(q, R,
+               [&](Epilogue& e, int li) {
+                   e.mode = EPI_SELF_QKV; e.C = q->qb; e.ldc = d;
+                   e.batch_ptrs = kv_ptrs_dev; e.row_slot = slot_dev; e.row_pos = ringpos_dev;
+                   e.layer = li; e.n_head = H; e.d_model = d; e.kv_len = q->ring;
+               },
+               [&](int li) {
+                   qwen_attention_kernel<T><<<dim3(H, n_jobs), 128, 0, q->st>>>((const T*)q->qb, jobs_dev, li, H, d, q->ring,
+                                                                               D.left_context_steps, D.block_bidirectional,
+                                                                               (T*)q->att);
+               });
+    run_head(q, R, nullptr);
 }
 
 // flush = false: forward_chunk (causal.py:713-782).  flush = true: flush_pending (causal.py:687-711) -- no new frames,
@@ -615,7 +700,9 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
             WLK_CHECK(keep >= 1, "round of %d steps exceeds the workspace (%d)", steps[0], q->max_rows);
             who.resize(keep); steps.resize(keep); R = acc; nj = keep;
         }
+        const size_t o_ch = carve((size_t)R * sizeof(WChunk));
         const size_t o_slot = carve((size_t)R * 4), o_ring = carve((size_t)R * 4), o_abs = carve((size_t)R * 4);
+        WChunk* chunks = reinterpret_cast<WChunk*>(q->stg_h + o_ch);
         QJob* jobs = reinterpret_cast<QJob*>(q->stg_h + o_jobs);
         void** kvp = reinterpret_cast<void**>(q->stg_h + o_kv);
         int32_t* slot = reinterpret_cast<int32_t*>(q->stg_h + o_slot);
@@ -632,6 +719,7 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
             CUDA_CHECK(cudaMemcpyAsync(q->mel + (size_t)r * 8 * D.n_mels, ready[i].data() + (size_t)done_steps[i] * 8 * D.n_mels,
                                        (size_t)steps[k] * 8 * D.n_mels * 4, cudaMemcpyHostToDevice, q->st));
             for (int t = 0; t < steps[k]; ++t, ++r) {
+                chunks[r] = WChunk{q->mel + (size_t)r * 8 * D.n_mels, 8, 8, r, 1};
                 slot[r] = k; abspos[r] = (int32_t)(start + t); ringpos[r] = (int32_t)((start + t) % q->ring);
             }
         }
@@ -641,8 +729,9 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
         const int32_t* slot_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_slot);
         const int32_t* ring_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_ring);
         const int32_t* abs_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_abs);
-        if (q->act == DT_F32) run_round_typed<float>(q, nj, R, jobs_dev, kv_dev, slot_dev, ring_dev, abs_dev);
-        else run_round_typed<bf16>(q, nj, R, jobs_dev, kv_dev, slot_dev, ring_dev, abs_dev);
+        const WChunk* chunks_dev = reinterpret_cast<const WChunk*>(q->stg_d + o_ch);
+        if (q->act == DT_F32) run_round_typed<float>(q, nj, R, jobs_dev, chunks_dev, kv_dev, slot_dev, ring_dev, abs_dev);
+        else run_round_typed<bf16>(q, nj, R, jobs_dev, chunks_dev, kv_dev, slot_dev, ring_dev, abs_dev);
         r = 0;
         for (int k = 0; k < nj; ++k) {
             const int i = who[k];
@@ -766,8 +855,7 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
 // rule) are compacted with positional rows 0..12; layers with block-diagonal bidirectional attention; the head only on
 // the rows the call emits.  All sessions of a call run in one pass, their rows back to back.
 //
-// Conv stem workspace: rounds of at most QW_CHUNKS_PER_ROUND chunks (im2col + GEMM, the same GEMMs as the causal
-// stem).  An implicit-GEMM conv would need a new GEMM operand path; a fixed round keeps conv2's im2col at
+// Conv stem workspace: rounds of at most QW_CHUNKS_PER_ROUND chunks of conv_stem (im2col + GEMM).  An implicit-GEMM conv would need a new GEMM operand path; a fixed round keeps conv2's im2col at
 // QW_CHUNKS_PER_ROUND x 800 x 9C elements (221 MB in bf16 at C = 480) whatever the batch, against 11.5 GB for 128
 // sessions' 13 chunks at once, and 32 chunks = 25600 conv2 rows still fill the GEMM grid.
 // =========================================================================================================
@@ -777,7 +865,7 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
 namespace wlk {
 namespace {
 
-constexpr int QW_T0 = 100, QW_T1 = 50, QW_T2 = 25, QW_T3 = 13;   // conv chunk frames -> steps after conv1 / 2 / 3
+constexpr int QW_T0 = 100, QW_T3 = 13;  // conv chunk frames, steps after conv3
 constexpr int QW_CHUNKS_PER_ROUND = 32;
 constexpr int QW_KMAX = 256;            // keys one attention block may hold (a full default window is 164 rows)
 constexpr int QW_QTILE = 64;            // query rows per attention CTA (4 warps x 16)
@@ -797,14 +885,6 @@ size_t session_bytes(const wlk_qwen* q) {
     return (size_t)q->dims.n_layer * 2 * q->dims.n_head * q->ring * 64 * q->es();
 }
 
-struct WChunk {                         // one conv chunk of one window (device array)
-    const float* src;                   // the chunk's first mel frame [frames][n_mels]
-    int32_t avail;                      // frames of the window inside the chunk; frames beyond are zero
-    int32_t p0;                         // conv input length: 100, or the window's length when it is under 100 frames
-    int32_t dst_row;                    // residual row of the chunk's first valid step
-    int32_t n_valid;                    // valid steps (mod-100 rule on avail)
-};
-
 struct WAttn {                          // one query tile of one attention block (device array)
     int32_t row0;                       // first row of the block
     int32_t len;                        // rows (= keys) of the block
@@ -823,63 +903,6 @@ __global__ void qwin_gather_kernel(const WChunk* __restrict__ jobs, float* __res
     }
 }
 
-// conv2d1 (1 -> C, 3x3, stride 2, pad 1, GELU) over chunks laid out [n][100][n_mels]; chunk k's input ends at p0
-// (the conv's zero padding starts there).  out NHWC [n][n_mels / 2][50][C]; steps past the chunk's conv length are
-// computed but never read.
-template <typename T>
-__global__ void qwin_conv1_kernel(const float* __restrict__ mel, const WChunk* __restrict__ jobs, const float* __restrict__ w,
-                                  const float* __restrict__ b, T* __restrict__ out, int n_chunks, int n_mels, int C) {
-    const int F1 = n_mels / 2;
-    const int64_t total = (int64_t)n_chunks * F1 * QW_T1 * C;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int c = i % C;
-        int64_t r = i / C;
-        const int t = r % QW_T1; r /= QW_T1;
-        const int f = r % F1;
-        const int64_t ch = r / F1;
-        const int p0 = jobs[ch].p0;
-        const float* x = mel + ch * QW_T0 * n_mels;
-        float acc = b[c];
-#pragma unroll
-        for (int kf = 0; kf < 3; ++kf) {
-            const int m = 2 * f - 1 + kf;
-            if (m < 0 || m >= n_mels) continue;
-#pragma unroll
-            for (int kt = 0; kt < 3; ++kt) {
-                const int fr = 2 * t - 1 + kt;
-                if (fr < 0 || fr >= p0) continue;
-                acc = fmaf(w[c * 9 + kf * 3 + kt], x[fr * n_mels + m], acc);
-            }
-        }
-        out[i] = from_f32<T>(gelu_erf(acc));
-    }
-}
-
-// im2col of a 3x3 / stride 2 / pad 1 conv over NHWC [n][Fi][Ti][C]: rows (n, fo, to), or (n, to, fo) when time_major
-// (conv3, so that conv_out reads one step's [F][C] features as one row); columns (tap, c).  Input steps at or past
-// the chunk's conv length at this stage read as zero (the conv's padding of a shorter input).
-template <typename T>
-__global__ void qwin_im2col_kernel(const T* __restrict__ src, const WChunk* __restrict__ jobs, T* __restrict__ dst, int n,
-                                   int Fi, int Ti, int stage, int C, int time_major) {
-    const int Fo = Fi / 2, To = (Ti + 1) / 2;
-    const int64_t total = (int64_t)n * Fo * To * 9 * C;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int c = i % C;
-        int64_t r = i / C;
-        const int tap = r % 9; r /= 9;
-        int fo, to;
-        if (time_major) { fo = r % Fo; r /= Fo; to = r % To; r /= To; }
-        else { to = r % To; r /= To; fo = r % Fo; r /= Fo; }
-        const int64_t ch = r;
-        int len = jobs[ch].p0;                                   // conv input length at this stage
-        for (int s = 0; s < stage; ++s) len = (len - 1) / 2 + 1;
-        const int f = 2 * fo - 1 + tap / 3, t = 2 * to - 1 + tap % 3;
-        T v = from_f32<T>(0.f);
-        if (f >= 0 && f < Fi && t >= 0 && t < len) v = src[((ch * Fi + f) * Ti + t) * C + c];
-        dst[i] = v;
-    }
-}
-
 // valid-step compaction: x[dst_row + j] = conv_out[chunk][j] + positional row j (rows restart in every chunk)
 __global__ void qwin_compact_kernel(const float* __restrict__ xc, const WChunk* __restrict__ jobs, const float* __restrict__ table,
                                     float* __restrict__ x, int d) {
@@ -887,17 +910,6 @@ __global__ void qwin_compact_kernel(const float* __restrict__ xc, const WChunk* 
     for (int s = 0; s < j.n_valid; ++s)
         for (int i = threadIdx.x; i < d; i += blockDim.x)
             x[(int64_t)(j.dst_row + s) * d + i] = xc[((int64_t)blockIdx.x * QW_T3 + s) * d + i] + table[(int64_t)s * d + i];
-}
-
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // Block-diagonal bidirectional attention, bf16 on tensor cores.  Grid (query tile, head), 4 warps.  The block's K and V
@@ -956,7 +968,7 @@ qwin_attn_mma_kernel(const bf16* __restrict__ qkv, const WAttn* __restrict__ ite
                 const bf16* kr = Ks + (kb + g) * QW_KSTRIDE + tq * 2;
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks)
-                    mma_bf16_16816(s[nt], qa[ks], *reinterpret_cast<const uint32_t*>(kr + ks * 16),
+                    ptx::mma_bf16_16816(s[nt], qa[ks], *reinterpret_cast<const uint32_t*>(kr + ks * 16),
                                    *reinterpret_cast<const uint32_t*>(kr + ks * 16 + 8));
             }
             const int k0 = kb + tq * 2;
@@ -986,8 +998,9 @@ qwin_attn_mma_kernel(const bf16* __restrict__ qkv, const WAttn* __restrict__ ite
         for (int j = 0; j < 4; ++j) {                          // 16 keys per MMA
             const int kb = kt + j * 16;
             if (kb >= nkp) break;
-            const uint32_t pa[4] = {pack_bf16(s[2 * j][0], s[2 * j][1]), pack_bf16(s[2 * j][2], s[2 * j][3]),
-                                    pack_bf16(s[2 * j + 1][0], s[2 * j + 1][1]), pack_bf16(s[2 * j + 1][2], s[2 * j + 1][3])};
+            const uint32_t pa[4] = {ptx::pack_bf16x2(s[2 * j][0], s[2 * j][1]), ptx::pack_bf16x2(s[2 * j][2], s[2 * j][3]),
+                                    ptx::pack_bf16x2(s[2 * j + 1][0], s[2 * j + 1][1]),
+                                    ptx::pack_bf16x2(s[2 * j + 1][2], s[2 * j + 1][3])};
             const bf16* v0 = Vs + (kb + tq * 2) * QW_KSTRIDE + g;
 #pragma unroll
             for (int nt = 0; nt < 8; ++nt) {
@@ -995,7 +1008,7 @@ qwin_attn_mma_kernel(const bf16* __restrict__ qkv, const WAttn* __restrict__ ite
                 __nv_bfloat162 b0, b1;
                 b0.x = v[0]; b0.y = v[QW_KSTRIDE];
                 b1.x = v[8 * QW_KSTRIDE]; b1.y = v[9 * QW_KSTRIDE];
-                mma_bf16_16816(o[nt], pa, *reinterpret_cast<uint32_t*>(&b0), *reinterpret_cast<uint32_t*>(&b1));
+                ptx::mma_bf16_16816(o[nt], pa, *reinterpret_cast<uint32_t*>(&b0), *reinterpret_cast<uint32_t*>(&b1));
             }
         }
     }
@@ -1108,63 +1121,30 @@ void launch_window_attention(int act, const void* qkv, const WAttn* items_dev, i
 void create_window(const wlk_qwen_window_dims* wdims, const wlk_config* cfg, wlk_qwen** out) {
     WLK_CHECK(wdims && cfg && out, "null argument");
     const wlk_qwen_window_dims& W = *wdims;
-    WLK_CHECK(W.n_mels % 8 == 0 && W.n_mels >= 8, "n_mels must be a multiple of 8");
-    WLK_CHECK(W.d_model % 64 == 0 && W.d_model / W.n_head == 64 && W.d_model <= 1280, "heads must be 64 wide, d_model <= 1280");
-    WLK_CHECK(W.conv_channels % 8 == 0, "conv_channels must be a multiple of 8");
     WLK_CHECK(W.n_window == 50, "the mod-100 length rule needs n_window = 50 (100-frame chunks), got %d", W.n_window);
     WLK_CHECK(W.n_window_infer == 0 || W.n_window_infer >= 2 * W.n_window, "n_window_infer must be 0 or >= %d", 2 * W.n_window);
     WLK_CHECK(W.left_context_frames > 0 && W.right_context_frames >= 0, "left_context_frames must be > 0, right >= 0");
     WLK_CHECK(W.max_positions >= QW_T3, "the positional table needs at least %d rows", QW_T3);
-    WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
     const int wframes = W.left_context_frames + W.right_context_frames;
     const int wrows = window_steps(wframes);
     const int chunks_per_block = W.n_window_infer / (2 * W.n_window);
     WLK_CHECK(std::min(wrows, W.n_window_infer ? QW_T3 * chunks_per_block : wrows) <= QW_KMAX,
               "attention blocks of more than %d rows are not supported", QW_KMAX);
-    const int num_sms = open_sm90_device(cfg->device);
-
-    auto* q = new wlk_qwen();
-    q->windowed = true; q->wd = W;
-    q->dims = wlk_qwen_dims{W.n_mels, W.conv_channels, W.d_model, W.n_head, W.n_layer, W.ffn_dim, W.out_dim, W.max_positions,
-                            8, 0, 1, 1, W.conv_out_bias, 0};
-    q->cfg = *cfg;
-    q->num_sms = num_sms;
-    q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
-    q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
-    q->win_rows = wrows;
-    q->win_block_chunks = chunks_per_block;
-    q->max_rows = cfg->max_batch * wrows;
-    CUDA_CHECK(cudaStreamCreateWithFlags(&q->st, cudaStreamNonBlocking));
-    if (q->act == DT_BF16) window_attention_opt_in();
-    alloc_weights(q);
-    const size_t es = q->es(), R = (size_t)q->max_rows, CH = QW_CHUNKS_PER_ROUND;
-    const int C = W.conv_channels, d = W.d_model, F = W.n_mels / 8, ffn = W.ffn_dim;
-    size_t* ws = &q->bytes_workspace;
-    q->mel_chunks = (float*)q->allocs.take(CH * QW_T0 * W.n_mels * 4, ws);
-    q->a1w = q->allocs.take(CH * (W.n_mels / 2) * QW_T1 * C * es, ws);
-    q->colw = q->allocs.take(CH * (W.n_mels / 4) * QW_T2 * 9 * C * es, ws);      // conv2's im2col is the larger one
-    q->a2w = q->allocs.take(CH * (W.n_mels / 4) * QW_T2 * C * es, ws);
-    q->a3w = q->allocs.take(CH * QW_T3 * F * C * es, ws);
-    q->xc = (float*)q->allocs.take(CH * QW_T3 * d * 4, ws);
-    q->x = (float*)q->allocs.take(R * d * 4, ws);
-    q->xn = q->allocs.take(R * d * es, ws);
-    q->qkv = q->allocs.take(R * 3 * d * es, ws);
-    q->att = q->allocs.take(R * d * es, ws);
-    q->hid = q->allocs.take(R * (size_t)std::max(ffn, d) * es, ws);
-    q->outbuf = (float*)q->allocs.take(R * W.out_dim * 4, ws);
-    q->win_scratch = (float*)q->allocs.take((size_t)wframes * W.n_mels * 4, ws);
-    q->audio_scratch = (float*)q->allocs.take((size_t)QMEL_AUDIO_CAP * 4, ws);
-    if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
-        q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
-        q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
-    }
+    const wlk_qwen_dims D{W.n_mels, W.conv_channels, W.d_model, W.n_head, W.n_layer, W.ffn_dim, W.out_dim, W.max_positions,
+                          8, 0, 1, 1, W.conv_out_bias, 0};
+    const size_t R = (size_t)cfg->max_batch * wrows;
     const size_t max_chunks = (size_t)cfg->max_batch * ((wframes + QW_T0 - 1) / QW_T0);
     const size_t max_items = (size_t)cfg->max_batch * ((wrows + QW_QTILE - 1) / QW_QTILE + wrows);
-    q->stg_bytes = R * 4 + max_chunks * sizeof(WChunk) + max_items * sizeof(WAttn)
-                 + (size_t)cfg->max_batch * (sizeof(MelJob) + 64) + 4096;
-    CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
-    q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
-    q->sess.resize(cfg->max_sessions);
+    const size_t stg = R * 4 + max_chunks * sizeof(WChunk) + max_items * sizeof(WAttn) + (size_t)cfg->max_batch * (sizeof(MelJob) + 64) + 4096;
+    wlk_qwen* q = create_common(D, cfg, (int)R, QW_CHUNKS_PER_ROUND, QW_T0, stg);
+    q->windowed = true; q->wd = W;
+    q->win_rows = wrows;
+    q->win_block_chunks = chunks_per_block;
+    if (q->act == DT_BF16) window_attention_opt_in();
+    size_t* ws = &q->bytes_workspace;
+    q->xc = (float*)q->allocs.take((size_t)QW_CHUNKS_PER_ROUND * QW_T3 * W.d_model * 4, ws);
+    q->qkv = q->allocs.take(R * 3 * W.d_model * q->es(), ws);
+    q->win_scratch = (float*)q->allocs.take((size_t)wframes * W.n_mels * 4, ws);
     *out = q;
 }
 
@@ -1175,8 +1155,7 @@ int64_t run_windows(wlk_qwen* q, const std::vector<const float*>& wins, const st
                     const std::vector<int>& lo, const std::vector<int>& hi) {
     const wlk_qwen_window_dims& W = q->wd;
     const int n = (int)wins.size();
-    const int C = W.conv_channels, d = W.d_model, F = W.n_mels / 8, ffn = W.ffn_dim, H = W.n_head;
-    const int F1 = W.n_mels / 2, F2 = W.n_mels / 4;
+    const int C = W.conv_channels, d = W.d_model, F = W.n_mels / 8, H = W.n_head;
     std::vector<int> row_off(n), rows(n), block(n);
     std::vector<WChunk> chunks;
     int R = 0;
@@ -1207,76 +1186,24 @@ int64_t run_windows(wlk_qwen* q, const std::vector<const float*>& wins, const st
     const WChunk* chunks_dev = reinterpret_cast<const WChunk*>(q->stg_d + o_ch);
     const WAttn* items_dev = reinterpret_cast<const WAttn*>(q->stg_d + o_it);
     const int32_t* emit_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_em);
-    auto blocks = [](int64_t total) { int64_t b = (total + 255) / 256; return (int)(b > 65535 * 16 ? 65535 * 16 : b); };
     // conv stem, in rounds of at most QW_CHUNKS_PER_ROUND chunks
     for (size_t c0 = 0; c0 < chunks.size(); c0 += QW_CHUNKS_PER_ROUND) {
         const int nc = (int)std::min<size_t>(QW_CHUNKS_PER_ROUND, chunks.size() - c0);
         const WChunk* jd = chunks_dev + c0;
-        qwin_gather_kernel<<<blocks((int64_t)nc * QW_T0 * W.n_mels), 256, 0, q->st>>>(jd, q->mel_chunks, nc, W.n_mels);
-        qwin_conv1_kernel<T><<<blocks((int64_t)nc * F1 * QW_T1 * C), 256, 0, q->st>>>(q->mel_chunks, jd, q->c1w, q->c1b, (T*)q->a1w, nc, W.n_mels, C);
-        qwin_im2col_kernel<T><<<blocks((int64_t)nc * F2 * QW_T2 * 9 * C), 256, 0, q->st>>>((const T*)q->a1w, jd, (T*)q->colw, nc, F1, QW_T1, 1, C, 0);
+        qwin_gather_kernel<<<grid_1d((int64_t)nc * QW_T0 * W.n_mels), 256, 0, q->st>>>(jd, q->mel, nc, W.n_mels);
+        conv_stem<T, QW_T0>(q, jd, nc);
         {   GemmArgs g;
-            g.A = q->colw; g.a_type = q->act; g.lda = 9 * C; g.W = q->W2c; g.w_type = q->act; g.ldw = 9 * C;
-            g.M = nc * F2 * QW_T2; g.N = C; g.K = 9 * C;
-            g.epi.bias = q->c2b; g.epi.gelu = 1; g.epi.C = q->a2w; g.epi.c_type = q->act; g.epi.ldc = C;
-            qgemm(q, g); }
-        qwin_im2col_kernel<T><<<blocks((int64_t)nc * F * QW_T3 * 9 * C), 256, 0, q->st>>>((const T*)q->a2w, jd, (T*)q->colw, nc, F2, QW_T2, 2, C, 1);
-        {   GemmArgs g;                                      // rows (chunk, step, f): one step's [F][C] is one conv_out row
-            g.A = q->colw; g.a_type = q->act; g.lda = 9 * C; g.W = q->W3c; g.w_type = q->act; g.ldw = 9 * C;
-            g.M = nc * QW_T3 * F; g.N = C; g.K = 9 * C;
-            g.epi.bias = q->c3b; g.epi.gelu = 1; g.epi.C = q->a3w; g.epi.c_type = q->act; g.epi.ldc = C;
-            qgemm(q, g); }
-        {   GemmArgs g;
-            g.A = q->a3w; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
+            g.A = q->a3; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
             g.M = nc * QW_T3; g.N = d; g.K = F * C;
             g.epi.bias = W.conv_out_bias ? q->bout : nullptr; g.epi.C = q->xc; g.epi.c_type = DT_F32; g.epi.ldc = d;
             qgemm(q, g); }
         qwin_compact_kernel<<<nc, 128, 0, q->st>>>(q->xc, jd, q->pos_table, q->x, d);
         CUDA_CHECK(cudaGetLastError());
     }
-    // pre-LN layers, block-diagonal attention
-    for (int li = 0; li < W.n_layer; ++li) {
-        QLayerW& L = q->L[li];
-        layernorm(q->x, d, L.ln1w, L.ln1b, q->xn, q->act, d, R, d, nullptr, q->st);
-        {   GemmArgs g;
-            g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = L.Wqkv; g.w_type = q->act; g.ldw = d;
-            g.M = R; g.N = 3 * d; g.K = d;
-            g.epi.bias = L.bqkv; g.epi.col_scale = 0.125f; g.epi.scale_cols = d;          // head_dim^-0.5 on q
-            g.epi.C = q->qkv; g.epi.ldc = 3 * d; g.epi.c_type = q->act;
-            qgemm(q, g); }
-        launch_window_attention(q->act, q->qkv, items_dev, (int)items.size(), H, d, q->att, q->st);
-        {   GemmArgs g;
-            g.A = q->att; g.a_type = q->act; g.lda = d; g.W = L.Wo; g.w_type = q->act; g.ldw = d;
-            g.M = R; g.N = d; g.K = d;
-            g.epi.bias = L.bo; g.epi.residual = q->x; g.epi.ldr = d; g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            qgemm(q, g); }
-        layernorm(q->x, d, L.ln2w, L.ln2b, q->xn, q->act, d, R, d, nullptr, q->st);
-        {   GemmArgs g;
-            g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = L.W1; g.w_type = q->act; g.ldw = d;
-            g.M = R; g.N = ffn; g.K = d;
-            g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = q->hid; g.epi.c_type = q->act; g.epi.ldc = ffn;
-            qgemm(q, g); }
-        {   GemmArgs g;
-            g.A = q->hid; g.a_type = q->act; g.lda = ffn; g.W = L.W2; g.w_type = q->act; g.ldw = ffn;
-            g.M = R; g.N = d; g.K = ffn;
-            g.epi.bias = L.b2; g.epi.residual = q->x; g.epi.ldr = d; g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            qgemm(q, g); }
-    }
-    // head on the emitted rows only (row-wise ops: the same values as over every row)
-    if (E > 0) {
-        layernorm(q->x, d, q->lnpw, q->lnpb, q->xn, q->act, d, E, d, emit_dev, q->st);
-        {   GemmArgs g;
-            g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = q->Wp1; g.w_type = q->act; g.ldw = d;
-            g.M = E; g.N = d; g.K = d;
-            g.epi.bias = q->bp1; g.epi.gelu = 1; g.epi.C = q->hid; g.epi.c_type = q->act; g.epi.ldc = d;
-            qgemm(q, g); }
-        {   GemmArgs g;
-            g.A = q->hid; g.a_type = q->act; g.lda = d; g.W = q->Wp2; g.w_type = q->act; g.ldw = d;
-            g.M = E; g.N = W.out_dim; g.K = d;
-            g.epi.bias = q->bp2; g.epi.C = q->outbuf; g.epi.c_type = DT_F32; g.epi.ldc = W.out_dim;
-            qgemm(q, g); }
-    }
-    CUDA_CHECK(cudaGetLastError());
+    // pre-LN layers, block-diagonal attention; the head on the emitted rows only
+    run_layers(q, R, [&](Epilogue& e, int) { e.C = q->qkv; e.ldc = 3 * d; },
+               [&](int) { launch_window_attention(q->act, q->qkv, items_dev, (int)items.size(), H, d, q->att, q->st); });
+    run_head(q, E, emit_dev);
     return E;
 }
 

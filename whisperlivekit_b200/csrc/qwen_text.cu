@@ -19,6 +19,7 @@
 #include "../../include/wlk_b200.h"
 #include "host.cuh"
 #include "kernels.cuh"
+#include "ptx.cuh"
 
 namespace wlk {
 namespace {
@@ -165,18 +166,6 @@ struct QTAttnTile { int32_t row0, n_rows, slot, pos0; };
 constexpr int QT_KT = 64;                         // keys per shared-memory tile
 constexpr int QT_KPAD = QT_HD + 8;                // padded row: the fragment loads of a quad hit distinct banks
 
-__device__ __forceinline__ void qt_mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t qt_pack(float lo, float hi) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t qt_pack_bf(bf16 lo, bf16 hi) {
-    return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
-}
 
 __global__ void __launch_bounds__(256)
 qt_attention_mma_kernel(const bf16* __restrict__ q, const QTAttnTile* __restrict__ tiles, void* const* __restrict__ kv_ptrs,
@@ -229,7 +218,7 @@ qt_attention_mma_kernel(const bf16* __restrict__ q, const QTAttnTile* __restrict
             for (int kk = 0; kk < 8; ++kk) {
                 const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&ks[8 * j + g][kk * 16 + 2 * t]);
                 const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&ks[8 * j + g][kk * 16 + 2 * t + 8]);
-                qt_mma16816(s[j], qa[kk], b0, b1);
+                ptx::mma_bf16_16816(s[j], qa[kk], b0, b1);
             }
         }
         float mx0 = m0, mx1 = m1;
@@ -267,15 +256,15 @@ qt_attention_mma_kernel(const bf16* __restrict__ q, const QTAttnTile* __restrict
         for (int n = 0; n < 16; ++n) { o[n][0] *= c0; o[n][1] *= c0; o[n][2] *= c1; o[n][3] *= c1; }
 #pragma unroll
         for (int kk = 0; kk < QT_KT / 16; ++kk) {
-            const uint32_t pa[4] = {qt_pack(s[2 * kk][0], s[2 * kk][1]), qt_pack(s[2 * kk][2], s[2 * kk][3]),
-                                    qt_pack(s[2 * kk + 1][0], s[2 * kk + 1][1]), qt_pack(s[2 * kk + 1][2], s[2 * kk + 1][3])};
+            const uint32_t pa[4] = {ptx::pack_bf16x2(s[2 * kk][0], s[2 * kk][1]), ptx::pack_bf16x2(s[2 * kk][2], s[2 * kk][3]),
+                                    ptx::pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]), ptx::pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3])};
             const int kr = 16 * kk + 2 * t;
 #pragma unroll
             for (int n = 0; n < 16; ++n) {
                 const int c = 8 * n + g;
-                const uint32_t b0 = qt_pack_bf(vs[kr][c], vs[kr + 1][c]);
-                const uint32_t b1 = qt_pack_bf(vs[kr + 8][c], vs[kr + 9][c]);
-                qt_mma16816(o[n], pa, b0, b1);
+                const uint32_t b0 = ptx::pack_bf16_pair(vs[kr][c], vs[kr + 1][c]);
+                const uint32_t b1 = ptx::pack_bf16_pair(vs[kr + 8][c], vs[kr + 9][c]);
+                ptx::mma_bf16_16816(o[n], pa, b0, b1);
             }
         }
         m0 = mx0; m1 = mx1;
@@ -284,8 +273,8 @@ qt_attention_mma_kernel(const bf16* __restrict__ q, const QTAttnTile* __restrict
 #pragma unroll
     for (int n = 0; n < 16; ++n) {
         const int c = h * QT_HD + 8 * n + 2 * t;
-        if (ok0) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g) * H * QT_HD + c) = qt_pack(o[n][0] * i0, o[n][1] * i0);
-        if (ok1) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g + 8) * H * QT_HD + c) = qt_pack(o[n][2] * i1, o[n][3] * i1);
+        if (ok0) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g) * H * QT_HD + c) = ptx::pack_bf16x2(o[n][0] * i0, o[n][1] * i0);
+        if (ok1) *reinterpret_cast<uint32_t*>(out + (int64_t)(tl.row0 + g + 8) * H * QT_HD + c) = ptx::pack_bf16x2(o[n][2] * i1, o[n][3] * i1);
     }
 }
 

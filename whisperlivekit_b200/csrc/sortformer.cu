@@ -29,6 +29,7 @@
 #include "../../include/wlk_b200.h"
 #include "host.cuh"
 #include "kernels.cuh"
+#include "ptx.cuh"
 
 namespace wlk {
 namespace {
@@ -288,14 +289,6 @@ sf_attention_kernel(const T* __restrict__ qkv, const SfJob* __restrict__ jobs, i
 //     P = exp(S * scale - max), row sums             a warp per 4 rows; P overwrites the row in place as bf16
 //     O = P V / sum                                  warps split the 8-wide output column tiles
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mma_bf16_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack2(bf16 lo, bf16 hi) {
-    return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
-}
 
 template <bool RELPOS>
 __global__ void __launch_bounds__(128)
@@ -351,7 +344,7 @@ sf_attention_mma_kernel(const bf16* __restrict__ qkv, const SfJob* __restrict__ 
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
-            if (ks < ksteps) { uint32_t b0, b1; bfrag(kr, ok, ks, b0, b1); mma_bf16_16816(acc, au[ks], b0, b1); }
+            if (ks < ksteps) { uint32_t b0, b1; bfrag(kr, ok, ks, b0, b1); ptx::mma_bf16_16816(acc, au[ks], b0, b1); }
         }
         const int c = 8 * nt + 2 * t;
         S[g][c] = acc[0] * score_scale; S[g][c + 1] = acc[1] * score_scale;
@@ -369,7 +362,7 @@ sf_attention_mma_kernel(const bf16* __restrict__ qkv, const SfJob* __restrict__ 
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
-                if (ks < ksteps) { uint32_t b0, b1; bfrag(pr, ok, ks, b0, b1); mma_bf16_16816(acc, av[ks], b0, b1); }
+                if (ks < ksteps) { uint32_t b0, b1; bfrag(pr, ok, ks, b0, b1); ptx::mma_bf16_16816(acc, av[ks], b0, b1); }
             }
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -419,8 +412,8 @@ sf_attention_mma_kernel(const bf16* __restrict__ qkv, const SfJob* __restrict__ 
             a[2] = *reinterpret_cast<const uint32_t*>(p0 + 8); a[3] = *reinterpret_cast<const uint32_t*>(p1 + 8);
             const int j0 = 16 * kk + 2 * t;
             auto vld = [&](int j) { return nok && j < T ? vbase[(int64_t)j * ld + n] : zero; };
-            const uint32_t b0 = pack2(vld(j0), vld(j0 + 1)), b1 = pack2(vld(j0 + 8), vld(j0 + 9));
-            mma_bf16_16816(acc, a, b0, b1);
+            const uint32_t b0 = ptx::pack_bf16_pair(vld(j0), vld(j0 + 1)), b1 = ptx::pack_bf16_pair(vld(j0 + 8), vld(j0 + 9));
+            ptx::mma_bf16_16816(acc, a, b0, b1);
         }
         const int c = 8 * ot + 2 * t;
         if (c < dh) {

@@ -12,27 +12,28 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib as L
-from .qwen_dims import QwenTowerDims
 
 
 def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
 
 
-class QwenTowerEngine:
-    def __init__(self, dims: QwenTowerDims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
+class _QwenEngineBase:
+    """The ctypes plumbing both tower engines share: one ``wlk_qwen`` handle, its weights, sessions and memory."""
+
+    def __init__(self, dims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8, gemm_backend: str = "auto"):
         self.lib = L.load()
         self.dims = dims
         self.precision = precision
         self.device = int(device)
         be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
-        cdims = L.wlk_qwen_dims(*dims.as_tuple())
+        cdims = self._DIMS(*dims.as_tuple())
         cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
                            max_sessions=max_sessions, max_batch=max_batch, gemm_backend=be[gemm_backend],
                            attn_backend=L.BACKEND_SIMT, max_align_heads=0, reserved=0)
         h = C.c_void_p()
-        L.check(self.lib.wlk_qwen_create(C.byref(cdims), C.byref(cfg), C.byref(h)))
+        L.check(getattr(self.lib, self._CREATE)(C.byref(cdims), C.byref(cfg), C.byref(h)))
         self.h = h
         self._closed = False
         if state_dict is not None:
@@ -50,7 +51,6 @@ class QwenTowerEngine:
         L.check(self.lib.wlk_qwen_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
         return dict(weights=w.value, sessions=s.value, workspace=k.value)
 
-    # -- sessions (QwenAudioCausalKVState, causal.py:44-57) ------------------------------------
     def open_session(self) -> int:
         sid = C.c_int32()
         L.check(self.lib.wlk_qwen_session_open(self.h, C.byref(sid)))
@@ -62,6 +62,41 @@ class QwenTowerEngine:
     def reset_session(self, sid: int) -> None:
         L.check(self.lib.wlk_qwen_session_reset(self.h, sid))
 
+    def _pack(self, sids, mels):
+        """(session ids, the mels [frames, n_mels] of every session back to back, frame offsets [n + 1])"""
+        n = len(sids)
+        if n != len(mels):
+            raise ValueError("sids and mels differ in length")
+        parts = [np.ascontiguousarray(m, np.float32).reshape(-1, self.dims.n_mels) for m in mels]
+        offs = np.zeros(n + 1, np.int32)
+        offs[1:] = np.cumsum([p.shape[0] for p in parts])
+        flat = np.concatenate(parts, axis=0) if offs[-1] else np.zeros((1, self.dims.n_mels), np.float32)
+        return np.asarray(list(sids), np.int32), flat, offs
+
+    def _device_out(self, cap: int):
+        import torch
+        out = torch.empty(max(cap, 1), self.dims.out_dim, dtype=torch.float32, device=f"cuda:{self.device}")
+        torch.cuda.current_stream(out.device).synchronize()   # the engine's stream does not order itself after torch's
+        return out
+
+    def close(self) -> None:
+        if not self._closed:
+            self._closed = True
+            L.check(self.lib.wlk_qwen_destroy(self.h))
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class QwenTowerEngine(_QwenEngineBase):
+    """The causal tower (wlk_qwen_create) over a QwenTowerDims geometry."""
+
+    _DIMS, _CREATE = L.wlk_qwen_dims, "wlk_qwen_create"
+
+    # -- sessions (QwenAudioCausalKVState, causal.py:44-57) ------------------------------------
     def _state(self, sid: int):
         p, e = C.c_int32(), C.c_int64()
         L.check(self.lib.wlk_qwen_session_state(self.h, sid, C.byref(p), C.byref(e)))
@@ -93,18 +128,13 @@ class QwenTowerEngine:
 
     # -- forward_chunk (causal.py:713-782), batched over sessions -----------------------------
     def _chunk_args(self, sids, mels):
-        n = len(sids)
-        if n != len(mels):
-            raise ValueError("sids and mels differ in length")
+        ids, flat, offs = self._pack(sids, mels)
         D = self.dims
-        parts = [np.ascontiguousarray(m, np.float32).reshape(-1, D.n_mels) for m in mels]
-        offs = np.zeros(n + 1, np.int32)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts, axis=0) if offs[-1] else np.zeros((1, D.n_mels), np.float32)
         consume = D.block_frames if D.block_frames > 0 else D.chunk_frames
-        cap = int(sum((self.pending_frames(s) + p.shape[0]) // consume * consume // D.chunk_frames for s, p in zip(sids, parts)))
-        cap += D.mutable_tail_steps * n                      # a mutable tail re-emits its steps with every call
-        return np.asarray(list(sids), np.int32), flat, offs, cap
+        cap = int(sum((self.pending_frames(s) + int(offs[i + 1] - offs[i])) // consume * consume // D.chunk_frames
+                      for i, s in enumerate(sids)))
+        cap += D.mutable_tail_steps * len(ids)               # a mutable tail re-emits its steps with every call
+        return ids, flat, offs, cap
 
     def forward_chunk(self, sids: Sequence[int], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
         ids, flat, offs, cap = self._chunk_args(sids, mels)
@@ -112,12 +142,6 @@ class QwenTowerEngine:
         rows = np.zeros(len(ids) + 1, np.int32)
         L.check(self.lib.wlk_qwen_forward_chunk(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
         return [out[rows[i]: rows[i + 1]].copy() for i in range(len(ids))]
-
-    def _device_out(self, cap: int):
-        import torch
-        out = torch.empty(max(cap, 1), self.dims.out_dim, dtype=torch.float32, device=f"cuda:{self.device}")
-        torch.cuda.current_stream(out.device).synchronize()   # the engine's stream does not order itself after torch's
-        return out
 
     def forward_chunk_device(self, sids: Sequence[int], mels: Sequence[np.ndarray]):
         """forward_chunk with the rows left on the device: (fp32 CUDA tensor [rows, out_dim], row offsets [n + 1])."""
@@ -177,68 +201,17 @@ class QwenTowerEngine:
         L.check(self.lib.wlk_qwen_flush_pending_device(self.h, _ptr(ids), len(ids), C.c_void_p(out.data_ptr()), cap, _ptr(rows)))
         return out[:int(rows[-1])], rows
 
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_qwen_destroy(self.h))
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class QwenWindowEngine:
+class QwenWindowEngine(_QwenEngineBase):
     """Host wrapper of the windowed Qwen3-ASR audio tower (wlk_qwen_window_* in include/wlk_b200.h).
 
     Mirrors QwenAudioSurgeryEncoder (third_party/qwen3-asr-causal/src/qwen3_asr_causal/model.py:441-608):
     ``forward_chunk(mels, state)`` becomes ``forward_chunk(sids, mels)`` over per-session device windows, batched over
     sessions; ``forward_full`` becomes ``encode``.  No CPU fallback."""
 
+    _DIMS, _CREATE = L.wlk_qwen_window_dims, "wlk_qwen_window_create"
     STATE_FIELDS = ("frames_seen", "window_start_frame", "emitted_steps", "last_input_frames", "last_recomputed_frames",
                     "last_recomputed_context_frames", "window_frames")
-
-    def __init__(self, dims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
-                 device: int = 0, max_sessions: int = 8, max_batch: int = 8, gemm_backend: str = "auto"):
-        self.lib = L.load()
-        self.dims = dims
-        self.precision = precision
-        self.device = int(device)
-        be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
-        cdims = L.wlk_qwen_window_dims(*dims.as_tuple())
-        cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
-                           max_sessions=max_sessions, max_batch=max_batch, gemm_backend=be[gemm_backend],
-                           attn_backend=L.BACKEND_SIMT, max_align_heads=0, reserved=0)
-        h = C.c_void_p()
-        L.check(self.lib.wlk_qwen_window_create(C.byref(cdims), C.byref(cfg), C.byref(h)))
-        self.h = h
-        self._closed = False
-        if state_dict is not None:
-            self.load_state_dict(state_dict)
-
-    def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
-        for name, arr in sd.items():
-            a = np.ascontiguousarray(arr, np.float32)
-            shape = (C.c_int64 * a.ndim)(*a.shape)
-            L.check(self.lib.wlk_qwen_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
-        L.check(self.lib.wlk_qwen_finalize_weights(self.h))
-
-    def memory(self) -> Dict[str, int]:
-        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        L.check(self.lib.wlk_qwen_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
-        return dict(weights=w.value, sessions=s.value, workspace=k.value)
-
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_qwen_session_open(self.h, C.byref(sid)))
-        return sid.value
-
-    def close_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_qwen_session_close(self.h, sid))
-
-    def reset_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_qwen_session_reset(self.h, sid))
 
     def state(self, sid: int) -> Dict[str, int]:
         """QwenAudioSurgeryState's counters (model.py:36-43) plus the frames the device window holds."""
@@ -246,23 +219,13 @@ class QwenWindowEngine:
         L.check(self.lib.wlk_qwen_window_state(self.h, sid, _ptr(f)))
         return dict(zip(self.STATE_FIELDS, (int(v) for v in f)))
 
-    def _args(self, sids, mels):
-        n = len(sids)
-        if n != len(mels):
-            raise ValueError("sids and mels differ in length")
-        parts = [np.ascontiguousarray(m, np.float32).reshape(-1, self.dims.n_mels) for m in mels]
-        offs = np.zeros(n + 1, np.int32)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts, axis=0) if offs[-1] else np.zeros((1, self.dims.n_mels), np.float32)
-        return np.asarray(list(sids), np.int32), flat, offs
-
     def _cap(self, n: int) -> int:
         from .qwen_dims import window_output_steps
         return n * window_output_steps(self.dims.window_frames)
 
     def forward_chunk(self, sids: Sequence[int], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
         """forward_chunk per session: new mel frames [frames, n_mels] in, the newly emitted rows [steps, out_dim] out."""
-        ids, flat, offs = self._args(sids, mels)
+        ids, flat, offs = self._pack(sids, mels)
         cap = self._cap(len(ids))
         out = np.zeros((max(cap, 1), self.dims.out_dim), np.float32)
         rows = np.zeros(len(ids) + 1, np.int32)
@@ -272,11 +235,9 @@ class QwenWindowEngine:
 
     def forward_chunk_device(self, sids: Sequence[int], mels: Sequence[np.ndarray]):
         """forward_chunk with the rows left on the device: (fp32 CUDA tensor [rows, out_dim], row offsets [n + 1])."""
-        import torch
-        ids, flat, offs = self._args(sids, mels)
+        ids, flat, offs = self._pack(sids, mels)
         cap = self._cap(len(ids))
-        out = torch.empty(max(cap, 1), self.dims.out_dim, dtype=torch.float32, device=f"cuda:{self.device}")
-        torch.cuda.current_stream(out.device).synchronize()   # the engine's stream does not order itself after torch's
+        out = self._device_out(cap)
         rows = np.zeros(len(ids) + 1, np.int32)
         L.check(self.lib.wlk_qwen_window_forward(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs),
                                                  C.c_void_p(out.data_ptr()), cap, _ptr(rows), 1))
@@ -285,23 +246,12 @@ class QwenWindowEngine:
     def encode(self, mels: Sequence[np.ndarray]) -> List[np.ndarray]:
         """forward_full: every row of each stateless window (at most left + right frames each)."""
         n = len(mels)
-        _, flat, offs = self._args(list(range(n)), mels)
+        _, flat, offs = self._pack(list(range(n)), mels)
         cap = self._cap(n)
         out = np.zeros((max(cap, 1), self.dims.out_dim), np.float32)
         rows = np.zeros(n + 1, np.int32)
         L.check(self.lib.wlk_qwen_window_encode(self.h, n, _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
         return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
-
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_qwen_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def window_attention(qkv, stream_rows: Sequence[int], block_rows: int, device: int = 0):

@@ -19,8 +19,40 @@ import numpy as np
 from .qwen_dims import QwenTowerDims
 
 
+class _SessionHandle:
+    """An engine session (``sid`` on ``engine``) that closes once, on close() or when the object is collected."""
+
+    def close(self):
+        if self.engine is not None:
+            self.engine.close_session(self.sid)
+            self.engine = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _check_mels(mels, n_mels: int):
+    if mels.ndim != 3:
+        raise ValueError("mels must have shape [batch, frames, n_mels]")
+    if mels.shape[-1] != n_mels:
+        raise ValueError(f"expected {n_mels} mel bins, got {mels.shape[-1]}")
+    if mels.shape[0] != 1:
+        raise ValueError("one stream per state: batch sessions through encode_rows")
+
+
+def _host_rows(hs, out_dim: int):
+    """Per-stream host rows -> (CPU tensor [total, out_dim], row offsets [N + 1])."""
+    import torch
+    offs = np.zeros(len(hs) + 1, np.int64)
+    offs[1:] = np.cumsum([h.shape[0] for h in hs])
+    return torch.from_numpy(np.ascontiguousarray(np.concatenate(hs) if hs else np.zeros((0, out_dim), np.float32))), offs
+
+
 @dataclass
-class B200QwenAudioState:
+class B200QwenAudioState(_SessionHandle):
     """Field-compatible with QwenAudioCausalKVState (causal.py:44-57) where callers read it."""
     sid: int
     engine: object = field(repr=False, default=None)
@@ -53,17 +85,6 @@ class B200QwenAudioState:
                 raise ValueError("mel_buffer must have shape [1, frames, n_mels]")
             m = value[0].detach().float().cpu().numpy() if hasattr(value, "detach") else np.asarray(value[0], np.float32)
         self.engine.set_pending(self.sid, m)      # like the reference, pending_frames follows at the next forward_chunk
-
-    def close(self):
-        if self.engine is not None:
-            self.engine.close_session(self.sid)
-            self.engine = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class B200QwenAudioCausalKVEncoder:
@@ -115,20 +136,11 @@ class B200QwenAudioCausalKVEncoder:
         state.pending_frames = self.engine.pending_frames(state.sid)
         state.mutable_steps = self.engine.mutable_steps(state.sid) if self.mutable_tail_steps else 0
 
-    def _check_mels(self, mels):
-        if mels.ndim != 3:
-            raise ValueError("mels must have shape [batch, frames, n_mels]")
-        if mels.shape[-1] != self.dims.n_mels:
-            raise ValueError(f"expected {self.dims.n_mels} mel bins, got {mels.shape[-1]}")
-        if mels.shape[0] != 1:
-            raise ValueError("one stream per state: batch sessions through engine.forward_chunk")
-
     def encode_rows(self, states, mels=None, flush: bool = False, device_rows: bool = True):
         """forward_chunk (flush=False, mels [1, frames, n_mels] per state) or flush_pending (flush=True) for N states in
         one engine call, with each state's fields updated as those two methods do.  Returns (rows [total, out_dim],
         row offsets [N + 1]): a CUDA tensor when the engine runs on the device and device_rows is set, else a CPU
         tensor."""
-        import torch
         if flush:
             before = [self.engine.pending_frames(s.sid) for s in states]
             sids = [s.sid for s in states]
@@ -139,7 +151,7 @@ class B200QwenAudioCausalKVEncoder:
                 hs = self.engine.flush_pending(sids)
         else:
             for m in mels:
-                self._check_mels(m)
+                _check_mels(m, self.dims.n_mels)
             ns = [int(m.shape[1]) for m in mels]
             for st, n in zip(states, ns):
                 st.last_input_frames = n
@@ -154,10 +166,7 @@ class B200QwenAudioCausalKVEncoder:
             else:
                 hs = self.engine.forward_chunk(sids, host)
         if not dev:
-            offs = np.zeros(len(states) + 1, np.int64)
-            offs[1:] = np.cumsum([h.shape[0] for h in hs])
-            rows = torch.from_numpy(np.ascontiguousarray(np.concatenate(hs) if hs else np.zeros((0, self.dims.out_dim),
-                                                                                              np.float32)))
+            rows, offs = _host_rows(hs, self.dims.out_dim)
         for i, st in enumerate(states):
             self._sync(st)
             if flush:
@@ -191,7 +200,7 @@ class B200QwenAudioCausalKVEncoder:
 
 
 @dataclass
-class B200QwenWindowState:
+class B200QwenWindowState(_SessionHandle):
     """Field-compatible with QwenAudioSurgeryState (reference model.py:36-43) where callers read it; the mel window
     itself lives on the device."""
     sid: int
@@ -202,17 +211,6 @@ class B200QwenWindowState:
     last_input_frames: int = 0
     last_recomputed_frames: int = 0
     last_recomputed_context_frames: int = 0
-
-    def close(self):
-        if self.engine is not None:
-            self.engine.close_session(self.sid)
-            self.engine = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class B200QwenAudioSurgeryEncoder:
@@ -290,33 +288,20 @@ class B200QwenAudioSurgeryEncoder:
     def init_state(self) -> B200QwenWindowState:
         return B200QwenWindowState(sid=self.engine.open_session(), engine=self.engine)
 
-    def _check_mels(self, mels):
-        if mels.ndim != 3:
-            raise ValueError("mels must have shape [batch, frames, n_mels]")
-        if mels.shape[-1] != self.dims.n_mels:
-            raise ValueError(f"expected {self.dims.n_mels} mel bins, got {mels.shape[-1]}")
-        if mels.shape[0] != 1:
-            raise ValueError("one stream per state: batch sessions through encode_rows")
-
     def encode_rows(self, states, mels, flush: bool = False, device_rows: bool = True):
         """forward_chunk for N states in one engine call, each state's fields updated as forward_chunk does.  Returns
         (rows [total, out_dim], row offsets [N + 1]): a CUDA tensor when the engine runs on the device and device_rows
         is set, else a CPU tensor."""
-        import torch
         if flush:
             raise ValueError("the windowed encoder has no flush: feed right_context_frames of zeros")
         for m in mels:
-            self._check_mels(m)
+            _check_mels(m, self.dims.n_mels)
         sids = [s.sid for s in states]
         host = [m[0].detach().float().cpu().numpy() for m in mels]
         if device_rows and hasattr(self.engine, "forward_chunk_device"):
             rows, offs = self.engine.forward_chunk_device(sids, host)
         else:
-            hs = self.engine.forward_chunk(sids, host)
-            offs = np.zeros(len(states) + 1, np.int64)
-            offs[1:] = np.cumsum([h.shape[0] for h in hs])
-            rows = torch.from_numpy(np.ascontiguousarray(np.concatenate(hs) if hs else np.zeros((0, self.dims.out_dim),
-                                                                                              np.float32)))
+            rows, offs = _host_rows(self.engine.forward_chunk(sids, host), self.dims.out_dim)
         for st in states:
             f = self.engine.state(st.sid)
             for k in ("frames_seen", "window_start_frame", "emitted_steps", "last_input_frames", "last_recomputed_frames",
@@ -327,7 +312,7 @@ class B200QwenAudioSurgeryEncoder:
     def forward_chunk(self, mels, state: Optional[B200QwenWindowState] = None):
         if state is None:
             state = self.init_state()
-        self._check_mels(mels)
+        _check_mels(mels, self.dims.n_mels)
         if mels.shape[1] == 0:                                             # model.py:568-570
             return mels.new_zeros(mels.shape[0], 0, self.dims.out_dim), state
         rows, _ = self.encode_rows([state], [mels], device_rows=False)
@@ -381,7 +366,7 @@ class B200StreamingMelExtractor:
         self._emitted = 0
 
 
-class B200DecoderRollingState:
+class B200DecoderRollingState(_SessionHandle):
     """Stands in for the reference's DecoderRollingState (model.py:53-68) in ``state.decoder``: the KV of
     [head + audio_steps] lives in an engine session, ``cache`` is that session's handle.  The session closes when the
     object is collected (segment rollover builds fresh decode states)."""
@@ -400,17 +385,6 @@ class B200DecoderRollingState:
 
     def get_seq_length(self) -> int:
         return self.engine.session_len(self.sid)
-
-    def close(self):
-        if self.engine is not None:
-            self.engine.close_session(self.sid)
-            self.engine = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class B200QwenTextDecoder:
