@@ -299,6 +299,37 @@ int wlk_qwen_window_state(wlk_qwen* q, int32_t sid, int64_t* fields);
  * blocks of block_rows rows start at its first row, the last one shorter (0 = one block per stream).               */
 int wlk_qwen_window_attention(int device, int precision, const void* qkv, void* out, int d_model, const int32_t* stream_rows,
                               int n_streams, int block_rows);
+/* Positional rows past the table (the causal engine): sin | cos of fp32(position) * inv_freq[j].  The optional tensor
+ * "positional_embedding.inv_freq" [d_model / 2] sets inv_freq; without it the engine evaluates the reference's recipe
+ * (exp of fp32(-ln(1e4) / (half - 1), a double rounded once) * j) with the host's expf, which can be one ulp away from the
+ * device's exp in a few entries, an error that grows with the position: hosts should load the tensor evaluated on the
+ * device (QwenTowerEngine does).
+ *
+ * ---- op-level entry points of the audio towers (kernel tests): one production launch on caller-owned device buffers,
+ *      with the engine's dims, precision and GEMM backend, on its stream, synchronized before returning.  "act" is fp32
+ *      in WLK_PREC_FP32 mode, bf16 otherwise.
+ * wlk_qwen_op_positions:  out fp32 [rows][d_model] = the positional rows of positions pos_host[r] in [0, 2^30): table rows
+ *                         inside the table, the closed form past it.  Needs only the positional table loaded.
+ * wlk_qwen_op_conv_stem:  the mode's conv stem over n_chunks chunks fp32 [n][T0][n_mels] (T0 = 8 causal, 100 windowed):
+ *                         a1 act [n][n_mels/2][T1][C], a2 act [n][n_mels/4][T2][C], a3 act [n][T3][n_mels/8][C]
+ *                         (T1 = T0 / 2, T2 = (T1 + 1) / 2, T3 = (T2 + 1) / 2).  Chunk k's conv input is p0_host[k] frames
+ *                         long; the windowed engine reads frames at or past avail_host[k] as zero (1 <= avail <= p0 <= 100),
+ *                         a causal chunk is 8 frames (avail = p0 = 8).  Steps past a stage's conv length are computed but
+ *                         meaningless.  Needs the conv2d1/2/3 tensors loaded; n_chunks is bounded by the conv workspace.
+ * wlk_qwen_op_qkv:        causal engine: the layer's QKV projection of xn act [rows][d_model] (rows <= max_batch * steps
+ *                         per round) with bias and head_dim^-0.5 on q -> q_out act [rows][d_model]; k and v of row r go to
+ *                         ring kv_ptrs_host[slot_host[r]] ([n_layer][K|V][n_head][ring][64] act, ring = left_context_steps
+ *                         + 128) at slot pos_host[r] % ring.  Needs that layer's q/k/v projections loaded.
+ * wlk_qwen_op_attention:  causal engine: one round's attention at a layer.  Job j owns the next n_steps_host[j] (1 .. 128)
+ *                         rows of q_dev / out_dev (act [rows][d_model], q pre-scaled) at positions start_host[j] .., its
+ *                         keys in ring kv_ptrs_host[j]; the engine's left context and block_bidirectional set the window. */
+int wlk_qwen_op_positions(wlk_qwen* q, const int32_t* pos_host, int32_t rows, float* out_dev);
+int wlk_qwen_op_conv_stem(wlk_qwen* q, const float* mel_dev, const int32_t* avail_host, const int32_t* p0_host, int32_t n_chunks,
+                          void* a1_dev, void* a2_dev, void* a3_dev);
+int wlk_qwen_op_qkv(wlk_qwen* q, int32_t layer, const void* xn_dev, const int32_t* slot_host, const int32_t* pos_host, int32_t rows,
+                    void* const* kv_ptrs_host, int32_t n_slots, void* q_out_dev);
+int wlk_qwen_op_attention(wlk_qwen* q, int32_t layer, const void* q_dev, const int32_t* start_host, const int32_t* n_steps_host,
+                          int32_t n_jobs, void* const* kv_ptrs_host, void* out_dev);
 
 /* =====================================================================================
  * Qwen3-ASR text decoder (HF Qwen3Model + lm_head, reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/

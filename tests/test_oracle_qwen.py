@@ -67,3 +67,29 @@ def test_sessions_are_independent_and_resettable():
     hb2 = orc.forward_chunk([b], [mels[:400]])[0]
     assert ha[0].shape[0] == 48 and ha[1].shape[0] == 24 and hb.shape[0] == 24
     np.testing.assert_allclose(hb2, ha[0], atol=1e-6)
+
+
+@pytest.mark.parametrize("d", [128, 896, 1024, 1280])
+def test_sinusoid_inv_freq_is_the_oracles_closed_form(d):
+    """The frequencies the engine loads for the positional rows past the table reproduce the oracle's closed form
+    (causal.py _position_embedding) bit for bit on the CPU, at the 0.6B width (896) and around it.  At 896 the scale
+    evaluated as an fp32 quotient of fp32 operands is one ulp away from the reference's double rounded once."""
+    import math
+
+    import torch
+    from oracle.qwen_oracle import QwenTowerOracle
+    from whisperlivekit_b200.qwen_dims import QwenTowerDims, sinusoid_inv_freq, sinusoid_table
+    T = 40
+    dims = QwenTowerDims(d_model=d, n_head=d // 64, max_positions=T)
+    orc = QwenTowerOracle(dims, {"positional_embedding.positional_embedding": sinusoid_table(T, d)})
+    inv = torch.from_numpy(sinusoid_inv_freq(d))
+    assert inv.dtype == torch.float32 and inv.shape == (d // 2,)
+    for offset, length in ((T, 24), (4095, 8), (45000, 24), (2 ** 20, 1)):
+        pos = torch.arange(offset, offset + length, dtype=torch.float32)
+        scaled = pos[:, None] * inv[None, :]
+        mine = torch.cat([scaled.sin(), scaled.cos()], dim=1)
+        assert torch.equal(mine, orc._pos(offset, length)), (d, offset)
+    half = d // 2
+    ref_scale = np.float32(-math.log(10000.0) / float(half - 1))
+    f32_scale = np.float32(-np.log(np.float32(10000.0))) / np.float32(half - 1)
+    assert (ref_scale != f32_scale) == (d == 896), (d, ref_scale, f32_scale)

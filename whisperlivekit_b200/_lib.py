@@ -104,6 +104,10 @@ SIGNATURES = {
     "wlk_qwen_window_encode": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, C.c_int64, _vp]),
     "wlk_qwen_window_state": (C.c_int, [_vp, C.c_int32, _vp]),
     "wlk_qwen_window_attention": (C.c_int, [C.c_int, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int]),
+    "wlk_qwen_op_positions": (C.c_int, [_vp, _vp, C.c_int32, _vp]),
+    "wlk_qwen_op_conv_stem": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp]),
+    "wlk_qwen_op_qkv": (C.c_int, [_vp, C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, _vp]),
+    "wlk_qwen_op_attention": (C.c_int, [_vp, C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp]),
     "wlk_qtext_create": (C.c_int, [_vp, _vp, _vp]),
     "wlk_qtext_destroy": (C.c_int, [_vp]),
     "wlk_qtext_load_tensor": (C.c_int, [_vp, C.c_char_p, _vp, _vp, C.c_int]),

@@ -101,6 +101,24 @@ struct WeightUpload {
     }
 };
 
+// Device copies of an op-level call's host index arrays, freed once the op's work on the stream is done.
+struct OpUpload {
+    cudaStream_t st;
+    std::vector<void*> bufs;
+    template <typename X>
+    const X* put(const X* host, size_t n) {
+        void* p = nullptr;
+        CUDA_CHECK(cudaMalloc(&p, (n > 1 ? n : 1) * sizeof(X)));
+        bufs.push_back(p);
+        CUDA_CHECK(cudaMemcpyAsync(p, host, n * sizeof(X), cudaMemcpyHostToDevice, st));
+        return (const X*)p;
+    }
+    ~OpUpload() {
+        cudaStreamSynchronize(st);
+        for (void* p : bufs) cudaFree(p);
+    }
+};
+
 inline int64_t numel(const int64_t* shape, int ndim) {
     int64_t n = 1;
     for (int i = 0; i < ndim; ++i) n *= shape[i];

@@ -113,9 +113,10 @@ __global__ void qwen_im2col_kernel(const T* __restrict__ src, const WChunk* __re
     }
 }
 
-// positional rows: table[pos] while pos is inside the table, else the closed form (reference causal.py:204-228)
-__global__ void qwen_pos_kernel(const int32_t* __restrict__ pos, const float* __restrict__ table, int max_positions,
-                                float* __restrict__ out, int rows, int d) {
+// positional rows: table[pos] while pos is inside the table, else the closed form sin | cos of fp32(pos) * inv_freq[j]
+// (reference causal.py:204-228; inv_freq [d / 2] holds the reference's fp32 frequencies, see load_tensor)
+__global__ void qwen_pos_kernel(const int32_t* __restrict__ pos, const float* __restrict__ table, const float* __restrict__ inv_freq,
+                                int max_positions, float* __restrict__ out, int rows, int d) {
     const int r = blockIdx.x;
     if (r >= rows) return;
     const int p = pos[r];
@@ -125,9 +126,7 @@ __global__ void qwen_pos_kernel(const int32_t* __restrict__ pos, const float* __
         if (p < max_positions) {
             v = table[(int64_t)p * d + i];
         } else {
-            const int j = i < half ? i : i - half;
-            const float inv = expf(-logf(10000.0f) / (float)max(1, half - 1) * (float)j);
-            const float a = (float)p * inv;
+            const float a = (float)p * inv_freq[i < half ? i : i - half];
             v = i < half ? sinf(a) : cosf(a);
         }
         out[(int64_t)r * d + i] = v;
@@ -235,13 +234,13 @@ struct wlk_qwen {
     wlk_qwen_dims dims{};
     wlk_config cfg{};
     int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
-    int ring = 0, max_rows = 0;
+    int ring = 0, max_rows = 0, conv_chunks = 0;                 // conv_chunks: chunks the conv stem's workspace holds
     cudaStream_t st = nullptr;
     std::mutex mu;
     DeviceAllocs allocs;
     size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
     // weights
-    float *c1w = nullptr, *c1b = nullptr, *c2b = nullptr, *c3b = nullptr, *bout = nullptr, *pos_table = nullptr;
+    float *c1w = nullptr, *c1b = nullptr, *c2b = nullptr, *c3b = nullptr, *bout = nullptr, *pos_table = nullptr, *pos_inv = nullptr;
     void *W2c = nullptr, *W3c = nullptr, *Wout = nullptr, *Wp1 = nullptr, *Wp2 = nullptr;
     float *lnpw = nullptr, *lnpb = nullptr, *bp1 = nullptr, *bp2 = nullptr;
     float *filtT = nullptr, *window = nullptr; float2* twiddle = nullptr; int2* filt_span = nullptr;   // mel front end
@@ -333,6 +332,7 @@ void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const 
         expect_shape(name.c_str(), shape, ndim, {D.max_positions, d});
         q->upload.put(host, n, q->pos_table, DT_F32, q->st);
     }
+    else if (name == "positional_embedding.inv_freq") vec(q->pos_inv, d / 2);   // optional: the host's own frequencies
     else if (name == "ln_post.weight") vec(q->lnpw, d);
     else if (name == "ln_post.bias") vec(q->lnpb, d);
     else if (name == "proj1.weight") mat(q->Wp1, d, d);
@@ -400,6 +400,7 @@ void alloc_weights(wlk_qwen* q) {
     q->W2c = q->allocs.take((size_t)C * 9 * C * es, aw); q->W3c = q->allocs.take((size_t)C * 9 * C * es, aw);
     q->Wout = q->allocs.take((size_t)d * C * F * es, aw); q->bout = (float*)q->allocs.take(d * 4, aw);
     q->pos_table = (float*)q->allocs.take((size_t)D.max_positions * d * 4, aw);
+    q->pos_inv = (float*)q->allocs.take((size_t)(d / 2) * 4, aw);
     q->lnpw = (float*)q->allocs.take(d * 4, aw); q->lnpb = (float*)q->allocs.take(d * 4, aw);
     q->Wp1 = q->allocs.take((size_t)d * d * es, aw); q->bp1 = (float*)q->allocs.take(d * 4, aw);
     q->Wp2 = q->allocs.take((size_t)D.out_dim * d * es, aw); q->bp2 = (float*)q->allocs.take(D.out_dim * 4, aw);
@@ -428,6 +429,17 @@ void alloc_weights(wlk_qwen* q) {
         CUDA_CHECK(cudaMemcpyAsync(q->twiddle, tw.data(), N_FFT * 8, cudaMemcpyHostToDevice, q->st));
         CUDA_CHECK(cudaStreamSynchronize(q->st));
     }
+    {   // default frequencies of the closed-form positional rows, the reference's recipe: the scale -ln(1e4) / (half - 1)
+        // is a double rounded once to fp32, times fp32(j), then fp32 exp.  The host's expf may still differ from the
+        // device's exp by an ulp in a few entries, so hosts load "positional_embedding.inv_freq" evaluated on the device
+        // (whisperlivekit_b200/qwen_engine.py always does)
+        const int half = d / 2;
+        const float scale = (float)(-std::log(10000.0) / (double)std::max(1, half - 1));
+        std::vector<float> f(half);
+        for (int j = 0; j < half; ++j) f[j] = std::exp(scale * (float)j);
+        CUDA_CHECK(cudaMemcpyAsync(q->pos_inv, f.data(), f.size() * 4, cudaMemcpyHostToDevice, q->st));
+        CUDA_CHECK(cudaStreamSynchronize(q->st));
+    }
 }
 
 // The creation both modes share: the checks on the shared geometry, device, precision and GEMM backend, stream, weights,
@@ -448,6 +460,7 @@ wlk_qwen* create_common(const wlk_qwen_dims& D, const wlk_config* cfg, int max_r
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     q->max_rows = max_rows;
+    q->conv_chunks = (int)conv_chunks;
     CUDA_CHECK(cudaStreamCreateWithFlags(&q->st, cudaStreamNonBlocking));
     alloc_weights(q);
     const size_t es = q->es(), R = (size_t)max_rows, CH = conv_chunks;
@@ -540,6 +553,21 @@ void conv_stem(wlk_qwen* q, const WChunk* chunks_dev, int nc) {
         qgemm(q, g); }
 }
 
+// The QKV projection of layer li over rows [0, R) of xn (causal.py:343-346): bias, head_dim^-0.5 on the q columns;
+// dst(epi) points the epilogue at the mode's destination
+template <typename QkvDst>
+void qkv_gemm(wlk_qwen* q, int li, const void* xn, int R, QkvDst dst) {
+    const int d = q->dims.d_model;
+    const QLayerW& L = q->L[li];
+    GemmArgs g;
+    g.A = xn; g.a_type = q->act; g.lda = d; g.W = L.Wqkv; g.w_type = q->act; g.ldw = d;
+    g.M = R; g.N = 3 * d; g.K = d;
+    g.epi.bias = L.bqkv; g.epi.col_scale = 0.125f; g.epi.scale_cols = d;
+    g.epi.c_type = q->act;
+    dst(g.epi);
+    qgemm(q, g);
+}
+
 // The n_layer pre-LN layers over rows [0, R) of q->x (causal.py:378-421): LN, QKV, attention, out-proj + residual, LN,
 // fc1 + GELU, fc2 + residual.  qkv_dst(epi, layer) points the QKV GEMM's epilogue at the mode's destination; attend(layer)
 // runs the mode's attention from there into q->att.
@@ -550,13 +578,7 @@ void run_layers(wlk_qwen* q, int R, QkvDst qkv_dst, Attend attend) {
     for (int li = 0; li < D.n_layer; ++li) {
         QLayerW& L = q->L[li];
         layernorm(q->x, d, L.ln1w, L.ln1b, q->xn, q->act, d, R, d, nullptr, q->st);
-        {   GemmArgs g;
-            g.A = q->xn; g.a_type = q->act; g.lda = d; g.W = L.Wqkv; g.w_type = q->act; g.ldw = d;
-            g.M = R; g.N = 3 * d; g.K = d;
-            g.epi.bias = L.bqkv; g.epi.col_scale = 0.125f; g.epi.scale_cols = d;          // head_dim^-0.5 on q (causal.py:343-346)
-            g.epi.c_type = q->act;
-            qkv_dst(g.epi, li);
-            qgemm(q, g); }
+        qkv_gemm(q, li, q->xn, R, [&](Epilogue& e) { qkv_dst(e, li); });
         attend(li);
         {   GemmArgs g;
             g.A = q->att; g.a_type = q->act; g.lda = d; g.W = L.Wo; g.w_type = q->act; g.ldw = d;
@@ -598,15 +620,37 @@ void run_head(wlk_qwen* q, int rows, const int32_t* row_idx) {
     CUDA_CHECK(cudaGetLastError());
 }
 
+// the positional rows of `rows` absolute positions (device array) -> out fp32 [rows][d]
+void launch_positions(wlk_qwen* q, const int32_t* pos_dev, float* out, int rows) {
+    qwen_pos_kernel<<<rows, 128, 0, q->st>>>(pos_dev, q->pos_table, q->pos_inv, q->dims.max_positions, out, rows, q->dims.d_model);
+}
+
+// the causal QKV destination: q -> qout [R][d]; k / v of row r -> ring kv_ptrs[slot[r]], layer li, ring slot ringpos[r]
+void causal_qkv_dst(wlk_qwen* q, Epilogue& e, int li, void* qout, void* const* kv_ptrs_dev, const int32_t* slot_dev,
+                    const int32_t* ringpos_dev) {
+    const wlk_qwen_dims& D = q->dims;
+    e.mode = EPI_SELF_QKV; e.C = qout; e.ldc = D.d_model;
+    e.batch_ptrs = kv_ptrs_dev; e.row_slot = slot_dev; e.row_pos = ringpos_dev;
+    e.layer = li; e.n_head = D.n_head; e.d_model = D.d_model; e.kv_len = q->ring;
+}
+
+// the causal attention of a round's jobs at layer li: q act [R][d] -> out act [R][d]
+template <typename T>
+void launch_causal_attention(wlk_qwen* q, int li, const void* qin, const QJob* jobs_dev, int n_jobs, void* out) {
+    const wlk_qwen_dims& D = q->dims;
+    qwen_attention_kernel<T><<<dim3(D.n_head, n_jobs), 128, 0, q->st>>>((const T*)qin, jobs_dev, li, D.n_head, D.d_model, q->ring,
+                                                                        D.left_context_steps, D.block_bidirectional, (T*)out);
+}
+
 // one causal round: R steps, one 8-frame chunk each, staged in q->mel; the sinusoid rows of their absolute positions
 // ride into conv_out as the GEMM's residual; the QKV GEMM scatters k / v into the session rings
 template <typename T>
 void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, const WChunk* chunks_dev, void* const* kv_ptrs_dev,
                      const int32_t* slot_dev, const int32_t* ringpos_dev, const int32_t* abspos_dev) {
     const wlk_qwen_dims& D = q->dims;
-    const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, H = D.n_head;
+    const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8;
     conv_stem<T, 8>(q, chunks_dev, R);
-    qwen_pos_kernel<<<R, 128, 0, q->st>>>(abspos_dev, q->pos_table, D.max_positions, q->posbuf, R, d);
+    launch_positions(q, abspos_dev, q->posbuf, R);
     {   GemmArgs g;
         g.A = q->a3; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
         g.M = R; g.N = d; g.K = F * C;
@@ -614,17 +658,8 @@ void run_round_typed(wlk_qwen* q, int n_jobs, int R, const QJob* jobs_dev, const
         g.epi.C = q->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
         qgemm(q, g); }
     CUDA_CHECK(cudaGetLastError());
-    run_layers(q, R,
-               [&](Epilogue& e, int li) {
-                   e.mode = EPI_SELF_QKV; e.C = q->qb; e.ldc = d;
-                   e.batch_ptrs = kv_ptrs_dev; e.row_slot = slot_dev; e.row_pos = ringpos_dev;
-                   e.layer = li; e.n_head = H; e.d_model = d; e.kv_len = q->ring;
-               },
-               [&](int li) {
-                   qwen_attention_kernel<T><<<dim3(H, n_jobs), 128, 0, q->st>>>((const T*)q->qb, jobs_dev, li, H, d, q->ring,
-                                                                               D.left_context_steps, D.block_bidirectional,
-                                                                               (T*)q->att);
-               });
+    run_layers(q, R, [&](Epilogue& e, int li) { causal_qkv_dst(q, e, li, q->qb, kv_ptrs_dev, slot_dev, ringpos_dev); },
+               [&](int li) { launch_causal_attention<T>(q, li, q->qb, jobs_dev, n_jobs, q->att); });
     run_head(q, R, nullptr);
 }
 
@@ -1101,6 +1136,11 @@ void attn_items(const std::vector<int>& row_off, const std::vector<int>& rows, c
 
 constexpr int QW_ATTN_SMEM = 2 * QW_KMAX * QW_KSTRIDE * 2;      // staged K and V of one block, bf16
 
+// the mel frames of nc windowed chunks -> q->mel [nc][100][n_mels], zero at and past each chunk's avail
+void launch_gather(wlk_qwen* q, const WChunk* chunks_dev, int nc) {
+    qwin_gather_kernel<<<grid_1d((int64_t)nc * QW_T0 * q->dims.n_mels), 256, 0, q->st>>>(chunks_dev, q->mel, nc, q->dims.n_mels);
+}
+
 // the bf16 kernel's dynamic shared memory exceeds the default 48 KB: opt in once per device (at create, or per op call)
 void window_attention_opt_in() {
     CUDA_CHECK(cudaFuncSetAttribute(qwin_attn_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QW_ATTN_SMEM));
@@ -1190,7 +1230,7 @@ int64_t run_windows(wlk_qwen* q, const std::vector<const float*>& wins, const st
     for (size_t c0 = 0; c0 < chunks.size(); c0 += QW_CHUNKS_PER_ROUND) {
         const int nc = (int)std::min<size_t>(QW_CHUNKS_PER_ROUND, chunks.size() - c0);
         const WChunk* jd = chunks_dev + c0;
-        qwin_gather_kernel<<<grid_1d((int64_t)nc * QW_T0 * W.n_mels), 256, 0, q->st>>>(jd, q->mel, nc, W.n_mels);
+        launch_gather(q, jd, nc);
         conv_stem<T, QW_T0>(q, jd, nc);
         {   GemmArgs g;
             g.A = q->a3; g.a_type = q->act; g.lda = (int64_t)F * C; g.W = q->Wout; g.w_type = q->act; g.ldw = (int64_t)F * C;
@@ -1326,6 +1366,103 @@ void window_encode(wlk_qwen* q, int n, const float* mels, const int32_t* frame_o
     }
     const int64_t E = run_windows_any(q, wins, wlen, lo, hi);
     CUDA_CHECK(cudaMemcpyAsync(out, q->outbuf, (size_t)E * W.out_dim * 4, cudaMemcpyDeviceToHost, q->st));
+    CUDA_CHECK(cudaStreamSynchronize(q->st));
+}
+
+// ---- op-level entry points (kernel tests): one production launch on caller-owned device buffers, with the engine's
+//      dims, precision and GEMM backend, on its stream, synchronized before returning ---------------------------------
+void op_require(const wlk_qwen* q, std::initializer_list<std::string> names) {
+    for (const std::string& n : names) WLK_CHECK(q->loaded.count(n), "tensor %s is not loaded", n.c_str());
+}
+
+void op_positions(wlk_qwen* q, const int32_t* pos, int rows, float* out) {
+    WLK_CHECK(pos && out, "null argument");
+    WLK_CHECK(rows >= 1 && rows <= (1 << 20), "rows %d outside [1, %d]", rows, 1 << 20);
+    op_require(q, {"positional_embedding.positional_embedding"});
+    for (int r = 0; r < rows; ++r) WLK_CHECK(pos[r] >= 0 && pos[r] < (1 << 30), "row %d: position %d outside [0, 2^30)", r, pos[r]);
+    OpUpload up{q->st};
+    launch_positions(q, up.put(pos, rows), out, rows);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(q->st));
+}
+
+void op_conv_stem(wlk_qwen* q, const float* mel, const int32_t* avail, const int32_t* p0, int n, void* a1, void* a2, void* a3) {
+    const wlk_qwen_dims& D = q->dims;
+    WLK_CHECK(mel && avail && p0 && a1 && a2 && a3, "null argument");
+    WLK_CHECK(n >= 1 && n <= q->conv_chunks, "%d chunks outside [1, %d] (the conv stem's workspace)", n, q->conv_chunks);
+    op_require(q, {"conv2d1.weight", "conv2d1.bias", "conv2d2.weight", "conv2d2.bias", "conv2d3.weight", "conv2d3.bias"});
+    const int T0 = q->windowed ? QW_T0 : 8;
+    std::vector<WChunk> chunks(n);
+    for (int k = 0; k < n; ++k) {
+        if (q->windowed)
+            WLK_CHECK(avail[k] >= 1 && avail[k] <= p0[k] && p0[k] <= T0, "chunk %d: avail %d, p0 %d (need 1 <= avail <= p0 <= %d)",
+                      k, avail[k], p0[k], T0);
+        else
+            WLK_CHECK(avail[k] == 8 && p0[k] == 8, "chunk %d: a causal chunk is 8 frames (avail %d, p0 %d)", k, avail[k], p0[k]);
+        chunks[k] = WChunk{mel + (size_t)k * T0 * D.n_mels, avail[k], p0[k], k, 0};
+    }
+    OpUpload up{q->st};
+    const WChunk* chunks_dev = up.put(chunks.data(), n);
+    if (q->windowed) launch_gather(q, chunks_dev, n);
+    else CUDA_CHECK(cudaMemcpyAsync(q->mel, mel, (size_t)n * 8 * D.n_mels * 4, cudaMemcpyDeviceToDevice, q->st));
+    if (q->act == DT_F32) { if (q->windowed) conv_stem<float, QW_T0>(q, chunks_dev, n); else conv_stem<float, 8>(q, chunks_dev, n); }
+    else { if (q->windowed) conv_stem<bf16, QW_T0>(q, chunks_dev, n); else conv_stem<bf16, 8>(q, chunks_dev, n); }
+    CUDA_CHECK(cudaGetLastError());
+    const int T1 = T0 / 2, T2 = (T1 + 1) / 2, T3 = (T2 + 1) / 2;
+    const size_t row = (size_t)D.conv_channels * q->es();
+    CUDA_CHECK(cudaMemcpyAsync(a1, q->a1, (size_t)n * (D.n_mels / 2) * T1 * row, cudaMemcpyDeviceToDevice, q->st));
+    CUDA_CHECK(cudaMemcpyAsync(a2, q->a2, (size_t)n * (D.n_mels / 4) * T2 * row, cudaMemcpyDeviceToDevice, q->st));
+    CUDA_CHECK(cudaMemcpyAsync(a3, q->a3, (size_t)n * T3 * (D.n_mels / 8) * row, cudaMemcpyDeviceToDevice, q->st));
+    CUDA_CHECK(cudaStreamSynchronize(q->st));
+}
+
+void op_qkv(wlk_qwen* q, int layer, const void* xn, const int32_t* slot, const int32_t* pos, int rows, void* const* kv,
+            int n_slots, void* qout) {
+    WLK_CHECK(!q->windowed, "a windowed engine has no K/V rings");
+    WLK_CHECK(xn && slot && pos && kv && qout, "null argument");
+    WLK_CHECK(layer >= 0 && layer < q->dims.n_layer, "layer %d outside [0, %d)", layer, q->dims.n_layer);
+    WLK_CHECK(rows >= 1 && rows <= q->max_rows, "rows %d outside [1, %d]", rows, q->max_rows);
+    WLK_CHECK(n_slots >= 1, "no K/V rings");
+    const std::string p = "layers." + std::to_string(layer) + ".self_attn.";
+    op_require(q, {p + "q_proj.weight", p + "k_proj.weight", p + "v_proj.weight", p + "q_proj.bias", p + "k_proj.bias",
+                   p + "v_proj.bias"});
+    std::vector<int32_t> ringpos(rows);
+    for (int r = 0; r < rows; ++r) {
+        WLK_CHECK(slot[r] >= 0 && slot[r] < n_slots, "row %d: slot %d outside [0, %d)", r, slot[r], n_slots);
+        WLK_CHECK(kv[slot[r]] != nullptr, "row %d: slot %d has no K/V ring", r, slot[r]);
+        WLK_CHECK(pos[r] >= 0 && pos[r] < (1 << 30), "row %d: position %d outside [0, 2^30)", r, pos[r]);
+        ringpos[r] = pos[r] % q->ring;
+    }
+    OpUpload up{q->st};
+    const int32_t* slot_d = up.put(slot, rows);
+    const int32_t* ring_d = up.put(ringpos.data(), rows);
+    void* const* kv_d = up.put(kv, n_slots);
+    qkv_gemm(q, layer, xn, rows, [&](Epilogue& e) { causal_qkv_dst(q, e, layer, qout, kv_d, slot_d, ring_d); });
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(q->st));
+}
+
+void op_attention(wlk_qwen* q, int layer, const void* qin, const int32_t* start, const int32_t* n_steps, int n_jobs,
+                  void* const* kv, void* out) {
+    WLK_CHECK(!q->windowed, "a windowed engine has no K/V rings");
+    WLK_CHECK(n_jobs >= 1 && n_jobs <= 65535, "%d jobs outside [1, 65535]", n_jobs);
+    WLK_CHECK(qin && start && n_steps && kv && out, "null argument");
+    WLK_CHECK(layer >= 0 && layer < q->dims.n_layer, "layer %d outside [0, %d)", layer, q->dims.n_layer);
+    std::vector<QJob> jobs(n_jobs);
+    int row = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        WLK_CHECK(n_steps[j] >= 1 && n_steps[j] <= Q_STEPS_CAP, "job %d: n_steps %d outside [1, %d]", j, n_steps[j], Q_STEPS_CAP);
+        WLK_CHECK(start[j] >= 0, "job %d: negative start %d", j, start[j]);
+        WLK_CHECK((int64_t)start[j] + n_steps[j] < ((int64_t)1 << 30), "job %d: stream position overflow", j);
+        WLK_CHECK(kv[j] != nullptr, "job %d has no K/V ring", j);
+        jobs[j] = QJob{kv[j], start[j], n_steps[j], row, 0};
+        row += n_steps[j];
+    }
+    OpUpload up{q->st};
+    const QJob* jobs_d = up.put(jobs.data(), n_jobs);
+    if (q->act == DT_F32) launch_causal_attention<float>(q, layer, qin, jobs_d, n_jobs, out);
+    else launch_causal_attention<bf16>(q, layer, qin, jobs_d, n_jobs, out);
+    CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaStreamSynchronize(q->st));
 }
 
@@ -1537,6 +1674,33 @@ int wlk_qwen_window_attention(int device, int precision, const void* qkv, void* 
     }
     cudaFree(items_dev);
     CUDA_CHECK(ce);
+    WLK_API_END
+}
+int wlk_qwen_op_positions(wlk_qwen* q, const int32_t* pos_host, int32_t rows, float* out_dev) {
+    WLK_API_BEGIN
+    WLK_ENTER(q, q->cfg.device);
+    op_positions(q, pos_host, rows, out_dev);
+    WLK_API_END
+}
+int wlk_qwen_op_conv_stem(wlk_qwen* q, const float* mel_dev, const int32_t* avail_host, const int32_t* p0_host, int32_t n_chunks,
+                          void* a1_dev, void* a2_dev, void* a3_dev) {
+    WLK_API_BEGIN
+    WLK_ENTER(q, q->cfg.device);
+    op_conv_stem(q, mel_dev, avail_host, p0_host, n_chunks, a1_dev, a2_dev, a3_dev);
+    WLK_API_END
+}
+int wlk_qwen_op_qkv(wlk_qwen* q, int32_t layer, const void* xn_dev, const int32_t* slot_host, const int32_t* pos_host, int32_t rows,
+                    void* const* kv_ptrs_host, int32_t n_slots, void* q_out_dev) {
+    WLK_API_BEGIN
+    WLK_ENTER(q, q->cfg.device);
+    op_qkv(q, layer, xn_dev, slot_host, pos_host, rows, kv_ptrs_host, n_slots, q_out_dev);
+    WLK_API_END
+}
+int wlk_qwen_op_attention(wlk_qwen* q, int32_t layer, const void* q_dev, const int32_t* start_host, const int32_t* n_steps_host,
+                          int32_t n_jobs, void* const* kv_ptrs_host, void* out_dev) {
+    WLK_API_BEGIN
+    WLK_ENTER(q, q->cfg.device);
+    op_attention(q, layer, q_dev, start_host, n_steps_host, n_jobs, kv_ptrs_host, out_dev);
     WLK_API_END
 }
 int wlk_qwen_memory(wlk_qwen* q, size_t* weights, size_t* sessions, size_t* workspace) {

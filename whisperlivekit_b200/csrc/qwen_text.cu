@@ -1009,23 +1009,6 @@ void logits_out(wlk_qtext* t, int row0, int rows, float* out) {
 }
 
 // ---- op-level entry points: one kernel of a round on caller-owned device buffers ----------------------------------
-// Device copies of an op call's host index arrays, freed once the op's work on the stream is done.
-struct OpUpload {
-    wlk_qtext* t;
-    std::vector<void*> bufs;
-    template <typename X>
-    const X* put(const X* host, size_t n) {
-        void* p = nullptr;
-        CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(X)));
-        bufs.push_back(p);
-        CUDA_CHECK(cudaMemcpyAsync(p, host, n * sizeof(X), cudaMemcpyHostToDevice, t->st));
-        return (const X*)p;
-    }
-    ~OpUpload() {
-        cudaStreamSynchronize(t->st);
-        for (void* p : bufs) cudaFree(p);
-    }
-};
 
 void op_rows(int rows) { WLK_CHECK(rows >= 1 && rows <= QT_ROUND_ROWS, "rows %d outside [1, %d]", rows, QT_ROUND_ROWS); }
 
@@ -1056,7 +1039,7 @@ void op_rmsnorm(wlk_qtext* t, const float* x, const float* w, void* out, int row
     WLK_CHECK(x && w && out, "null argument");
     op_rows(rows);
     if (out_row) for (int r = 0; r < rows; ++r) WLK_CHECK(out_row[r] >= -1, "row %d: output row %d", r, out_row[r]);
-    OpUpload up{t};
+    OpUpload up{t->st};
     const int32_t* out_row_d = out_row ? up.put(out_row, rows) : nullptr;
     if (t->act == DT_F32) launch_rmsnorm<float>(t, x, w, out, out_row_d, rows, t->dims.rms_eps);
     else launch_rmsnorm<bf16>(t, x, w, out, out_row_d, rows, t->dims.rms_eps);
@@ -1068,7 +1051,7 @@ void op_qk_rope(wlk_qtext* t, const float* qkv, const float* qn, const float* kn
                 void* const* kv, int n_slots, int layer, void* qout) {
     WLK_CHECK(qkv && qn && kn && pos && slot && kv && qout, "null argument");
     op_check_rows(t, pos, slot, rows, kv, n_slots, layer, false);
-    OpUpload up{t};
+    OpUpload up{t->st};
     const int32_t* pos_d = up.put(pos, rows);
     const int32_t* slot_d = up.put(slot, rows);
     void* const* kv_d = up.put(kv, n_slots);
@@ -1084,7 +1067,7 @@ void op_attention(wlk_qtext* t, const void* q, const int32_t* pos, const int32_t
     op_check_rows(t, pos, slot, rows, kv, n_slots, layer, true);
     std::vector<QTAttnTile> tiles(rows);
     const int n_tiles = make_tiles(pos, slot, rows, tiles.data());
-    OpUpload up{t};
+    OpUpload up{t->st};
     const int32_t* pos_d = up.put(pos, rows);
     const int32_t* slot_d = up.put(slot, rows);
     void* const* kv_d = up.put(kv, n_slots);

@@ -130,6 +130,19 @@ def sinusoid_table(max_positions: int, d_model: int) -> np.ndarray:
     return np.concatenate([np.sin(scaled), np.cos(scaled)], axis=1).astype(np.float32)
 
 
+def sinusoid_inv_freq(d_model: int, device="cpu") -> np.ndarray:
+    """Inverse frequencies [d_model / 2] of the positional rows past the table, exactly as the reference's closed form
+    computes them (causal.py ``_position_embedding``): the scale ``-ln(1e4) / (half - 1)`` is a Python double, rounded
+    to fp32 once when torch multiplies it into the fp32 ``arange``, then fp32 ``exp`` on ``device``.  An fp32 quotient
+    of fp32 operands can land one ulp away (it does at d_model 896), and the angle error grows with the position."""
+    import math
+
+    import torch
+    half = d_model // 2
+    inv = torch.exp(-math.log(10000.0) / float(max(1, half - 1)) * torch.arange(half, device=device, dtype=torch.float32))
+    return inv.cpu().numpy().astype(np.float32)
+
+
 def synthetic_tower_state_dict(dims: QwenTowerDims, seed: int = 0) -> Dict[str, np.ndarray]:
     """Seeded weights with the tower's own parameter names, scaled for unit-variance activations."""
     rng = np.random.default_rng(seed)

@@ -12,6 +12,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib as L
+from .qwen_dims import sinusoid_inv_freq
 
 
 def _ptr(a: np.ndarray):
@@ -36,14 +37,20 @@ class _QwenEngineBase:
         L.check(getattr(self.lib, self._CREATE)(C.byref(cdims), C.byref(cfg), C.byref(h)))
         self.h = h
         self._closed = False
+        # the reference's fp32 frequencies of the positional rows past the table, evaluated on this device like the
+        # reference evaluates them on its own
+        self.load_tensor("positional_embedding.inv_freq", sinusoid_inv_freq(dims.d_model, f"cuda:{self.device}"))
         if state_dict is not None:
             self.load_state_dict(state_dict)
 
+    def load_tensor(self, name: str, arr) -> None:
+        a = np.ascontiguousarray(arr, np.float32)
+        shape = (C.c_int64 * a.ndim)(*a.shape)
+        L.check(self.lib.wlk_qwen_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
+
     def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
         for name, arr in sd.items():
-            a = np.ascontiguousarray(arr, np.float32)
-            shape = (C.c_int64 * a.ndim)(*a.shape)
-            L.check(self.lib.wlk_qwen_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
+            self.load_tensor(name, arr)
         L.check(self.lib.wlk_qwen_finalize_weights(self.h))
 
     def memory(self) -> Dict[str, int]:
@@ -78,6 +85,44 @@ class _QwenEngineBase:
         out = torch.empty(max(cap, 1), self.dims.out_dim, dtype=torch.float32, device=f"cuda:{self.device}")
         torch.cuda.current_stream(out.device).synchronize()   # the engine's stream does not order itself after torch's
         return out
+
+    # -- op-level (device pointers, e.g. torch tensors' data_ptr(); "act" is fp32 or bf16 as the precision) ------------
+    def op_positions(self, positions: Sequence[int], out_ptr) -> None:
+        """The positional rows fp32 [rows][d_model] of absolute positions: table rows, the closed form past the table."""
+        pos = np.ascontiguousarray(positions, np.int32)
+        L.check(self.lib.wlk_qwen_op_positions(self.h, _ptr(pos), len(pos), out_ptr))
+
+    def op_conv_stem(self, mel_ptr, avail: Sequence[int], p0: Sequence[int], a1_ptr, a2_ptr, a3_ptr) -> None:
+        """The mode's conv stem over chunks fp32 [n][T0][n_mels] (T0 = 8 causal, 100 windowed) -> the three activations
+        in act: a1 [n][n_mels/2][T1][C], a2 [n][n_mels/4][T2][C], a3 [n][T3][n_mels/8][C]."""
+        av = np.ascontiguousarray(avail, np.int32)
+        pz = np.ascontiguousarray(p0, np.int32)
+        if len(av) != len(pz):
+            raise ValueError("avail and p0 differ in length")
+        L.check(self.lib.wlk_qwen_op_conv_stem(self.h, mel_ptr, _ptr(av), _ptr(pz), len(av), a1_ptr, a2_ptr, a3_ptr))
+
+    def op_qkv(self, layer: int, xn_ptr, row_slot: Sequence[int], row_pos: Sequence[int], kv_ptrs: Sequence[int],
+               q_out_ptr) -> None:
+        """Causal engine: the QKV projection of xn act [rows][d_model] with the round's epilogue (bias, head_dim^-0.5 on
+        q) -> q act [rows][d_model], k / v into ring kv_ptrs[row_slot[r]] at slot row_pos[r] % ring of layer."""
+        slot = np.ascontiguousarray(row_slot, np.int32)
+        pos = np.ascontiguousarray(row_pos, np.int32)
+        if len(slot) != len(pos):
+            raise ValueError("row_slot and row_pos differ in length")
+        kv = (C.c_void_p * len(kv_ptrs))(*[int(p) for p in kv_ptrs])
+        L.check(self.lib.wlk_qwen_op_qkv(self.h, int(layer), xn_ptr, _ptr(slot), _ptr(pos), len(pos), kv, len(kv_ptrs),
+                                         q_out_ptr))
+
+    def op_attention(self, layer: int, q_ptr, starts: Sequence[int], n_steps: Sequence[int], kv_ptrs: Sequence[int],
+                     out_ptr) -> None:
+        """Causal engine: one round's attention.  Job j owns the next n_steps[j] rows of q / out (act [rows][d_model]) at
+        positions starts[j] ..; its keys are in ring kv_ptrs[j]."""
+        st = np.ascontiguousarray(starts, np.int32)
+        ns = np.ascontiguousarray(n_steps, np.int32)
+        if not (len(st) == len(ns) == len(kv_ptrs)):
+            raise ValueError("starts, n_steps and kv_ptrs differ in length")
+        kv = (C.c_void_p * max(len(kv_ptrs), 1))(*[int(p) for p in kv_ptrs])
+        L.check(self.lib.wlk_qwen_op_attention(self.h, int(layer), q_ptr, _ptr(st), _ptr(ns), len(st), kv, out_ptr))
 
     def close(self) -> None:
         if not self._closed:
@@ -254,14 +299,16 @@ class QwenWindowEngine(_QwenEngineBase):
         return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
 
 
-def window_attention(qkv, stream_rows: Sequence[int], block_rows: int, device: int = 0):
+def window_attention(qkv, stream_rows: Sequence[int], block_rows: int, device: int = 0, out=None):
     """The windowed tower's block-diagonal attention kernel on a CUDA tensor qkv [rows, 3 * d_model] (fp32 runs the SIMT
-    parity kernel, bf16 the tensor-core one; q pre-scaled) -> [rows, d_model] of the same dtype.  Kernel tests only."""
+    parity kernel, bf16 the tensor-core one; q pre-scaled) -> [rows, d_model] of the same dtype (written into ``out``
+    when given: rows past the streams are left as they are).  Kernel tests only."""
     import torch
     lib = L.load()
     d = qkv.shape[1] // 3
     qkv = qkv.contiguous()
-    out = torch.empty(qkv.shape[0], d, dtype=qkv.dtype, device=qkv.device)
+    if out is None:
+        out = torch.empty(qkv.shape[0], d, dtype=qkv.dtype, device=qkv.device)
     torch.cuda.synchronize(qkv.device)
     rows = np.asarray(list(stream_rows), np.int32)
     prec = L.PREC_FP32 if qkv.dtype == torch.float32 else L.PREC_BF16
