@@ -406,6 +406,30 @@ int wlk_qtext_generate_full(wlk_qtext* t, const int32_t* sids, int32_t n, const 
                             const int32_t* stop_ids, int32_t n_stop, const int32_t* suppress, int32_t n_suppress,
                             float repetition_penalty, int32_t no_repeat_ngram_size, int32_t max_consecutive,
                             int32_t wait_token_id, int32_t* tokens_out, int32_t* n_tokens_out);
+/* generate_full_hypothesis_rolling (model.py:991-1250) for n caller-owned sessions in one call.  Session i holds the KV of
+ * its reused prefix (it was reset by the caller when its rolling state does not validate); its rows (row_src /
+ * row_offsets and embeds as wlk_qtext_generate_full: lead tokens, delta audio rows, template tail, then the draft) bring
+ * it to prefix_len[i] + draft_len[i] positions, prefix_len[i] = head + audio_steps + tail_len, and the last draft_len[i]
+ * rows are the draft tokens (already cut at the first stop id and to max_new_tokens).
+ *   verify: one forward with draft_len + 1 logit rows per session; the picks (controls as wlk_qtext_pick, row j after
+ *     draft[:j]) and the draft check stay on the device; the host reads (accepted, next pick) per session once and
+ *     crops a session whose draft was rejected at j to prefix + j.
+ *   continuation: every step forwards one row per session still decoding, picks over its device history and downloads
+ *     4 bytes per live session.  A session stops on a stop id or at max_new_tokens tokens.
+ * On return every session holds prefix_len - tail_len positions ([head + audio_steps]); tokens_out [n][max_new_tokens]
+ * (row i's first n_tokens_out[i] entries set: the accepted draft, then the picks); stats_out [n][4]: draft_accepted,
+ * decode_steps, all of a non-empty draft accepted (0/1), draft corrected (0/1).
+ * Fails before any work, changing no session, on n outside [1, max_batch], a repeated or closed session, max_new_tokens
+ * < 1, draft_len outside [0, min(max_new_tokens, rows - 1)], a non-token draft row, rows that do not bring the session to
+ * prefix_len + draft_len, prefix_len + draft_len + max_new_tokens past max_ctx, more verify rows than the engine keeps
+ * or a row source out of range.  A failure after the work started resets every named session, so a rolling state the
+ * caller kept no longer validates and the next call rebuilds it.  No logit rows are kept for wlk_qtext_pick / logits. */
+int wlk_qtext_generate_rolling(wlk_qtext* t, const int32_t* sids, int32_t n, const int32_t* row_src, const int32_t* row_offsets,
+                               const float* embeds, int64_t embeds_ld, int32_t n_embeds, const int32_t* draft_len,
+                               const int32_t* prefix_len, int32_t tail_len, int32_t max_new_tokens, const int32_t* stop_ids,
+                               int32_t n_stop, const int32_t* suppress, int32_t n_suppress, float repetition_penalty,
+                               int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id,
+                               int32_t* tokens_out, int32_t* n_tokens_out, int32_t* stats_out);
 /* raw lm_head outputs [n_rows][vocab] fp32 of logit rows row0 .. row0 + n_rows of the last forward */
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host);
 /* RoPE frequencies: the optional tensor "rotary_emb.inv_freq" [head_dim / 2] (HF's non-persistent buffer of that name,

@@ -126,6 +126,9 @@ SIGNATURES = {
                                  C.c_int32, _vp, _vp]),
     "wlk_qtext_generate_full": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp,
                                           C.c_int32, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
+    "wlk_qtext_generate_rolling": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int64, C.c_int32, _vp, _vp, C.c_int32,
+                                             C.c_int32, _vp, C.c_int32, _vp, C.c_int32, C.c_float, C.c_int32, C.c_int32,
+                                             C.c_int32, _vp, _vp, _vp]),
     "wlk_qtext_logits": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp]),
     "wlk_qtext_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp]),
     "wlk_qtext_op_qk_rope": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),

@@ -47,6 +47,9 @@ _OPS = {
     # QwenTowerEngine (QwenAudioCausalKVEncoder.forward_chunk / StreamingMelExtractor.append per stream: mel_append)
     "forward_chunk": (True, False), "mel_append": (True, False), "mel_flush": (False, False),
     "flush_pending": (False, False),
+    # B200QwenRealtimeModel (qwen_plugin._RealtimeOps): one CachedAudioDecodeState per session, flushes merged apart
+    "append_audio_to_cache": (True, False), "flush_audio_to_cache": (False, False),
+    "generate_full_hypothesis_rolling": (True, False), "generate_full_hypothesis_from_cached_audio": (True, False),
 }
 _BATCHED = tuple(_OPS)
 

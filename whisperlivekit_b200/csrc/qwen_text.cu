@@ -2,8 +2,9 @@
 //   reference third_party/qwen3-asr-causal/src/qwen3_asr_causal/model.py:
 //     text model wiring :1498-1507, generate_full_hypothesis_rolling :991-1250,
 //     generate_full_hypothesis_from_cached_audio :839-989, _GreedyControlSession :254-438
-// The host drives the generate logic (whisperlivekit_b200/qwen_text_engine.py); this file owns the forward over a
-// croppable per-session KV cache and the decode controls + argmax over the logit rows.
+// The host's TextDecodeDriver (whisperlivekit_b200/qwen_text_engine.py) holds the reference generate logic; this file owns
+// the forward over a croppable per-session KV cache, the decode controls + argmax over the logit rows, and the two
+// generate loops run in one call each (generate_full, generate_rolling).
 //
 // Data layout (per round, R <= QT_ROUND_ROWS rows packed over the sessions of the call, each session's rows in position
 // order, so a row always finds the keys of its predecessors either in earlier rounds or in this round's scatter):
@@ -296,8 +297,9 @@ struct PickArgs {
     float penalty; int penalize; int ngram; int max_consec; int wait_id;
     int32_t* picks; float* values;
     // device-resident histories (gen != null): row j picks for session row_sess[j], whose history is its first `step`
-    // tokens gen[row_sess[j]][0 .. step); the pick is appended there and left in next[row_sess[j]] for the next forward
-    int32_t* gen; int gen_ld; const int32_t* row_sess; int step; int32_t* next;
+    // tokens gen[row_sess[j]][0 .. step) (row_step[j] tokens instead when row_step is set); the pick is appended there
+    // and left in next[row_sess[j]] for the next forward
+    int32_t* gen; int gen_ld; const int32_t* row_sess; int step; int32_t* next; const int32_t* row_step;
 };
 
 // _GreedyControlSession.controlled_logits + argmax (model.py:335-418), one CTA per logit row, in place on the row:
@@ -313,11 +315,11 @@ __global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
     const int sess = a.gen ? a.row_sess[row] : 0;
     int32_t* gh = a.gen ? a.gen + (int64_t)sess * a.gen_ld : nullptr;
     const int32_t* h = a.gen ? gh : a.hist + a.hist_off[row];
-    const int n = a.gen ? a.step : a.hist_len[row];
+    const int n = a.gen ? (a.row_step ? a.row_step[row] : a.step) : a.hist_len[row];
     auto emit = [&](int pick, float value) {                          // thread 0, after every read of the history
         a.picks[row] = pick;
         if (a.values) a.values[row] = value;
-        if (gh) { gh[a.step] = pick; a.next[sess] = pick; }
+        if (gh) { gh[n] = pick; a.next[sess] = pick; }
     };
     const int words = (a.vocab + 31) / 32;
     const float fmin = -3.4028234663852886e38f;
@@ -372,6 +374,36 @@ __global__ void __launch_bounds__(QT_PICK_THREADS) qt_pick_kernel(PickArgs a) {
             if (bv[w] > best || (bv[w] == best && bi[w] < besti)) { best = bv[w]; besti = bi[w]; }
         if (besti == 0x7fffffff) besti = 0;                            // NaN row: torch.argmax would say 0 too
         emit(besti, best);
+    }
+}
+
+// Draft verification of generate_full_hypothesis_rolling (model.py:991-1250), one CTA per session.  Session i's verify
+// picks are picks[base[i] .. base[i] + dl[i]], row j picked after draft[:j]; accepted = the first j whose pick differs
+// from draft[j], else dl.  The pick after the accepted prefix (the correction, or the tail's first pick when all of the
+// draft stands) starts the continuation: gen row i becomes draft[:accepted] + [that pick] (the pick only while it fits
+// gen_ld), next[i] holds it for the next forward and res[i] = (accepted, pick) is what the host reads.
+__global__ void qt_verify_kernel(const int32_t* __restrict__ picks, const int32_t* __restrict__ base,
+                                 const int32_t* __restrict__ draft, const int32_t* __restrict__ draft_off,
+                                 const int32_t* __restrict__ dl, int32_t* __restrict__ gen, int gen_ld,
+                                 int32_t* __restrict__ next, int32_t* __restrict__ res) {
+    __shared__ int acc;
+    const int i = blockIdx.x, n = dl[i];
+    const int32_t* p = picks + base[i];
+    const int32_t* d = draft + draft_off[i];
+    if (threadIdx.x == 0) acc = n;
+    __syncthreads();
+    for (int j = threadIdx.x; j < n; j += blockDim.x)
+        if (p[j] != d[j]) atomicMin(&acc, j);
+    __syncthreads();
+    const int a = acc;
+    int32_t* g = gen + (int64_t)i * gen_ld;
+    for (int j = threadIdx.x; j < a; j += blockDim.x) g[j] = d[j];
+    if (threadIdx.x == 0) {
+        const int tok = p[a];
+        if (a < gen_ld) g[a] = tok;
+        next[i] = tok;
+        res[2 * i] = a;
+        res[2 * i + 1] = tok;
     }
 }
 
@@ -875,7 +907,7 @@ void launch_picks(wlk_qtext* t, int N, const PickArgs& a) {
         head_group(t, g0, rows);
         PickArgs b = a;
         b.logits = t->logits; b.ld = D.vocab; b.vocab = D.vocab;
-        if (b.gen) b.row_sess += g0;
+        if (b.gen) { b.row_sess += g0; if (b.row_step) b.row_step += g0; }
         else { b.hist_off += g0; b.hist_len += g0; }
         b.picks += g0;
         if (b.values) b.values += g0;
@@ -908,6 +940,19 @@ void pick(wlk_qtext* t, const int32_t* hist, int n_hist, const int32_t* hist_off
     CUDA_CHECK(cudaMemcpyAsync(picks, t->picks_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
     if (values) CUDA_CHECK(cudaMemcpyAsync(values, t->values_d, (size_t)N * 4, cudaMemcpyDeviceToHost, t->st));
     CUDA_CHECK(cudaStreamSynchronize(t->st));            // the one host sync of a forward + pick phase
+}
+
+// The generate loops' device histories: gen_d holds n rows of max_new tokens, then n next tokens (returned).
+int32_t* gen_buffer(wlk_qtext* t, int n, int max_new) {
+    const size_t need = (size_t)n * max_new + n;
+    if (need > t->gen_cap) {
+        CUDA_CHECK(cudaStreamSynchronize(t->st));
+        if (t->gen_d) CUDA_CHECK(cudaFree(t->gen_d));
+        t->gen_d = nullptr;
+        t->gen_cap = std::max(need, (size_t)1 << 14);
+        CUDA_CHECK(cudaMalloc(&t->gen_d, t->gen_cap * 4));
+    }
+    return t->gen_d + (size_t)n * max_new;
 }
 
 // generate_full_hypothesis_from_cached_audio's cached path (model.py:839-989) for n caller-owned sessions at once: each
@@ -944,15 +989,7 @@ void generate_full(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_
         for (int i = 0; i < n; ++i) n_out[i] = 0;
         if (max_new > 0) {
             const std::vector<int32_t> sup = pick_suppress(t, suppress, n_suppress, &wait_id);
-            const size_t gen_need = (size_t)n * max_new + n;
-            if (gen_need > t->gen_cap) {
-                CUDA_CHECK(cudaStreamSynchronize(t->st));
-                if (t->gen_d) CUDA_CHECK(cudaFree(t->gen_d));
-                t->gen_d = nullptr;
-                t->gen_cap = std::max(gen_need, (size_t)1 << 14);
-                CUDA_CHECK(cudaMalloc(&t->gen_d, t->gen_cap * 4));
-            }
-            int32_t* next_d = t->gen_d + (size_t)n * max_new;
+            int32_t* next_d = gen_buffer(t, n, max_new);
             // pick buffer: [suppress][row -> session index of the step]
             int32_t* sup_d = pick_buffer(t, sup.size() + (size_t)n + 1);
             int32_t* row_sess_d = sup_d + sup.size();
@@ -995,6 +1032,137 @@ void generate_full(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_
         throw;
     }
     reset();
+}
+
+// generate_full_hypothesis_rolling (model.py:991-1250) for n caller-owned sessions at once, with the rules of
+// TextDecodeDriver._generate_rolling.  Session i holds the KV of its reused prefix; its rows (row_src / row_offsets, the
+// last draft_len[i] of them the draft tokens) bring it to prefix_len[i] + draft_len[i] positions.  One forward keeps
+// draft_len + 1 logit rows per session, picks on them with the draft prefixes as histories and verifies the drafts on the
+// device (qt_verify_kernel); one download of (accepted, pick) per session lets the host crop each session to prefix +
+// accepted.  Then every step forwards one row per session still decoding and picks over its device history; a step
+// downloads only its picks.  On return every session holds prefix_len - tail_len positions ([head + audio_steps]); a
+// failure after the checks resets every named session.
+void generate_rolling(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, const int32_t* row_off,
+                      const float* embeds, int n_embeds, int64_t embeds_ld, const int32_t* draft_len, const int32_t* prefix_len,
+                      int tail_len, int max_new, const int32_t* stop, int n_stop, const int32_t* suppress, int n_suppress,
+                      float penalty, int ngram, int max_consec, int wait_id, int32_t* tokens_out, int32_t* n_out,
+                      int32_t* stats_out) {
+    const wlk_qtext_dims& D = t->dims;
+    WLK_CHECK(t->finalized, "weights not finalized");
+    WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
+    WLK_CHECK(max_new >= 1, "max_new_tokens %d < 1", max_new);
+    WLK_CHECK(tail_len >= 0, "tail_len %d < 0", tail_len);
+    int n_verify = 0, n_draft = 0;
+    for (int i = 0; i < n; ++i) {
+        const QTSession& s = tsession(t, sids[i]);
+        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        const int r = row_off[i + 1] - row_off[i], dl = draft_len[i], p = prefix_len[i];
+        WLK_CHECK(dl >= 0 && dl <= max_new && dl + 1 <= r, "session %d: draft_len %d outside [0, min(max_new_tokens %d, rows %d - 1)]",
+                  sids[i], dl, max_new, r);
+        WLK_CHECK(p >= tail_len && s.len + r == p + dl, "session %d: %d held + %d rows is not prefix_len %d + draft_len %d "
+                  "(tail_len %d)", sids[i], s.len, r, p, dl, tail_len);
+        WLK_CHECK((int64_t)p + dl + max_new <= D.max_ctx, "session %d: prefix %d + draft %d + max_new_tokens %d exceed max_ctx %d",
+                  sids[i], p, dl, max_new, D.max_ctx);
+        for (int k = row_off[i + 1] - dl; k < row_off[i + 1]; ++k)
+            WLK_CHECK(row_src[k] >= 0, "session %d: draft row %d is not a token", sids[i], k - row_off[i]);
+        n_verify += dl + 1;
+        n_draft += dl;
+    }
+    WLK_CHECK(n_verify <= t->logit_cap, "%d verify rows exceed the engine's %d logit rows", n_verify, t->logit_cap);
+    for (int r = row_off[0]; r < row_off[n]; ++r)
+        WLK_CHECK(row_src[r] < D.vocab && (row_src[r] >= 0 || -1 - row_src[r] < n_embeds),
+                  "row %d: source %d is neither a token id nor an embedding row", r - row_off[0], row_src[r]);
+    try {
+        const std::vector<int32_t> sup = pick_suppress(t, suppress, n_suppress, &wait_id);
+        int32_t* next_d = gen_buffer(t, n, max_new);
+        // one upload: [suppress][hist_off V][hist_len V][drafts][base n][draft_off n][dl n]; then the per-step
+        // [row_sess n][row_step n] and the verify results res [2n]
+        std::vector<int32_t> meta(sup);
+        const size_t o_hoff = meta.size(), o_hlen = o_hoff + n_verify, o_draft = o_hlen + n_verify,
+                     o_base = o_draft + n_draft, o_doff = o_base + n, o_dl = o_doff + n, o_rs = o_dl + n, o_step = o_rs + n,
+                     o_res = o_step + n;
+        meta.resize(o_rs);
+        std::vector<int32_t> logit_rows(n);
+        for (int i = 0, v = 0, dd = 0; i < n; ++i) {
+            const int dl = draft_len[i];
+            meta[o_base + i] = v; meta[o_doff + i] = dd; meta[o_dl + i] = dl;
+            for (int j = 0; j <= dl; ++j, ++v) { meta[o_hoff + v] = dd; meta[o_hlen + v] = j; }
+            for (int j = 0; j < dl; ++j) meta[o_draft + dd + j] = row_src[row_off[i + 1] - dl + j];
+            dd += dl;
+            logit_rows[i] = dl + 1;
+        }
+        int32_t* buf = pick_buffer(t, o_res + 2 * (size_t)n);
+        CUDA_CHECK(cudaMemcpyAsync(buf, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, t->st));
+        PickArgs a{};
+        a.suppress = buf; a.n_suppress = (int)sup.size();
+        a.penalty = penalty; a.penalize = penalty != 1.0f && penalty > 0.0f; a.ngram = ngram; a.max_consec = max_consec;
+        a.wait_id = wait_id; a.picks = t->picks_d; a.values = nullptr;
+
+        // verify pass: every block in one forward, its picks and the draft check on the device
+        forward(t, sids, n, row_src, row_off, embeds, n_embeds, logit_rows.data(), embeds_ld);
+        PickArgs va = a;
+        va.hist = buf + o_draft; va.hist_off = buf + o_hoff; va.hist_len = buf + o_hlen;
+        launch_picks(t, n_verify, va);
+        qt_verify_kernel<<<n, 128, 0, t->st>>>(t->picks_d, buf + o_base, buf + o_draft, buf + o_doff, buf + o_dl, t->gen_d,
+                                                max_new, next_d, buf + o_res);
+        CUDA_CHECK(cudaGetLastError());
+        std::vector<int32_t> res(2 * (size_t)n), glen(n), steps(n), live, live_sids(n), offs(n + 1), ones(n, 1), picks(n),
+            step_meta(2 * (size_t)n);
+        CUDA_CHECK(cudaMemcpyAsync(res.data(), buf + o_res, res.size() * 4, cudaMemcpyDeviceToHost, t->st));
+        CUDA_CHECK(cudaStreamSynchronize(t->st));        // the one host sync of the verify pass
+        auto stops = [&](int tok) { for (int s = 0; s < n_stop; ++s) if (stop[s] == tok) return true; return false; };
+        for (int i = 0; i < n; ++i) {
+            const int dl = draft_len[i], acc = res[2 * i], tok = res[2 * i + 1];
+            int32_t* out = tokens_out + (size_t)i * max_new;
+            for (int j = 0; j < acc; ++j) out[j] = row_src[row_off[i + 1] - dl + j];
+            glen[i] = acc;
+            steps[i] = 0;
+            if (acc < dl) t->sess[sids[i]].len = prefix_len[i] + acc;     // the corrected pick replaces draft[acc]
+            if (acc < max_new) {                                          // the correction, or the tail's first pick
+                out[glen[i]++] = tok;
+                steps[i] = 1;
+                if (!stops(tok) && glen[i] < max_new) live.push_back(i);
+            }
+            stats_out[4 * i] = acc;
+            stats_out[4 * i + 2] = dl > 0 && acc == dl;
+            stats_out[4 * i + 3] = acc < dl;
+        }
+        for (int i = 0; i <= n; ++i) offs[i] = i;
+        // continuation: one row per live session, its device history growing by the step's pick
+        while (!live.empty()) {
+            const int m = (int)live.size();
+            for (int k = 0; k < m; ++k) {
+                live_sids[k] = sids[live[k]];
+                step_meta[k] = live[k];
+                step_meta[m + k] = glen[live[k]];
+            }
+            forward(t, live_sids.data(), m, live.data(), offs.data(), nullptr, 0, ones.data(), 0, next_d, n);
+            CUDA_CHECK(cudaMemcpyAsync(buf + o_rs, step_meta.data(), (size_t)2 * m * 4, cudaMemcpyHostToDevice, t->st));
+            PickArgs sa = a;
+            sa.gen = t->gen_d; sa.gen_ld = max_new; sa.row_sess = buf + o_rs; sa.row_step = buf + o_rs + m; sa.next = next_d;
+            launch_picks(t, m, sa);
+            CUDA_CHECK(cudaMemcpyAsync(picks.data(), t->picks_d, (size_t)m * 4, cudaMemcpyDeviceToHost, t->st));
+            CUDA_CHECK(cudaStreamSynchronize(t->st));    // the one host sync of a step
+            int kept = 0;
+            for (int k = 0; k < m; ++k) {
+                const int i = live[k], tok = picks[k];
+                tokens_out[(size_t)i * max_new + glen[i]++] = tok;
+                steps[i]++;
+                if (!stops(tok) && glen[i] < max_new) live[kept++] = i;
+            }
+            live.resize(kept);
+        }
+        for (int i = 0; i < n; ++i) {
+            n_out[i] = glen[i];
+            stats_out[4 * i + 1] = steps[i];
+            t->sess[sids[i]].len = prefix_len[i] - tail_len;
+        }
+        t->n_logit = 0;
+    } catch (...) {
+        for (int i = 0; i < n; ++i) t->sess[sids[i]].len = 0;   // the checks above found every session open
+        t->n_logit = 0;
+        throw;
+    }
 }
 
 void logits_out(wlk_qtext* t, int row0, int rows, float* out) {
@@ -1271,6 +1439,23 @@ int wlk_qtext_generate_full(wlk_qtext* t, const int32_t* sids, int32_t n, const 
     WLK_CHECK(embeds_ld == 0 || embeds_ld >= t->dims.d_model, "embeds_ld %lld < d_model %d", (long long)embeds_ld, t->dims.d_model);
     generate_full(t, sids, n, row_src, row_offsets, embeds, n_embeds, embeds_ld, max_new_tokens, stop_ids, n_stop, suppress,
                   n_suppress, repetition_penalty, no_repeat_ngram_size, max_consecutive, wait_token_id, tokens_out, n_tokens_out);
+    WLK_API_END
+}
+int wlk_qtext_generate_rolling(wlk_qtext* t, const int32_t* sids, int32_t n, const int32_t* row_src, const int32_t* row_offsets,
+                               const float* embeds, int64_t embeds_ld, int32_t n_embeds, const int32_t* draft_len,
+                               const int32_t* prefix_len, int32_t tail_len, int32_t max_new_tokens, const int32_t* stop_ids,
+                               int32_t n_stop, const int32_t* suppress, int32_t n_suppress, float repetition_penalty,
+                               int32_t no_repeat_ngram_size, int32_t max_consecutive, int32_t wait_token_id,
+                               int32_t* tokens_out, int32_t* n_tokens_out, int32_t* stats_out) {
+    WLK_API_BEGIN
+    WLK_ENTER(t, t->cfg.device);
+    WLK_CHECK(sids && row_src && row_offsets && (embeds || n_embeds == 0) && draft_len && prefix_len &&
+              (stop_ids || n_stop == 0) && (suppress || n_suppress == 0) && tokens_out && n_tokens_out && stats_out,
+              "null argument");
+    WLK_CHECK(embeds_ld == 0 || embeds_ld >= t->dims.d_model, "embeds_ld %lld < d_model %d", (long long)embeds_ld, t->dims.d_model);
+    generate_rolling(t, sids, n, row_src, row_offsets, embeds, n_embeds, embeds_ld, draft_len, prefix_len, tail_len,
+                     max_new_tokens, stop_ids, n_stop, suppress, n_suppress, repetition_penalty, no_repeat_ngram_size,
+                     max_consecutive, wait_token_id, tokens_out, n_tokens_out, stats_out);
     WLK_API_END
 }
 int wlk_qtext_logits(wlk_qtext* t, int32_t row0, int32_t n_rows, float* out_host) {

@@ -113,6 +113,43 @@ def uninstall():
 
 
 # ---------------------------------------------------------------------------------------------------------------
+# qwen3-streaming seam: cohorts over a realtime model installed with batching=True
+# ---------------------------------------------------------------------------------------------------------------
+def install_qwen_cohorts(realtime, processor_cls=None):
+    """Bracket every ``Qwen3StreamingOnlineProcessor.process_iter`` (qwen3_asr_causal/online.py) with the cohort of
+    ``realtime.batcher`` (a ``B200QwenRealtimeModel`` installed with ``batching=True``), as ``install(batching=True)``
+    does for AlignAtt: the worker threads' iterations advance together, so every session's append and generate land in
+    the cohort's merged engine calls.  ``processor_cls`` defaults to the class WhisperLiveKit's qwen3-streaming backend
+    instantiates.  ``uninstall_qwen_cohorts(processor_cls)`` restores it."""
+    if realtime.batcher is None:
+        raise ValueError("the realtime model was installed without batching=True")
+    if processor_cls is None:
+        from qwen3_asr_causal.online import Qwen3StreamingOnlineProcessor as processor_cls
+    orig = processor_cls.__dict__.get("_b200_process_iter", processor_cls.process_iter)
+    batcher = realtime.batcher
+
+    def process_iter(self, *a, **k):
+        batcher.begin_iter()
+        try:
+            return orig(self, *a, **k)
+        finally:
+            batcher.end_iter()
+
+    processor_cls._b200_process_iter = orig
+    processor_cls.process_iter = process_iter
+    return processor_cls
+
+
+def uninstall_qwen_cohorts(processor_cls=None):
+    if processor_cls is None:
+        from qwen3_asr_causal.online import Qwen3StreamingOnlineProcessor as processor_cls
+    orig = processor_cls.__dict__.get("_b200_process_iter")
+    if orig is not None:
+        processor_cls.process_iter = orig
+        del processor_cls._b200_process_iter
+
+
+# ---------------------------------------------------------------------------------------------------------------
 # diarization seam (SURVEY.md section 8b item 3)
 # ---------------------------------------------------------------------------------------------------------------
 def sortformer_state_dict_from_nemo(path: str):

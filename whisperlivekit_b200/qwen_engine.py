@@ -28,6 +28,7 @@ class _QwenEngineBase:
         self.dims = dims
         self.precision = precision
         self.device = int(device)
+        self.max_batch = int(max_batch)
         be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
         cdims = self._DIMS(*dims.as_tuple())
         cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
@@ -64,6 +65,8 @@ class _QwenEngineBase:
         return sid.value
 
     def close_session(self, sid: int) -> None:
+        if self._closed:            # destroyed first (a session handle collected in the same garbage cycle): its
+            return                  # sessions went with it, and the handle must not be touched
         L.check(self.lib.wlk_qwen_session_close(self.h, sid))
 
     def reset_session(self, sid: int) -> None:

@@ -465,29 +465,24 @@ class B200QwenTextDecoder:
         kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
                             max_consecutive_text_tokens)
         ctl = self.engine.make_controls(**kw)
-        fh = self._rows(frame_hidden)
+        outs = self.full_tokens([frame_hidden[b] for b in range(batch)], token_rows(prefix_token_ids, batch),
+                                token_rows(prompt_token_ids, batch), audio_placeholder_token_id, max_new_tokens, ctl)
+        return padded_tokens(outs, ctl, device)
 
-        def rows(ids, b):
-            if ids is None:
-                return None
-            t = torch.as_tensor(ids).long()
-            return (t if t.ndim == 1 else t[b]).tolist()
-
-        prefixes = [self.engine.full_prefix(fh[b], prefix_token_ids=rows(prefix_token_ids, b),
+    def full_tokens(self, frame_rows, prefix_rows, prompt_rows, audio_placeholder_token_id, max_new_tokens: int, ctl):
+        """The cached path's tokens per stream: frame_rows[b] [steps, d], prefix_rows[b] / prompt_rows[b] token lists or
+        None.  Streams with an empty prefix get no tokens; the others run in one generate_full_batch (waves of
+        max_batch)."""
+        prefixes = [self.engine.full_prefix(self._rows(f), prefix_token_ids=p,
                                             audio_placeholder_token_id=audio_placeholder_token_id,
-                                            prompt_token_ids=rows(prompt_token_ids, b), bos_token_id=self.model.bos_token_id)
-                    for b in range(batch)]
-        live = [b for b in range(batch) if prefixes[b][0].shape[0]]
-        outs = [[] for _ in range(batch)]
+                                            prompt_token_ids=q, bos_token_id=self.model.bos_token_id)
+                    for f, p, q in zip(frame_rows, prefix_rows, prompt_rows)]
+        live = [b for b in range(len(prefixes)) if prefixes[b][0].shape[0]]
+        outs = [[] for _ in prefixes]
         for b, toks in zip(live, self._generate_full([prefixes[b][1] for b in live], [prefixes[b][0] for b in live],
                                                      max_new_tokens, ctl)):
             outs[b] = toks
-        # rows that stopped early are filled with the stop-fill id while the others decode (model.py:419-436)
-        width = max(len(o) for o in outs)
-        if ctl.stop_ids:
-            fill = ctl.eos_token_id if ctl.eos_token_id is not None else min(ctl.stop_ids)
-            outs = [o + [fill] * (width - len(o)) for o in outs]
-        return torch.tensor(outs, dtype=torch.long, device=device).reshape(batch, width)
+        return outs
 
     def _generate_full(self, frame_rows, srcs, max_new_tokens: int, ctl):
         """engine.generate_full_batch over the scratch sessions, in waves of the engine's max_batch."""
@@ -571,15 +566,35 @@ class B200QwenTextDecoder:
                 prevs.append(RollingState(dec.head_token_ids, dec.head_len, dec.audio_steps))
             decs.append(dec)
         controls.setdefault("wait_token_id", self.model.wait_token_id)
-        toks, stats, new = self.engine.generate_rolling(
+        toks, stats, new = self.engine.generate_rolling_batch(
             [d.sid for d in decs], [self._rows(f) for f in frame_rows], prevs, template_token_ids,
             audio_placeholder_token_id, [None if d is None else [int(t) for t in d] for d in drafts],
-            max_new_tokens=max_new_tokens, bos_token_id=self.model.bos_token_id, **controls)
+            max_new_tokens=max_new_tokens, bos_token_id=self.model.bos_token_id, scratch=self._scratch, **controls)
         for dec, state, st, s in zip(decs, states, new, stats):
             if s.get("decoder_path") != "full":
                 dec.head_token_ids, dec.head_len, dec.audio_steps = st.head_token_ids, st.head_len, st.audio_steps
                 state.decoder = dec
         return toks, stats
+
+
+def token_rows(ids, batch: int):
+    """A generate method's prefix_token_ids / prompt_token_ids ([steps] shared, or [batch, steps]) as one list per row."""
+    if ids is None:
+        return [None] * batch
+    import torch
+    t = torch.as_tensor(ids).long()
+    return [(t if t.ndim == 1 else t[b]).tolist() for b in range(batch)]
+
+
+def padded_tokens(outs, ctl, device):
+    """Tokens per row -> the reference's [batch, width] long tensor: rows that stopped early are filled with the
+    stop-fill id while the others decode (model.py:419-436)."""
+    import torch
+    width = max(len(o) for o in outs)
+    if ctl.stop_ids:
+        fill = ctl.eos_token_id if ctl.eos_token_id is not None else min(ctl.stop_ids)
+        outs = [o + [fill] * (width - len(o)) for o in outs]
+    return torch.tensor(outs, dtype=torch.long, device=device).reshape(len(outs), width)
 
 
 def adapter_tensors(adapter) -> dict:
@@ -616,19 +631,36 @@ class B200QwenRealtimeModel:
     (N = 1), plus ``flush_audio_to_cache`` for the causal model only: the windowed model has none, so the streamer's
     ``flush_pending_audio`` returns None as in the reference.  With CUDA engines ``state.frame_hidden`` is a device
     tensor and the generate methods read it in place: no frame row reaches the host.  The reference streamers
-    (``SegmentedCachedFullHypothesisStreamer``) run over the installed model unchanged."""
+    (``SegmentedCachedFullHypothesisStreamer``) run over the installed model unchanged.
+
+    ``batching=True`` serves many sessions, each driven from its own thread, in shared engine calls: the four seam
+    methods submit to a ``batching.BatchingEngine`` whose dispatcher thread merges concurrent calls of one kind and equal
+    static arguments (template, placeholder id, max_new_tokens, decode controls) into one call of
+    ``RealtimeFrames.append`` (appends and flushes apart), ``generate_rolling_batch`` or the cached path's batch.  While
+    it is on, the dispatcher thread is the only caller of the engines' compute; callers only open, close and read their
+    sessions.  Bracket each caller's iteration (one ``process_iter``) with ``batcher.begin_iter()`` /
+    ``batcher.end_iter()`` (``plugin.install_qwen_cohorts`` does it for ``Qwen3StreamingOnlineProcessor``) so that a
+    cohort's appends and generates land in the same merged calls.  A merged call that fails is replayed one caller at
+    a time, so an error reaches only the caller whose session caused it.  ``close()`` stops the dispatcher."""
 
     def __init__(self, model, encoder, decoder):
         from .qwen_realtime import RealtimeFrames
         self.model, self.encoder, self.decoder = model, encoder, decoder
         self.frames = RealtimeFrames(encoder, decoder.engine, decoder.dims.d_model)
+        self.batcher = None
 
     @classmethod
     def install(cls, model, precision: str = "bf16", max_ctx: int = 1024, max_sessions: int = 8, tower_factory=None,
-                text_factory=None, attention_blocks: Optional[bool] = None):
+                text_factory=None, attention_blocks: Optional[bool] = None, batching: bool = False,
+                max_batch: Optional[int] = None, max_wait_s: float = 0.002):
         """tower_factory(dims, state_dict) / text_factory(dims, state_dict): engines to use instead of the CUDA ones
-        (the CPU oracles in tests).  attention_blocks: the windowed tower's, as B200QwenAudioSurgeryEncoder.dims_of."""
-        tower_kw = {} if tower_factory else dict(precision=precision, max_sessions=max_sessions)
+        (the CPU oracles in tests).  attention_blocks: the windowed tower's, as B200QwenAudioSurgeryEncoder.dims_of.
+        max_batch: sessions per call of both CUDA engines (their default, 8, when None).  batching: coalesce
+        concurrent seam calls (see the class docstring), at most as many sessions per merged call as the smaller of the
+        two engines' max_batch, so that no merged call exceeds what the engines take.  Size max_sessions for every
+        stream's tower and decoder session plus max_batch scratch sessions of the non-rolling generate."""
+        engine_kw = {} if max_batch is None else dict(max_batch=int(max_batch))
+        tower_kw = {} if tower_factory else dict(precision=precision, max_sessions=max_sessions, **engine_kw)
         windowed = _is_window_encoder(model.audio_encoder)
         if windowed:
             encoder = B200QwenAudioSurgeryEncoder.from_reference(model.audio_encoder, engine_factory=tower_factory,
@@ -640,7 +672,8 @@ class B200QwenRealtimeModel:
             raise ValueError(f"tower rows are {encoder.dims.out_dim} wide, the adapter takes "
                              f"{model.adapter.proj.weight.shape[1]}")
         decoder = B200QwenTextDecoder.install(model, engine_factory=text_factory, precision=precision, max_ctx=max_ctx,
-                                              max_sessions=max_sessions, extra_tensors=adapter_tensors(model.adapter))
+                                              max_sessions=max_sessions, extra_tensors=adapter_tensors(model.adapter),
+                                              **engine_kw)
         rt = cls(model, encoder, decoder)
         if "audio_encoder" in getattr(model, "_modules", {}):
             del model._modules["audio_encoder"]        # an nn.Module takes only modules as child attributes
@@ -648,17 +681,139 @@ class B200QwenRealtimeModel:
         model.append_audio_to_cache = rt.append_audio_to_cache
         if not windowed:
             model.flush_audio_to_cache = rt.flush_audio_to_cache
+        if batching:
+            from .batching import BatchingEngine
+            caps = [int(e.max_batch) for e in (encoder.engine, decoder.engine) if getattr(e, "max_batch", None)]
+            cap = min(caps) if caps else (max_batch or 64)        # the CPU oracles take any batch
+            rt.batcher = BatchingEngine(_RealtimeOps(rt), max_batch=min(cap, max_batch or cap), max_wait_s=max_wait_s)
+            model.generate_full_hypothesis_rolling = rt.generate_full_hypothesis_rolling
+            model.generate_full_hypothesis_from_cached_audio = rt.generate_full_hypothesis_from_cached_audio
         model.b200_realtime = rt
         return rt
 
     def append_audio_to_cache(self, mels, state=None):
         if state is None:
             state = self.model.init_cached_audio_decode_state()
-        (cached, delta), = self.frames.append([state], [mels])
+        if self.batcher is not None:
+            (cached, delta), = self.batcher.submit("append_audio_to_cache", [state], [mels]).result()
+        else:
+            (cached, delta), = self.frames.append([state], [mels])
         return cached, delta, state
 
     def flush_audio_to_cache(self, state=None):
         if state is None:
             state = self.model.init_cached_audio_decode_state()
-        (cached, delta), = self.frames.append([state], flush=True)
+        if self.batcher is not None:
+            (cached, delta), = self.batcher.submit("flush_audio_to_cache", [state]).result()
+        else:
+            (cached, delta), = self.frames.append([state], flush=True)
         return cached, delta, state
+
+    # -- the generate methods with batching on (without it they are B200QwenTextDecoder's) -------------------------
+    def _controls(self, eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                  max_consecutive_text_tokens):
+        """The decode controls as a merge key: hashable, equal when the decoder would build equal controls."""
+        return dict(eos_token_id=None if eos_token_id is None else int(eos_token_id),
+                    stop_token_ids=None if stop_token_ids is None else tuple(int(t) for t in stop_token_ids),
+                    suppress_token_ids=None if suppress_token_ids is None else tuple(int(t) for t in suppress_token_ids),
+                    repetition_penalty=float(repetition_penalty), no_repeat_ngram_size=int(no_repeat_ngram_size),
+                    max_consecutive_text_tokens=int(max_consecutive_text_tokens))
+
+    def generate_full_hypothesis_from_cached_audio(self, frame_hidden, *, prefix_token_ids=None,
+                                                   audio_placeholder_token_id=None, prompt_token_ids=None,
+                                                   max_new_tokens: int = 128, eos_token_id=None, stop_token_ids=None,
+                                                   suppress_token_ids=None, repetition_penalty: float = 1.0,
+                                                   no_repeat_ngram_size: int = 0, max_consecutive_text_tokens: int = 0,
+                                                   use_decoder_kv_cache: bool = True):
+        import torch
+        if frame_hidden.ndim != 3:
+            raise ValueError("frame_hidden must have shape [batch, steps, hidden]")
+        if max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        batch = int(frame_hidden.shape[0])
+        if max_new_tokens == 0:
+            return torch.empty(batch, 0, dtype=torch.long, device=frame_hidden.device)
+        kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                            max_consecutive_text_tokens)
+        items = list(zip([frame_hidden[b] for b in range(batch)], token_rows(prefix_token_ids, batch),
+                         token_rows(prompt_token_ids, batch)))
+        outs = self.batcher.submit("generate_full_hypothesis_from_cached_audio", [object() for _ in items], items,
+                                   audio_placeholder_token_id=audio_placeholder_token_id,
+                                   max_new_tokens=int(max_new_tokens), **kw).result()
+        return padded_tokens(outs, self.decoder.engine.make_controls(**kw), frame_hidden.device)
+
+    def generate_full_hypothesis_rolling(self, frame_hidden, *, state, template_token_ids, audio_placeholder_token_id,
+                                         draft_token_ids=None, max_new_tokens: int = 128, eos_token_id=None,
+                                         stop_token_ids=None, suppress_token_ids=None, repetition_penalty: float = 1.0,
+                                         no_repeat_ngram_size: int = 0, max_consecutive_text_tokens: int = 0):
+        import torch
+        from .qwen_text_engine import split_template
+        if frame_hidden.ndim != 3:
+            raise ValueError("frame_hidden must have shape [batch, steps, hidden]")
+        head, tail = split_template(template_token_ids, audio_placeholder_token_id)
+        kw = self._controls(eos_token_id, stop_token_ids, suppress_token_ids, repetition_penalty, no_repeat_ngram_size,
+                            max_consecutive_text_tokens)
+        audio_steps = int(frame_hidden.shape[1])
+        if int(frame_hidden.shape[0]) != 1 or max_new_tokens <= 0 or audio_steps == 0:
+            expanded = head + [int(audio_placeholder_token_id)] * audio_steps + tail
+            toks = self.generate_full_hypothesis_from_cached_audio(
+                frame_hidden, prefix_token_ids=expanded, audio_placeholder_token_id=audio_placeholder_token_id,
+                max_new_tokens=max_new_tokens, **kw)
+            return toks, {"decoder_path": "full"}
+        draft = None if draft_token_ids is None else [int(t) for t in draft_token_ids]
+        (toks, stats), = self.batcher.submit(
+            "generate_full_hypothesis_rolling", [state], [(frame_hidden[0], draft)],
+            template_token_ids=tuple(int(t) for t in template_token_ids),
+            audio_placeholder_token_id=int(audio_placeholder_token_id), max_new_tokens=int(max_new_tokens), **kw).result()
+        return torch.tensor([toks], dtype=torch.long, device=frame_hidden.device), stats
+
+    def close(self) -> None:
+        """Stop the dispatcher of batching=True (pending calls fail)."""
+        if self.batcher is not None:
+            self.batcher.close()
+
+
+class _RealtimeOps:
+    """The realtime model's seam calls in the batch form BatchingEngine's dispatcher makes them: the first argument is
+    one key per caller row (the CachedAudioDecodeStates; placeholders for the stateless cached path)."""
+
+    def __init__(self, rt: B200QwenRealtimeModel):
+        self.rt = rt
+
+    def _append(self, states, mels=None, flush: bool = False):
+        engine = self.rt.encoder.engine
+        for st in states:                          # fail before any session is touched: the batch is then replayed
+            if getattr(st.audio, "engine", None) is not engine:
+                raise ValueError("the stream's audio session is closed")
+        saved = [(st.audio.frames_seen, st.audio.last_input_frames) for st in states]
+        try:
+            return self.rt.frames.append(states, mels, flush=flush)
+        except BaseException:
+            for st, (seen, last) in zip(states, saved):
+                st.audio.frames_seen, st.audio.last_input_frames = seen, last
+            raise
+
+    def append_audio_to_cache(self, states, mels):
+        return self._append(states, mels)
+
+    def flush_audio_to_cache(self, states):
+        return self._append(states, flush=True)
+
+    def generate_full_hypothesis_rolling(self, states, items, *, template_token_ids, audio_placeholder_token_id,
+                                         max_new_tokens, **controls):
+        dec = self.rt.decoder
+        toks, stats = dec.generate_rolling_batch([fh for fh, _ in items], states, [d for _, d in items],
+                                                 template_token_ids=list(template_token_ids),
+                                                 audio_placeholder_token_id=audio_placeholder_token_id,
+                                                 max_new_tokens=max_new_tokens, **controls)
+        return list(zip(toks, stats))
+
+    def generate_full_hypothesis_from_cached_audio(self, keys, items, *, audio_placeholder_token_id, max_new_tokens,
+                                                   **controls):
+        dec = self.rt.decoder
+        ctl = dec.engine.make_controls(wait_token_id=dec.model.wait_token_id, **controls)
+        return dec.full_tokens([fh for fh, _, _ in items], [p for _, p, _ in items], [q for _, _, q in items],
+                               audio_placeholder_token_id, max_new_tokens, ctl)
+
+    def close(self):
+        pass

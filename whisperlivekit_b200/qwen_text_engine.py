@@ -12,6 +12,10 @@ greedy decode controls + argmax (``pick``).  ``TextDecodeDriver`` runs the refer
   * ``generate_full_batch`` - the same cached path for N caller-owned sessions in lockstep: one forward of every prefix,
     then one forward + pick per step over the sessions still decoding.  ``generate_full`` is its N = 1 case.
 
+``QwenTextEngine`` runs ``generate_full_batch`` and ``generate_rolling_batch`` (``generate_rolling`` in one call) as single
+engine calls (wlk_qtext_generate_full / wlk_qtext_generate_rolling); its ``generate_full`` and ``generate_rolling`` stay
+the driver loops over forward / pick, the reference the engine calls are tested against.
+
 The CPU oracle (oracle/qwen_text_oracle.py) implements the same primitives, so both run the same driver code."""
 from __future__ import annotations
 
@@ -93,6 +97,11 @@ class TextDecodeDriver:
         with self.phase_lock:
             return self._generate_full_batch(*args, **kwargs)
 
+    def generate_rolling_batch(self, *args, scratch: Optional[list] = None, **kwargs):
+        """generate_rolling; an engine that runs the whole call in one engine call overrides it.  scratch: sessions
+        the full path may use (generate_full opens and closes its own here)."""
+        return self.generate_rolling(*args, **kwargs)
+
     def make_controls(self, *, eos_token_id=None, stop_token_ids=None, suppress_token_ids=None, repetition_penalty=1.0,
                       no_repeat_ngram_size=0, max_consecutive_text_tokens=0, wait_token_id=None) -> Controls:
         stop = {int(t) for t in (stop_token_ids or ())}
@@ -130,60 +139,16 @@ class TextDecodeDriver:
                                  no_repeat_ngram_size=no_repeat_ngram_size,
                                  max_consecutive_text_tokens=max_consecutive_text_tokens, wait_token_id=wait_token_id)
         n = len(sids)
-        drafts = list(drafts) if drafts is not None else [None] * n
         out_tokens: List[Optional[List[int]]] = [None] * n
         out_stats: List[Optional[Dict]] = [None] * n
         new_states = list(states)
-        live = []                       # (i, block rows, draft, stats skeleton)
-
-        def fallback(i, fh):
+        full, live = self._rolling_plan(sids, frame_hidden, states, head, tail, drafts, max_new_tokens, ctl)
+        for i, fh in full:
             expanded = head + [int(audio_placeholder_token_id)] * fh.shape[0] + tail
             out_tokens[i] = self.generate_full(fh, prefix_token_ids=expanded,
                                                audio_placeholder_token_id=audio_placeholder_token_id,
                                                max_new_tokens=max_new_tokens, controls=ctl, bos_token_id=bos_token_id)
             out_stats[i] = {"decoder_path": "full"}
-
-        for i in range(n):
-            fh = _frame_rows(frame_hidden[i])
-            audio_steps = int(fh.shape[0])
-            if max_new_tokens <= 0 or audio_steps == 0:
-                fallback(i, fh)
-                continue
-            draft = [int(t) for t in (drafts[i] or [])]
-            for k, t in enumerate(draft):
-                if t in ctl.stop_ids:
-                    draft = draft[:k]
-                    break
-            draft = draft[:int(max_new_tokens)]
-            st = states[i]
-            valid = (st is not None and st.head_token_ids == tuple(head) and 0 <= st.audio_steps <= audio_steps
-                     and self.session_len(sids[i]) == st.head_len + st.audio_steps)
-            if valid:
-                reused = int(st.audio_steps)
-                audio_rows = fh[reused:]
-                lead: List[int] = []
-            else:
-                reused = 0
-                audio_rows = fh
-                lead = list(head)
-            if len(lead) + audio_rows.shape[0] + len(tail) + len(draft) == 0:
-                fallback(i, fh)
-                continue
-            src = np.concatenate([np.asarray(lead, np.int32), -1 - np.arange(audio_rows.shape[0], dtype=np.int32),
-                                  np.asarray(tail + draft, np.int32)])
-            if not valid:
-                self.reset_session(sids[i])
-            live.append((i, (src, audio_rows), draft, {
-                "decoder_path": "rolling+draft" if draft else "rolling",
-                "decoder_rebuilt": not valid,
-                "draft_tokens": len(draft),
-                "prefill_positions": int(src.shape[0]),
-                "audio_steps": audio_steps,
-                "audio_delta_steps": int(audio_rows.shape[0]),
-                "reused_audio_steps": reused,
-                "prompt_head_tokens": len(head),
-                "template_tail_tokens": len(tail),
-            }))
         if not live:
             return out_tokens, out_stats, new_states
 
@@ -240,11 +205,67 @@ class TextDecodeDriver:
             self.crop(sids[i], len(head) + stats["audio_steps"])
             new_states[i] = RollingState(tuple(head), len(head), stats["audio_steps"])
             stats["decode_steps"] = steps.get(i, 0) + (1 if corrected else 0)
-            out_stats[i] = {k: stats[k] for k in (
-                "decoder_path", "decoder_rebuilt", "draft_tokens", "draft_accepted", "draft_all_accepted", "decode_steps",
-                "prefill_positions", "audio_steps", "audio_delta_steps", "reused_audio_steps", "prompt_head_tokens",
-                "template_tail_tokens")}
+            out_stats[i] = self._rolling_stats(stats)
         return out_tokens, out_stats, new_states
+
+    _ROLLING_STATS = ("decoder_path", "decoder_rebuilt", "draft_tokens", "draft_accepted", "draft_all_accepted",
+                      "decode_steps", "prefill_positions", "audio_steps", "audio_delta_steps", "reused_audio_steps",
+                      "prompt_head_tokens", "template_tail_tokens")
+
+    @classmethod
+    def _rolling_stats(cls, stats: Dict) -> Dict:
+        return {k: stats[k] for k in cls._ROLLING_STATS}
+
+    def _rolling_plan(self, sids, frame_hidden, states, head: List[int], tail: List[int], drafts, max_new_tokens: int,
+                      ctl: Controls):
+        """generate_rolling's per-session decisions before any forward.  Returns (full, live): the sessions that take
+        the full path as (i, frame rows), the others as (i, (row sources, delta frame rows), draft, stats skeleton).
+        A session whose state does not validate is reset here, so its block rebuilds [head + audio] from scratch."""
+        n = len(sids)
+        drafts = list(drafts) if drafts is not None else [None] * n
+        full, live = [], []
+        for i in range(n):
+            fh = _frame_rows(frame_hidden[i])
+            audio_steps = int(fh.shape[0])
+            if max_new_tokens <= 0 or audio_steps == 0:
+                full.append((i, fh))
+                continue
+            draft = [int(t) for t in (drafts[i] or [])]
+            for k, t in enumerate(draft):
+                if t in ctl.stop_ids:
+                    draft = draft[:k]
+                    break
+            draft = draft[:int(max_new_tokens)]
+            st = states[i]
+            valid = (st is not None and st.head_token_ids == tuple(head) and 0 <= st.audio_steps <= audio_steps
+                     and self.session_len(sids[i]) == st.head_len + st.audio_steps)
+            if valid:
+                reused = int(st.audio_steps)
+                audio_rows = fh[reused:]
+                lead: List[int] = []
+            else:
+                reused = 0
+                audio_rows = fh
+                lead = list(head)
+            if len(lead) + audio_rows.shape[0] + len(tail) + len(draft) == 0:
+                full.append((i, fh))
+                continue
+            src = np.concatenate([np.asarray(lead, np.int32), -1 - np.arange(audio_rows.shape[0], dtype=np.int32),
+                                  np.asarray(tail + draft, np.int32)])
+            if not valid:
+                self.reset_session(sids[i])
+            live.append((i, (src, audio_rows), draft, {
+                "decoder_path": "rolling+draft" if draft else "rolling",
+                "decoder_rebuilt": not valid,
+                "draft_tokens": len(draft),
+                "prefill_positions": int(src.shape[0]),
+                "audio_steps": audio_steps,
+                "audio_delta_steps": int(audio_rows.shape[0]),
+                "reused_audio_steps": reused,
+                "prompt_head_tokens": len(head),
+                "template_tail_tokens": len(tail),
+            }))
+        return full, live
 
     # -- generate_full_hypothesis_from_cached_audio (model.py:839-989), cached path -----------------------------------
     def full_prefix(self, frame_hidden, *, prefix_token_ids: Optional[Sequence[int]] = None,
@@ -386,6 +407,8 @@ class QwenTextEngine(TextDecodeDriver):
         return sid.value
 
     def close_session(self, sid: int) -> None:
+        if self._closed:            # destroyed first (a session handle collected in the same garbage cycle): its
+            return                  # sessions went with it, and the handle must not be touched
         L.check(self.lib.wlk_qtext_session_close(self.h, int(sid)))
 
     def reset_session(self, sid: int) -> None:
@@ -486,6 +509,92 @@ class QwenTextEngine(TextDecodeDriver):
                 ctl.max_consecutive, ctl.wait_id, _ptr(toks), _ptr(counts)))
             self._n_logit = 0
         return [toks[i, :counts[i]].tolist() for i in range(n)]
+
+    def generate_rolling_batch(self, sids: Sequence[int], frame_hidden: Sequence, states: Sequence[Optional[RollingState]],
+                               template_token_ids: Sequence[int], audio_placeholder_token_id: int,
+                               drafts: Optional[Sequence[Optional[Sequence[int]]]] = None, *, max_new_tokens: int = 128,
+                               bos_token_id=None, scratch: Optional[list] = None, **control_kwargs):
+        """TextDecodeDriver.generate_rolling with its verify pass and decode loop in one engine call
+        (wlk_qtext_generate_rolling): the picks, the draft check and the generated histories stay on the device.  Same
+        rounds, tokens, stats and states.
+
+        Sessions take the full path when they have no audio steps, when max_new_tokens <= 0 or when their block would
+        be empty; those go through one generate_full_batch on scratch sessions: the open sessions of the caller's
+        `scratch` list (B200QwenTextDecoder passes the ones it keeps for the non-rolling generate), and for the rest
+        sessions opened for the call and closed after it, which need free slots within max_sessions while it runs.
+
+        Sessions whose rolling state does not validate are reset before the engine call, as the driver resets them.
+        Input the engine rejects raises WlkError before any work and changes no session beyond that reset; a failure
+        after the work started resets every named session.  Either way the states the caller keeps no longer validate
+        for the reset sessions, and the next call rebuilds them."""
+        head, tail = split_template(template_token_ids, audio_placeholder_token_id)
+        ctl = self.make_controls(**control_kwargs)
+        n = len(sids)
+        if n and max_new_tokens < 0:
+            raise ValueError("max_new_tokens must be >= 0")
+        out_tokens: List[Optional[List[int]]] = [None] * n
+        out_stats: List[Optional[Dict]] = [None] * n
+        new_states = list(states)
+        with self.phase_lock:
+            full, live = self._rolling_plan(sids, frame_hidden, states, head, tail, drafts, max_new_tokens, ctl)
+            if full:
+                self._generate_full_scratch(full, head, tail, audio_placeholder_token_id, max_new_tokens, ctl,
+                                            out_tokens, out_stats, scratch)
+            if not live:
+                return out_tokens, out_stats, new_states
+            m = len(live)
+            flat, off, rows, n_rows, ld = self._pack([blk for _, blk, _, _ in live])
+            ids = np.asarray([sids[i] for i, *_ in live], np.int32)
+            dl = np.asarray([len(d) for _, _, d, _ in live], np.int32)
+            prefix = np.asarray([len(head) + st["audio_steps"] + len(tail) for *_, st in live], np.int32)
+            stop = np.asarray(sorted(ctl.stop_ids), np.int32) if ctl.stop_ids else np.zeros(1, np.int32)
+            sup = ctl.suppress if len(ctl.suppress) else np.zeros(1, np.int32)
+            toks = np.zeros((m, int(max_new_tokens)), np.int32)
+            counts = np.zeros(m, np.int32)
+            res = np.zeros((m, 4), np.int32)
+            try:
+                L.check(self.lib.wlk_qtext_generate_rolling(
+                    self.h, _ptr(ids), m, _ptr(flat), _ptr(off), self._rows_ptr(rows, ld), ld, n_rows, _ptr(dl),
+                    _ptr(prefix), len(tail), int(max_new_tokens), _ptr(stop), len(ctl.stop_ids), _ptr(sup),
+                    len(ctl.suppress), float(ctl.penalty), ctl.ngram, ctl.max_consecutive, ctl.wait_id, _ptr(toks),
+                    _ptr(counts), _ptr(res)))
+            finally:
+                self._n_logit = 0
+        for k, (i, _, _, stats) in enumerate(live):
+            accepted, decode_steps, all_accepted, _ = (int(v) for v in res[k])
+            out_tokens[i] = toks[k, :counts[k]].tolist()
+            stats.update(draft_accepted=accepted, draft_all_accepted=bool(all_accepted), decode_steps=decode_steps)
+            out_stats[i] = self._rolling_stats(stats)
+            new_states[i] = RollingState(tuple(head), len(head), stats["audio_steps"])
+        return out_tokens, out_stats, new_states
+
+    def _generate_full_scratch(self, full, head, tail, placeholder, max_new_tokens, ctl, out_tokens, out_stats,
+                               keep: Optional[list] = None):
+        """generate_rolling_batch's full-path sessions [(i, frame rows)]: generate_full_batch in waves of max_batch
+        over the open sessions of `keep`, plus sessions opened for the call and closed after it for the rest."""
+        srcs = []
+        for i, fh in full:
+            expanded = head + [int(placeholder)] * fh.shape[0] + tail
+            srcs.append(self.full_prefix(fh, prefix_token_ids=expanded, audio_placeholder_token_id=placeholder)[0])
+            out_tokens[i] = []
+            out_stats[i] = {"decoder_path": "full"}
+        todo = [k for k, s in enumerate(srcs) if s.shape[0]] if max_new_tokens > 0 else []
+        need = min(len(todo), self.max_batch)
+        scratch = list(keep or [])[:need]
+        temp = []
+        try:
+            while len(scratch) < need:
+                temp.append(self.open_session())
+                scratch.append(temp[-1])
+            for a in range(0, len(todo), self.max_batch):
+                wave = todo[a: a + self.max_batch]
+                got = self.generate_full_batch(scratch[:len(wave)], [full[k][1] for k in wave], [srcs[k] for k in wave],
+                                               max_new_tokens=max_new_tokens, controls=ctl)
+                for k, g in zip(wave, got):
+                    out_tokens[full[k][0]] = g
+        finally:
+            for sid in temp:
+                self.close_session(sid)
 
     def adapter_dims(self) -> Tuple[int, int, int]:
         """(in_dim, blocks, hidden width) of the loaded frame adapter; in_dim 0 without one."""
