@@ -93,17 +93,11 @@ struct ProfRec { int cls; cudaEvent_t a, b; double flops, bytes; };
 
 using namespace wlk;
 
-struct wlk_engine {
+struct wlk_engine : EngineBase {       // act: also the type of every session buffer
     wlk_dims dims{};
-    wlk_config cfg{};
-    int act = DT_F32;                 // activation type (and type of every session buffer)
     int wt = DT_F32;                  // weight-matrix type: = act, or DT_BF16X2 (hi + lo bf16 planes) in WLK_PREC_BF16X3
     void* a_split = nullptr; size_t a_split_elems = 0;   // BF16X3: (hi, lo) planes of a GEMM's fp32 activation operand
     int gemm_backend = WLK_BACKEND_SIMT, attn_backend = WLK_BACKEND_SIMT;
-    int num_sms = 132;
-    cudaStream_t st = nullptr;
-    std::mutex mu;
-    DeviceAllocs allocs;              // buffers kept from create (or first use) until destroy
     // token-step CUDA graphs: the ~390 launches of one decoder step depend only on the batch size (every per-session
     // quantity travels in the staged job arrays), so they are captured once per batch size and replayed
     bool graphs_on = true;
@@ -115,11 +109,9 @@ struct wlk_engine {
 
     Arena arena;
     Weights w;
-    std::set<std::string> loaded;
-    bool finalized = false;
     float* stage_f32 = nullptr; size_t stage_cap = 0;
 
-    std::vector<Session> sess;
+    SessionTable<Session> sess;
     std::vector<int32_t> align_rank_host;     // [L*H] -> rank or -1
     int32_t* align_rank_dev = nullptr;
     uint8_t* kv_maps_dev = nullptr;           // [max_sessions] CUtensorMap (128 B each) over each session's cross-K/V
@@ -137,14 +129,10 @@ struct wlk_engine {
     void** xptrs_dev = nullptr;               // x + b*1500*d
     float* audio_scratch = nullptr;
     void* beam_scratch = nullptr; size_t beam_scratch_cap = 0;   // staging for wlk_sessions_gather_decoder
-    float* sk_scratch = nullptr; int* sk_counters = nullptr;     // this engine's split-K workspace (GemmArgs)
     float* mel_scratch = nullptr;             // fp32 [MEL_ROWS][n_mels] for the read_mel tap
     // decoder workspace
     int dec_rows_max = 0;
     float* dx = nullptr; void *dxn = nullptr, *dq = nullptr, *datt = nullptr, *dhid = nullptr, *dsel = nullptr;
-    // staging (pinned host mirror + device copy)
-    uint8_t *stg_host = nullptr, *stg_dev = nullptr; size_t stg_bytes = 0;
-    cudaEvent_t stg_done = nullptr;
     StepResult *res_dev = nullptr, *res_host = nullptr;
     float* tap_host = nullptr; size_t tap_cap = 0;
     float* all_logits_dev = nullptr; size_t all_logits_cap = 0;
@@ -153,9 +141,7 @@ struct wlk_engine {
     bool prof_on = false;
     std::vector<ProfRec> prof;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool;
-    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
 
-    size_t es() const { return dtype_size(act); }
     size_t wes() const { return dtype_size(wt); }
 };
 
@@ -428,50 +414,20 @@ void run_gemm(wlk_engine* e, GemmArgs& g, int cls) {
     ProfScope ps(e, cls, 2.0 * g.M * (double)g.N * g.K,
                  (double)g.M * g.K * dtype_size(g.a_type) + (double)g.N * g.K * dtype_size(g.w_type) +
                      (double)g.M * g.N * dtype_size(g.epi.c_type));
-    g.sk_scratch = e->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
-    g.sk_counters = e->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
     if (e->wt == DT_BF16X2) {
         // every weight matrix is one whole [N, ldw] allocation: the lo plane sits right behind the hi plane
         g.W_lo = reinterpret_cast<const bf16*>(g.W) + (size_t)g.N * g.ldw;
         g.a_split = e->a_split; g.a_split_elems = e->a_split_elems;
-        std::string why;
-        WLK_CHECK(gemm_tcgen05_supported(g, &why), "bf16x3 GEMM (M=%d N=%d K=%d): %s", g.M, g.N, g.K, why.c_str());
-        gemm_tcgen05(g, e->st, e->num_sms);
+        e->gemm.run(g, true, e->st, e->num_sms, "bf16x3");
         return;
     }
-    bool tc = e->gemm_backend == WLK_BACKEND_TCGEN05 && gemm_tcgen05_supported(g, nullptr);
-    if (tc) gemm_tcgen05(g, e->st, e->num_sms);
-    else gemm_simt(g, e->st);
+    e->gemm.run(g, e->gemm_backend == WLK_BACKEND_TCGEN05, e->st, e->num_sms);
 }
 
-// ---------------------------------------------------------------------------------------
-// staging: a pinned host block mirrored on the device, carved per call
-// ---------------------------------------------------------------------------------------
-struct Stager {
-    wlk_engine* e; size_t used = 0;
-    explicit Stager(wlk_engine* e_) : e(e_) { CUDA_CHECK(cudaEventSynchronize(e->stg_done)); }
-    template <typename T> T* host(size_t count, T** dev) {
-        size_t off = (used + 255) / 256 * 256;
-        size_t bytes = count * sizeof(T);
-        WLK_CHECK(off + bytes <= e->stg_bytes, "staging buffer overflow (%zu + %zu > %zu)", off, bytes, e->stg_bytes);
-        used = off + bytes;
-        *dev = reinterpret_cast<T*>(e->stg_dev + off);
-        return reinterpret_cast<T*>(e->stg_host + off);
-    }
-    void upload() {
-        if (used) CUDA_CHECK(cudaMemcpyAsync(e->stg_dev, e->stg_host, used, cudaMemcpyHostToDevice, e->st));
-        CUDA_CHECK(cudaEventRecord(e->stg_done, e->st));
-    }
-};
-
-Session& get_session(wlk_engine* e, int32_t sid) {
-    WLK_CHECK(sid >= 0 && sid < (int)e->sess.size() && e->sess[sid].open, "invalid session id %d", sid);
-    return e->sess[sid];
-}
 // the session whose encoder output / cross-K/V / content length `s` decodes against (itself unless a beam fork)
 Session& enc_owner(wlk_engine* e, Session& s) { return s.parent >= 0 ? e->sess[s.parent] : s; }
 Session& get_root_session(wlk_engine* e, int32_t sid, const char* what) {
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(s.parent < 0, "session %d is a beam fork of session %d: %s belongs to the parent", sid, s.parent, what);
     return s;
 }
@@ -527,12 +483,12 @@ void encode_batch(wlk_engine* e, const int32_t* sids, int n, int32_t* content_ou
     const size_t es = e->es();
     WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
     // first pass: validation only (no session state is touched until the whole batch is known to be good)
+    e->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
         Session& s = get_root_session(e, sids[i], "encode");
         WLK_CHECK(s.audio_len > 0, "session %d has no audio", sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
     }
-    Stager sg(e);
+    Stager sg(e->stg);
     MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(n, &mj_dev);
     void** xkv_dev; void** xkv = sg.host<void*>(n, &xkv_dev);
     int max_frames = 1;
@@ -542,7 +498,7 @@ void encode_batch(wlk_engine* e, const int32_t* sids, int n, int32_t* content_ou
         content_out[i] = s.content_len;
         xkv[i] = s.cross_kv;
     }
-    sg.upload();
+    sg.upload(e->st);
 
     {   ProfScope ps(e, WLK_KC_MEL, 0, (double)n * (480000.0 * 4 + 3000.0 * nm * es));
         mel_forward(mj_dev, n, nm, W.filtT, W.window, W.twiddle, W.filt_span, e->act, max_frames, e->st); }
@@ -696,14 +652,14 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
     WLK_CHECK(e->act == DT_BF16 && e->wt == DT_BF16 && e->attn_backend == WLK_BACKEND_TCGEN05 && e->gemm_backend == WLK_BACKEND_TCGEN05,
               "the incremental encoder runs in the bf16 wgmma mode only");
     WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
+    e->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
         Session& s = get_root_session(e, sids[i], "encode");
         WLK_CHECK(s.audio_len > 0, "session %d has no audio", sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
     }
     for (int i = 0; i < n; ++i) ensure_incremental(e, e->sess[sids[i]], sids[i]);
 
-    Stager sg(e);
+    Stager sg(e->stg);
     MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(n, &mj_dev);
     IncJob* ij_dev; IncJob* ij = sg.host<IncJob>(n, &ij_dev);
     DecJob* dj_dev; DecJob* dj = sg.host<DecJob>(n, &dj_dev);
@@ -738,7 +694,7 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
         R += len; R1 += 2 * len + 1;
         max_rows = std::max(max_rows, len);
     }
-    sg.upload();
+    sg.upload(e->st);
     {   ProfScope ps(e, WLK_KC_MEL, 0, (double)n * (480000.0 * 4 + 3000.0 * nm * es));
         mel_forward(mj_dev, n, nm, W.filtT, W.window, W.twiddle, W.filt_span, e->act, max_frames, e->st); }
 
@@ -830,7 +786,8 @@ void decode_batch(wlk_engine* e, const int32_t* sids, int n, const int32_t* toke
     const int R = offsets[n] - offsets[0];
     WLK_CHECK(R >= n && R <= e->dec_rows_max, "decode rows %d outside [%d, %d]", R, n, e->dec_rows_max);
 
-    Stager sg(e);
+    e->sess.check_batch(sids, n);
+    Stager sg(e->stg);
     DecJob* dj_dev; DecJob* dj = sg.host<DecJob>(n, &dj_dev);
     int32_t *tok_dev, *pos_dev, *slot_dev, *sel_dev;
     int32_t* tok = sg.host<int32_t>(R, &tok_dev);
@@ -841,8 +798,7 @@ void decode_batch(wlk_engine* e, const int32_t* sids, int n, const int32_t* toke
     void** lptr_dev; void** lptr = sg.host<void*>(2 * n, &lptr_dev);
     int n_sel = 0, r = 0, max_tq = 0;
     for (int i = 0; i < n; ++i) {
-        Session& s = get_session(e, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        Session& s = e->sess[sids[i]];
         WLK_CHECK(enc_owner(e, s).encoded, "session %d: decode before encode", sids[i]);
         const int tq = offsets[i + 1] - offsets[i];
         WLK_CHECK(tq >= 1, "session %d: empty token list", sids[i]);
@@ -863,7 +819,7 @@ void decode_batch(wlk_engine* e, const int32_t* sids, int n, const int32_t* toke
         if (first) { sel[n_sel] = dj[i].row_off + sot_index; lptr[n_sel] = s.logits_sot; ++n_sel; }
         sel[n_sel] = r - 1; lptr[n_sel] = s.logits_last; ++n_sel;
     }
-    sg.upload();
+    sg.upload(e->st);
 
     auto launch_all = [&]() {
     {   ProfScope ps(e, WLK_KC_MISC);
@@ -1034,7 +990,7 @@ void alloc_session(wlk_engine* e, Session& s) {
     if (e->act == DT_BF16) {
         alignas(64) uint8_t tmap[128];
         make_cross_kv_tmap(tmap, s.cross_kv, D.n_text_layer, D.n_text_head);
-        const size_t slot = (size_t)(&s - e->sess.data());
+        const size_t slot = (size_t)(&s - e->sess.slots.data());
         CUDA_CHECK(cudaMemcpy(e->kv_maps_dev + slot * 128, tmap, 128, cudaMemcpyHostToDevice));
         make_self_kv_tmap(tmap, s.self_kv, D.n_text_layer, D.n_text_head, D.n_text_ctx);
         CUDA_CHECK(cudaMemcpy(e->self_maps_dev + slot * 128, tmap, 128, cudaMemcpyHostToDevice));
@@ -1074,7 +1030,7 @@ void alloc_fork(wlk_engine* e, Session& s, int parent) {
     if (e->act == DT_BF16) {
         alignas(64) uint8_t tmap[128];
         make_cross_kv_tmap(tmap, p.cross_kv, D.n_text_layer, D.n_text_head);
-        const size_t slot = (size_t)(&s - e->sess.data());
+        const size_t slot = (size_t)(&s - e->sess.slots.data());
         CUDA_CHECK(cudaMemcpy(e->kv_maps_dev + slot * 128, tmap, 128, cudaMemcpyHostToDevice));
         make_self_kv_tmap(tmap, s.self_kv, D.n_text_layer, D.n_text_head, D.n_text_ctx);
         CUDA_CHECK(cudaMemcpy(e->self_maps_dev + slot * 128, tmap, 128, cudaMemcpyHostToDevice));
@@ -1089,13 +1045,12 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     WLK_CHECK(dims->n_text_state % 64 == 0 && dims->n_text_state / dims->n_text_head == 64, "text heads must be 64 wide");
     WLK_CHECK(dims->n_mels % 8 == 0 && dims->n_mels <= 128, "n_mels must be 80 or 128");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    const int num_sms = open_sm90_device(cfg->device);
-
-    auto* e = new wlk_engine();
-    e->dims = *dims; e->cfg = *cfg;
-    e->num_sms = num_sms;
     WLK_CHECK(cfg->precision == WLK_PREC_FP32 || cfg->precision == WLK_PREC_BF16 || cfg->precision == WLK_PREC_BF16X3,
               "unknown precision %d", cfg->precision);
+
+    auto* e = new wlk_engine();
+    e->open(*cfg);
+    e->dims = *dims;
     e->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     e->wt = cfg->precision == WLK_PREC_BF16X3 ? DT_BF16X2 : e->act;
     e->gemm_backend = cfg->gemm_backend != WLK_BACKEND_AUTO ? cfg->gemm_backend
@@ -1109,12 +1064,9 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
         e->gemm_backend = WLK_BACKEND_TCGEN05;
         e->attn_backend = cfg->attn_backend == WLK_BACKEND_SIMT ? WLK_BACKEND_SIMT : WLK_BACKEND_TCGEN05;
     }
-    CUDA_CHECK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
     {   const char* v = getenv("WLK_GRAPHS"); e->graphs_on = !(v && v[0] == '0'); }
     {   const char* v = getenv("WLK_MEL_INCREMENTAL"); e->mel_incremental = !(v && v[0] == '0'); }
     for (auto& t : e->timers) CUDA_CHECK(cudaEventCreate(&t));
-    CUDA_CHECK(cudaEventCreateWithFlags(&e->stg_done, cudaEventDisableTiming));
-    CUDA_CHECK(cudaEventRecord(e->stg_done, e->st));
 
     // weights arena: dry run for the size, then the real layout
     layout_weights(e);
@@ -1146,10 +1098,7 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     e->hid = e->allocs.take((size_t)B * N_CTX * 4 * d * es, acct);
     e->audio_scratch = (float*)e->allocs.take(AUDIO_CAP * sizeof(float), acct);
     e->mel_scratch = (float*)e->allocs.take((size_t)MEL_STORE_FRAMES * D.n_mels * sizeof(float), acct);
-    if (e->gemm_backend == WLK_BACKEND_TCGEN05) {
-        e->sk_scratch = (float*)e->allocs.take(SK_SCRATCH_FLOATS * sizeof(float), acct);
-        e->sk_counters = (int*)e->allocs.take(SK_MAX_TILES * sizeof(int), acct);
-    }
+    if (e->gemm_backend == WLK_BACKEND_TCGEN05) e->gemm.alloc(e->allocs, acct);
     {
         std::vector<int64_t> rows(2 * B);
         std::vector<void*> xp(B);
@@ -1178,12 +1127,10 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
         e->a_split_elems = (m + 7) / 8 * 8;
         e->a_split = e->allocs.take(e->a_split_elems * 2 * 2, acct);
     }
-    e->stg_bytes = (size_t)B * 2048 + R * 16 + 65536 + 1024 * 8 * 4;
-    CUDA_CHECK(cudaMallocHost(&e->stg_host, e->stg_bytes));
-    e->stg_dev = reinterpret_cast<uint8_t*>(e->allocs.take(e->stg_bytes, acct));
+    e->stg.alloc((size_t)B * 2048 + R * 16 + 65536 + 1024 * 8 * 4, e->allocs, acct);
     e->res_dev = (StepResult*)e->allocs.take(B * sizeof(StepResult), acct);
     CUDA_CHECK(cudaMallocHost(&e->res_host, sizeof(StepResult) * B));
-    e->sess.resize(cfg->max_sessions);
+    e->sess.slots.resize(cfg->max_sessions);
     e->kv_maps_dev = reinterpret_cast<uint8_t*>(e->allocs.take((size_t)cfg->max_sessions * 128, acct));
     e->self_maps_dev = reinterpret_cast<uint8_t*>(e->allocs.take((size_t)cfg->max_sessions * 128, acct));
     e->align_rank_host.assign((size_t)D.n_text_layer * D.n_text_head, -1);
@@ -1193,20 +1140,17 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
 }
 
 void destroy_engine(wlk_engine* e) {
-    cudaStreamSynchronize(e->st);
-    for (auto& s : e->sess) if (s.open && s.parent >= 0) free_session(e, s);     // forks before their parents
-    for (auto& s : e->sess) if (s.open) free_session(e, s);
-    for (void* p : {(void*)e->stage_f32, e->beam_scratch, (void*)e->all_logits_dev}) if (p) cudaFree(p);
-    e->allocs.free_all();
-    if (e->stg_host) cudaFreeHost(e->stg_host);
-    if (e->res_host) cudaFreeHost(e->res_host);
-    if (e->tap_host) cudaFreeHost(e->tap_host);
-    for (auto& t : e->timers) if (t) cudaEventDestroy(t);
-    for (auto& p : e->prof) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }
-    for (auto& p : e->ev_pool) { cudaEventDestroy(p.first); cudaEventDestroy(p.second); }
-    if (e->stg_done) cudaEventDestroy(e->stg_done);
-    for (auto& kv : e->dec_graphs) cudaGraphExecDestroy(kv.second.exec);
-    cudaStreamDestroy(e->st);
+    e->close([e] {
+        for (auto& s : e->sess) if (s.open && s.parent >= 0) free_session(e, s);     // forks before their parents
+        for (auto& s : e->sess) if (s.open) free_session(e, s);
+        for (void* p : {(void*)e->stage_f32, e->beam_scratch, (void*)e->all_logits_dev}) if (p) cudaFree(p);
+        if (e->res_host) cudaFreeHost(e->res_host);
+        if (e->tap_host) cudaFreeHost(e->tap_host);
+        for (auto& t : e->timers) if (t) cudaEventDestroy(t);
+        for (auto& p : e->prof) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }
+        for (auto& p : e->ev_pool) { cudaEventDestroy(p.first); cudaEventDestroy(p.second); }
+        for (auto& kv : e->dec_graphs) cudaGraphExecDestroy(kv.second.exec);
+    });
     delete e;
 }
 
@@ -1305,9 +1249,7 @@ int wlk_engine_sync(wlk_engine* e) {
 int wlk_engine_memory(wlk_engine* e, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    if (weights) *weights = e->bytes_weights;
-    if (sessions) *sessions = e->bytes_sessions;
-    if (workspace) *workspace = e->bytes_workspace;
+    e->memory(weights, sessions, workspace);
     WLK_API_END
 }
 
@@ -1317,9 +1259,7 @@ int wlk_session_open(wlk_engine* e, int32_t* sid) {
     WLK_CHECK(sid, "null out pointer");
     WLK_CHECK(e->finalized, "weights not finalized");
     WLK_CHECK(e->n_align > 0, "alignment heads not set");
-    int found = -1;
-    for (int i = 0; i < (int)e->sess.size(); ++i) if (!e->sess[i].open) { found = i; break; }
-    WLK_CHECK(found >= 0, "all %d sessions in use", (int)e->sess.size());
+    const int found = e->sess.free_slot();
     alloc_session(e, e->sess[found]);
     e->sess[found].open = true;
     *sid = found;
@@ -1328,7 +1268,7 @@ int wlk_session_open(wlk_engine* e, int32_t* sid) {
 int wlk_session_close(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(s.n_forks == 0, "session %d still has %d beam fork(s): close them first", sid, s.n_forks);
     CUDA_CHECK(cudaStreamSynchronize(e->st));
     free_session(e, s);
@@ -1339,9 +1279,7 @@ int wlk_session_fork(wlk_engine* e, int32_t parent, int32_t* child) {
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(child, "null out pointer");
     get_root_session(e, parent, "forking");
-    int found = -1;
-    for (int i = 0; i < (int)e->sess.size(); ++i) if (!e->sess[i].open) { found = i; break; }
-    WLK_CHECK(found >= 0, "all %d sessions in use", (int)e->sess.size());
+    const int found = e->sess.free_slot();
     alloc_fork(e, e->sess[found], parent);
     e->sess[found].open = true;
     *child = found;
@@ -1355,13 +1293,12 @@ int wlk_sessions_gather_decoder(wlk_engine* e, const int32_t* sids, const int32_
     const size_t es = e->es();
     const size_t pitch = (size_t)D.n_text_ctx * 64 * es;                 // one (layer, k|v, head) plane of the self-K/V
     const size_t planes = (size_t)D.n_text_layer * 2 * D.n_text_head;
+    e->sess.check_batch(sids, n);
     std::vector<int> moved;
     for (int i = 0; i < n; ++i) {
-        Session& d = get_session(e, sids[i]);
         WLK_CHECK(src[i] >= 0 && src[i] < n, "source index %d out of range", src[i]);
-        Session& s = get_session(e, sids[src[i]]);
+        Session &d = e->sess[sids[i]], &s = e->sess[sids[src[i]]];
         WLK_CHECK(&enc_owner(e, d) == &enc_owner(e, s), "sessions %d and %d do not share an encoder output", sids[i], sids[src[i]]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice", sids[i]);
         if (src[i] != i) moved.push_back(i);
     }
     if (moved.empty()) return 0;
@@ -1432,7 +1369,7 @@ int wlk_session_drop_audio(wlk_engine* e, int32_t sid, int64_t n) {
 int wlk_session_clear_audio(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     s.audio_len = 0; s.mel_n = -1; s.mel_dropped = 0; s.inc_valid = false;
     WLK_API_END
 }
@@ -1440,14 +1377,14 @@ int wlk_session_audio_len(wlk_engine* e, int32_t sid, int64_t* n) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(n, "null out pointer");
-    *n = get_session(e, sid).audio_len;
+    *n = e->sess.at(sid).audio_len;
     WLK_API_END
 }
 
 int wlk_session_reset_decoder(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear();
     WLK_API_END
 }
@@ -1487,10 +1424,10 @@ int wlk_encode_mel(wlk_engine* e, int32_t sid, const float* mel_host, int32_t co
     Session& s = get_root_session(e, sid, "encode");
     WLK_CHECK(mel_host && content_mel_len >= 0, "bad arguments");
     const int nm = e->dims.n_mels;
-    Stager sg(e);
+    Stager sg(e->stg);
     void** xkv_dev; void** xkv = sg.host<void*>(1, &xkv_dev);
     xkv[0] = s.cross_kv;
-    sg.upload();
+    sg.upload(e->st);
     CUDA_CHECK(cudaMemcpyAsync(e->mel_scratch, mel_host, (size_t)nm * N_FRAMES * 4, cudaMemcpyHostToDevice, e->st));
     {   ProfScope ps(e, WLK_KC_MEL);
         mel_import(e->mel_scratch, e->mel_t, e->act, nm, e->st); }
@@ -1520,7 +1457,7 @@ int wlk_decode_all_logits(wlk_engine* e, int32_t sid, const int32_t* tokens, int
 int wlk_read_align_rows(wlk_engine* e, int32_t sid, float* out, int64_t capacity, int32_t* n_align, int32_t* rows) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(out && n_align && rows, "null argument");
     const int R = s.align_rows, A = e->n_align;
     WLK_CHECK((int64_t)A * R * N_CTX <= capacity, "output buffer too small: need %d x %d x %d", A, R, N_CTX);
@@ -1536,14 +1473,14 @@ int wlk_no_speech_prob(wlk_engine* e, const int32_t* sids, int n, float* prob_ou
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && prob_out && n >= 1 && n <= e->cfg.max_batch, "bad arguments");
-    Stager sg(e);
+    Stager sg(e->stg);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
     for (int i = 0; i < n; ++i) {
-        Session& s = get_session(e, sids[i]);
+        Session& s = e->sess.at(sids[i]);
         WLK_CHECK(!s.iter_row_start.empty(), "session %d: no decode call in this epoch", sids[i]);
         lj[i] = make_logit_job(e, s, 16, 0);
     }
-    sg.upload();
+    sg.upload(e->st);
     const int no_speech = (e->dims.n_vocab >= 51865 ? 50257 : 50256) + 2 + (e->dims.n_vocab - 51765 - (e->dims.n_vocab >= 51865 ? 1 : 0)) + 4;
     {   ProfScope ps(e, WLK_KC_LOGITS);
         no_speech_prob(lj_dev, n, e->dims.n_vocab, no_speech, e->res_dev, e->st); }
@@ -1556,15 +1493,15 @@ int wlk_suppress(wlk_engine* e, const int32_t* sids, int n, const int32_t* token
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && n >= 1 && n <= e->cfg.max_batch && n_tokens >= 0 && n_tokens <= 4096, "bad arguments");
-    Stager sg(e);
+    Stager sg(e->stg);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
     int32_t* tk_dev; int32_t* tk = sg.host<int32_t>(n_tokens > 0 ? n_tokens : 1, &tk_dev);
-    for (int i = 0; i < n; ++i) lj[i] = make_logit_job(e, get_session(e, sids[i]), 16, 0);
+    for (int i = 0; i < n; ++i) lj[i] = make_logit_job(e, e->sess.at(sids[i]), 16, 0);
     for (int i = 0; i < n_tokens; ++i) {
         WLK_CHECK(token_ids[i] >= 0 && token_ids[i] < e->dims.n_vocab, "token %d out of range", token_ids[i]);
         tk[i] = token_ids[i];
     }
-    sg.upload();
+    sg.upload(e->st);
     {   ProfScope ps(e, WLK_KC_LOGITS);
         suppress_tokens(lj_dev, n, tk_dev, n_tokens, e->st); }
     WLK_API_END
@@ -1572,17 +1509,17 @@ int wlk_suppress(wlk_engine* e, const int32_t* sids, int n, const int32_t* token
 int wlk_add_logit_bias(wlk_engine* e, int32_t sid, const int32_t* token_ids, const float* bias, int n) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(n >= 0 && n <= 4096, "bad count");
     if (n) {
-        Stager sg(e);
+        Stager sg(e->stg);
         int32_t* tk_dev; int32_t* tk = sg.host<int32_t>(n, &tk_dev);
         float* b_dev; float* b = sg.host<float>(n, &b_dev);
         for (int i = 0; i < n; ++i) {
             WLK_CHECK(token_ids[i] >= 0 && token_ids[i] < e->dims.n_vocab, "token %d out of range", token_ids[i]);
             tk[i] = token_ids[i]; b[i] = bias[i];
         }
-        sg.upload();
+        sg.upload(e->st);
         add_logit_bias(s.logits_last, tk_dev, b_dev, n, e->st);
     }
     WLK_API_END
@@ -1592,14 +1529,14 @@ int wlk_greedy_and_align(wlk_engine* e, const int32_t* sids, int n, int32_t wind
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(sids && token_out && logprob_out && frame_out && n >= 1 && n <= e->cfg.max_batch && window_iters >= 1, "bad arguments");
-    Stager sg(e);
+    Stager sg(e->stg);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
     for (int i = 0; i < n; ++i) {
-        Session& s = get_session(e, sids[i]);
+        Session& s = e->sess.at(sids[i]);
         WLK_CHECK(!s.iter_row_start.empty(), "session %d: no decode call in this epoch", sids[i]);
         lj[i] = make_logit_job(e, s, window_iters, 0);
     }
-    sg.upload();
+    sg.upload(e->st);
     {   ProfScope ps(e, WLK_KC_LOGITS);
         greedy_pick(lj_dev, n, e->dims.n_vocab, e->res_dev, e->st); }
     {   ProfScope ps(e, WLK_KC_ALIGN);
@@ -1624,7 +1561,8 @@ int wlk_select(wlk_engine* e, const int32_t* sids, int n, const int32_t* suppres
     WLK_CHECK(n_suppress >= 0 && n_suppress <= 4096 && n_first >= 0 && n_first <= 64, "bad suppression lists");
     const int n_bias = bias_offsets ? bias_offsets[n] : 0;
     WLK_CHECK(n_bias >= 0 && n_bias <= 64 * n, "bad bias lists");
-    Stager sg(e);
+    e->sess.check_batch(sids, n);
+    Stager sg(e->stg);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(n, &lj_dev);
     LogitJob* fj_dev; LogitJob* fj = sg.host<LogitJob>(n, &fj_dev);
     int32_t* sup_dev; int32_t* sup = sg.host<int32_t>(n_suppress > 0 ? n_suppress : 1, &sup_dev);
@@ -1634,9 +1572,8 @@ int wlk_select(wlk_engine* e, const int32_t* sids, int n, const int32_t* suppres
     float* bv_dev; float* bv = sg.host<float>(n_bias > 0 ? n_bias : 1, &bv_dev);
     int nf = 0;
     for (int i = 0; i < n; ++i) {
-        Session& s = get_session(e, sids[i]);
+        Session& s = e->sess[sids[i]];
         WLK_CHECK(!s.iter_row_start.empty(), "session %d: no decode call in this epoch", sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
         lj[i] = make_logit_job(e, s, window_iters, 0);
         if (first_mask && first_mask[i]) fj[nf++] = lj[i];
         if (n_bias) {
@@ -1655,7 +1592,7 @@ int wlk_select(wlk_engine* e, const int32_t* sids, int n, const int32_t* suppres
     };
     check_ids(suppress_ids, n_suppress, sup);
     check_ids(first_ids, n_first, fst);
-    sg.upload();
+    sg.upload(e->st);
     {   ProfScope ps(e, WLK_KC_LOGITS);
         if (nf && n_first) suppress_tokens(fj_dev, nf, fst_dev, n_first, e->st);
         suppress_tokens(lj_dev, n, sup_dev, n_suppress, e->st);
@@ -1679,7 +1616,7 @@ int wlk_read_mel(wlk_engine* e, int32_t sid, float* out) {
     WLK_CHECK(out && s.encoded, "session not encoded");
     const int nm = e->dims.n_mels;
     // re-run the finalize pass into an fp32 time-major scratch (att is free between calls)
-    Stager sg(e);
+    Stager sg(e->stg);
     MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(1, &mj_dev);
     const int64_t N = s.audio_len;
     int64_t n_compute = (N + 199) / HOP + 1;
@@ -1691,7 +1628,7 @@ int wlk_read_mel(wlk_engine* e, int32_t sid, float* out) {
     // the tap shows what the encoder consumed: the session's cached raw rows (however they were produced -- moved or
     // recomputed) go through the clamp / scale pass again; only audio longer than the stored rows is recomputed
     mj[0].keep_lo = 0; mj[0].keep_hi = n_compute <= MEL_STORE_FRAMES ? (int32_t)n_compute : 0;
-    sg.upload();
+    sg.upload(e->st);
     mel_forward(mj_dev, 1, nm, e->w.filtT, e->w.window, e->w.twiddle, e->w.filt_span, DT_F32, (int)n_compute, e->st);
     float* h = tap_buffer(e, (size_t)MEL_ROWS * nm);
     CUDA_CHECK(cudaMemcpyAsync(h, scratch, (size_t)MEL_ROWS * nm * 4, cudaMemcpyDeviceToHost, e->st));
@@ -1703,7 +1640,7 @@ int wlk_read_mel(wlk_engine* e, int32_t sid, float* out) {
 int wlk_read_encoder(wlk_engine* e, int32_t sid, float* out) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = enc_owner(e, get_session(e, sid));
+    Session& s = enc_owner(e, e->sess.at(sid));
     WLK_CHECK(out && s.encoded, "session not encoded");
     const size_t n = (size_t)N_CTX * e->dims.n_audio_state;
     float* h = tap_buffer(e, n);
@@ -1718,7 +1655,7 @@ int wlk_read_encoder(wlk_engine* e, int32_t sid, float* out) {
 int wlk_read_logits(wlk_engine* e, int32_t sid, int32_t which, float* out) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(out && !s.iter_row_start.empty(), "no decode call in this epoch");
     CUDA_CHECK(cudaMemcpyAsync(out, which ? s.logits_sot : s.logits_last, (size_t)e->dims.n_vocab * 4, cudaMemcpyDeviceToHost, e->st));
     CUDA_CHECK(cudaStreamSynchronize(e->st));
@@ -1727,14 +1664,14 @@ int wlk_read_logits(wlk_engine* e, int32_t sid, int32_t which, float* out) {
 int wlk_read_align_attn(wlk_engine* e, int32_t sid, float* out, int64_t capacity, int32_t* rows, int32_t* cols) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = get_session(e, sid);
+    Session& s = e->sess.at(sid);
     WLK_CHECK(out && rows && cols && !s.iter_row_start.empty(), "no decode call in this epoch");
-    Stager sg(e);
+    Stager sg(e->stg);
     LogitJob* lj_dev; LogitJob* lj = sg.host<LogitJob>(1, &lj_dev);
     lj[0] = make_logit_job(e, s, 16, 1);
     const int T = lj[0].row_end - lj[0].row_begin, C = lj[0].content_len;
     WLK_CHECK((int64_t)T * C <= capacity, "output buffer too small: need %d x %d", T, C);
-    sg.upload();
+    sg.upload(e->st);
     align_reduce(lj_dev, 1, e->n_align, e->dims.n_text_ctx, e->res_dev, e->st);
     float* h = tap_buffer(e, (size_t)T * N_CTX);
     CUDA_CHECK(cudaMemcpyAsync(h, s.attn_out, (size_t)T * N_CTX * 4, cudaMemcpyDeviceToHost, e->st));
@@ -1752,8 +1689,7 @@ int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t l
     GemmArgs g;
     g.A = A; g.a_type = a_type; g.lda = lda; g.W = Wm; g.w_type = w_type; g.ldw = ldw; g.M = M; g.N = N; g.K = K;
     g.epi.bias = bias; g.epi.gelu = gelu & 1; g.epi.C = C; g.epi.c_type = c_type; g.epi.ldc = ldc;
-    g.sk_scratch = e->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
-    g.sk_counters = e->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
+    e->gemm.wire(g);
     if (gelu & 2) { WLK_CHECK(c_type == DT_F32, "in-place accumulation needs an fp32 output"); g.epi.residual = (const float*)C; g.epi.ldr = ldc; }
     ProfScope ps(e, WLK_KC_MISC, 2.0 * M * (double)N * K, 0);
     if (backend == WLK_BACKEND_TCGEN05) gemm_tcgen05(g, e->st, e->num_sms, 0);

@@ -1,5 +1,6 @@
 // Host plumbing shared by the C-ABI units: the entry-point guard, device selection, device buffers kept until
-// destroy, the fp32 weight upload and the checks on loaded tensors.
+// destroy, the fp32 weight upload, the checks on loaded tensors, the staging block, the GEMM dispatch, the session
+// table and the state every engine handle holds.
 #pragma once
 
 #include <initializer_list>
@@ -8,6 +9,7 @@
 #include <string>
 #include <vector>
 
+#include "../../include/wlk_b200.h"
 #include "kernels.cuh"
 
 // The body of every extern "C" entry point runs between these.  No exception crosses the C ABI: the message goes to
@@ -141,5 +143,145 @@ inline void require_loaded(const std::set<std::string>& loaded, const std::vecto
         if (!loaded.count(r) && nmiss++ < 5) missing += r + " ";
     WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
 }
+
+// A pinned host block mirrored on the device: a call lays out its small per-call arrays (jobs, row maps, pointer
+// tables) in it with a Stager and sends them in one H2D copy.  The event recorded after that copy guards the host
+// block: the next layout waits on it before it writes.
+struct Staging {
+    uint8_t *host = nullptr, *dev = nullptr;
+    size_t bytes = 0;
+    cudaEvent_t done = nullptr;
+
+    void alloc(size_t n, DeviceAllocs& allocs, size_t* acct) {
+        bytes = n;
+        CUDA_CHECK(cudaMallocHost(&host, n));
+        dev = reinterpret_cast<uint8_t*>(allocs.take(n, acct));
+        CUDA_CHECK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    }
+    void release() {                                     // `dev` belongs to the DeviceAllocs
+        if (host) cudaFreeHost(host);
+        if (done) cudaEventDestroy(done);
+        host = nullptr;
+        done = nullptr;
+    }
+};
+
+// One layout of the staging block.  Arrays go in call order, each at a 256-byte-aligned offset, so the same sequence of
+// sizes always gives the same device pointers (captured CUDA graphs replay them).
+struct Stager {
+    Staging& stg;
+    size_t used = 0;
+    explicit Stager(Staging& s) : stg(s) { CUDA_CHECK(cudaEventSynchronize(stg.done)); }
+    template <typename T>
+    T* host(size_t count, T** dev) {
+        size_t off = (used + 255) / 256 * 256;
+        size_t bytes = count * sizeof(T);
+        WLK_CHECK(off + bytes <= stg.bytes, "staging buffer overflow (%zu + %zu > %zu)", off, bytes, stg.bytes);
+        used = off + bytes;
+        *dev = reinterpret_cast<T*>(stg.dev + off);
+        return reinterpret_cast<T*>(stg.host + off);
+    }
+    void upload(cudaStream_t st) {
+        if (used) CUDA_CHECK(cudaMemcpyAsync(stg.dev, stg.host, used, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaEventRecord(stg.done, st));
+    }
+};
+
+// An engine's GEMM launch: the split-K scratch of the wgmma kernels and the choice between them and the SIMT kernel.
+// Each engine decides by its own rule whether a GEMM should run on the tensor cores and passes the result as `tc`.
+struct GemmDispatch {
+    float* sk_scratch = nullptr;
+    int* sk_counters = nullptr;
+
+    // Taken only by an engine that runs wgmma GEMMs.
+    void alloc(DeviceAllocs& allocs, size_t* acct) {
+        sk_scratch = (float*)allocs.take(SK_SCRATCH_FLOATS * sizeof(float), acct);
+        sk_counters = (int*)allocs.take(SK_MAX_TILES * sizeof(int), acct);
+    }
+    void wire(GemmArgs& g) const {
+        g.sk_scratch = sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
+        g.sk_counters = sk_counters; g.sk_max_tiles = SK_MAX_TILES;
+    }
+    // A shape the wgmma kernels do not take runs on the SIMT kernel, unless `strict` names the caller: then it raises.
+    void run(GemmArgs& g, bool tc, cudaStream_t st, int num_sms, const char* strict = nullptr) const {
+        if (g.M <= 0) return;
+        wire(g);
+        if (tc) {
+            std::string why;
+            if (gemm_tcgen05_supported(g, strict ? &why : nullptr)) { gemm_tcgen05(g, st, num_sms); return; }
+            WLK_CHECK(!strict, "%s GEMM %dx%dx%d has no wgmma kernel: %s", strict, g.M, g.N, g.K, why.c_str());
+        }
+        gemm_simt(g, st);
+    }
+};
+
+// An engine's session slots.  S has a `bool open`; a closed slot is free.
+template <typename S>
+struct SessionTable {
+    std::vector<S> slots;
+
+    int size() const { return (int)slots.size(); }
+    S& operator[](int32_t sid) { return slots[sid]; }    // a sid that at() or check_batch() accepted
+    typename std::vector<S>::iterator begin() { return slots.begin(); }
+    typename std::vector<S>::iterator end() { return slots.end(); }
+
+    int free_slot() const {
+        for (int i = 0; i < size(); ++i)
+            if (!slots[i].open) return i;
+        WLK_CHECK(false, "all %d sessions in use", size());
+        return -1;
+    }
+    S& at(int32_t sid) {
+        WLK_CHECK(sid >= 0 && sid < size() && slots[sid].open, "invalid session id %d", sid);
+        return slots[sid];
+    }
+    // Every sid of a batch names an open session, and none appears twice.
+    void check_batch(const int32_t* sids, int n) {
+        for (int i = 0; i < n; ++i) {
+            at(sids[i]);
+            for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        }
+    }
+};
+
+// What every engine handle holds.  Calls on a handle take `mu` and make cfg.device current (WLK_ENTER).
+struct EngineBase {
+    wlk_config cfg{};
+    int act = DT_F32;                    // activation type
+    int num_sms = 132;
+    cudaStream_t st = nullptr;
+    std::mutex mu;
+    DeviceAllocs allocs;                 // buffers kept from create (or first use) until destroy
+    WeightUpload upload;
+    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
+    std::set<std::string> loaded;
+    bool finalized = false;
+    Staging stg;
+    GemmDispatch gemm;
+
+    size_t es() const { return dtype_size(act); }
+
+    // The device (sm_90a only), then the engine's non-blocking stream.
+    void open(const wlk_config& c) {
+        cfg = c;
+        num_sms = open_sm90_device(c.device);
+        CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    }
+    // Waits for the stream, lets the engine free its sessions and its own buffers, then frees what every engine holds.
+    template <typename F>
+    void close(F&& free_own) {
+        cudaStreamSynchronize(st);
+        free_own();
+        allocs.free_all();
+        upload.release();
+        stg.release();
+        cudaStreamDestroy(st);
+    }
+    void memory(size_t* weights, size_t* sessions, size_t* workspace) const {
+        if (weights) *weights = bytes_weights;
+        if (sessions) *sessions = bytes_sessions;
+        if (workspace) *workspace = bytes_workspace;
+    }
+};
 
 }  // namespace wlk

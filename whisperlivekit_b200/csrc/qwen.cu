@@ -230,15 +230,10 @@ struct QSession {
 
 using namespace wlk;
 
-struct wlk_qwen {
+struct wlk_qwen : EngineBase {
     wlk_qwen_dims dims{};
-    wlk_config cfg{};
-    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
+    int gemm_backend = WLK_BACKEND_SIMT;
     int ring = 0, max_rows = 0, conv_chunks = 0;                 // conv_chunks: chunks the conv stem's workspace holds
-    cudaStream_t st = nullptr;
-    std::mutex mu;
-    DeviceAllocs allocs;
-    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
     // weights
     float *c1w = nullptr, *c1b = nullptr, *c2b = nullptr, *c3b = nullptr, *bout = nullptr, *pos_table = nullptr, *pos_inv = nullptr;
     void *W2c = nullptr, *W3c = nullptr, *Wout = nullptr, *Wp1 = nullptr, *Wp2 = nullptr;
@@ -247,16 +242,11 @@ struct wlk_qwen {
     bool have_filters = false;
     float* mel_out = nullptr; size_t mel_out_cap = 0; float* audio_scratch = nullptr;
     std::vector<QLayerW> L;
-    std::set<std::string> loaded;
-    bool finalized = false;
-    WeightUpload upload;
     // sessions and workspaces
-    std::vector<QSession> sess;
+    SessionTable<QSession> sess;
     float *mel = nullptr, *x = nullptr, *outbuf = nullptr;                      // conv chunks, residual, head output
     void *a1 = nullptr, *col = nullptr, *a2 = nullptr, *a3 = nullptr;           // conv stem
     void *xn = nullptr, *att = nullptr, *hid = nullptr;                         // layer stack and head
-    float* sk_scratch = nullptr; int* sk_counters = nullptr;      // this engine's split-K workspace (GemmArgs)
-    uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
     // causal engine: the positional rows of a round, q of a round (k / v go to the session rings)
     float* posbuf = nullptr; void* qb = nullptr;
     // windowed engine (wlk_qwen_window_create): geometry, rows of a full window, conv_out's rows, q/k/v, window scratch
@@ -265,18 +255,11 @@ struct wlk_qwen {
     int win_rows = 0, win_block_chunks = 0;
     void* qkv = nullptr;
     float *xc = nullptr, *win_scratch = nullptr;
-    size_t es() const { return dtype_size(act); }
 };
 
 namespace {
 
-void qgemm(wlk_qwen* q, GemmArgs& g) {
-    if (g.M <= 0) return;
-    g.sk_scratch = q->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
-    g.sk_counters = q->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
-    if (q->gemm_backend == WLK_BACKEND_TCGEN05 && gemm_tcgen05_supported(g, nullptr)) gemm_tcgen05(g, q->st, q->num_sms);
-    else gemm_simt(g, q->st);
-}
+void qgemm(wlk_qwen* q, GemmArgs& g) { q->gemm.run(g, q->gemm_backend == WLK_BACKEND_TCGEN05, q->st, q->num_sms); }
 
 void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const int64_t* shape, int ndim) {
     const wlk_qwen_dims& D = q->dims;
@@ -452,16 +435,14 @@ wlk_qwen* create_common(const wlk_qwen_dims& D, const wlk_config* cfg, int max_r
     WLK_CHECK(D.d_model % 64 == 0 && D.d_model / D.n_head == 64 && D.d_model <= 1280, "heads must be 64 wide, d_model <= 1280");
     WLK_CHECK(D.conv_channels % 8 == 0, "conv_channels must be a multiple of 8");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    const int num_sms = open_sm90_device(cfg->device);
 
     auto* q = new wlk_qwen();
-    q->dims = D; q->cfg = *cfg;
-    q->num_sms = num_sms;
+    q->open(*cfg);
+    q->dims = D;
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     q->max_rows = max_rows;
     q->conv_chunks = (int)conv_chunks;
-    CUDA_CHECK(cudaStreamCreateWithFlags(&q->st, cudaStreamNonBlocking));
     alloc_weights(q);
     const size_t es = q->es(), R = (size_t)max_rows, CH = conv_chunks;
     const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
@@ -478,14 +459,9 @@ wlk_qwen* create_common(const wlk_qwen_dims& D, const wlk_config* cfg, int max_r
     q->hid = q->allocs.take(R * (size_t)std::max(ffn, d) * es, ws);
     q->outbuf = (float*)q->allocs.take(R * D.out_dim * 4, ws);
     q->audio_scratch = (float*)q->allocs.take((size_t)QMEL_AUDIO_CAP * 4, ws);
-    if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
-        q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
-        q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
-    }
-    q->stg_bytes = stg_bytes;
-    CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
-    q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
-    q->sess.resize(cfg->max_sessions);
+    if (q->gemm_backend == WLK_BACKEND_TCGEN05) q->gemm.alloc(q->allocs, ws);
+    q->stg.alloc(stg_bytes, q->allocs, ws);
+    q->sess.slots.resize(cfg->max_sessions);
     return q;
 }
 
@@ -511,19 +487,11 @@ void create(const wlk_qwen_dims* dims, const wlk_config* cfg, wlk_qwen** out) {
 }
 
 void destroy(wlk_qwen* q) {
-    cudaStreamSynchronize(q->st);
-    for (auto& s : q->sess) { if (s.kv) cudaFree(s.kv); if (s.win) cudaFree(s.win); if (s.audio) cudaFree(s.audio); if (s.mel_raw) cudaFree(s.mel_raw); if (s.mel_blockmax) cudaFree(s.mel_blockmax); }
-    if (q->mel_out) cudaFree(q->mel_out);
-    q->allocs.free_all();
-    q->upload.release();
-    if (q->stg_h) cudaFreeHost(q->stg_h);
-    cudaStreamDestroy(q->st);
+    q->close([q] {
+        for (auto& s : q->sess) { if (s.kv) cudaFree(s.kv); if (s.win) cudaFree(s.win); if (s.audio) cudaFree(s.audio); if (s.mel_raw) cudaFree(s.mel_raw); if (s.mel_blockmax) cudaFree(s.mel_blockmax); }
+        if (q->mel_out) cudaFree(q->mel_out);
+    });
     delete q;
-}
-
-QSession& qsession(wlk_qwen* q, int32_t sid) {
-    WLK_CHECK(sid >= 0 && sid < (int)q->sess.size() && q->sess[sid].open, "invalid session id %d", sid);
-    return q->sess[sid];
 }
 
 int grid_1d(int64_t total) { const int64_t b = (total + 255) / 256; return (int)(b > 65535 * 16 ? 65535 * 16 : b); }
@@ -680,9 +648,9 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
     std::vector<std::vector<float>> ready(n), rest(n), new_tail(n);
     std::vector<int> done_steps(n, 0), total_steps(n, 0), freeze(n, 0);
     int64_t rows_total = 0;
+    q->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
-        QSession& s = qsession(q, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        QSession& s = q->sess[sids[i]];
         std::vector<float> all(s.pending);
         if (!flush) {
             const int nf = frame_off[i + 1] - frame_off[i];
@@ -722,10 +690,9 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
         for (int i = 0; i < n; ++i) if (done_steps[i] < total_steps[i]) who.push_back(i);
         if (who.empty()) break;
         int nj = (int)who.size();
-        // carve the staging block
-        size_t off = 0;
-        auto carve = [&](size_t bytes) { size_t o = (off + 255) / 256 * 256; off = o + bytes; WLK_CHECK(off <= q->stg_bytes, "staging overflow"); return o; };
-        const size_t o_jobs = carve(nj * sizeof(QJob)), o_kv = carve(nj * sizeof(void*));
+        Stager sg(q->stg);
+        QJob* jobs_dev; QJob* jobs = sg.host<QJob>(nj, &jobs_dev);
+        void** kv_dev; void** kvp = sg.host<void*>(nj, &kv_dev);
         int R = 0;
         std::vector<int> steps(nj);
         for (int k = 0; k < nj; ++k) { steps[k] = std::min(steps_cap, total_steps[who[k]] - done_steps[who[k]]); R += steps[k]; }
@@ -735,14 +702,11 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
             WLK_CHECK(keep >= 1, "round of %d steps exceeds the workspace (%d)", steps[0], q->max_rows);
             who.resize(keep); steps.resize(keep); R = acc; nj = keep;
         }
-        const size_t o_ch = carve((size_t)R * sizeof(WChunk));
-        const size_t o_slot = carve((size_t)R * 4), o_ring = carve((size_t)R * 4), o_abs = carve((size_t)R * 4);
-        WChunk* chunks = reinterpret_cast<WChunk*>(q->stg_h + o_ch);
-        QJob* jobs = reinterpret_cast<QJob*>(q->stg_h + o_jobs);
-        void** kvp = reinterpret_cast<void**>(q->stg_h + o_kv);
-        int32_t* slot = reinterpret_cast<int32_t*>(q->stg_h + o_slot);
-        int32_t* ringpos = reinterpret_cast<int32_t*>(q->stg_h + o_ring);
-        int32_t* abspos = reinterpret_cast<int32_t*>(q->stg_h + o_abs);
+        WChunk* chunks_dev; WChunk* chunks = sg.host<WChunk>(R, &chunks_dev);
+        int32_t *slot_dev, *ring_dev, *abs_dev;
+        int32_t* slot = sg.host<int32_t>(R, &slot_dev);
+        int32_t* ringpos = sg.host<int32_t>(R, &ring_dev);
+        int32_t* abspos = sg.host<int32_t>(R, &abs_dev);
         int r = 0;
         for (int k = 0; k < nj; ++k) {
             const int i = who[k];
@@ -758,13 +722,7 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
                 slot[r] = k; abspos[r] = (int32_t)(start + t); ringpos[r] = (int32_t)((start + t) % q->ring);
             }
         }
-        CUDA_CHECK(cudaMemcpyAsync(q->stg_d, q->stg_h, off, cudaMemcpyHostToDevice, q->st));
-        const QJob* jobs_dev = reinterpret_cast<const QJob*>(q->stg_d + o_jobs);
-        void* const* kv_dev = reinterpret_cast<void* const*>(q->stg_d + o_kv);
-        const int32_t* slot_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_slot);
-        const int32_t* ring_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_ring);
-        const int32_t* abs_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_abs);
-        const WChunk* chunks_dev = reinterpret_cast<const WChunk*>(q->stg_d + o_ch);
+        sg.upload(q->st);
         if (q->act == DT_F32) run_round_typed<float>(q, nj, R, jobs_dev, chunks_dev, kv_dev, slot_dev, ring_dev, abs_dev);
         else run_round_typed<bf16>(q, nj, R, jobs_dev, chunks_dev, kv_dev, slot_dev, ring_dev, abs_dev);
         r = 0;
@@ -777,7 +735,7 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
             done_steps[i] += steps[k];
             q->sess[sids[i]].emitted += M > 0 ? freeze[i] : steps[k];    // a mutable tail: only the frozen steps count (:638)
         }
-        CUDA_CHECK(cudaStreamSynchronize(q->st));        // the staging block and outbuf are reused by the next round
+        CUDA_CHECK(cudaStreamSynchronize(q->st));        // outbuf is reused by the next round
     }
     for (int i = 0; i < n; ++i) {                        // commit the host-side buffers
         QSession& s = q->sess[sids[i]];
@@ -797,9 +755,9 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
     std::vector<Plan> plan(n, Plan{0, 0, 0});
     std::vector<int> who;
     int64_t rows = 0;
+    q->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
-        QSession& s = qsession(q, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        QSession& s = q->sess[sids[i]];
         if (!s.audio) {
             CUDA_CHECK(cudaMalloc(&s.audio, (size_t)QMEL_AUDIO_CAP * 4));
             CUDA_CHECK(cudaMalloc(&s.mel_raw, (size_t)MEL_STORE_FRAMES * D.n_mels * 4));
@@ -844,12 +802,10 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
         q->mel_out_cap = (size_t)rows * D.n_mels * 2;
         CUDA_CHECK(cudaMalloc(&q->mel_out, q->mel_out_cap * 4));
     }
-    size_t off = 0;
-    auto carve = [&](size_t bytes) { size_t o = (off + 255) / 256 * 256; off = o + bytes; WLK_CHECK(off <= q->stg_bytes, "staging overflow"); return o; };
-    const size_t o_jobs = carve(nj * sizeof(MelJob)), o_rng = carve(nj * sizeof(int2)), o_off = carve(nj * sizeof(int64_t));
-    MelJob* mj = reinterpret_cast<MelJob*>(q->stg_h + o_jobs);
-    int2* rng = reinterpret_cast<int2*>(q->stg_h + o_rng);
-    int64_t* ooff = reinterpret_cast<int64_t*>(q->stg_h + o_off);
+    Stager sg(q->stg);
+    MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(nj, &mj_dev);
+    int2* rng_dev; int2* rng = sg.host<int2>(nj, &rng_dev);
+    int64_t* ooff_dev; int64_t* ooff = sg.host<int64_t>(nj, &ooff_dev);
     int max_frames = 1;
     for (int k = 0; k < nj; ++k) {
         const int i = who[k];
@@ -859,10 +815,9 @@ void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, con
         rng[k] = make_int2(plan[i].first, plan[i].last);
         ooff[k] = frame_off[i];
     }
-    CUDA_CHECK(cudaMemcpyAsync(q->stg_d, q->stg_h, off, cudaMemcpyHostToDevice, q->st));
-    mel_window_forward(reinterpret_cast<const MelJob*>(q->stg_d + o_jobs), reinterpret_cast<const int2*>(q->stg_d + o_rng),
-                       reinterpret_cast<const int64_t*>(q->stg_d + o_off), q->mel_out, nj, D.n_mels, q->filtT, q->window,
-                       q->twiddle, q->filt_span, max_frames, q->st);
+    sg.upload(q->st);
+    mel_window_forward(mj_dev, rng_dev, ooff_dev, q->mel_out, nj, D.n_mels, q->filtT, q->window, q->twiddle, q->filt_span,
+                       max_frames, q->st);
     CUDA_CHECK(cudaMemcpyAsync(out, q->mel_out, (size_t)rows * D.n_mels * 4, cudaMemcpyDeviceToHost, q->st));
     // drop the samples no longer needed: keep MARGIN (8) frames of history before the next frame to emit (features.py:77-83)
     for (int k = 0; k < nj; ++k) {
@@ -1216,16 +1171,12 @@ int64_t run_windows(wlk_qwen* q, const std::vector<const float*>& wins, const st
     std::vector<int32_t> emit;
     for (int i = 0; i < n; ++i) for (int r = lo[i]; r < hi[i]; ++r) emit.push_back(row_off[i] + r);
     const int E = (int)emit.size();
-    size_t off = 0;
-    auto carve = [&](size_t bytes) { size_t o = (off + 255) / 256 * 256; off = o + bytes; WLK_CHECK(off <= q->stg_bytes, "staging overflow"); return o; };
-    const size_t o_ch = carve(chunks.size() * sizeof(WChunk)), o_it = carve(items.size() * sizeof(WAttn)), o_em = carve((size_t)E * 4);
-    memcpy(q->stg_h + o_ch, chunks.data(), chunks.size() * sizeof(WChunk));
-    memcpy(q->stg_h + o_it, items.data(), items.size() * sizeof(WAttn));
-    memcpy(q->stg_h + o_em, emit.data(), (size_t)E * 4);
-    CUDA_CHECK(cudaMemcpyAsync(q->stg_d, q->stg_h, off, cudaMemcpyHostToDevice, q->st));
-    const WChunk* chunks_dev = reinterpret_cast<const WChunk*>(q->stg_d + o_ch);
-    const WAttn* items_dev = reinterpret_cast<const WAttn*>(q->stg_d + o_it);
-    const int32_t* emit_dev = reinterpret_cast<const int32_t*>(q->stg_d + o_em);
+    Stager sg(q->stg);
+    WChunk* chunks_dev; WAttn* items_dev; int32_t* emit_dev;
+    memcpy(sg.host<WChunk>(chunks.size(), &chunks_dev), chunks.data(), chunks.size() * sizeof(WChunk));
+    memcpy(sg.host<WAttn>(items.size(), &items_dev), items.data(), items.size() * sizeof(WAttn));
+    memcpy(sg.host<int32_t>(E, &emit_dev), emit.data(), (size_t)E * 4);
+    sg.upload(q->st);
     // conv stem, in rounds of at most QW_CHUNKS_PER_ROUND chunks
     for (size_t c0 = 0; c0 < chunks.size(); c0 += QW_CHUNKS_PER_ROUND) {
         const int nc = (int)std::min<size_t>(QW_CHUNKS_PER_ROUND, chunks.size() - c0);
@@ -1264,9 +1215,9 @@ void window_forward(wlk_qwen* q, const int32_t* sids, int n, const float* mels, 
     struct Plan { int nf, keep, drop_old, lo, hi, take; };
     std::vector<Plan> plan(n);
     int64_t rows_total = 0;
+    q->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {                            // validate and plan; no session changes before the encode
-        QSession& s = qsession(q, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        QSession& s = q->sess[sids[i]];
         const int nf = frame_off[i + 1] - frame_off[i];
         WLK_CHECK(nf >= 0, "negative frame count");
         Plan p{nf, (int)s.win_len, 0, 0, 0, 0};
@@ -1501,9 +1452,7 @@ int wlk_qwen_session_open(wlk_qwen* q, int32_t* sid) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sid, "null out pointer");
-    int found = -1;
-    for (int i = 0; i < (int)q->sess.size(); ++i) if (!q->sess[i].open) { found = i; break; }
-    WLK_CHECK(found >= 0, "all %d sessions in use", (int)q->sess.size());
+    const int found = q->sess.free_slot();
     QSession& s = q->sess[found];
     const size_t bytes = session_bytes(q);
     CUDA_CHECK(cudaMalloc(q->windowed ? (void**)&s.win : &s.kv, bytes));
@@ -1515,7 +1464,7 @@ int wlk_qwen_session_open(wlk_qwen* q, int32_t* sid) {
 int wlk_qwen_session_close(wlk_qwen* q, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     cudaFree(q->windowed ? (void*)s.win : s.kv);
     q->bytes_sessions -= session_bytes(q);
@@ -1529,7 +1478,7 @@ int wlk_qwen_session_close(wlk_qwen* q, int32_t sid) {
 int wlk_qwen_session_reset(wlk_qwen* q, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     s.emitted = 0; s.pending.clear(); s.tail.clear();
     s.buf_len = s.buf_start_frame = s.mel_emitted = s.total_samples = 0;       // StreamingMelExtractor.reset, features.py:112
     s.win_len = s.frames_seen = s.window_start = s.last_in = s.last_rec = s.last_ctx = 0;
@@ -1538,7 +1487,7 @@ int wlk_qwen_session_reset(wlk_qwen* q, int32_t sid) {
 int wlk_qwen_session_state(wlk_qwen* q, int32_t sid, int32_t* pending_frames, int64_t* emitted_steps) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     if (pending_frames) *pending_frames = (int32_t)(s.pending.size() / q->dims.n_mels);
     if (emitted_steps) *emitted_steps = s.emitted;
     WLK_API_END
@@ -1546,7 +1495,7 @@ int wlk_qwen_session_state(wlk_qwen* q, int32_t sid, int32_t* pending_frames, in
 int wlk_qwen_session_mutable_steps(wlk_qwen* q, int32_t sid, int32_t* mutable_steps) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     WLK_CHECK(mutable_steps != nullptr, "null argument");
     *mutable_steps = (int32_t)(s.tail.size() / ((size_t)8 * q->dims.n_mels));
     WLK_API_END
@@ -1590,7 +1539,7 @@ int wlk_qwen_flush_pending_device(wlk_qwen* q, const int32_t* sids, int n, float
 int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int64_t capacity_frames, int32_t* n_frames) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     WLK_CHECK(n_frames, "null argument");
     const int64_t have = (int64_t)(s.pending.size() / q->dims.n_mels);
     WLK_CHECK(have <= capacity_frames, "%lld pending frames exceed the buffer's %lld", (long long)have, (long long)capacity_frames);
@@ -1602,7 +1551,7 @@ int wlk_qwen_session_get_pending(wlk_qwen* q, int32_t sid, float* mels_host, int
 int wlk_qwen_session_set_pending(wlk_qwen* q, int32_t sid, const float* mels_host, int32_t n_frames) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     WLK_CHECK(n_frames >= 0 && (mels_host || n_frames == 0), "bad arguments");
     s.pending.assign(mels_host, mels_host + (size_t)n_frames * q->dims.n_mels);
     WLK_API_END
@@ -1645,7 +1594,7 @@ int wlk_qwen_window_state(wlk_qwen* q, int32_t sid, int64_t* fields) {
     WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(q->windowed, "not a windowed engine");
     WLK_CHECK(fields != nullptr, "null argument");
-    QSession& s = qsession(q, sid);
+    QSession& s = q->sess.at(sid);
     const int64_t v[7] = {s.frames_seen, s.window_start, s.emitted, s.last_in, s.last_rec, s.last_ctx, s.win_len};
     memcpy(fields, v, sizeof(v));
     WLK_API_END
@@ -1706,9 +1655,7 @@ int wlk_qwen_op_attention(wlk_qwen* q, int32_t layer, const void* q_dev, const i
 int wlk_qwen_memory(wlk_qwen* q, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    if (weights) *weights = q->bytes_weights;
-    if (sessions) *sessions = q->bytes_sessions;
-    if (workspace) *workspace = q->bytes_workspace;
+    q->memory(weights, sessions, workspace);
     WLK_API_END
 }
 

@@ -438,53 +438,31 @@ constexpr float QT_ADAPTER_EPS = 1e-6f;
 
 using namespace wlk;
 
-struct wlk_qtext {
+struct wlk_qtext : EngineBase {
     wlk_qtext_dims dims{};
-    wlk_config cfg{};
-    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
-    cudaStream_t st = nullptr;
-    std::mutex mu;
-    DeviceAllocs allocs;
-    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0, kv_bytes = 0;
+    size_t kv_bytes = 0;
     float *emb = nullptr, *normw = nullptr, *inv_freq = nullptr;
     void* head = nullptr;                               // lm_head [V][d] act type (the embedding table when tied)
     std::vector<QTLayerW> L;
-    std::set<std::string> loaded;
-    bool finalized = false;
-    WeightUpload upload;
-    std::vector<QTSession> sess;
+    SessionTable<QTSession> sess;
     float *x = nullptr, *qkv = nullptr, *gu = nullptr, *up = nullptr, *logits = nullptr, *values_d = nullptr;
     void *xn = nullptr, *qb = nullptr, *att = nullptr, *hid = nullptr, *hlog = nullptr;
     int32_t* picks_d = nullptr;
     float* up_h = nullptr;                               // pinned: the round's host embedding rows, one H2D copy per round
-    cudaEvent_t stg_ev = nullptr;                        // recorded after the last H2D copy out of stg_h / up_h
     int32_t* pick_d = nullptr; size_t pick_cap = 0;      // device copy of a pick call's histories, suppress list, offsets
     int32_t* gen_d = nullptr; size_t gen_cap = 0;        // generate_full: per-session token histories + next tokens
     int logit_group = 0;
     int up_rows = 0;                                     // rows of `up` (uploaded embedding rows)
     int logit_cap = 0, n_logit = 0;                      // rows of hlog; rows the last forward kept
-    float* sk_scratch = nullptr; int* sk_counters = nullptr;
-    uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
     std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> adapter_stash;   // until finalize
     bool has_adapter = false;
     QTAdapter ad;
-    size_t es() const { return dtype_size(act); }
 };
 
 namespace {
 
-void tgemm(wlk_qtext* t, GemmArgs& g) {
-    if (g.M <= 0) return;
-    g.sk_scratch = t->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
-    g.sk_counters = t->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
-    if (t->gemm_backend == WLK_BACKEND_TCGEN05) {
-        std::string why;
-        WLK_CHECK(gemm_tcgen05_supported(g, &why), "text decoder GEMM %dx%dx%d has no wgmma kernel: %s", g.M, g.N, g.K, why.c_str());
-        gemm_tcgen05(g, t->st, t->num_sms);
-    } else {
-        gemm_simt(g, t->st);
-    }
-}
+// bf16 runs every GEMM on the wgmma kernels (cfg->gemm_backend is not consulted); a shape they do not take is an error
+void tgemm(wlk_qtext* t, GemmArgs& g) { t->gemm.run(g, t->act == DT_BF16, t->st, t->num_sms, "text decoder"); }
 
 void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const int64_t* shape, int ndim) {
     const wlk_qtext_dims& D = t->dims;
@@ -616,14 +594,11 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     WLK_CHECK(D.max_ctx >= 1 && D.max_ctx <= 32768, "max_ctx must be in [1, 32768]");
     WLK_CHECK((size_t)(D.vocab + 31) / 32 * 4 <= 200 * 1024, "vocab too large for the pick kernel's bitmap");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    const int num_sms = open_sm90_device(cfg->device);
 
     auto* t = new wlk_qtext();
-    t->dims = D; t->cfg = *cfg;
-    t->num_sms = num_sms;
+    t->open(*cfg);
+    t->dims = D;
     t->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
-    t->gemm_backend = t->act == DT_BF16 ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
-    CUDA_CHECK(cudaStreamCreateWithFlags(&t->st, cudaStreamNonBlocking));
     const size_t es = t->es();
     const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
     const size_t W = (size_t)(H + 2 * KV) * QT_HD;
@@ -665,38 +640,23 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     t->logits = (float*)t->allocs.take((size_t)t->logit_group * D.vocab * 4, ws);
     t->picks_d = (int32_t*)t->allocs.take((size_t)t->logit_cap * 4, ws);
     t->values_d = (float*)t->allocs.take((size_t)t->logit_cap * 4, ws);
-    if (t->gemm_backend == WLK_BACKEND_TCGEN05) {
-        t->sk_scratch = (float*)t->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
-        t->sk_counters = (int*)t->allocs.take(SK_MAX_TILES * 4, ws);
-    }
-    t->stg_bytes = R * 32 + (size_t)cfg->max_batch * 16 + 8192;
-    CUDA_CHECK(cudaMallocHost(&t->stg_h, t->stg_bytes));
+    if (t->act == DT_BF16) t->gemm.alloc(t->allocs, ws);
+    t->stg.alloc(R * 32 + (size_t)cfg->max_batch * 16 + 8192, t->allocs, ws);
     CUDA_CHECK(cudaMallocHost(&t->up_h, R * d * 4));
-    CUDA_CHECK(cudaEventCreateWithFlags(&t->stg_ev, cudaEventDisableTiming));
-    t->stg_d = (uint8_t*)t->allocs.take(t->stg_bytes, ws);
     t->kv_bytes = (size_t)D.n_layer * 2 * KV * D.max_ctx * QT_HD * es;
-    t->sess.resize(cfg->max_sessions);
+    t->sess.slots.resize(cfg->max_sessions);
     CUDA_CHECK(cudaFuncSetAttribute(qt_pick_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     *out = t;
 }
 
 void destroy(wlk_qtext* t) {
-    cudaStreamSynchronize(t->st);
-    for (auto& s : t->sess) if (s.kv) cudaFree(s.kv);
-    t->allocs.free_all();
-    t->upload.release();
-    if (t->stg_h) cudaFreeHost(t->stg_h);
-    if (t->up_h) cudaFreeHost(t->up_h);
-    if (t->pick_d) cudaFree(t->pick_d);
-    if (t->gen_d) cudaFree(t->gen_d);
-    if (t->stg_ev) cudaEventDestroy(t->stg_ev);
-    cudaStreamDestroy(t->st);
+    t->close([t] {
+        for (auto& s : t->sess) if (s.kv) cudaFree(s.kv);
+        if (t->up_h) cudaFreeHost(t->up_h);
+        if (t->pick_d) cudaFree(t->pick_d);
+        if (t->gen_d) cudaFree(t->gen_d);
+    });
     delete t;
-}
-
-QTSession& tsession(wlk_qtext* t, int32_t sid) {
-    WLK_CHECK(sid >= 0 && sid < (int)t->sess.size() && t->sess[sid].open, "invalid session id %d", sid);
-    return t->sess[sid];
 }
 
 // Attention tiles of one round (the bf16 kernel's CTAs): <= 16 consecutive rows of one slot, a new tile whenever the
@@ -794,9 +754,9 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
     WLK_CHECK(t->finalized, "weights not finalized");
     WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
     int n_logit = 0;
+    t->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
-        QTSession& s = tsession(t, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        QTSession& s = t->sess[sids[i]];
         const int r = row_off[i + 1] - row_off[i];
         WLK_CHECK(r >= 1, "session %d has no rows", sids[i]);
         WLK_CHECK(s.len + r <= D.max_ctx, "context full: session %d holds %d positions, %d more exceed max_ctx %d", sids[i], s.len, r, D.max_ctx);
@@ -823,17 +783,14 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
     }
     for (int r0 = 0; r0 < total; r0 += QT_ROUND_ROWS) {
         const int R = std::min(QT_ROUND_ROWS, total - r0);
-        size_t off = 0;
-        auto carve = [&](size_t bytes) { size_t o = (off + 255) / 256 * 256; off = o + bytes; WLK_CHECK(off <= t->stg_bytes, "staging overflow"); return o; };
-        const size_t o_src = carve((size_t)R * 4), o_pos = carve((size_t)R * 4), o_slot = carve((size_t)R * 4),
-                     o_log = carve((size_t)R * 4), o_kv = carve((size_t)n * sizeof(void*)),
-                     o_tile = carve((size_t)R * sizeof(QTAttnTile));
-        CUDA_CHECK(cudaEventSynchronize(t->stg_ev));     // the previous H2D copy out of stg_h / up_h has been consumed
-        int32_t* src = reinterpret_cast<int32_t*>(t->stg_h + o_src);
-        int32_t* pos = reinterpret_cast<int32_t*>(t->stg_h + o_pos);
-        int32_t* slot = reinterpret_cast<int32_t*>(t->stg_h + o_slot);
-        int32_t* lrow = reinterpret_cast<int32_t*>(t->stg_h + o_log);
-        void** kvp = reinterpret_cast<void**>(t->stg_h + o_kv);
+        Stager sg(t->stg);                               // also waits until the previous round's copy out of up_h is done
+        int32_t *src_d, *pos_d, *slot_d, *log_d;
+        int32_t* src = sg.host<int32_t>(R, &src_d);
+        int32_t* pos = sg.host<int32_t>(R, &pos_d);
+        int32_t* slot = sg.host<int32_t>(R, &slot_d);
+        int32_t* lrow = sg.host<int32_t>(R, &log_d);
+        void** kv_d; void** kvp = sg.host<void*>(n, &kv_d);
+        QTAttnTile* tiles_d; QTAttnTile* tiles = sg.host<QTAttnTile>(R, &tiles_d);
         for (int i = 0; i < n; ++i) kvp[i] = t->sess[sids[i]].kv;
         // embedding rows of this round go to `up` in the order they appear: packed into pinned memory, one copy
         int n_up = 0;
@@ -846,17 +803,9 @@ void forward(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_src, c
             }
             src[k] = s; pos[k] = r_pos[r]; slot[k] = r_sess[r]; lrow[k] = r_log[r];
         }
-        QTAttnTile* tiles = reinterpret_cast<QTAttnTile*>(t->stg_h + o_tile);
         const int n_tiles = make_tiles(pos, slot, R, tiles);
         if (n_up) CUDA_CHECK(cudaMemcpyAsync(t->up, t->up_h, (size_t)n_up * D.d_model * 4, cudaMemcpyHostToDevice, t->st));
-        CUDA_CHECK(cudaMemcpyAsync(t->stg_d, t->stg_h, off, cudaMemcpyHostToDevice, t->st));
-        CUDA_CHECK(cudaEventRecord(t->stg_ev, t->st));
-        const int32_t* src_d = reinterpret_cast<const int32_t*>(t->stg_d + o_src);
-        const int32_t* pos_d = reinterpret_cast<const int32_t*>(t->stg_d + o_pos);
-        const int32_t* slot_d = reinterpret_cast<const int32_t*>(t->stg_d + o_slot);
-        const int32_t* log_d = reinterpret_cast<const int32_t*>(t->stg_d + o_log);
-        void* const* kv_d = reinterpret_cast<void* const*>(t->stg_d + o_kv);
-        const QTAttnTile* tiles_d = reinterpret_cast<const QTAttnTile*>(t->stg_d + o_tile);
+        sg.upload(t->st);                                // its event guards up_h as well
         const float* up = dev_rows ? embeds : t->up;
         const int64_t up_ld = dev_rows ? embeds_ld : D.d_model;
         if (t->act == DT_F32) run_round<float>(t, R, src_d, pos_d, slot_d, kv_d, log_d, tiles_d, n_tiles, up, up_ld, tok_d);
@@ -974,9 +923,8 @@ void generate_full(wlk_qtext* t, const int32_t* sids, int n, const int32_t* row_
         WLK_CHECK(t->finalized, "weights not finalized");
         WLK_CHECK(n >= 1 && n <= t->cfg.max_batch, "batch %d outside [1, %d]", n, t->cfg.max_batch);
         WLK_CHECK(max_new >= 0, "max_new_tokens %d < 0", max_new);
+        t->sess.check_batch(sids, n);
         for (int i = 0; i < n; ++i) {
-            tsession(t, sids[i]);
-            for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
             const int r = row_off[i + 1] - row_off[i];
             WLK_CHECK(r >= 1, "session %d has no rows", sids[i]);
             WLK_CHECK((int64_t)r + max_new <= D.max_ctx, "session %d: prefix %d + max_new_tokens %d exceed max_ctx %d", sids[i], r,
@@ -1053,9 +1001,9 @@ void generate_rolling(wlk_qtext* t, const int32_t* sids, int n, const int32_t* r
     WLK_CHECK(max_new >= 1, "max_new_tokens %d < 1", max_new);
     WLK_CHECK(tail_len >= 0, "tail_len %d < 0", tail_len);
     int n_verify = 0, n_draft = 0;
+    t->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
-        const QTSession& s = tsession(t, sids[i]);
-        for (int j = 0; j < i; ++j) WLK_CHECK(sids[j] != sids[i], "session %d appears twice in the batch", sids[i]);
+        const QTSession& s = t->sess[sids[i]];
         const int r = row_off[i + 1] - row_off[i], dl = draft_len[i], p = prefix_len[i];
         WLK_CHECK(dl >= 0 && dl <= max_new && dl + 1 <= r, "session %d: draft_len %d outside [0, min(max_new_tokens %d, rows %d - 1)]",
                   sids[i], dl, max_new, r);
@@ -1335,18 +1283,14 @@ int wlk_qtext_finalize_weights(wlk_qtext* t) {
 int wlk_qtext_memory(wlk_qtext* t, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
-    if (weights) *weights = t->bytes_weights;
-    if (sessions) *sessions = t->bytes_sessions;
-    if (workspace) *workspace = t->bytes_workspace;
+    t->memory(weights, sessions, workspace);
     WLK_API_END
 }
 int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(sid, "null out pointer");
-    int found = -1;
-    for (int i = 0; i < (int)t->sess.size(); ++i) if (!t->sess[i].open) { found = i; break; }
-    WLK_CHECK(found >= 0, "all %d sessions in use", (int)t->sess.size());
+    const int found = t->sess.free_slot();
     QTSession& s = t->sess[found];
     CUDA_CHECK(cudaMalloc(&s.kv, t->kv_bytes));
     t->bytes_sessions += t->kv_bytes;
@@ -1357,7 +1301,7 @@ int wlk_qtext_session_open(wlk_qtext* t, int32_t* sid) {
 int wlk_qtext_session_close(wlk_qtext* t, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
-    QTSession& s = tsession(t, sid);
+    QTSession& s = t->sess.at(sid);
     CUDA_CHECK(cudaStreamSynchronize(t->st));
     cudaFree(s.kv);
     t->bytes_sessions -= t->kv_bytes;
@@ -1367,20 +1311,20 @@ int wlk_qtext_session_close(wlk_qtext* t, int32_t sid) {
 int wlk_qtext_session_reset(wlk_qtext* t, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
-    tsession(t, sid).len = 0;
+    t->sess.at(sid).len = 0;
     WLK_API_END
 }
 int wlk_qtext_session_len(wlk_qtext* t, int32_t sid, int32_t* len) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(len, "null out pointer");
-    *len = tsession(t, sid).len;
+    *len = t->sess.at(sid).len;
     WLK_API_END
 }
 int wlk_qtext_crop(wlk_qtext* t, int32_t sid, int32_t len) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
-    QTSession& s = tsession(t, sid);
+    QTSession& s = t->sess.at(sid);
     WLK_CHECK(len >= 0 && len <= s.len, "crop to %d outside [0, %d]", len, s.len);
     s.len = len;
     WLK_API_END

@@ -21,7 +21,6 @@
 
 #include <map>
 #include <mutex>
-#include <set>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -692,16 +691,11 @@ struct SfSession {
 
 using namespace wlk;
 
-struct wlk_sf {
+struct wlk_sf : EngineBase {
     wlk_sf_dims dims{};
-    wlk_config cfg{};
-    int act = DT_F32, gemm_backend = WLK_BACKEND_SIMT, num_sms = 132;
+    int gemm_backend = WLK_BACKEND_SIMT;
     int F1 = 0, F2 = 0, F3 = 0, frames_per_chunk = 0, prev_keep = 99, chunk_samples = 0, n_freq = 0;
     int max_T = 0, max_T3 = 0, max_feat = 0, max_pop = 0, max_chunk_cap = 0;
-    cudaStream_t st = nullptr;
-    std::mutex mu;
-    DeviceAllocs allocs;
-    size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
     // front end + conv stem
     float *window = nullptr, *fbT = nullptr; float2* twiddle = nullptr; int2* span = nullptr;
     float *c0w = nullptr, *c0b = nullptr, *dw1w = nullptr, *dw1b = nullptr, *dw2w = nullptr, *dw2b = nullptr, *pw1b = nullptr, *pw2b = nullptr, *outb = nullptr;
@@ -710,28 +704,14 @@ struct wlk_sf {
     std::vector<SfTLayerW> TL;
     void *Wproj = nullptr, *Wh = nullptr; float *bproj = nullptr, *bh = nullptr, *Wspk = nullptr, *bspk = nullptr;
     float* pe_table = nullptr;          // [2 SF_MAX_T - 1][D] RelPositionalEncoding rows, fp32 (input of the per-layer tables)
-    std::set<std::string> loaded;
-    bool finalized = false;
-    WeightUpload upload;
-    std::vector<SfSession> sess;
+    SessionTable<SfSession> sess;
     // workspaces
     float *pcm = nullptr, *feats = nullptr, *chunk = nullptr, *x = nullptr, *y = nullptr, *preds = nullptr, *out_preds = nullptr;
     void *a1 = nullptr, *a2 = nullptr, *a2p = nullptr, *a3 = nullptr, *a3p = nullptr, *xn = nullptr, *qkv = nullptr, *att = nullptr, *hid = nullptr, *cv = nullptr;
-    float* sk_scratch = nullptr; int* sk_counters = nullptr;
-    uint8_t *stg_h = nullptr, *stg_d = nullptr; size_t stg_bytes = 0;
     float* out_h = nullptr;
-    size_t es() const { return dtype_size(act); }
 };
 
 namespace {
-
-void sfgemm(wlk_sf* q, GemmArgs& g) {
-    if (g.M <= 0) return;
-    g.sk_scratch = q->sk_scratch; g.sk_scratch_floats = SK_SCRATCH_FLOATS;
-    g.sk_counters = q->sk_counters; g.sk_max_tiles = SK_MAX_TILES;
-    if (q->gemm_backend == WLK_BACKEND_TCGEN05 && gemm_tcgen05_supported(g, nullptr)) gemm_tcgen05(g, q->st, q->num_sms);
-    else gemm_simt(g, q->st);
-}
 
 void gemm(wlk_sf* q, const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K, const float* bias, int act_fn,
           void* C, int c_type, int64_t ldc, const float* residual = nullptr, float scale = 1.f, int scale_cols = 0) {
@@ -740,7 +720,7 @@ void gemm(wlk_sf* q, const void* A, int64_t lda, const void* W, int64_t ldw, int
     g.M = M; g.N = N; g.K = K;
     g.epi.bias = bias; g.epi.gelu = act_fn; g.epi.C = C; g.epi.c_type = c_type; g.epi.ldc = ldc;
     g.epi.residual = residual; g.epi.ldr = ldc; g.epi.col_scale = scale; g.epi.scale_cols = scale_cols;
-    sfgemm(q, g);
+    q->gemm.run(g, q->gemm_backend == WLK_BACKEND_TCGEN05, q->st, q->num_sms);
 }
 
 void expect(const std::string& name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
@@ -941,11 +921,10 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     WLK_CHECK(D.n_spk >= 1 && D.n_spk <= 8, "n_spk must be in [1, 8]");
     WLK_CHECK(D.spkcache_len >= D.n_spk * (1 + D.spkcache_sil_frames_per_spk), "speaker cache too short for n_spk");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    const int num_sms = open_sm90_device(cfg->device);
 
     auto* q = new wlk_sf();
-    q->dims = D; q->cfg = *cfg;
-    q->num_sms = num_sms;
+    q->open(*cfg);
+    q->dims = D;
     q->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
     q->gemm_backend = q->act == DT_BF16 && cfg->gemm_backend != WLK_BACKEND_SIMT ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT;
     q->n_freq = D.n_fft / 2 + 1;
@@ -964,7 +943,6 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
         int mp = D.spkcache_update_period > mc ? D.spkcache_update_period : mc;
         if (mp > mc + D.fifo_len) mp = mc + D.fifo_len;
         q->max_pop = mp; }
-    CUDA_CHECK(cudaStreamCreateWithFlags(&q->st, cudaStreamNonBlocking));
     const size_t es = q->es();
     const int C = D.conv_channels, d = D.d_model, t = D.tf_d_model, ff = D.ff_mult * d, K = D.conv_kernel, S = D.n_spk;
     size_t* aw = &q->bytes_weights;
@@ -1028,14 +1006,9 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
     q->preds = (float*)q->allocs.take(R * S * 4, ws);
     q->out_preds = (float*)q->allocs.take(B * q->max_chunk_cap * S * 4, ws);
     CUDA_CHECK(cudaMallocHost(&q->out_h, B * q->max_chunk_cap * S * 4));
-    if (q->gemm_backend == WLK_BACKEND_TCGEN05) {
-        q->sk_scratch = (float*)q->allocs.take(SK_SCRATCH_FLOATS * 4, ws);
-        q->sk_counters = (int*)q->allocs.take(SK_MAX_TILES * 4, ws);
-    }
-    q->stg_bytes = B * sizeof(SfJob) + 4096;
-    CUDA_CHECK(cudaMallocHost(&q->stg_h, q->stg_bytes));
-    q->stg_d = (uint8_t*)q->allocs.take(q->stg_bytes, ws);
-    q->sess.resize(cfg->max_sessions);
+    if (q->gemm_backend == WLK_BACKEND_TCGEN05) q->gemm.alloc(q->allocs, ws);
+    q->stg.alloc(B * sizeof(SfJob) + 4096, q->allocs, ws);
+    q->sess.slots.resize(cfg->max_sessions);
     *out = q;
 }
 
@@ -1050,19 +1023,11 @@ void free_session(SfSession& s) {
 }
 
 void destroy(wlk_sf* q) {
-    cudaStreamSynchronize(q->st);
-    for (auto& s : q->sess) free_session(s);
-    q->allocs.free_all();
-    q->upload.release();
-    if (q->stg_h) cudaFreeHost(q->stg_h);
-    if (q->out_h) cudaFreeHost(q->out_h);
-    cudaStreamDestroy(q->st);
+    q->close([q] {
+        for (auto& s : q->sess) free_session(s);
+        if (q->out_h) cudaFreeHost(q->out_h);
+    });
     delete q;
-}
-
-SfSession& session(wlk_sf* q, int32_t sid) {
-    WLK_CHECK(sid >= 0 && sid < (int)q->sess.size() && q->sess[sid].open, "invalid session id %d", sid);
-    return q->sess[sid];
 }
 
 void reset_session(wlk_sf* q, SfSession& s) {         // _init_streaming_state (sortformer_backend.py:212-234)
@@ -1156,11 +1121,10 @@ void step(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const in
     const int S = D.n_spk, d = D.d_model;
     // ---- pass 1: validate and plan without touching any session
     std::vector<SfJob> jobs(n);
-    std::set<int32_t> seen;
     int feat_rows = 0, r1 = 0, r2 = 0, r3 = 0, R = 0, out_off = 0;
+    q->sess.check_batch(sids, n);
     for (int i = 0; i < n; ++i) {
-        SfSession& s = session(q, sids[i]);
-        WLK_CHECK(seen.insert(sids[i]).second, "session %d appears twice in the batch", sids[i]);
+        SfSession& s = q->sess[sids[i]];
         SfJob& j = jobs[i];
         memset(&j, 0, sizeof(j));
         int n_feat;
@@ -1205,7 +1169,7 @@ void step(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const in
     }
     // ---- total_preds room (trim like sortformer_backend.py:301-305, before the step's rows are appended)
     for (int i = 0; i < n; ++i) {
-        SfSession& s = session(q, sids[i]);
+        SfSession& s = q->sess[sids[i]];
         if (s.tp_rows + jobs[i].max_chunk > SF_TP_CAP) {
             CUDA_CHECK(cudaMemcpyAsync(s.total_preds, s.total_preds + (size_t)(s.tp_rows - SF_TP_KEEP) * S, (size_t)SF_TP_KEEP * S * 4,
                                        cudaMemcpyDeviceToDevice, q->st));
@@ -1213,9 +1177,10 @@ void step(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const in
         }
         jobs[i].total_preds = s.total_preds + (size_t)s.tp_rows * S;
     }
-    memcpy(q->stg_h, jobs.data(), sizeof(SfJob) * n);
-    CUDA_CHECK(cudaMemcpyAsync(q->stg_d, q->stg_h, sizeof(SfJob) * n, cudaMemcpyHostToDevice, q->st));
-    const SfJob* jd = reinterpret_cast<const SfJob*>(q->stg_d);
+    Stager sg(q->stg);
+    SfJob* jd;
+    memcpy(sg.host<SfJob>(n, &jd), jobs.data(), sizeof(SfJob) * n);
+    sg.upload(q->st);
     if (pcm_host) {
         for (int i = 0; i < n; ++i)
             CUDA_CHECK(cudaMemcpyAsync(q->pcm + (size_t)i * q->chunk_samples, pcm_host + sample_off[i], (size_t)q->chunk_samples * 4,
@@ -1253,7 +1218,7 @@ void step(wlk_sf* q, const int32_t* sids, int n, const float* pcm_host, const in
     // ---- commit (the device work of the step has succeeded)
     int o = 0;
     for (int i = 0; i < n; ++i) {
-        SfSession& s = session(q, sids[i]);
+        SfSession& s = q->sess[sids[i]];
         const SfJob& j = jobs[i];
         s.flip ^= 1;
         s.sl = std::min(j.sl + j.pop, D.spkcache_len);
@@ -1302,34 +1267,30 @@ int wlk_sf_session_open(wlk_sf* q, int32_t* sid) {
     WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(sid != nullptr, "null argument");
     const wlk_sf_dims& D = q->dims;
-    for (size_t i = 0; i < q->sess.size(); ++i) {
-        SfSession& s = q->sess[i];
-        if (s.open) continue;
-        size_t* acct = &q->bytes_sessions;
-        auto al = [&](size_t bytes) { void* p = nullptr; CUDA_CHECK(cudaMalloc(&p, bytes)); *acct += bytes; return p; };
-        for (int k = 0; k < 2; ++k) {
-            s.cache[k] = (float*)al((size_t)D.spkcache_len * D.d_model * 4);
-            s.fifo[k] = (float*)al((size_t)D.fifo_len * D.d_model * 4);
-            s.cache_preds[k] = (float*)al((size_t)D.spkcache_len * D.n_spk * 4);
-        }
-        s.fifo_preds = (float*)al((size_t)D.fifo_len * D.n_spk * 4);
-        s.mean_sil = (float*)al((size_t)D.d_model * 4);
-        s.prev_mel = (float*)al((size_t)q->frames_per_chunk * D.n_mels * 4);
-        s.total_preds = (float*)al((size_t)SF_TP_CAP * D.n_spk * 4);
-        s.n_sil = (int32_t*)al(16);
-        s.open = true;
-        reset_session(q, s);
-        CUDA_CHECK(cudaStreamSynchronize(q->st));
-        *sid = (int32_t)i;
-        return 0;
+    const int found = q->sess.free_slot();
+    SfSession& s = q->sess[found];
+    size_t* acct = &q->bytes_sessions;
+    auto al = [&](size_t bytes) { void* p = nullptr; CUDA_CHECK(cudaMalloc(&p, bytes)); *acct += bytes; return p; };
+    for (int k = 0; k < 2; ++k) {
+        s.cache[k] = (float*)al((size_t)D.spkcache_len * D.d_model * 4);
+        s.fifo[k] = (float*)al((size_t)D.fifo_len * D.d_model * 4);
+        s.cache_preds[k] = (float*)al((size_t)D.spkcache_len * D.n_spk * 4);
     }
-    WLK_CHECK(false, "all %zu sessions in use", q->sess.size());
+    s.fifo_preds = (float*)al((size_t)D.fifo_len * D.n_spk * 4);
+    s.mean_sil = (float*)al((size_t)D.d_model * 4);
+    s.prev_mel = (float*)al((size_t)q->frames_per_chunk * D.n_mels * 4);
+    s.total_preds = (float*)al((size_t)SF_TP_CAP * D.n_spk * 4);
+    s.n_sil = (int32_t*)al(16);
+    s.open = true;
+    reset_session(q, s);
+    CUDA_CHECK(cudaStreamSynchronize(q->st));
+    *sid = found;
     WLK_API_END
 }
 int wlk_sf_session_close(wlk_sf* q, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    SfSession& s = session(q, sid);
+    SfSession& s = q->sess.at(sid);
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     free_session(s);
     WLK_API_END
@@ -1337,7 +1298,7 @@ int wlk_sf_session_close(wlk_sf* q, int32_t sid) {
 int wlk_sf_session_reset(wlk_sf* q, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    reset_session(q, session(q, sid));
+    reset_session(q, q->sess.at(sid));
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     WLK_API_END
 }
@@ -1361,7 +1322,7 @@ int wlk_sf_step_features(wlk_sf* q, const int32_t* sids, int n, const float* fea
 int wlk_sf_total_preds(wlk_sf* q, int32_t sid, const float** preds_dev, int32_t* n_rows) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    SfSession& s = session(q, sid);
+    SfSession& s = q->sess.at(sid);
     if (preds_dev) *preds_dev = s.total_preds;
     if (n_rows) *n_rows = s.tp_rows;
     WLK_API_END
@@ -1370,7 +1331,7 @@ int wlk_sf_read_state(wlk_sf* q, int32_t sid, int32_t* lengths /*[4]: spkcache, 
                       float* spkcache_preds_host, float* fifo_host, float* mean_sil_host) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    SfSession& s = session(q, sid);
+    SfSession& s = q->sess.at(sid);
     const wlk_sf_dims& D = q->dims;
     CUDA_CHECK(cudaStreamSynchronize(q->st));
     if (lengths) {
@@ -1387,9 +1348,7 @@ int wlk_sf_read_state(wlk_sf* q, int32_t sid, int32_t* lengths /*[4]: spkcache, 
 int wlk_sf_memory(wlk_sf* q, size_t* weights, size_t* sessions, size_t* workspace) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    if (weights) *weights = q->bytes_weights;
-    if (sessions) *sessions = q->bytes_sessions;
-    if (workspace) *workspace = q->bytes_workspace;
+    q->memory(weights, sessions, workspace);
     WLK_API_END
 }
 
