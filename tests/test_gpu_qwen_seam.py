@@ -103,7 +103,7 @@ def test_engine_call_equals_driver_loop(precision, controls, device_rows):
 
 def _raw_call(eng, sids, srcs, dl, prefix, tail, max_new, rows=None):
     import ctypes as C
-    from whisperlivekit_b200.qwen_text_engine import _ptr
+    from whisperlivekit_b200._lib import _ptr
     ids = np.asarray(sids, np.int32)
     flat = np.concatenate(srcs).astype(np.int32) if srcs else np.zeros(1, np.int32)
     off = np.zeros(len(srcs) + 1, np.int32)

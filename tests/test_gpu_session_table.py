@@ -1,6 +1,7 @@
 """GPU: the session table every engine shares -- a full table refuses another session, a batch that names a session
 twice or a closed session is refused, and every refusal leaves the open sessions working.  Each engine at its smallest
-geometry with max_sessions=2, through the batch entry point it exposes (a Whisper session gets its audio on open)."""
+geometry with max_sessions=2, through the batch entry point it exposes (a Whisper session gets its audio on open).
+And the handle every wrapper shares: once the engine is closed, no call reaches the destroyed engine."""
 import numpy as np
 import pytest
 
@@ -41,6 +42,13 @@ def _sortformer():
     return eng, lambda sids: eng.step_audio(sids, [np.zeros(16000, np.float32)] * len(sids)), None
 
 
+def _vad():
+    from oracle.vad_oracle import synthetic_vad_state_dict
+    from whisperlivekit_b200.vad import VadEngine
+    eng = VadEngine(synthetic_vad_state_dict(seed=9), max_sessions=2)
+    return eng, lambda sids: eng.forward(sids, [np.zeros(512, np.float32)] * len(sids)), None
+
+
 @pytest.mark.parametrize("make", [_whisper, _tower, _text, _sortformer], ids=["whisper", "tower", "text", "sortformer"])
 def test_session_table_refusals(make):
     from whisperlivekit_b200._lib import WlkError
@@ -68,3 +76,23 @@ def test_session_table_refusals(make):
         call([b, a])
     finally:
         eng.close()
+
+
+@pytest.mark.parametrize("make", [_whisper, _tower, _text, _sortformer, _vad],
+                         ids=["whisper", "tower", "text", "sortformer", "vad"])
+def test_closed_engine(make):
+    """A session handle may be collected after its engine (in the same garbage cycle): closing the session then does
+    nothing, a second close() does nothing, and any other call is refused as a null handle instead of reaching the
+    destroyed engine."""
+    from whisperlivekit_b200._lib import WlkError
+    eng, call, prepare = make()
+    sid = eng.open_session()
+    if prepare:
+        prepare(sid)
+    call([sid])
+    eng.close()
+    assert eng.h is None
+    eng.close_session(sid)
+    eng.close()
+    with pytest.raises(WlkError, match="null engine"):
+        call([sid])

@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "csrc", "libwlk_b200.so")
 
@@ -53,6 +55,8 @@ class wlk_config(C.Structure):
 
 PREC_FP32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
 BACKEND_AUTO, BACKEND_SIMT, BACKEND_TCGEN05 = 0, 1, 2
+PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "bf16x3": PREC_BF16X3}
+BACKENDS = {"auto": BACKEND_AUTO, "simt": BACKEND_SIMT, "tcgen05": BACKEND_TCGEN05}
 KERNEL_CLASSES = ["mel", "gemm_enc", "attn_enc", "layernorm", "gemm_xkv", "gemm_dec",
                   "attn_dec_self", "attn_dec_cross", "logits", "align", "misc"]
 
@@ -217,3 +221,105 @@ def load():
 def check(rc: int):
     if rc != 0:
         raise WlkError(load().wlk_last_error().decode("utf-8", "replace"))
+
+
+def _ptr(a: np.ndarray):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def pack(parts, dtype, shape=(), offs_dtype=np.int32):
+    """Per-stream arrays -> (their rows [*shape] of ``dtype`` back to back, offsets [n + 1] of ``offs_dtype``): stream i
+    is flat[offs[i]: offs[i + 1]].  Without any row, flat is one zero row, so the engine is never handed a null pointer."""
+    parts = [np.ascontiguousarray(p, dtype).reshape(-1, *shape) for p in parts]
+    offs = np.zeros(len(parts) + 1, offs_dtype)
+    offs[1:] = np.cumsum([p.shape[0] for p in parts])
+    flat = np.concatenate(parts) if offs[-1] else np.zeros((1, *shape), dtype)
+    return flat, offs
+
+
+def split(out: np.ndarray, offs):
+    """Per-stream copies of the rows of ``out``: stream i owns rows offs[i] .. offs[i + 1]."""
+    return [out[offs[i]: offs[i + 1]].copy() for i in range(len(offs) - 1)]
+
+
+class Engine:
+    """One engine handle of the library: create, weights, memory, sessions and one destroy.
+
+    A subclass names its entry points as the class data below, each ``wlk_*`` name in full; where the library has no
+    such entry point, the subclass sets the method that would call it to None.  ``close`` destroys the
+    handle once and sets ``h`` to None: a later call reaches the library as a null handle, which every entry point
+    refuses ("null engine"), instead of a pointer into the freed engine."""
+
+    CREATE = DESTROY = LOAD_TENSOR = FINALIZE = MEMORY = SESSION_OPEN = SESSION_CLOSE = SESSION_RESET = None
+    precisions = ("fp32", "bf16")                         # the precision names the engine takes
+    h = None
+
+    def _create_handle(self, device: int, *args) -> None:
+        """h = CREATE(*args, &h) for an engine on ``device``."""
+        self.lib = load()
+        self.device = int(device)
+        h = C.c_void_p()
+        check(getattr(self.lib, self.CREATE)(*args, C.byref(h)))
+        self.h = h
+
+    def _create(self, cdims, *, precision: str, device: int, max_sessions: int, max_batch: int, gemm_backend: str = "auto",
+                attn_backend: str = "simt", max_align_heads: int = 0) -> None:
+        """CREATE(&cdims, &config) with the config built from the precision and backend names."""
+        if precision not in self.precisions:
+            raise KeyError(precision)
+        cfg = wlk_config(device=device, precision=PRECISIONS[precision], max_sessions=max_sessions, max_batch=max_batch,
+                         gemm_backend=BACKENDS[gemm_backend], attn_backend=BACKENDS[attn_backend],
+                         max_align_heads=max_align_heads, reserved=0)
+        self.precision = precision
+        self.max_batch = int(max_batch)
+        self._create_handle(device, C.byref(cdims), C.byref(cfg))
+
+    def close(self) -> None:
+        h, self.h = self.h, None
+        if h is not None:
+            check(getattr(self.lib, self.DESTROY)(h))
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    # -- weights ------------------------------------------------------------------------------------------------------
+    def load_tensor(self, name: str, arr) -> None:
+        a = np.ascontiguousarray(arr, np.float32)
+        shape = (C.c_int64 * a.ndim)(*a.shape)
+        check(getattr(self.lib, self.LOAD_TENSOR)(self.h, name.encode(), _ptr(a), shape, a.ndim))
+
+    def finalize(self) -> None:
+        check(getattr(self.lib, self.FINALIZE)(self.h))
+
+    @staticmethod
+    def _skip(name: str, arr) -> bool:
+        """Whether load_state_dict leaves this checkpoint entry out."""
+        return False
+
+    def load_state_dict(self, sd) -> None:
+        for name, arr in sd.items():
+            if not self._skip(name, arr):
+                self.load_tensor(name, arr)
+        self.finalize()
+
+    def memory(self) -> dict:
+        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
+        check(getattr(self.lib, self.MEMORY)(self.h, C.byref(w), C.byref(s), C.byref(k)))
+        return dict(weights=w.value, sessions=s.value, workspace=k.value)
+
+    # -- sessions -----------------------------------------------------------------------------------------------------
+    def open_session(self) -> int:
+        sid = C.c_int32()
+        check(getattr(self.lib, self.SESSION_OPEN)(self.h, C.byref(sid)))
+        return sid.value
+
+    def close_session(self, sid: int) -> None:
+        if self.h is None:          # destroyed first (a session handle collected in the same garbage cycle): its
+            return                  # sessions went with it
+        check(getattr(self.lib, self.SESSION_CLOSE)(self.h, int(sid)))
+
+    def reset_session(self, sid: int) -> None:
+        check(getattr(self.lib, self.SESSION_RESET)(self.h, int(sid)))

@@ -15,6 +15,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib as L
+from ._lib import _ptr, pack
 from .dims import ModelDimensions, SpecialTokens, default_alignment_heads
 from .weights import hann_window, mel_filterbank
 
@@ -23,35 +24,25 @@ def _i32(a) -> np.ndarray:
     return np.ascontiguousarray(np.asarray(a, dtype=np.int32))
 
 
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-class WhisperEngine:
+class WhisperEngine(L.Engine):
     backend = "b200-cuda"
+    CREATE, DESTROY = "wlk_engine_create", "wlk_engine_destroy"
+    LOAD_TENSOR, FINALIZE, MEMORY = "wlk_engine_load_tensor", "wlk_engine_finalize_weights", "wlk_engine_memory"
+    SESSION_OPEN, SESSION_CLOSE = "wlk_session_open", "wlk_session_close"
+    precisions = ("fp32", "bf16", "bf16x3")
+    reset_session = None            # no whole-session reset: reset_decoder / reset_incremental reset its parts
 
     def __init__(self, dims: ModelDimensions, state_dict: Optional[Dict[str, np.ndarray]] = None,
                  align_heads: Optional[Sequence[Tuple[int, int]]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8,
                  gemm_backend: str = "auto", attn_backend: str = "auto"):
-        self.lib = L.load()
         self.dims = dims
         self.specials = SpecialTokens.for_dims(dims)
-        self.precision = precision
-        self.device = int(device)
         heads = list(align_heads) if align_heads is not None else default_alignment_heads(dims)
         self.align_heads = [tuple(int(v) for v in h) for h in heads]
-        be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
-        cdims = L.wlk_dims(*dims.as_tuple())
-        cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16, "bf16x3": L.PREC_BF16X3}[precision],
-                           max_sessions=max_sessions, max_batch=max_batch,
-                           gemm_backend=be[gemm_backend], attn_backend=be[attn_backend],
-                           max_align_heads=max(len(self.align_heads), 1), reserved=0)
-        self.max_batch = max_batch
-        h = C.c_void_p()
-        L.check(self.lib.wlk_engine_create(C.byref(cdims), C.byref(cfg), C.byref(h)))
-        self.h = h
-        self._closed = False
+        self._create(L.wlk_dims(*dims.as_tuple()), precision=precision, device=device, max_sessions=max_sessions,
+                     max_batch=max_batch, gemm_backend=gemm_backend, attn_backend=attn_backend,
+                     max_align_heads=max(len(self.align_heads), 1))
         self.load_tensor("mel_filters", mel_filterbank(dims.n_mels))
         self.load_tensor("hann_window", hann_window())
         pairs = _i32(self.align_heads).reshape(-1)
@@ -61,17 +52,9 @@ class WhisperEngine:
             self.load_state_dict(state_dict)
 
     # -- weights -----------------------------------------------------------------
-    def load_tensor(self, name: str, arr) -> None:
-        a = np.ascontiguousarray(np.asarray(arr, dtype=np.float32))
-        shape = (C.c_int64 * a.ndim)(*a.shape)
-        L.check(self.lib.wlk_engine_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
-
-    def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
-        for k, v in sd.items():
-            if k.endswith("alignment_heads") or k.endswith(".mask"):
-                continue
-            self.load_tensor(k, v)
-        L.check(self.lib.wlk_engine_finalize_weights(self.h))
+    @staticmethod
+    def _skip(name: str, arr) -> bool:
+        return name.endswith(("alignment_heads", ".mask"))
 
     def weight_blob(self) -> Tuple[int, int]:
         """(device pointer, nbytes) of the packed weights -- broadcast target for NCCL at init."""
@@ -82,11 +65,6 @@ class WhisperEngine:
     def adopt_weights(self) -> None:
         L.check(self.lib.wlk_engine_adopt_weights(self.h))
 
-    def memory(self) -> Dict[str, int]:
-        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        L.check(self.lib.wlk_engine_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
-        return dict(weights=w.value, sessions=s.value, workspace=k.value)
-
     def stream(self) -> int:
         p = C.c_void_p()
         L.check(self.lib.wlk_engine_stream(self.h, C.byref(p)))
@@ -96,14 +74,6 @@ class WhisperEngine:
         L.check(self.lib.wlk_engine_sync(self.h))
 
     # -- sessions ------------------------------------------------------------------
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_session_open(self.h, C.byref(sid)))
-        return int(sid.value)
-
-    def close_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_session_close(self.h, sid))
-
     def append_audio(self, sid: int, pcm) -> None:
         a = np.ascontiguousarray(np.asarray(pcm, dtype=np.float32).reshape(-1))
         L.check(self.lib.wlk_session_append_audio(self.h, sid, _ptr(a), a.shape[0]))
@@ -163,9 +133,9 @@ class WhisperEngine:
 
     def decode(self, sids: Sequence[int], tokens: Sequence[Sequence[int]], sot_index: int = 0) -> None:
         s = _i32(sids)
-        offs = np.zeros(len(s) + 1, np.int32)
-        offs[1:] = np.cumsum([len(t) for t in tokens])
-        flat = _i32([t for ts in tokens for t in ts])
+        if len(tokens) != len(s):
+            raise ValueError("sids and tokens differ in length")
+        flat, offs = pack(tokens, np.int32)
         L.check(self.lib.wlk_decode(self.h, _ptr(s), len(s), _ptr(flat), _ptr(offs), int(sot_index)))
 
     # -- LocalAgreement path ---------------------------------------------------------
@@ -324,15 +294,3 @@ class WhisperEngine:
         xd = torch.from_numpy(x).to(f"cuda:{self.device}")
         torch.cuda.synchronize()
         return self.op_dtw(xd.data_ptr(), x.shape[0], x.shape[1])
-
-    # -- lifetime ------------------------------------------------------------------------
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_engine_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

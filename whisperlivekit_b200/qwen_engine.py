@@ -12,75 +12,34 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib as L
+from ._lib import _ptr, pack, split
 from .qwen_dims import sinusoid_inv_freq
 
 
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+class _QwenEngineBase(L.Engine):
+    """What both tower engines share: one ``wlk_qwen`` handle, its weights, sessions and memory."""
 
-
-class _QwenEngineBase:
-    """The ctypes plumbing both tower engines share: one ``wlk_qwen`` handle, its weights, sessions and memory."""
+    DESTROY = "wlk_qwen_destroy"
+    LOAD_TENSOR, FINALIZE, MEMORY = "wlk_qwen_load_tensor", "wlk_qwen_finalize_weights", "wlk_qwen_memory"
+    SESSION_OPEN, SESSION_CLOSE, SESSION_RESET = "wlk_qwen_session_open", "wlk_qwen_session_close", "wlk_qwen_session_reset"
 
     def __init__(self, dims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8, gemm_backend: str = "auto"):
-        self.lib = L.load()
         self.dims = dims
-        self.precision = precision
-        self.device = int(device)
-        self.max_batch = int(max_batch)
-        be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
-        cdims = self._DIMS(*dims.as_tuple())
-        cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
-                           max_sessions=max_sessions, max_batch=max_batch, gemm_backend=be[gemm_backend],
-                           attn_backend=L.BACKEND_SIMT, max_align_heads=0, reserved=0)
-        h = C.c_void_p()
-        L.check(getattr(self.lib, self._CREATE)(C.byref(cdims), C.byref(cfg), C.byref(h)))
-        self.h = h
-        self._closed = False
+        self._create(self._DIMS(*dims.as_tuple()), precision=precision, device=device, max_sessions=max_sessions,
+                     max_batch=max_batch, gemm_backend=gemm_backend)
         # the reference's fp32 frequencies of the positional rows past the table, evaluated on this device like the
         # reference evaluates them on its own
         self.load_tensor("positional_embedding.inv_freq", sinusoid_inv_freq(dims.d_model, f"cuda:{self.device}"))
         if state_dict is not None:
             self.load_state_dict(state_dict)
 
-    def load_tensor(self, name: str, arr) -> None:
-        a = np.ascontiguousarray(arr, np.float32)
-        shape = (C.c_int64 * a.ndim)(*a.shape)
-        L.check(self.lib.wlk_qwen_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
-
-    def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
-        for name, arr in sd.items():
-            self.load_tensor(name, arr)
-        L.check(self.lib.wlk_qwen_finalize_weights(self.h))
-
-    def memory(self) -> Dict[str, int]:
-        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        L.check(self.lib.wlk_qwen_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
-        return dict(weights=w.value, sessions=s.value, workspace=k.value)
-
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_qwen_session_open(self.h, C.byref(sid)))
-        return sid.value
-
-    def close_session(self, sid: int) -> None:
-        if self._closed:            # destroyed first (a session handle collected in the same garbage cycle): its
-            return                  # sessions went with it, and the handle must not be touched
-        L.check(self.lib.wlk_qwen_session_close(self.h, sid))
-
-    def reset_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_qwen_session_reset(self.h, sid))
-
     def _pack(self, sids, mels):
         """(session ids, the mels [frames, n_mels] of every session back to back, frame offsets [n + 1])"""
         n = len(sids)
         if n != len(mels):
             raise ValueError("sids and mels differ in length")
-        parts = [np.ascontiguousarray(m, np.float32).reshape(-1, self.dims.n_mels) for m in mels]
-        offs = np.zeros(n + 1, np.int32)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts, axis=0) if offs[-1] else np.zeros((1, self.dims.n_mels), np.float32)
+        flat, offs = pack(mels, np.float32, (self.dims.n_mels,))
         return np.asarray(list(sids), np.int32), flat, offs
 
     def _device_out(self, cap: int):
@@ -127,22 +86,11 @@ class _QwenEngineBase:
         kv = (C.c_void_p * max(len(kv_ptrs), 1))(*[int(p) for p in kv_ptrs])
         L.check(self.lib.wlk_qwen_op_attention(self.h, int(layer), q_ptr, _ptr(st), _ptr(ns), len(st), kv, out_ptr))
 
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_qwen_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class QwenTowerEngine(_QwenEngineBase):
     """The causal tower (wlk_qwen_create) over a QwenTowerDims geometry."""
 
-    _DIMS, _CREATE = L.wlk_qwen_dims, "wlk_qwen_create"
+    _DIMS, CREATE = L.wlk_qwen_dims, "wlk_qwen_create"
 
     # -- sessions (QwenAudioCausalKVState, causal.py:44-57) ------------------------------------
     def _state(self, sid: int):
@@ -189,7 +137,7 @@ class QwenTowerEngine(_QwenEngineBase):
         out = np.zeros((max(cap, 1), self.dims.out_dim), np.float32)
         rows = np.zeros(len(ids) + 1, np.int32)
         L.check(self.lib.wlk_qwen_forward_chunk(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(len(ids))]
+        return split(out, rows)
 
     def forward_chunk_device(self, sids: Sequence[int], mels: Sequence[np.ndarray]):
         """forward_chunk with the rows left on the device: (fp32 CUDA tensor [rows, out_dim], row offsets [n + 1])."""
@@ -203,23 +151,17 @@ class QwenTowerEngine(_QwenEngineBase):
     # -- incremental log-mel front end (StreamingMelExtractor, features.py:32-112) on the device -------------
     def load_mel_filters(self, filters: Optional[np.ndarray] = None) -> None:
         from .weights import mel_filterbank
-        a = np.ascontiguousarray(mel_filterbank(self.dims.n_mels) if filters is None else filters, np.float32)
-        shape = (C.c_int64 * 2)(*a.shape)
-        L.check(self.lib.wlk_qwen_load_tensor(self.h, b"mel_filters", _ptr(a), shape, 2))
+        self.load_tensor("mel_filters", mel_filterbank(self.dims.n_mels) if filters is None else filters)
 
     def _mel_call(self, sids, audios, flush: bool) -> List[np.ndarray]:
         n = len(sids)
-        D = self.dims
-        parts = [np.ascontiguousarray(a, np.float32).reshape(-1) for a in audios] if not flush else [np.zeros(0, np.float32)] * n
-        offs = np.zeros(n + 1, np.int64)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts) if offs[-1] else np.zeros(1, np.float32)
-        cap = int(offs[-1] // 160 + 4 * n + 8) if not flush else 4 * n + 8
-        out = np.zeros((cap, D.n_mels), np.float32)
+        flat, offs = pack([()] * n if flush else audios, np.float32, offs_dtype=np.int64)
+        cap = int(offs[-1] // 160 + 4 * n + 8)
+        out = np.zeros((cap, self.dims.n_mels), np.float32)
         rows = np.zeros(n + 1, np.int32)
         ids = np.asarray(list(sids), np.int32)
         L.check(self.lib.wlk_qwen_append_audio(self.h, _ptr(ids), n, _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows), int(flush)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+        return split(out, rows)
 
     def mel_append(self, sids: Sequence[int], audios: Sequence[np.ndarray]) -> List[np.ndarray]:
         """StreamingMelExtractor.append per session: raw samples in, newly determined mel frames [frames, n_mels] out."""
@@ -238,7 +180,7 @@ class QwenTowerEngine(_QwenEngineBase):
         rows = np.zeros(n + 1, np.int32)
         ids = np.asarray(list(sids), np.int32)
         L.check(self.lib.wlk_qwen_flush_pending(self.h, _ptr(ids), n, _ptr(out), cap, _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+        return split(out, rows)
 
     def flush_pending_device(self, sids: Sequence[int]):
         """flush_pending with the rows left on the device, as forward_chunk_device returns them."""
@@ -257,7 +199,7 @@ class QwenWindowEngine(_QwenEngineBase):
     ``forward_chunk(mels, state)`` becomes ``forward_chunk(sids, mels)`` over per-session device windows, batched over
     sessions; ``forward_full`` becomes ``encode``.  No CPU fallback."""
 
-    _DIMS, _CREATE = L.wlk_qwen_window_dims, "wlk_qwen_window_create"
+    _DIMS, CREATE = L.wlk_qwen_window_dims, "wlk_qwen_window_create"
     STATE_FIELDS = ("frames_seen", "window_start_frame", "emitted_steps", "last_input_frames", "last_recomputed_frames",
                     "last_recomputed_context_frames", "window_frames")
 
@@ -279,7 +221,7 @@ class QwenWindowEngine(_QwenEngineBase):
         rows = np.zeros(len(ids) + 1, np.int32)
         L.check(self.lib.wlk_qwen_window_forward(self.h, _ptr(ids), len(ids), _ptr(flat), _ptr(offs), _ptr(out), cap,
                                                  _ptr(rows), 0))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(len(ids))]
+        return split(out, rows)
 
     def forward_chunk_device(self, sids: Sequence[int], mels: Sequence[np.ndarray]):
         """forward_chunk with the rows left on the device: (fp32 CUDA tensor [rows, out_dim], row offsets [n + 1])."""
@@ -299,7 +241,7 @@ class QwenWindowEngine(_QwenEngineBase):
         out = np.zeros((max(cap, 1), self.dims.out_dim), np.float32)
         rows = np.zeros(n + 1, np.int32)
         L.check(self.lib.wlk_qwen_window_encode(self.h, n, _ptr(flat), _ptr(offs), _ptr(out), cap, _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+        return split(out, rows)
 
 
 def window_attention(qkv, stream_rows: Sequence[int], block_rows: int, device: int = 0, out=None):

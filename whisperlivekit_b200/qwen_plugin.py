@@ -16,6 +16,7 @@ from typing import Optional
 
 import numpy as np
 
+from ._lib import pack
 from .qwen_dims import QwenTowerDims
 
 
@@ -46,9 +47,8 @@ def _check_mels(mels, n_mels: int):
 def _host_rows(hs, out_dim: int):
     """Per-stream host rows -> (CPU tensor [total, out_dim], row offsets [N + 1])."""
     import torch
-    offs = np.zeros(len(hs) + 1, np.int64)
-    offs[1:] = np.cumsum([h.shape[0] for h in hs])
-    return torch.from_numpy(np.ascontiguousarray(np.concatenate(hs) if hs else np.zeros((0, out_dim), np.float32))), offs
+    flat, offs = pack(hs, np.float32, (out_dim,), np.int64)
+    return torch.from_numpy(flat[:offs[-1]]), offs
 
 
 @dataclass

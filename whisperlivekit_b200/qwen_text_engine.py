@@ -27,11 +27,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib as L
+from ._lib import _ptr
 from .qwen_dims import QwenTextDims, rope_inv_freq
-
-
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _frame_rows(x):
@@ -355,64 +352,27 @@ class TextDecodeDriver:
                 self.reset_session(sid)
 
 
-class QwenTextEngine(TextDecodeDriver):
+class QwenTextEngine(TextDecodeDriver, L.Engine):
     """The text decoder on the H100.  No CPU fallback: construction fails without the CUDA library or a device.
     Embedding rows may be host arrays or fp32 CUDA tensors; the latter are read in place by the forward."""
 
     device_rows = True
+    CREATE, DESTROY = "wlk_qtext_create", "wlk_qtext_destroy"
+    LOAD_TENSOR, FINALIZE, MEMORY = "wlk_qtext_load_tensor", "wlk_qtext_finalize_weights", "wlk_qtext_memory"
+    SESSION_OPEN, SESSION_CLOSE, SESSION_RESET = "wlk_qtext_session_open", "wlk_qtext_session_close", "wlk_qtext_session_reset"
 
     def __init__(self, dims: QwenTextDims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8):
-        self.lib = L.load()
         self.dims = dims
         self.vocab = dims.vocab
-        self.precision = precision
-        self.max_batch = max_batch
-        cdims = L.wlk_qtext_dims(*dims.as_tuple())
-        cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
-                           max_sessions=max_sessions, max_batch=max_batch, gemm_backend=L.BACKEND_AUTO,
-                           attn_backend=L.BACKEND_SIMT, max_align_heads=0, reserved=0)
-        h = C.c_void_p()
-        L.check(self.lib.wlk_qtext_create(C.byref(cdims), C.byref(cfg), C.byref(h)))
-        self.h = h
-        self._closed = False
+        self._create(L.wlk_qtext_dims(*dims.as_tuple()), precision=precision, device=device, max_sessions=max_sessions,
+                     max_batch=max_batch)
         self._n_logit = 0
         self._dev_rows = None                    # device rows the last forward reads: alive until its pick synchronizes
         # HF's fp32 RoPE frequencies; a state dict that carries the model's own buffer overrides them
         self.load_tensor("rotary_emb.inv_freq", rope_inv_freq(dims.rope_theta, dims.head_dim))
         if state_dict is not None:
             self.load_state_dict(state_dict)
-
-    def load_tensor(self, name: str, arr) -> None:
-        a = np.ascontiguousarray(arr, np.float32)
-        shape = (C.c_int64 * a.ndim)(*a.shape)
-        L.check(self.lib.wlk_qtext_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
-
-    def finalize(self) -> None:
-        L.check(self.lib.wlk_qtext_finalize_weights(self.h))
-
-    def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
-        for name, arr in sd.items():
-            self.load_tensor(name, arr)
-        self.finalize()
-
-    def memory(self) -> Dict[str, int]:
-        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        L.check(self.lib.wlk_qtext_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
-        return dict(weights=w.value, sessions=s.value, workspace=k.value)
-
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_qtext_session_open(self.h, C.byref(sid)))
-        return sid.value
-
-    def close_session(self, sid: int) -> None:
-        if self._closed:            # destroyed first (a session handle collected in the same garbage cycle): its
-            return                  # sessions went with it, and the handle must not be touched
-        L.check(self.lib.wlk_qtext_session_close(self.h, int(sid)))
-
-    def reset_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_qtext_session_reset(self.h, int(sid)))
 
     def session_len(self, sid: int) -> int:
         n = C.c_int32()
@@ -662,14 +622,3 @@ class QwenTextEngine(TextDecodeDriver):
 
     def op_swiglu(self, gu_ptr, hid_ptr, rows: int) -> None:
         L.check(self.lib.wlk_qtext_op_swiglu(self.h, gu_ptr, hid_ptr, int(rows)))
-
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_qtext_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -19,13 +19,10 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib as L
+from ._lib import _ptr, pack, split
 from .diarization import DiarizationSegmenter, SpeakerSegment, resolve_max_speakers
 from .sortformer_dims import SortformerDims
 from .weights import mel_filterbank
-
-
-def _ptr(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 _INT_FIELDS = ("n_mels", "n_fft", "win_length", "hop", "conv_channels", "d_model", "n_head", "n_layer", "ff_mult", "conv_kernel",
@@ -35,85 +32,54 @@ _FLOAT_FIELDS = ("pred_score_threshold", "scores_boost_latest", "sil_threshold",
                  "min_pos_scores_rate")
 
 
-class SortformerEngine:
+class SortformerEngine(L.Engine):
+    CREATE, DESTROY = "wlk_sf_create", "wlk_sf_destroy"
+    LOAD_TENSOR, FINALIZE, MEMORY = "wlk_sf_load_tensor", "wlk_sf_finalize_weights", "wlk_sf_memory"
+    SESSION_OPEN, SESSION_CLOSE, SESSION_RESET = "wlk_sf_session_open", "wlk_sf_session_close", "wlk_sf_session_reset"
+
     def __init__(self, dims: SortformerDims, state_dict: Optional[Dict[str, np.ndarray]] = None, *, precision: str = "bf16",
                  device: int = 0, max_sessions: int = 8, max_batch: int = 8, gemm_backend: str = "auto"):
-        self.lib = L.load()
         self.dims = dims
-        self.precision = precision
-        self.device = int(device)
-        self.max_batch = int(max_batch)
-        be = {"auto": L.BACKEND_AUTO, "simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}
         cd = L.wlk_sf_dims(**{k: int(getattr(dims, k)) for k in _INT_FIELDS}, **{k: float(getattr(dims, k)) for k in _FLOAT_FIELDS})
-        cfg = L.wlk_config(device=device, precision={"fp32": L.PREC_FP32, "bf16": L.PREC_BF16}[precision],
-                           max_sessions=max_sessions, max_batch=max_batch, gemm_backend=be[gemm_backend],
-                           attn_backend=L.BACKEND_SIMT, max_align_heads=0, reserved=0)
-        h = C.c_void_p()
-        L.check(self.lib.wlk_sf_create(C.byref(cd), C.byref(cfg), C.byref(h)))
-        self.h = h
-        self._closed = False
+        self._create(cd, precision=precision, device=device, max_sessions=max_sessions, max_batch=max_batch,
+                     gemm_backend=gemm_backend)
         self.chunk_samples = dims.chunk_len * dims.subsampling_factor * dims.hop
         self.chunk_duration_seconds = self.chunk_samples / 16000.0           # sortformer_backend.py:190-194
         if state_dict is not None:
             self.load_state_dict(state_dict)
 
     def load_state_dict(self, sd: Dict[str, np.ndarray]) -> None:
-        d = self.dims
         full = dict(sd)
-        full.setdefault("mel_filters", mel_filterbank(d.n_mels, 16000, d.n_fft))
-        for name, arr in full.items():
-            a = np.ascontiguousarray(arr, np.float32)
-            # a NeMo checkpoint also carries buffers of modules this path replaces or never calls: the preprocessor's window /
-            # filterbank (the front end is rebuilt from the geometry), BatchNorm's counter, the unused hidden_to_spks layer
-            if (a.ndim == 0 or name.startswith(("preprocessor.", "sortformer_modules.hidden_to_spks."))
-                    or name.endswith("num_batches_tracked")):
-                continue
-            shape = (C.c_int64 * a.ndim)(*a.shape)
-            L.check(self.lib.wlk_sf_load_tensor(self.h, name.encode(), _ptr(a), shape, a.ndim))
-        L.check(self.lib.wlk_sf_finalize_weights(self.h))
+        full.setdefault("mel_filters", mel_filterbank(self.dims.n_mels, 16000, self.dims.n_fft))
+        super().load_state_dict(full)
 
-    def memory(self) -> Dict[str, int]:
-        w, s, k = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        L.check(self.lib.wlk_sf_memory(self.h, C.byref(w), C.byref(s), C.byref(k)))
-        return dict(weights=w.value, sessions=s.value, workspace=k.value)
-
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_sf_session_open(self.h, C.byref(sid)))
-        return sid.value
-
-    def close_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_sf_session_close(self.h, sid))
-
-    def reset_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_sf_session_reset(self.h, sid))
+    @staticmethod
+    def _skip(name: str, arr) -> bool:
+        # a NeMo checkpoint also carries buffers of modules this path replaces or never calls: the preprocessor's window /
+        # filterbank (the front end is rebuilt from the geometry), BatchNorm's counter, the unused hidden_to_spks layer
+        return (np.ndim(arr) == 0 or name.startswith(("preprocessor.", "sortformer_modules.hidden_to_spks."))
+                or name.endswith("num_batches_tracked"))
 
     def step_audio(self, sids: Sequence[int], chunks: Sequence[np.ndarray], want_preds: bool = True) -> List[np.ndarray]:
         """diarize()'s device part for n streams: one ``chunk_samples`` chunk each -> chunk_preds [rows, n_spk] each."""
         n = len(sids)
-        parts = [np.ascontiguousarray(c, np.float32).reshape(-1) for c in chunks]
-        offs = np.zeros(n + 1, np.int64)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts)
+        flat, offs = pack(chunks, np.float32, offs_dtype=np.int64)
         ids = np.asarray(list(sids), np.int32)
         rows = np.zeros(n + 1, np.int32)
         out = np.zeros((n * 32, self.dims.n_spk), np.float32)
         L.check(self.lib.wlk_sf_step_audio(self.h, _ptr(ids), n, _ptr(flat), _ptr(offs), _ptr(out) if want_preds else None, _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)] if want_preds else [rows[i + 1] - rows[i] for i in range(n)]
+        return split(out, rows) if want_preds else [rows[i + 1] - rows[i] for i in range(n)]
 
     def step_features(self, sids: Sequence[int], feats: Sequence[np.ndarray], left_offset: int, right_offset: int) -> List[np.ndarray]:
         """forward_streaming_step for n streams: time-major features [frames, n_mels] each."""
         n = len(sids)
-        parts = [np.ascontiguousarray(f, np.float32).reshape(-1, self.dims.n_mels) for f in feats]
-        offs = np.zeros(n + 1, np.int32)
-        offs[1:] = np.cumsum([p.shape[0] for p in parts])
-        flat = np.concatenate(parts, axis=0)
+        flat, offs = pack(feats, np.float32, (self.dims.n_mels,))
         ids = np.asarray(list(sids), np.int32)
         rows = np.zeros(n + 1, np.int32)
         out = np.zeros((n * 32, self.dims.n_spk), np.float32)
         L.check(self.lib.wlk_sf_step_features(self.h, _ptr(ids), n, _ptr(flat), _ptr(offs), int(left_offset), int(right_offset),
                                               _ptr(out), _ptr(rows)))
-        return [out[rows[i]: rows[i + 1]].copy() for i in range(n)]
+        return split(out, rows)
 
     def total_preds(self, sid: int):
         """(device address of the stream's total_preds [rows, n_spk], rows)"""
@@ -131,17 +97,6 @@ class SortformerEngine:
         L.check(self.lib.wlk_sf_read_state(self.h, sid, _ptr(lengths), _ptr(cache), _ptr(cpreds), _ptr(fifo), _ptr(msil)))
         return dict(spkcache_len=int(lengths[0]), fifo_len=int(lengths[1]), n_sil=int(lengths[2]), chunk_index=int(lengths[3]),
                     spkcache=cache, spkcache_preds=cpreds, fifo=fifo, mean_sil_emb=msil)
-
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_sf_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 # ---------------------------------------------------------------------------------------------------------------

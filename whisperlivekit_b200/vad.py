@@ -9,68 +9,42 @@ The weights are the scripted model's own ``state_dict()`` (names kept).  No CPU 
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, List, Sequence
 
 import numpy as np
 
 from . import _lib as L
+from ._lib import _ptr, pack, split
 
 WINDOW = 512
 
 
-class VadEngine:
+class VadEngine(L.Engine):
+    CREATE, DESTROY = "wlk_vad_create", "wlk_vad_destroy"
+    SESSION_OPEN, SESSION_CLOSE, SESSION_RESET = "wlk_vad_session_open", "wlk_vad_session_close", "wlk_vad_session_reset"
+    load_tensor = finalize = load_state_dict = memory = None     # wlk_vad_load_tensor takes element counts: see __init__
+
     def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, max_sessions: int = 64):
-        self.lib = L.load()
-        h = C.c_void_p()
-        L.check(self.lib.wlk_vad_create(int(device), int(max_sessions), C.byref(h)))
-        self.h = h
-        self._closed = False
+        self._create_handle(device, int(device), int(max_sessions))
         for k, v in state_dict.items():
             name = k[7:] if k.startswith("_model.") else k
             if name.startswith("_model_8k") or k.startswith("_model_8k"):
                 continue                                              # the 8 kHz branch of the scripted model is not used at 16 kHz
             a = np.ascontiguousarray(np.asarray(v, np.float32))
-            L.check(self.lib.wlk_vad_load_tensor(self.h, name.encode(), a.ctypes.data_as(C.c_void_p), a.size))
-
-    def open_session(self) -> int:
-        sid = C.c_int32()
-        L.check(self.lib.wlk_vad_session_open(self.h, C.byref(sid)))
-        return int(sid.value)
-
-    def reset_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_vad_session_reset(self.h, int(sid)))
-
-    def close_session(self, sid: int) -> None:
-        L.check(self.lib.wlk_vad_session_close(self.h, int(sid)))
+            L.check(self.lib.wlk_vad_load_tensor(self.h, name.encode(), _ptr(a), a.size))
 
     def forward(self, sids: Sequence[int], audios: Sequence[np.ndarray]) -> List[np.ndarray]:
         """audios[i]: fp32 samples of stream i, a whole number of 512-sample windows -> probabilities per window."""
         s = np.ascontiguousarray(sids, np.int32)
-        wins = []
-        offs = np.zeros(len(s) + 1, np.int32)
-        for i, a in enumerate(audios):
-            a = np.ascontiguousarray(np.asarray(a, np.float32).reshape(-1))
-            if a.shape[0] % WINDOW:
-                raise ValueError("VAD input must be whole 512-sample windows (FixedVADIterator buffers the remainder)")
-            wins.append(a)
-            offs[i + 1] = offs[i] + a.shape[0] // WINDOW
-        pcm = np.concatenate(wins) if wins else np.zeros(0, np.float32)
+        wins = [np.asarray(a, np.float32).reshape(-1) for a in audios]
+        if len(wins) != len(s):
+            raise ValueError("sids and audios differ in length")
+        if any(w.shape[0] % WINDOW for w in wins):
+            raise ValueError("VAD input must be whole 512-sample windows (FixedVADIterator buffers the remainder)")
+        pcm, offs = pack(wins, np.float32, (WINDOW,))
         probs = np.zeros(int(offs[-1]), np.float32)
-        L.check(self.lib.wlk_vad_forward(self.h, s.ctypes.data_as(C.c_void_p), len(s), pcm.ctypes.data_as(C.c_void_p),
-                                         offs.ctypes.data_as(C.c_void_p), probs.ctypes.data_as(C.c_void_p)))
-        return [probs[offs[i]: offs[i + 1]].copy() for i in range(len(s))]
-
-    def close(self) -> None:
-        if not self._closed:
-            self._closed = True
-            L.check(self.lib.wlk_vad_destroy(self.h))
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        L.check(self.lib.wlk_vad_forward(self.h, _ptr(s), len(s), _ptr(pcm), _ptr(offs), _ptr(probs)))
+        return split(probs, offs)
 
 
 class B200VadModel:
