@@ -1,4 +1,4 @@
-// Engine: weights arena, per-session device state, batched encode/decode orchestration and the C ABI
+// Engine: weights, per-session device state, batched encode/decode orchestration and the C ABI
 // declared in include/wlk_b200.h.  One CUDA stream per engine; calls are serialised by a mutex and
 // concurrency comes from batching sessions into one call.
 #include <algorithm>
@@ -29,20 +29,9 @@ void set_last_error(const std::string& msg) { g_last_error = msg; }
 namespace {
 
 constexpr int AUDIO_CAP = 2 * 480000;       // samples a session may buffer (reference keeps <= 30 s + one chunk)
-constexpr size_t ALIGN = 256;
 
 static const char* kClassNames[WLK_KC_COUNT] = {"mel", "gemm_enc", "attn_enc", "layernorm", "gemm_xkv", "gemm_dec",
                                                 "attn_dec_self", "attn_dec_cross", "logits", "align", "misc"};
-
-struct Arena {                       // bump allocator over one device allocation (the weight blob)
-    uint8_t* base = nullptr;
-    size_t cap = 0, used = 0;
-    void* take(size_t bytes) {
-        size_t off = (used + ALIGN - 1) / ALIGN * ALIGN;
-        used = off + bytes;
-        return base ? base + off : reinterpret_cast<void*>(off);   // dry run when base == nullptr
-    }
-};
 
 struct EncLayerW { float *ln1w, *ln1b, *bqkv, *bo, *ln2w, *ln2b, *b1, *b2; void *Wqkv, *Wo, *W1, *W2; };
 struct DecLayerW {
@@ -107,9 +96,7 @@ struct wlk_engine : EngineBase {       // act: also the type of every session bu
     std::set<uint64_t> dec_graph_seen;
     uint64_t dec_graph_tick = 0;
 
-    Arena arena;
     Weights w;
-    float* stage_f32 = nullptr; size_t stage_cap = 0;
 
     SessionTable<Session> sess;
     std::vector<int32_t> align_rank_host;     // [L*H] -> rank or -1
@@ -187,224 +174,78 @@ struct ProfScope {
 // ---------------------------------------------------------------------------------------
 // weights
 // ---------------------------------------------------------------------------------------
-void layout_weights(wlk_engine* e) {
-    const wlk_dims& D = e->dims;
-    Arena& A = e->arena;
-    Weights& W = e->w;
-    const size_t es = e->wes();
-    const int d = D.n_audio_state, dt = D.n_text_state;
-    auto f32 = [&](size_t n) { return reinterpret_cast<float*>(A.take(n * 4)); };
-    auto mat = [&](size_t n) { return A.take(n * es); };
-    W.filtT = f32((size_t)N_FREQ * D.n_mels);
-    W.window = f32(N_FFT);
-    W.twiddle = reinterpret_cast<float2*>(A.take(N_FFT * 8));
-    W.filt_span = reinterpret_cast<int2*>(A.take((size_t)D.n_mels * 8));
-    W.Wc1 = mat((size_t)d * 3 * D.n_mels); W.bc1 = f32(d);
-    W.Wc2 = mat((size_t)d * 3 * d); W.bc2 = f32(d);
-    W.enc_pos = f32((size_t)D.n_audio_ctx * d);
-    W.enc.resize(D.n_audio_layer);
-    for (auto& l : W.enc) {
-        l.ln1w = f32(d); l.ln1b = f32(d);
-        l.Wqkv = mat((size_t)3 * d * d); l.bqkv = f32(3 * d);
-        l.Wo = mat((size_t)d * d); l.bo = f32(d);
-        l.ln2w = f32(d); l.ln2b = f32(d);
-        l.W1 = mat((size_t)4 * d * d); l.b1 = f32(4 * d);
-        l.W2 = mat((size_t)4 * d * d); l.b2 = f32(d);
-    }
-    W.lnpw = f32(d); W.lnpb = f32(d);
-    W.emb_f32 = f32((size_t)D.n_vocab * dt);
-    W.emb_act = (e->wt == DT_F32) ? (void*)W.emb_f32 : mat((size_t)D.n_vocab * dt);
-    W.dec_pos = f32((size_t)D.n_text_ctx * dt);
-    W.dec.resize(D.n_text_layer);
-    for (auto& l : W.dec) {
-        l.ln1w = f32(dt); l.ln1b = f32(dt);
-        l.Wqkv = mat((size_t)3 * dt * dt); l.bqkv = f32(3 * dt);
-        l.Wo = mat((size_t)dt * dt); l.bo = f32(dt);
-        l.lncw = f32(dt); l.lncb = f32(dt);
-        l.Wqc = mat((size_t)dt * dt); l.bqc = f32(dt);
-        l.Woc = mat((size_t)dt * dt); l.boc = f32(dt);
-        l.ln2w = f32(dt); l.ln2b = f32(dt);
-        l.W1 = mat((size_t)4 * dt * dt); l.b1 = f32(4 * dt);
-        l.W2 = mat((size_t)4 * dt * dt); l.b2 = f32(dt);
-    }
-    W.lnw = f32(dt); W.lnb = f32(dt);
-    W.Wxkv = mat((size_t)D.n_text_layer * 2 * dt * d);
-    W.bxkv = f32((size_t)D.n_text_layer * 2 * dt);
-}
-
-float* stage_reserve(wlk_engine* e, size_t n) {
-    if (n > e->stage_cap) {
-        if (e->stage_f32) CUDA_CHECK(cudaFree(e->stage_f32));
-        size_t cap = n < (1u << 20) ? (1u << 20) : n;
-        CUDA_CHECK(cudaMalloc(&e->stage_f32, cap * 4));
-        e->stage_cap = cap;
-    }
-    return e->stage_f32;
-}
-float* stage(wlk_engine* e, const float* host, size_t n) {
-    float* s = stage_reserve(e, n);
-    CUDA_CHECK(cudaMemcpyAsync(s, host, n * 4, cudaMemcpyHostToDevice, e->st));
-    return s;
-}
-void put_f32(wlk_engine* e, float* dst, const float* host, size_t n) {
-    CUDA_CHECK(cudaMemcpyAsync(dst, host, n * 4, cudaMemcpyHostToDevice, e->st));
-    CUDA_CHECK(cudaStreamSynchronize(e->st));
-}
-// device fp32 -> `n` elements at element offset `off` of a weight matrix of `total` elements (planar in DT_BF16X2)
-void store_mat(wlk_engine* e, void* base, size_t total, size_t off, const float* src_dev, size_t n) {
-    if (e->wt == DT_BF16X2) {
-        bf16* hi = reinterpret_cast<bf16*>(base) + off;
-        split_f32_to_planes(src_dev, hi, hi + total, (int64_t)n, e->st);
-    } else {
-        convert_f32_to(src_dev, reinterpret_cast<uint8_t*>(base) + off * e->wes(), e->wt, (int64_t)n, e->st);
-    }
-    CUDA_CHECK(cudaStreamSynchronize(e->st));
-}
-void put_mat(wlk_engine* e, void* base, size_t total, size_t off, const float* host, size_t n) {
-    store_mat(e, base, total, off, stage(e, host, n), n);
-}
 uint8_t* offs(void* p, size_t elems, size_t es) { return reinterpret_cast<uint8_t*>(p) + elems * es; }
-// conv weight [c_out, c_in, 3] -> tap-major [c_out, 3 * c_in] in the weight type (via an fp32 staging copy in BF16X3)
-void put_conv(wlk_engine* e, void* dst, const float* host, int c_out, int c_in) {
-    const size_t n = (size_t)c_out * c_in * 3;
-    float* s = stage_reserve(e, 2 * n);                         // second half: the packed fp32 copy
-    CUDA_CHECK(cudaMemcpyAsync(s, host, n * 4, cudaMemcpyHostToDevice, e->st));
-    if (e->wt == DT_BF16X2) {
-        pack_conv_weight(s, s + n, DT_F32, c_out, c_in, e->st);
-        store_mat(e, dst, n, 0, s + n, n);
-    } else {
-        pack_conv_weight(s, dst, e->wt, c_out, c_in, e->st);
-        CUDA_CHECK(cudaStreamSynchronize(e->st));
-    }
-}
 
-void load_tensor(wlk_engine* e, const std::string& name, const float* host, const int64_t* shape, int ndim) {
+// Every tensor in the order of the weight blob, which bench.py broadcasts across ranks (weight_blob / adopt_weights)
+void declare_weights(wlk_engine* e) {
     const wlk_dims& D = e->dims;
     Weights& W = e->w;
-    const int d = D.n_audio_state, dt = D.n_text_state;
-    const size_t es = e->es();
-    const int64_t n = numel(shape, ndim);
-    auto expect = [&](int64_t want) {
-        WLK_CHECK(n == want, "tensor %s has %lld elements, expected %lld", name.c_str(), (long long)n, (long long)want);
+    WeightTable& T = e->weights;
+    T.rule = WeightTable::NUMEL;
+    T.wt = e->wt;
+    const int wt = e->wt, d = D.n_audio_state, dt = D.n_text_state;
+    T.buf(W.filtT, (size_t)N_FREQ * D.n_mels * 4);
+    T.f32("hann_window", W.window, {N_FFT});
+    T.buf(W.twiddle, N_FFT * 8);
+    T.buf(W.filt_span, (size_t)D.n_mels * 8);
+    declare_mel_filters(T, W.filtT, W.filt_span, D.n_mels, N_FREQ);
+    T.mat("encoder.conv1.weight", W.Wc1, {d, D.n_mels, 3}, swap_inner_axes(d, D.n_mels, 3));
+    T.f32("encoder.conv1.bias", W.bc1, {d});
+    T.mat("encoder.conv2.weight", W.Wc2, {d, d, 3}, swap_inner_axes(d, d, 3));
+    T.f32("encoder.conv2.bias", W.bc2, {d});
+    T.f32("encoder.positional_embedding", W.enc_pos, {D.n_audio_ctx, d});
+    // the parts every block has: self-attention (q / k / v rows fused; key has no bias) and the MLP around `between`
+    auto block = [&](const std::string& p, int dm, auto& l, auto&& between) {
+        T.f32(p + "attn_ln.weight", l.ln1w, {dm});
+        T.f32(p + "attn_ln.bias", l.ln1b, {dm});
+        T.fused(l.Wqkv, wt, {{p + "attn.query.weight", dm}, {p + "attn.key.weight", dm}, {p + "attn.value.weight", dm}}, dm);
+        T.fused(l.bqkv, DT_F32, {{p + "attn.query.bias", dm}, {"", dm}, {p + "attn.value.bias", dm}}, 0);
+        T.mat(p + "attn.out.weight", l.Wo, {dm, dm});
+        T.f32(p + "attn.out.bias", l.bo, {dm});
+        between();
+        T.f32(p + "mlp_ln.weight", l.ln2w, {dm});
+        T.f32(p + "mlp_ln.bias", l.ln2b, {dm});
+        T.mat(p + "mlp.0.weight", l.W1, {4 * dm, dm});
+        T.f32(p + "mlp.0.bias", l.b1, {4 * dm});
+        T.mat(p + "mlp.2.weight", l.W2, {dm, 4 * dm});
+        T.f32(p + "mlp.2.bias", l.b2, {dm});
     };
-    if (name == "mel_filters") {
-        expect((int64_t)D.n_mels * N_FREQ);
-        std::vector<float> t((size_t)n);
-        for (int m = 0; m < D.n_mels; ++m)
-            for (int k = 0; k < N_FREQ; ++k) t[(size_t)k * D.n_mels + m] = host[(size_t)m * N_FREQ + k];
-        put_f32(e, W.filtT, t.data(), n);
-        std::vector<int2> span(D.n_mels);                     // non-zero span of every (triangular) filter
-        for (int m = 0; m < D.n_mels; ++m) {
-            int lo = N_FREQ, hi = 0;
-            for (int k = 0; k < N_FREQ; ++k)
-                if (host[(size_t)m * N_FREQ + k] != 0.f) { if (k < lo) lo = k; hi = k + 1; }
-            if (lo >= hi) { lo = 0; hi = 0; }
-            span[m] = make_int2(lo, hi);
-        }
-        CUDA_CHECK(cudaMemcpyAsync(W.filt_span, span.data(), span.size() * 8, cudaMemcpyHostToDevice, e->st));
-        CUDA_CHECK(cudaStreamSynchronize(e->st));
-    } else if (name == "hann_window") {
-        expect(N_FFT);
-        put_f32(e, W.window, host, n);
-    } else if (name == "encoder.conv1.weight") {
-        expect((int64_t)d * D.n_mels * 3);
-        put_conv(e, W.Wc1, host, d, D.n_mels);
-    } else if (name == "encoder.conv2.weight") {
-        expect((int64_t)d * d * 3);
-        put_conv(e, W.Wc2, host, d, d);
-    } else if (name == "encoder.conv1.bias") { expect(d); put_f32(e, W.bc1, host, n);
-    } else if (name == "encoder.conv2.bias") { expect(d); put_f32(e, W.bc2, host, n);
-    } else if (name == "encoder.positional_embedding") { expect((int64_t)D.n_audio_ctx * d); put_f32(e, W.enc_pos, host, n);
-    } else if (name == "encoder.ln_post.weight") { expect(d); put_f32(e, W.lnpw, host, n);
-    } else if (name == "encoder.ln_post.bias") { expect(d); put_f32(e, W.lnpb, host, n);
-    } else if (name == "decoder.token_embedding.weight") {
-        expect((int64_t)D.n_vocab * dt);
-        put_f32(e, W.emb_f32, host, n);
-        if (e->wt != DT_F32) store_mat(e, W.emb_act, (size_t)n, 0, W.emb_f32, (size_t)n);
-    } else if (name == "decoder.positional_embedding") { expect((int64_t)D.n_text_ctx * dt); put_f32(e, W.dec_pos, host, n);
-    } else if (name == "decoder.ln.weight") { expect(dt); put_f32(e, W.lnw, host, n);
-    } else if (name == "decoder.ln.bias") { expect(dt); put_f32(e, W.lnb, host, n);
-    } else if (name.rfind("encoder.blocks.", 0) == 0 || name.rfind("decoder.blocks.", 0) == 0) {
-        const bool is_dec = name[0] == 'd';
-        size_t p0 = strlen("encoder.blocks.");
-        size_t p1 = name.find('.', p0);
-        int li = std::stoi(name.substr(p0, p1 - p0));
-        std::string rest = name.substr(p1 + 1);
-        const int dm = is_dec ? dt : d;
-        WLK_CHECK(li >= 0 && li < (is_dec ? D.n_text_layer : D.n_audio_layer), "layer index out of range in %s", name.c_str());
-        if (!is_dec) {
-            EncLayerW& L = W.enc[li];
-            if (rest == "attn.query.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, 0, host, n); }
-            else if (rest == "attn.key.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, (size_t)dm * dm, host, n); }
-            else if (rest == "attn.value.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, (size_t)2 * dm * dm, host, n); }
-            else if (rest == "attn.query.bias") { expect(dm); put_f32(e, L.bqkv, host, n); }
-            else if (rest == "attn.value.bias") { expect(dm); put_f32(e, L.bqkv + 2 * dm, host, n); }
-            else if (rest == "attn.out.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wo, (size_t)dm * dm, 0, host, n); }
-            else if (rest == "attn.out.bias") { expect(dm); put_f32(e, L.bo, host, n); }
-            else if (rest == "attn_ln.weight") { expect(dm); put_f32(e, L.ln1w, host, n); }
-            else if (rest == "attn_ln.bias") { expect(dm); put_f32(e, L.ln1b, host, n); }
-            else if (rest == "mlp.0.weight") { expect((int64_t)4 * dm * dm); put_mat(e, L.W1, (size_t)4 * dm * dm, 0, host, n); }
-            else if (rest == "mlp.0.bias") { expect(4 * dm); put_f32(e, L.b1, host, n); }
-            else if (rest == "mlp.2.weight") { expect((int64_t)4 * dm * dm); put_mat(e, L.W2, (size_t)4 * dm * dm, 0, host, n); }
-            else if (rest == "mlp.2.bias") { expect(dm); put_f32(e, L.b2, host, n); }
-            else if (rest == "mlp_ln.weight") { expect(dm); put_f32(e, L.ln2w, host, n); }
-            else if (rest == "mlp_ln.bias") { expect(dm); put_f32(e, L.ln2b, host, n); }
-            else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-        } else {
-            DecLayerW& L = W.dec[li];
-            const size_t xrow = (size_t)li * 2 * dt;      // row offset inside Wxkv / bxkv
-            if (rest == "attn.query.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, 0, host, n); }
-            else if (rest == "attn.key.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, (size_t)dm * dm, host, n); }
-            else if (rest == "attn.value.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqkv, (size_t)3 * dm * dm, (size_t)2 * dm * dm, host, n); }
-            else if (rest == "attn.query.bias") { expect(dm); put_f32(e, L.bqkv, host, n); }
-            else if (rest == "attn.value.bias") { expect(dm); put_f32(e, L.bqkv + 2 * dm, host, n); }
-            else if (rest == "attn.out.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wo, (size_t)dm * dm, 0, host, n); }
-            else if (rest == "attn.out.bias") { expect(dm); put_f32(e, L.bo, host, n); }
-            else if (rest == "attn_ln.weight") { expect(dm); put_f32(e, L.ln1w, host, n); }
-            else if (rest == "attn_ln.bias") { expect(dm); put_f32(e, L.ln1b, host, n); }
-            else if (rest == "cross_attn.query.weight") { expect((int64_t)dm * dm); put_mat(e, L.Wqc, (size_t)dm * dm, 0, host, n); }
-            else if (rest == "cross_attn.query.bias") { expect(dm); put_f32(e, L.bqc, host, n); }
-            else if (rest == "cross_attn.key.weight") { expect((int64_t)dt * d); put_mat(e, W.Wxkv, (size_t)D.n_text_layer * 2 * dt * d, xrow * d, host, n); }
-            else if (rest == "cross_attn.value.weight") { expect((int64_t)dt * d); put_mat(e, W.Wxkv, (size_t)D.n_text_layer * 2 * dt * d, (xrow + dt) * d, host, n); }
-            else if (rest == "cross_attn.value.bias") { expect(dt); put_f32(e, W.bxkv + xrow + dt, host, n); }
-            else if (rest == "cross_attn.out.weight") { expect((int64_t)dm * dm); put_mat(e, L.Woc, (size_t)dm * dm, 0, host, n); }
-            else if (rest == "cross_attn.out.bias") { expect(dm); put_f32(e, L.boc, host, n); }
-            else if (rest == "cross_attn_ln.weight") { expect(dm); put_f32(e, L.lncw, host, n); }
-            else if (rest == "cross_attn_ln.bias") { expect(dm); put_f32(e, L.lncb, host, n); }
-            else if (rest == "mlp.0.weight") { expect((int64_t)4 * dm * dm); put_mat(e, L.W1, (size_t)4 * dm * dm, 0, host, n); }
-            else if (rest == "mlp.0.bias") { expect(4 * dm); put_f32(e, L.b1, host, n); }
-            else if (rest == "mlp.2.weight") { expect((int64_t)4 * dm * dm); put_mat(e, L.W2, (size_t)4 * dm * dm, 0, host, n); }
-            else if (rest == "mlp.2.bias") { expect(dm); put_f32(e, L.b2, host, n); }
-            else if (rest == "mlp_ln.weight") { expect(dm); put_f32(e, L.ln2w, host, n); }
-            else if (rest == "mlp_ln.bias") { expect(dm); put_f32(e, L.ln2b, host, n); }
-            else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-        }
-    } else {
-        WLK_CHECK(false, "unknown tensor %s", name.c_str());
+    W.enc.resize(D.n_audio_layer);
+    for (int i = 0; i < D.n_audio_layer; ++i) block("encoder.blocks." + std::to_string(i) + ".", d, W.enc[i], [] {});
+    T.f32("encoder.ln_post.weight", W.lnpw, {d});
+    T.f32("encoder.ln_post.bias", W.lnpb, {d});
+    // the token embedding in fp32 (the decoder's input rows) and, unless that is the weight type, in the weight type
+    // (the logits GEMM); in fp32 both are the same buffer
+    WeightTable::Entry& emb = T.f32("decoder.token_embedding.weight", W.emb_f32, {D.n_vocab, dt});
+    if (wt != DT_F32) {
+        T.buf(W.emb_act, (size_t)D.n_vocab * dt * e->wes());
+        emb.dst.push_back(WeightTable::Dst(W.emb_act, 0, wt, (size_t)D.n_vocab * dt));
     }
-    e->loaded.insert(name);
-}
-
-std::vector<std::string> required_tensors(const wlk_dims& D) {
-    std::vector<std::string> r = {"mel_filters", "hann_window", "encoder.conv1.weight", "encoder.conv1.bias",
-                                  "encoder.conv2.weight", "encoder.conv2.bias", "encoder.positional_embedding",
-                                  "encoder.ln_post.weight", "encoder.ln_post.bias", "decoder.token_embedding.weight",
-                                  "decoder.positional_embedding", "decoder.ln.weight", "decoder.ln.bias"};
-    const char* att[] = {"query.weight", "query.bias", "key.weight", "value.weight", "value.bias", "out.weight", "out.bias"};
-    const char* com[] = {"attn_ln.weight", "attn_ln.bias", "mlp.0.weight", "mlp.0.bias", "mlp.2.weight", "mlp.2.bias",
-                         "mlp_ln.weight", "mlp_ln.bias"};
-    for (int l = 0; l < D.n_audio_layer; ++l) {
-        std::string p = "encoder.blocks." + std::to_string(l) + ".";
-        for (auto a : att) r.push_back(p + "attn." + a);
-        for (auto c : com) r.push_back(p + c);
+    T.f32("decoder.positional_embedding", W.dec_pos, {D.n_text_ctx, dt});
+    W.dec.resize(D.n_text_layer);
+    for (int i = 0; i < D.n_text_layer; ++i) {
+        const std::string p = "decoder.blocks." + std::to_string(i) + ".";
+        DecLayerW& l = W.dec[i];
+        block(p, dt, l, [&] {
+            T.f32(p + "cross_attn_ln.weight", l.lncw, {dt});
+            T.f32(p + "cross_attn_ln.bias", l.lncb, {dt});
+            T.mat(p + "cross_attn.query.weight", l.Wqc, {dt, dt});
+            T.f32(p + "cross_attn.query.bias", l.bqc, {dt});
+            T.mat(p + "cross_attn.out.weight", l.Woc, {dt, dt});
+            T.f32(p + "cross_attn.out.bias", l.boc, {dt});
+        });
     }
-    for (int l = 0; l < D.n_text_layer; ++l) {
-        std::string p = "decoder.blocks." + std::to_string(l) + ".";
-        for (auto a : att) { r.push_back(p + "attn." + a); r.push_back(p + "cross_attn." + a); }
-        for (auto c : com) r.push_back(p + c);
-        r.push_back(p + "cross_attn_ln.weight"); r.push_back(p + "cross_attn_ln.bias");
+    T.f32("decoder.ln.weight", W.lnw, {dt});
+    T.f32("decoder.ln.bias", W.lnb, {dt});
+    // every decoder layer's cross K/V projection in one matrix [L * 2 * dt][d] (key has no bias)
+    std::vector<std::pair<std::string, int64_t>> xkv, xkv_bias;
+    for (int i = 0; i < D.n_text_layer; ++i) {
+        const std::string p = "decoder.blocks." + std::to_string(i) + ".cross_attn.";
+        xkv.insert(xkv.end(), {{p + "key.weight", dt}, {p + "value.weight", dt}});
+        xkv_bias.insert(xkv_bias.end(), {{"", dt}, {p + "value.bias", dt}});
     }
-    return r;
+    T.fused(W.Wxkv, wt, xkv, d);
+    T.fused(W.bxkv, DT_F32, xkv_bias, 0);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1068,13 +909,9 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     {   const char* v = getenv("WLK_MEL_INCREMENTAL"); e->mel_incremental = !(v && v[0] == '0'); }
     for (auto& t : e->timers) CUDA_CHECK(cudaEventCreate(&t));
 
-    // weights arena: dry run for the size, then the real layout
-    layout_weights(e);
-    const size_t wbytes = e->arena.used + ALIGN;
-    e->arena = Arena{};
-    e->arena.base = reinterpret_cast<uint8_t*>(e->allocs.take(wbytes, &e->bytes_weights));
-    e->arena.cap = wbytes;
-    layout_weights(e);
+    declare_weights(e);
+    e->weights.allocate(e->allocs, &e->bytes_weights);
+    if (e->wt == DT_F32) e->w.emb_act = e->w.emb_f32;
     {   // DFT twiddles exp(-2 pi i t / 400) in double -> float
         std::vector<float2> tw(N_FFT);
         for (int t = 0; t < N_FFT; ++t) {
@@ -1143,7 +980,7 @@ void destroy_engine(wlk_engine* e) {
     e->close([e] {
         for (auto& s : e->sess) if (s.open && s.parent >= 0) free_session(e, s);     // forks before their parents
         for (auto& s : e->sess) if (s.open) free_session(e, s);
-        for (void* p : {(void*)e->stage_f32, e->beam_scratch, (void*)e->all_logits_dev}) if (p) cudaFree(p);
+        for (void* p : {e->beam_scratch, (void*)e->all_logits_dev}) if (p) cudaFree(p);
         if (e->res_host) cudaFreeHost(e->res_host);
         if (e->tap_host) cudaFreeHost(e->tap_host);
         for (auto& t : e->timers) if (t) cudaEventDestroy(t);
@@ -1190,14 +1027,14 @@ int wlk_engine_load_tensor(wlk_engine* e, const char* name, const float* host, c
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
-    load_tensor(e, name, host, shape, ndim);
+    e->weights.load(name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_engine_finalize_weights(wlk_engine* e) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    require_loaded(e->loaded, required_tensors(e->dims));
-    if (e->stage_f32) { CUDA_CHECK(cudaFree(e->stage_f32)); e->stage_f32 = nullptr; e->stage_cap = 0; }
+    e->weights.require_all();
+    e->upload.release();
     e->finalized = true;
     WLK_API_END
 }
@@ -1206,7 +1043,7 @@ int wlk_engine_weight_blob(wlk_engine* e, void** dev, size_t* nbytes) {
     WLK_ENTER(e, e->cfg.device);
     WLK_CHECK(dev && nbytes, "null out pointer");
     CUDA_CHECK(cudaStreamSynchronize(e->st));
-    *dev = e->arena.base; *nbytes = e->arena.cap;
+    *dev = e->weights.blob; *nbytes = e->weights.bytes;
     WLK_API_END
 }
 int wlk_engine_adopt_weights(wlk_engine* e) {

@@ -1,9 +1,11 @@
 // Host plumbing shared by the C-ABI units: the entry-point guard, device selection, device buffers kept until
-// destroy, the fp32 weight upload, the checks on loaded tensors, the staging block, the GEMM dispatch, the session
-// table and the state every engine handle holds.
+// destroy, the fp32 weight upload, the weight table, the staging block, the GEMM dispatch, the session table and the
+// state every engine handle holds.
 #pragma once
 
-#include <initializer_list>
+#include <cstring>
+#include <functional>
+#include <map>
 #include <mutex>
 #include <set>
 #include <string>
@@ -84,8 +86,9 @@ struct WeightUpload {
     float* buf = nullptr;
     size_t cap = 0;
 
-    // n floats -> dst as fp32 (a copy) or as dst_type (a conversion).  Synchronous: `host` may be reused on return.
-    void put(const float* host, size_t n, void* dst, int dst_type, cudaStream_t st) {
+    // n floats -> dst as fp32 (a copy) or as dst_type (a conversion).  DT_BF16X2 puts the hi plane at dst and the lo
+    // plane `plane` elements behind it.  Synchronous: `host` may be reused on return.
+    void put(const float* host, size_t n, void* dst, int dst_type, cudaStream_t st, size_t plane = 0) {
         if (n > cap) {
             if (buf) { CUDA_CHECK(cudaStreamSynchronize(st)); CUDA_CHECK(cudaFree(buf)); }
             CUDA_CHECK(cudaMalloc(&buf, n * 4));
@@ -93,6 +96,7 @@ struct WeightUpload {
         }
         CUDA_CHECK(cudaMemcpyAsync(buf, host, n * 4, cudaMemcpyHostToDevice, st));
         if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, buf, n * 4, cudaMemcpyDeviceToDevice, st));
+        else if (dst_type == DT_BF16X2) split_f32_to_planes(buf, (bf16*)dst, (bf16*)dst + plane, (int64_t)n, st);
         else convert_f32_to(buf, dst, dst_type, (int64_t)n, st);
         CUDA_CHECK(cudaStreamSynchronize(st));
     }
@@ -127,21 +131,156 @@ inline int64_t numel(const int64_t* shape, int ndim) {
     return n;
 }
 
-// The tensor's shape must be exactly `want`.
-inline void expect_shape(const char* name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
-    bool ok = (int)want.size() == ndim;
-    int i = 0;
-    for (int64_t w : want) { if (ok && shape[i] != w) ok = false; ++i; }
-    WLK_CHECK(ok, "tensor %s has the wrong shape for this geometry", name);
+// An engine's weights.  At create the engine declares every checkpoint tensor once -- its name, its canonical shape and
+// where its elements go -- together with the unnamed buffers it derives itself, then allocate() places them all in one
+// device blob.  load() checks a tensor against its declaration by the engine's shape rule and uploads it; require_all()
+// names the declared tensors that were not loaded.
+struct WeightTable {
+    // element count only; element count and leading axis (Conv kernels may carry trailing singleton axes); exact shape
+    enum Rule { NUMEL, LEADING, EXACT };
+    using Perm = std::function<std::vector<float>(const float* host)>;   // host rearrangement before the upload
+    struct Dst {
+        void** base;
+        size_t off = 0;                  // element offset from *base (into the hi plane in DT_BF16X2)
+        int type = DT_F32;
+        size_t plane = 0;                // DT_BF16X2: elements from the hi plane to the lo plane (the whole matrix)
+        Perm perm = nullptr;
+        template <typename T>
+        Dst(T*& b, size_t o = 0, int t = DT_F32, size_t p = 0, Perm f = nullptr)
+            : base(reinterpret_cast<void**>(&b)), off(o), type(t), plane(p), perm(std::move(f)) {}
+    };
+    struct Entry {
+        std::string name;
+        std::vector<int64_t> shape;
+        std::vector<Dst> dst;            // none: accepted and dropped
+        bool optional = false;
+    };
+
+    WeightUpload& up;
+    cudaStream_t& st;
+    Rule rule = EXACT;
+    int wt = DT_F32;                     // type of the weight matrices
+    std::vector<Entry> entries;          // in declaration order, the order require_all() reports in
+    std::map<std::string, size_t> index;
+    std::vector<std::pair<void**, size_t>> slots;   // pointer to set, byte offset in the blob
+    size_t used = 0;
+    uint8_t* blob = nullptr;
+    size_t bytes = 0;
+    std::set<std::string> loaded;
+
+    // `nbytes` of the blob at the next 256-byte boundary; *slot points there once allocate() ran, so a slot must not
+    // move in between (resize per-layer vectors before declaring)
+    template <typename T>
+    void buf(T*& slot, size_t nbytes) {
+        used = (used + 255) / 256 * 256;
+        slots.push_back({reinterpret_cast<void**>(&slot), used});
+        used += nbytes;
+    }
+    Entry& add(const std::string& name, std::vector<int64_t> shape, std::vector<Dst> dst) {
+        index[name] = entries.size();
+        entries.push_back({name, std::move(shape), std::move(dst)});
+        return entries.back();
+    }
+    // a tensor in a buffer of its own: an fp32 vector, or a matrix in the weight type
+    Entry& f32(const std::string& name, float*& slot, std::vector<int64_t> shape) {
+        buf(slot, (size_t)numel(shape.data(), (int)shape.size()) * 4);
+        return add(name, std::move(shape), {Dst(slot)});
+    }
+    Entry& mat(const std::string& name, void*& slot, std::vector<int64_t> shape, Perm perm = nullptr) {
+        const size_t n = (size_t)numel(shape.data(), (int)shape.size());
+        buf(slot, n * dtype_size(wt));
+        return add(name, std::move(shape), {Dst(slot, 0, wt, n, std::move(perm))});
+    }
+    // Tensors one after another in one buffer of `type`: [sum of rows][cols], or a vector when cols is 0.  A part without a
+    // name is left zero.
+    template <typename T>
+    void fused(T*& slot, int type, const std::vector<std::pair<std::string, int64_t>>& parts, int64_t cols) {
+        int64_t rows = 0;
+        for (auto& p : parts) rows += p.second;
+        const size_t n = (size_t)rows * (cols ? cols : 1);
+        buf(slot, n * dtype_size(type));
+        int64_t r = 0;
+        for (auto& p : parts) {
+            if (!p.first.empty())
+                add(p.first, cols ? std::vector<int64_t>{p.second, cols} : std::vector<int64_t>{p.second},
+                    {Dst(slot, (size_t)r * (cols ? cols : 1), type, n)});
+            r += p.second;
+        }
+    }
+
+    // The blob (with 256 bytes of tail slack), zero-filled, and every declared pointer into it.
+    void allocate(DeviceAllocs& allocs, size_t* acct) {
+        bytes = used + 256;
+        blob = reinterpret_cast<uint8_t*>(allocs.take(bytes, acct));
+        for (auto& s : slots) *s.first = blob + s.second;
+    }
+
+    void check_shape(const Entry& e, const int64_t* shape, int ndim) const {
+        const int64_t n = numel(shape, ndim), want = numel(e.shape.data(), (int)e.shape.size());
+        if (rule == NUMEL) {
+            WLK_CHECK(n == want, "tensor %s has %lld elements, expected %lld", e.name.c_str(), (long long)n, (long long)want);
+            return;
+        }
+        const bool ok = rule == LEADING ? n == want && shape[0] == e.shape[0]
+                                        : std::vector<int64_t>(shape, shape + ndim) == e.shape;
+        WLK_CHECK(ok, "tensor %s has the wrong shape for this geometry", e.name.c_str());
+    }
+
+    void load(const std::string& name, const float* host, const int64_t* shape, int ndim) {
+        auto it = index.find(name);
+        WLK_CHECK(it != index.end(), "unknown tensor %s", name.c_str());
+        const Entry& e = entries[it->second];
+        const int64_t n = numel(shape, ndim);
+        if (!e.dst.empty()) check_shape(e, shape, ndim);      // an entry without a destination takes any shape
+        for (const Dst& d : e.dst) {
+            std::vector<float> tmp;
+            if (d.perm) tmp = d.perm(host);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(*d.base) + d.off * (d.type == DT_F32 ? 4 : 2);
+            up.put(d.perm ? tmp.data() : host, d.perm ? tmp.size() : (size_t)n, dst, d.type, st, d.plane);
+        }
+        loaded.insert(name);
+    }
+
+    // Every declared tensor that is not optional was loaded; the error names the first few that were not.
+    void require_all() const {
+        std::string missing;
+        int nmiss = 0;
+        for (auto& e : entries)
+            if (!e.optional && !loaded.count(e.name) && nmiss++ < 5) missing += e.name + " ";
+        WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+    }
+};
+
+// [a][b][c] -> [a][c][b].  A Conv weight [Co][Ci][K] becomes tap-major [Co][K][Ci] (a tap's input channels are
+// contiguous, like the im2col rows); a projection over channel-major features [d][C][F] reads [F][C] activations.
+inline WeightTable::Perm swap_inner_axes(int64_t a, int64_t b, int64_t c) {
+    return [=](const float* s) {
+        std::vector<float> t((size_t)(a * b * c));
+        for (int64_t i = 0; i < a; ++i)
+            for (int64_t j = 0; j < b; ++j)
+                for (int64_t k = 0; k < c; ++k) t[(size_t)((i * c + k) * b + j)] = s[(i * b + j) * c + k];
+        return t;
+    };
 }
 
-// Every name in `required` must have been loaded; the error names the first few that were not.
-inline void require_loaded(const std::set<std::string>& loaded, const std::vector<std::string>& required) {
-    std::string missing;
-    int nmiss = 0;
-    for (auto& r : required)
-        if (!loaded.count(r) && nmiss++ < 5) missing += r + " ";
-    WLK_CHECK(nmiss == 0, "%d tensors missing, e.g. %s", nmiss, missing.c_str());
+// "mel_filters" [n_mels][n_freq] (a Slaney filterbank): transposed to [n_freq][n_mels] at `filtT`, and the non-zero
+// span [lo, hi) of every (triangular) filter at `span`.  The engine reserves both buffers.
+inline WeightTable::Entry& declare_mel_filters(WeightTable& T, float*& filtT, int2*& span, int n_mels, int n_freq) {
+    auto spans = [=](const float* s) {
+        std::vector<float> out(2 * (size_t)n_mels);     // int2 per filter, carried bit for bit by the fp32 copy
+        for (int m = 0; m < n_mels; ++m) {
+            int lo = n_freq, hi = 0;
+            for (int k = 0; k < n_freq; ++k)
+                if (s[(size_t)m * n_freq + k] != 0.f) { if (k < lo) lo = k; hi = k + 1; }
+            if (lo >= hi) { lo = 0; hi = 0; }
+            const int2 v = make_int2(lo, hi);
+            memcpy(&out[2 * (size_t)m], &v, sizeof(v));
+        }
+        return out;
+    };
+    return T.add("mel_filters", {n_mels, n_freq},
+                 {WeightTable::Dst(filtT, 0, DT_F32, 0, swap_inner_axes(1, n_mels, n_freq)),
+                  WeightTable::Dst(span, 0, DT_F32, 0, spans)});
 }
 
 // A pinned host block mirrored on the device: a call lays out its small per-call arrays (jobs, row maps, pointer
@@ -253,8 +392,8 @@ struct EngineBase {
     std::mutex mu;
     DeviceAllocs allocs;                 // buffers kept from create (or first use) until destroy
     WeightUpload upload;
+    WeightTable weights{upload, st};
     size_t bytes_weights = 0, bytes_sessions = 0, bytes_workspace = 0;
-    std::set<std::string> loaded;
     bool finalized = false;
     Staging stg;
     GemmDispatch gemm;

@@ -347,23 +347,6 @@ void split_f32_to_planes(const float* src, bf16* hi, bf16* lo, int64_t n, cudaSt
     CUDA_CHECK(cudaGetLastError());
 }
 
-template <typename T>
-__global__ void pack_conv_kernel(const float* w, T* dst, int c_out, int c_in) {
-    // dst[co][k * c_in + ci] = w[co][ci][k]
-    int64_t n = (int64_t)c_out * c_in * 3;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        int co = (int)(i / (3 * c_in));
-        int rem = (int)(i - (int64_t)co * 3 * c_in);
-        int k = rem / c_in, ci = rem - k * c_in;
-        dst[i] = from_f32<T>(w[((int64_t)co * c_in + ci) * 3 + k]);
-    }
-}
-void pack_conv_weight(const float* w, void* dst, int dst_type, int c_out, int c_in, cudaStream_t st) {
-    if (dst_type == DT_F32) pack_conv_kernel<float><<<1024, 256, 0, st>>>(w, (float*)dst, c_out, c_in);
-    else pack_conv_kernel<bf16><<<1024, 256, 0, st>>>(w, (bf16*)dst, c_out, c_in);
-    CUDA_CHECK(cudaGetLastError());
-}
-
 // =====================================================================================
 // LayerNorm (fp32 statistics, reference whisper/model.py:39-41), one warp per row
 // =====================================================================================

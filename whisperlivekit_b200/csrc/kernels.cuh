@@ -141,7 +141,5 @@ void convert_to_f32(const void* src, int src_type, float* dst, int64_t n, cudaSt
 // WLK_PREC_BF16X3 weights: hi = bf16(x), lo = bf16(x - hi)
 void split_f32_to_planes(const float* src, bf16* hi, bf16* lo, int64_t n, cudaStream_t st);
 void pcm16_to_f32(const int16_t* src_dev, float* dst_dev, int64_t n, cudaStream_t st);
-// conv weight [c_out, c_in, 3] -> [c_out, 3 * c_in] (tap-major) in the destination type
-void pack_conv_weight(const float* w, void* dst, int dst_type, int c_out, int c_in, cudaStream_t st);
 
 }  // namespace wlk

@@ -114,7 +114,7 @@ __global__ void qwen_im2col_kernel(const T* __restrict__ src, const WChunk* __re
 }
 
 // positional rows: table[pos] while pos is inside the table, else the closed form sin | cos of fp32(pos) * inv_freq[j]
-// (reference causal.py:204-228; inv_freq [d / 2] holds the reference's fp32 frequencies, see load_tensor)
+// (reference causal.py:204-228; inv_freq [d / 2] holds the reference's fp32 frequencies, see alloc_weights)
 __global__ void qwen_pos_kernel(const int32_t* __restrict__ pos, const float* __restrict__ table, const float* __restrict__ inv_freq,
                                 int max_positions, float* __restrict__ out, int rows, int d) {
     const int r = blockIdx.x;
@@ -239,7 +239,6 @@ struct wlk_qwen : EngineBase {
     void *W2c = nullptr, *W3c = nullptr, *Wout = nullptr, *Wp1 = nullptr, *Wp2 = nullptr;
     float *lnpw = nullptr, *lnpb = nullptr, *bp1 = nullptr, *bp2 = nullptr;
     float *filtT = nullptr, *window = nullptr; float2* twiddle = nullptr; int2* filt_span = nullptr;   // mel front end
-    bool have_filters = false;
     float* mel_out = nullptr; size_t mel_out_cap = 0; float* audio_scratch = nullptr;
     std::vector<QLayerW> L;
     // sessions and workspaces
@@ -261,145 +260,55 @@ namespace {
 
 void qgemm(wlk_qwen* q, GemmArgs& g) { q->gemm.run(g, q->gemm_backend == WLK_BACKEND_TCGEN05, q->st, q->num_sms); }
 
-void load_tensor(wlk_qwen* q, const std::string& name, const float* host, const int64_t* shape, int ndim) {
-    const wlk_qwen_dims& D = q->dims;
-    const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
-    const int64_t n = numel(shape, ndim);
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect_shape(name.c_str(), shape, ndim, {rows, cols}); q->upload.put(host, n, dst, q->act, q->st); };
-    auto vec = [&](float* dst, int64_t len) { expect_shape(name.c_str(), shape, ndim, {len}); q->upload.put(host, n, dst, DT_F32, q->st); };
-    if (name == "mel_filters") {
-        // optional: only wlk_qwen_append_audio needs it.  [n_mels][201] (Slaney filterbank of the feature extractor)
-        expect_shape(name.c_str(), shape, ndim, {D.n_mels, N_FREQ});
-        std::vector<float> t((size_t)n);
-        std::vector<int2> span(D.n_mels);
-        for (int m = 0; m < D.n_mels; ++m) {
-            int lo = N_FREQ, hi = 0;
-            for (int k = 0; k < N_FREQ; ++k) {
-                t[(size_t)k * D.n_mels + m] = host[(size_t)m * N_FREQ + k];
-                if (host[(size_t)m * N_FREQ + k] != 0.f) { if (k < lo) lo = k; hi = k + 1; }
-            }
-            if (lo >= hi) { lo = 0; hi = 0; }
-            span[m] = make_int2(lo, hi);
-        }
-        q->upload.put(t.data(), n, q->filtT, DT_F32, q->st);
-        CUDA_CHECK(cudaMemcpyAsync(q->filt_span, span.data(), span.size() * 8, cudaMemcpyHostToDevice, q->st));
-        CUDA_CHECK(cudaStreamSynchronize(q->st));
-        q->have_filters = true;
-    }
-    else if (name == "conv2d1.weight") { expect_shape(name.c_str(), shape, ndim, {C, 1, 3, 3}); q->upload.put(host, n, q->c1w, DT_F32, q->st); }
-    else if (name == "conv2d1.bias") vec(q->c1b, C);
-    else if (name == "conv2d2.weight" || name == "conv2d3.weight") {
-        // [Co][Ci][3][3] -> [Co][tap][Ci]: a tap's input channels are contiguous, like the im2col rows
-        expect_shape(name.c_str(), shape, ndim, {C, C, 3, 3});
-        std::vector<float> packed((size_t)n);
-        for (int co = 0; co < C; ++co)
-            for (int ci = 0; ci < C; ++ci)
-                for (int tap = 0; tap < 9; ++tap)
-                    packed[((size_t)co * 9 + tap) * C + ci] = host[((size_t)co * C + ci) * 9 + tap];
-        q->upload.put(packed.data(), n, name == "conv2d2.weight" ? q->W2c : q->W3c, q->act, q->st);
-    }
-    else if (name == "conv2d2.bias") vec(q->c2b, C);
-    else if (name == "conv2d3.bias") vec(q->c3b, C);
-    else if (name == "conv_out.weight") {
-        // the reference flattens [C][F] (channel-major, causal.py:240-242); activations here are [F][C]
-        expect_shape(name.c_str(), shape, ndim, {d, (int64_t)C * F});
-        std::vector<float> packed((size_t)n);
-        for (int o = 0; o < d; ++o)
-            for (int c = 0; c < C; ++c)
-                for (int f = 0; f < F; ++f)
-                    packed[(size_t)o * C * F + (size_t)f * C + c] = host[(size_t)o * C * F + (size_t)c * F + f];
-        q->upload.put(packed.data(), n, q->Wout, q->act, q->st);
-    }
-    else if (name == "conv_out.bias") { WLK_CHECK(D.conv_out_bias, "this geometry has no conv_out bias"); vec(q->bout, d); }
-    else if (name == "positional_embedding.positional_embedding") {
-        expect_shape(name.c_str(), shape, ndim, {D.max_positions, d});
-        q->upload.put(host, n, q->pos_table, DT_F32, q->st);
-    }
-    else if (name == "positional_embedding.inv_freq") vec(q->pos_inv, d / 2);   // optional: the host's own frequencies
-    else if (name == "ln_post.weight") vec(q->lnpw, d);
-    else if (name == "ln_post.bias") vec(q->lnpb, d);
-    else if (name == "proj1.weight") mat(q->Wp1, d, d);
-    else if (name == "proj1.bias") vec(q->bp1, d);
-    else if (name == "proj2.weight") mat(q->Wp2, D.out_dim, d);
-    else if (name == "proj2.bias") vec(q->bp2, D.out_dim);
-    else if (name.rfind("layers.", 0) == 0) {
-        const size_t dot = name.find('.', 7);
-        WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
-        const int li = atoi(name.substr(7, dot - 7).c_str());
-        WLK_CHECK(li >= 0 && li < D.n_layer, "layer index out of range in %s", name.c_str());
-        const std::string rest = name.substr(dot + 1);
-        QLayerW& Lw = q->L[li];
-        const size_t es = q->es();
-        auto part = [&](int which, bool is_weight) {            // q / k / v rows of the fused projection
-            if (is_weight) { expect_shape(name.c_str(), shape, ndim, {d, d}); q->upload.put(host, n, (char*)Lw.Wqkv + (size_t)which * d * d * es, q->act, q->st); }
-            else { expect_shape(name.c_str(), shape, ndim, {d}); q->upload.put(host, n, Lw.bqkv + (size_t)which * d, DT_F32, q->st); }
-        };
-        if (rest == "self_attn.q_proj.weight") part(0, true);
-        else if (rest == "self_attn.k_proj.weight") part(1, true);
-        else if (rest == "self_attn.v_proj.weight") part(2, true);
-        else if (rest == "self_attn.q_proj.bias") part(0, false);
-        else if (rest == "self_attn.k_proj.bias") part(1, false);
-        else if (rest == "self_attn.v_proj.bias") part(2, false);
-        else if (rest == "self_attn.out_proj.weight") mat(Lw.Wo, d, d);
-        else if (rest == "self_attn.out_proj.bias") vec(Lw.bo, d);
-        else if (rest == "self_attn_layer_norm.weight") vec(Lw.ln1w, d);
-        else if (rest == "self_attn_layer_norm.bias") vec(Lw.ln1b, d);
-        else if (rest == "final_layer_norm.weight") vec(Lw.ln2w, d);
-        else if (rest == "final_layer_norm.bias") vec(Lw.ln2b, d);
-        else if (rest == "fc1.weight") mat(Lw.W1, ffn, d);
-        else if (rest == "fc1.bias") vec(Lw.b1, ffn);
-        else if (rest == "fc2.weight") mat(Lw.W2, d, ffn);
-        else if (rest == "fc2.bias") vec(Lw.b2, d);
-        else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    }
-    else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    q->loaded.insert(name);
-}
-
-std::vector<std::string> required(const wlk_qwen_dims& D) {
-    std::vector<std::string> r = {"conv2d1.weight", "conv2d1.bias", "conv2d2.weight", "conv2d2.bias", "conv2d3.weight",
-                                  "conv2d3.bias", "conv_out.weight", "positional_embedding.positional_embedding",
-                                  "ln_post.weight", "ln_post.bias", "proj1.weight", "proj1.bias", "proj2.weight", "proj2.bias"};
-    if (D.conv_out_bias) r.push_back("conv_out.bias");
-    for (int i = 0; i < D.n_layer; ++i) {
-        const std::string p = "layers." + std::to_string(i) + ".";
-        for (const char* s : {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.out_proj", "fc1", "fc2",
-                              "self_attn_layer_norm", "final_layer_norm"}) {
-            r.push_back(p + s + ".weight");
-            r.push_back(p + s + ".bias");
-        }
-    }
-    return r;
-}
-
-// the tower's weights (shared by the causal and the windowed engine) and the mel front end's constants
+// The tower's weights (shared by the causal and the windowed engine) and the mel front end's constants.  The positional
+// frequencies and the filterbank (only wlk_qwen_append_audio needs it) are optional.
 void alloc_weights(wlk_qwen* q) {
     const wlk_qwen_dims& D = q->dims;
-    const size_t es = q->es();
+    WeightTable& T = q->weights;
+    T.rule = WeightTable::EXACT;
+    T.wt = q->act;
     const int C = D.conv_channels, d = D.d_model, F = D.n_mels / 8, ffn = D.ffn_dim;
-    size_t* aw = &q->bytes_weights;
-    q->c1w = (float*)q->allocs.take((size_t)C * 9 * 4, aw); q->c1b = (float*)q->allocs.take(C * 4, aw);
-    q->c2b = (float*)q->allocs.take(C * 4, aw); q->c3b = (float*)q->allocs.take(C * 4, aw);
-    q->W2c = q->allocs.take((size_t)C * 9 * C * es, aw); q->W3c = q->allocs.take((size_t)C * 9 * C * es, aw);
-    q->Wout = q->allocs.take((size_t)d * C * F * es, aw); q->bout = (float*)q->allocs.take(d * 4, aw);
-    q->pos_table = (float*)q->allocs.take((size_t)D.max_positions * d * 4, aw);
-    q->pos_inv = (float*)q->allocs.take((size_t)(d / 2) * 4, aw);
-    q->lnpw = (float*)q->allocs.take(d * 4, aw); q->lnpb = (float*)q->allocs.take(d * 4, aw);
-    q->Wp1 = q->allocs.take((size_t)d * d * es, aw); q->bp1 = (float*)q->allocs.take(d * 4, aw);
-    q->Wp2 = q->allocs.take((size_t)D.out_dim * d * es, aw); q->bp2 = (float*)q->allocs.take(D.out_dim * 4, aw);
+    T.f32("conv2d1.weight", q->c1w, {C, 1, 3, 3});
+    T.f32("conv2d1.bias", q->c1b, {C});
+    T.mat("conv2d2.weight", q->W2c, {C, C, 3, 3}, swap_inner_axes(C, C, 9));
+    T.f32("conv2d2.bias", q->c2b, {C});
+    T.mat("conv2d3.weight", q->W3c, {C, C, 3, 3}, swap_inner_axes(C, C, 9));
+    T.f32("conv2d3.bias", q->c3b, {C});
+    // the reference flattens [C][F] (channel-major, causal.py:240-242)
+    T.mat("conv_out.weight", q->Wout, {d, (int64_t)C * F}, swap_inner_axes(d, C, F));
+    if (D.conv_out_bias) T.f32("conv_out.bias", q->bout, {d});
+    T.f32("positional_embedding.positional_embedding", q->pos_table, {D.max_positions, d});
+    T.f32("positional_embedding.inv_freq", q->pos_inv, {d / 2}).optional = true;
+    T.f32("ln_post.weight", q->lnpw, {d});
+    T.f32("ln_post.bias", q->lnpb, {d});
+    T.mat("proj1.weight", q->Wp1, {d, d});
+    T.f32("proj1.bias", q->bp1, {d});
+    T.mat("proj2.weight", q->Wp2, {D.out_dim, d});
+    T.f32("proj2.bias", q->bp2, {D.out_dim});
     q->L.resize(D.n_layer);
-    for (auto& Lw : q->L) {
-        Lw.Wqkv = q->allocs.take((size_t)3 * d * d * es, aw); Lw.bqkv = (float*)q->allocs.take(3 * d * 4, aw);
-        Lw.Wo = q->allocs.take((size_t)d * d * es, aw); Lw.bo = (float*)q->allocs.take(d * 4, aw);
-        Lw.W1 = q->allocs.take((size_t)ffn * d * es, aw); Lw.b1 = (float*)q->allocs.take(ffn * 4, aw);
-        Lw.W2 = q->allocs.take((size_t)d * ffn * es, aw); Lw.b2 = (float*)q->allocs.take(d * 4, aw);
-        Lw.ln1w = (float*)q->allocs.take(d * 4, aw); Lw.ln1b = (float*)q->allocs.take(d * 4, aw);
-        Lw.ln2w = (float*)q->allocs.take(d * 4, aw); Lw.ln2b = (float*)q->allocs.take(d * 4, aw);
+    for (int i = 0; i < D.n_layer; ++i) {
+        const std::string p = "layers." + std::to_string(i) + ".";
+        QLayerW& Lw = q->L[i];
+        const std::string a = p + "self_attn.";
+        T.fused(Lw.Wqkv, q->act, {{a + "q_proj.weight", d}, {a + "k_proj.weight", d}, {a + "v_proj.weight", d}}, d);
+        T.fused(Lw.bqkv, DT_F32, {{a + "q_proj.bias", d}, {a + "k_proj.bias", d}, {a + "v_proj.bias", d}}, 0);
+        T.mat(a + "out_proj.weight", Lw.Wo, {d, d});
+        T.f32(a + "out_proj.bias", Lw.bo, {d});
+        T.mat(p + "fc1.weight", Lw.W1, {ffn, d});
+        T.f32(p + "fc1.bias", Lw.b1, {ffn});
+        T.mat(p + "fc2.weight", Lw.W2, {d, ffn});
+        T.f32(p + "fc2.bias", Lw.b2, {d});
+        T.f32(p + "self_attn_layer_norm.weight", Lw.ln1w, {d});
+        T.f32(p + "self_attn_layer_norm.bias", Lw.ln1b, {d});
+        T.f32(p + "final_layer_norm.weight", Lw.ln2w, {d});
+        T.f32(p + "final_layer_norm.bias", Lw.ln2b, {d});
     }
-    q->filtT = (float*)q->allocs.take((size_t)N_FREQ * D.n_mels * 4, aw);
-    q->window = (float*)q->allocs.take(N_FFT * 4, aw);
-    q->twiddle = (float2*)q->allocs.take(N_FFT * 8, aw);
-    q->filt_span = (int2*)q->allocs.take((size_t)D.n_mels * 8, aw);
+    T.buf(q->filtT, (size_t)N_FREQ * D.n_mels * 4);
+    T.buf(q->window, N_FFT * 4);
+    T.buf(q->twiddle, N_FFT * 8);
+    T.buf(q->filt_span, (size_t)D.n_mels * 8);
+    declare_mel_filters(T, q->filtT, q->filt_span, D.n_mels, N_FREQ).optional = true;
+    T.allocate(q->allocs, &q->bytes_weights);
     {   // periodic Hann window and DFT twiddles exp(-2 pi i t / 400), evaluated in double
         std::vector<float> win(N_FFT);
         std::vector<float2> tw(N_FFT);
@@ -749,7 +658,7 @@ void forward_chunk(wlk_qwen* q, const int32_t* sids, int n, const float* mels, c
 void append_audio(wlk_qwen* q, const int32_t* sids, int n, const float* pcm, const int64_t* sample_off, float* out,
                   int64_t cap_frames, int32_t* frame_off, bool flush) {
     const wlk_qwen_dims& D = q->dims;
-    WLK_CHECK(q->have_filters, "load the \"mel_filters\" tensor [n_mels][201] before appending audio");
+    WLK_CHECK(q->weights.loaded.count("mel_filters"), "load the \"mel_filters\" tensor [n_mels][201] before appending audio");
     WLK_CHECK(n >= 1 && n <= q->cfg.max_batch, "batch %d outside [1, %d]", n, q->cfg.max_batch);
     struct Plan { int first, last, frames; };
     std::vector<Plan> plan(n, Plan{0, 0, 0});
@@ -1323,7 +1232,7 @@ void window_encode(wlk_qwen* q, int n, const float* mels, const int32_t* frame_o
 // ---- op-level entry points (kernel tests): one production launch on caller-owned device buffers, with the engine's
 //      dims, precision and GEMM backend, on its stream, synchronized before returning ---------------------------------
 void op_require(const wlk_qwen* q, std::initializer_list<std::string> names) {
-    for (const std::string& n : names) WLK_CHECK(q->loaded.count(n), "tensor %s is not loaded", n.c_str());
+    for (const std::string& n : names) WLK_CHECK(q->weights.loaded.count(n), "tensor %s is not loaded", n.c_str());
 }
 
 void op_positions(wlk_qwen* q, const int32_t* pos, int rows, float* out) {
@@ -1437,13 +1346,13 @@ int wlk_qwen_load_tensor(wlk_qwen* q, const char* name, const float* host, const
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
-    load_tensor(q, name, host, shape, ndim);
+    q->weights.load(name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_qwen_finalize_weights(wlk_qwen* q) {
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
-    require_loaded(q->loaded, required(q->dims));
+    q->weights.require_all();
     q->upload.release();
     q->finalized = true;
     WLK_API_END

@@ -464,62 +464,6 @@ namespace {
 // bf16 runs every GEMM on the wgmma kernels (cfg->gemm_backend is not consulted); a shape they do not take is an error
 void tgemm(wlk_qtext* t, GemmArgs& g) { t->gemm.run(g, t->act == DT_BF16, t->st, t->num_sms, "text decoder"); }
 
-void load_tensor(wlk_qtext* t, const std::string& name, const float* host, const int64_t* shape, int ndim) {
-    const wlk_qtext_dims& D = t->dims;
-    const int d = D.d_model, F = D.ffn_dim, qd = D.n_head * QT_HD, kvd = D.n_kv_head * QT_HD;
-    const int64_t n = numel(shape, ndim);
-    const size_t es = t->es();
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect_shape(name.c_str(), shape, ndim, {rows, cols}); t->upload.put(host, n, dst, t->act, t->st); };
-    auto vec = [&](float* dst, int64_t len) { expect_shape(name.c_str(), shape, ndim, {len}); t->upload.put(host, n, dst, DT_F32, t->st); };
-    if (name == "embed_tokens.weight") {
-        expect_shape(name.c_str(), shape, ndim, {D.vocab, d});
-        t->upload.put(host, n, t->emb, DT_F32, t->st);
-        if (D.tied) t->upload.put(host, n, t->head, t->act, t->st);
-    }
-    else if (name == "lm_head.weight") { WLK_CHECK(!D.tied, "this geometry ties lm_head to embed_tokens"); mat(t->head, D.vocab, d); }
-    else if (name == "norm.weight") vec(t->normw, d);
-    else if (name == "rotary_emb.inv_freq") vec(t->inv_freq, QT_HD / 2);     // optional: the host's own RoPE frequencies
-    else if (name.rfind("adapter.", 0) == 0) {                                   // optional: the frame adapter, packed by finalize
-        WLK_CHECK(!t->finalized, "adapter tensor %s loaded after finalize", name.c_str());
-        t->adapter_stash[name] = {std::vector<int64_t>(shape, shape + ndim), std::vector<float>(host, host + n)};
-    }
-    else if (name.rfind("layers.", 0) == 0) {
-        const size_t dot = name.find('.', 7);
-        WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
-        const int li = atoi(name.substr(7, dot - 7).c_str());
-        WLK_CHECK(li >= 0 && li < D.n_layer, "layer index out of range in %s", name.c_str());
-        const std::string rest = name.substr(dot + 1);
-        QTLayerW& Lw = t->L[li];
-        if (rest == "self_attn.q_proj.weight") { expect_shape(name.c_str(), shape, ndim, {qd, d}); t->upload.put(host, n, Lw.Wqkv, t->act, t->st); }
-        else if (rest == "self_attn.k_proj.weight") { expect_shape(name.c_str(), shape, ndim, {kvd, d}); t->upload.put(host, n, (char*)Lw.Wqkv + (size_t)qd * d * es, t->act, t->st); }
-        else if (rest == "self_attn.v_proj.weight") { expect_shape(name.c_str(), shape, ndim, {kvd, d}); t->upload.put(host, n, (char*)Lw.Wqkv + (size_t)(qd + kvd) * d * es, t->act, t->st); }
-        else if (rest == "self_attn.o_proj.weight") mat(Lw.Wo, d, qd);
-        else if (rest == "self_attn.q_norm.weight") vec(Lw.qn, QT_HD);
-        else if (rest == "self_attn.k_norm.weight") vec(Lw.kn, QT_HD);
-        else if (rest == "mlp.gate_proj.weight") { expect_shape(name.c_str(), shape, ndim, {F, d}); t->upload.put(host, n, Lw.Wgu, t->act, t->st); }
-        else if (rest == "mlp.up_proj.weight") { expect_shape(name.c_str(), shape, ndim, {F, d}); t->upload.put(host, n, (char*)Lw.Wgu + (size_t)F * d * es, t->act, t->st); }
-        else if (rest == "mlp.down_proj.weight") mat(Lw.Wd, d, F);
-        else if (rest == "input_layernorm.weight") vec(Lw.ln1, d);
-        else if (rest == "post_attention_layernorm.weight") vec(Lw.ln2, d);
-        else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    }
-    else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    t->loaded.insert(name);
-}
-
-std::vector<std::string> required(const wlk_qtext_dims& D) {
-    std::vector<std::string> r = {"embed_tokens.weight", "norm.weight"};
-    if (!D.tied) r.push_back("lm_head.weight");
-    for (int i = 0; i < D.n_layer; ++i) {
-        const std::string p = "layers." + std::to_string(i) + ".";
-        for (const char* s : {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "self_attn.q_norm",
-                              "self_attn.k_norm", "mlp.gate_proj", "mlp.up_proj", "mlp.down_proj", "input_layernorm",
-                              "post_attention_layernorm"})
-            r.push_back(p + s + ".weight");
-    }
-    return r;
-}
-
 // Pack the stashed adapter tensors (no-op when none were loaded).
 void build_adapter(wlk_qtext* t) {
     auto& st = t->adapter_stash;
@@ -602,20 +546,34 @@ void create(const wlk_qtext_dims* dims, const wlk_config* cfg, wlk_qtext** out) 
     const size_t es = t->es();
     const int d = D.d_model, F = D.ffn_dim, H = D.n_head, KV = D.n_kv_head;
     const size_t W = (size_t)(H + 2 * KV) * QT_HD;
-    size_t* aw = &t->bytes_weights;
-    t->emb = (float*)t->allocs.take((size_t)D.vocab * d * 4, aw);
-    t->head = t->allocs.take((size_t)D.vocab * d * es, aw);
-    t->normw = (float*)t->allocs.take((size_t)d * 4, aw);
-    t->inv_freq = (float*)t->allocs.take(QT_HD / 2 * 4, aw);
-    t->L.resize(D.n_layer);
-    for (auto& Lw : t->L) {
-        Lw.Wqkv = t->allocs.take(W * d * es, aw);
-        Lw.Wo = t->allocs.take((size_t)d * H * QT_HD * es, aw);
-        Lw.Wgu = t->allocs.take((size_t)2 * F * d * es, aw);
-        Lw.Wd = t->allocs.take((size_t)d * F * es, aw);
-        Lw.qn = (float*)t->allocs.take(QT_HD * 4, aw); Lw.kn = (float*)t->allocs.take(QT_HD * 4, aw);
-        Lw.ln1 = (float*)t->allocs.take((size_t)d * 4, aw); Lw.ln2 = (float*)t->allocs.take((size_t)d * 4, aw);
+    WeightTable& T = t->weights;
+    T.rule = WeightTable::EXACT;
+    T.wt = t->act;
+    // the fp32 embedding rows, and lm_head in the activation type: a copy of the embedding table when tied
+    WeightTable::Entry& emb = T.f32("embed_tokens.weight", t->emb, {D.vocab, d});
+    if (D.tied) {
+        T.buf(t->head, (size_t)D.vocab * d * es);
+        emb.dst.push_back(WeightTable::Dst(t->head, 0, t->act));
+    } else {
+        T.mat("lm_head.weight", t->head, {D.vocab, d});
     }
+    T.f32("norm.weight", t->normw, {d});
+    T.f32("rotary_emb.inv_freq", t->inv_freq, {QT_HD / 2}).optional = true;   // the host's own RoPE frequencies
+    t->L.resize(D.n_layer);
+    for (int i = 0; i < D.n_layer; ++i) {
+        const std::string p = "layers." + std::to_string(i) + ".";
+        QTLayerW& Lw = t->L[i];
+        const std::string a = p + "self_attn.", m = p + "mlp.";
+        T.fused(Lw.Wqkv, t->act, {{a + "q_proj.weight", H * QT_HD}, {a + "k_proj.weight", KV * QT_HD}, {a + "v_proj.weight", KV * QT_HD}}, d);
+        T.mat(a + "o_proj.weight", Lw.Wo, {d, H * QT_HD});
+        T.fused(Lw.Wgu, t->act, {{m + "gate_proj.weight", F}, {m + "up_proj.weight", F}}, d);
+        T.mat(m + "down_proj.weight", Lw.Wd, {d, F});
+        T.f32(a + "q_norm.weight", Lw.qn, {QT_HD});
+        T.f32(a + "k_norm.weight", Lw.kn, {QT_HD});
+        T.f32(p + "input_layernorm.weight", Lw.ln1, {d});
+        T.f32(p + "post_attention_layernorm.weight", Lw.ln2, {d});
+    }
+    T.allocate(t->allocs, &t->bytes_weights);
     {   // default inv_freq = 1 / theta^(2i / 128) in fp32 arithmetic like HF's default rope init (fp32 exponent, pow, then
         // 1 / x); libm's powf can still land one ulp away from torch's pow in a few entries, so hosts load
         // "rotary_emb.inv_freq" (whisperlivekit_b200/qwen_text_engine.py always does)
@@ -1268,13 +1226,18 @@ int wlk_qtext_load_tensor(wlk_qtext* t, const char* name, const float* host, con
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
-    load_tensor(t, name, host, shape, ndim);
+    if (std::string(name).rfind("adapter.", 0) == 0) {       // optional: the frame adapter, packed by finalize
+        WLK_CHECK(!t->finalized, "adapter tensor %s loaded after finalize", name);
+        t->adapter_stash[name] = {std::vector<int64_t>(shape, shape + ndim), std::vector<float>(host, host + numel(shape, ndim))};
+    } else {
+        t->weights.load(name, host, shape, ndim);
+    }
     WLK_API_END
 }
 int wlk_qtext_finalize_weights(wlk_qtext* t) {
     WLK_API_BEGIN
     WLK_ENTER(t, t->cfg.device);
-    require_loaded(t->loaded, required(t->dims));
+    t->weights.require_all();
     build_adapter(t);
     t->upload.release();
     t->finalized = true;

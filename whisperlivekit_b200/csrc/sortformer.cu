@@ -723,159 +723,11 @@ void gemm(wlk_sf* q, const void* A, int64_t lda, const void* W, int64_t ldw, int
     q->gemm.run(g, q->gemm_backend == WLK_BACKEND_TCGEN05, q->st, q->num_sms);
 }
 
-void expect(const std::string& name, const int64_t* shape, int ndim, std::initializer_list<int64_t> want) {
-    int64_t nw = 1, ns = numel(shape, ndim);
-    for (int64_t w : want) nw *= w;
-    // trailing singleton axes (Conv1d / Conv2d kernels of size 1) are accepted either way: the element count and the
-    // leading axis pin the layout
-    WLK_CHECK(ns == nw && shape[0] == *want.begin(), "tensor %s has the wrong shape for this geometry", name.c_str());
-}
-
 int sub_len(int t) { for (int i = 0; i < 3; ++i) t = (t + 2 - 3) / 2 + 1; return t; }
-
-void load_tensor(wlk_sf* q, const std::string& name, const float* host, const int64_t* shape, int ndim) {
-    const wlk_sf_dims& D = q->dims;
-    const int C = D.conv_channels, d = D.d_model, t = D.tf_d_model, ff = D.ff_mult * D.d_model, K = D.conv_kernel;
-    const int64_t n = numel(shape, ndim);
-    auto mat = [&](void* dst, int64_t rows, int64_t cols) { expect(name, shape, ndim, {rows, cols}); q->upload.put(host, n, dst, q->act, q->st); };
-    auto vec = [&](float* dst, int64_t len) { expect(name, shape, ndim, {len}); q->upload.put(host, n, dst, DT_F32, q->st); };
-    const std::string pe = "encoder.pre_encode.";
-    if (name == "mel_filters") {                    // [n_mels][n_freq] Slaney bank (librosa.filters.mel, as NeMo builds it)
-        expect(name, shape, ndim, {D.n_mels, q->n_freq});
-        std::vector<float> tr((size_t)n);
-        std::vector<int2> span(D.n_mels);
-        for (int m = 0; m < D.n_mels; ++m) {
-            int lo = q->n_freq, hi = 0;
-            for (int k = 0; k < q->n_freq; ++k) {
-                const float v = host[(size_t)m * q->n_freq + k];
-                tr[(size_t)k * D.n_mels + m] = v;
-                if (v != 0.f) { if (k < lo) lo = k; hi = k + 1; }
-            }
-            if (lo >= hi) { lo = 0; hi = 0; }
-            span[m] = make_int2(lo, hi);
-        }
-        q->upload.put(tr.data(), n, q->fbT, DT_F32, q->st);
-        CUDA_CHECK(cudaMemcpyAsync(q->span, span.data(), span.size() * 8, cudaMemcpyHostToDevice, q->st));
-        CUDA_CHECK(cudaStreamSynchronize(q->st));
-    }
-    else if (name == pe + "conv.0.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->c0w, DT_F32, q->st); }
-    else if (name == pe + "conv.0.bias") vec(q->c0b, C);
-    else if (name == pe + "conv.2.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->dw1w, DT_F32, q->st); }
-    else if (name == pe + "conv.2.bias") vec(q->dw1b, C);
-    else if (name == pe + "conv.3.weight") mat(q->Wpw1, C, C);
-    else if (name == pe + "conv.3.bias") vec(q->pw1b, C);
-    else if (name == pe + "conv.5.weight") { expect(name, shape, ndim, {C, 9}); q->upload.put(host, n, q->dw2w, DT_F32, q->st); }
-    else if (name == pe + "conv.5.bias") vec(q->dw2b, C);
-    else if (name == pe + "conv.6.weight") mat(q->Wpw2, C, C);
-    else if (name == pe + "conv.6.bias") vec(q->pw2b, C);
-    else if (name == pe + "out.weight") {
-        // NeMo flattens [C][F] channel-major (x.transpose(1, 2).reshape(b, t, -1)); activations here are [F][C]
-        const int F = q->F3;
-        expect(name, shape, ndim, {d, (int64_t)C * F});
-        std::vector<float> packed((size_t)n);
-        for (int o = 0; o < d; ++o)
-            for (int c = 0; c < C; ++c)
-                for (int f = 0; f < F; ++f)
-                    packed[(size_t)o * C * F + (size_t)f * C + c] = host[(size_t)o * C * F + (size_t)c * F + f];
-        q->upload.put(packed.data(), n, q->Wout, q->act, q->st);
-    }
-    else if (name == pe + "out.bias") vec(q->outb, d);
-    else if (name.rfind("encoder.layers.", 0) == 0) {
-        const size_t dot = name.find('.', 15);
-        WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
-        const int li = atoi(name.substr(15, dot - 15).c_str());
-        WLK_CHECK(li >= 0 && li < D.n_layer, "layer index out of range in %s", name.c_str());
-        const std::string r = name.substr(dot + 1);
-        SfLayerW& L = q->L[li];
-        const size_t es = q->es();
-        auto part = [&](int which, bool w) {
-            if (w) { expect(name, shape, ndim, {d, d}); q->upload.put(host, n, (char*)L.Wqkv + (size_t)which * d * d * es, q->act, q->st); }
-            else { expect(name, shape, ndim, {d}); q->upload.put(host, n, L.bqkv + (size_t)which * d, DT_F32, q->st); }
-        };
-        if (r == "norm_feed_forward1.weight") vec(L.ln_ff1w, d); else if (r == "norm_feed_forward1.bias") vec(L.ln_ff1b, d);
-        else if (r == "feed_forward1.linear1.weight") mat(L.W_ff1a, ff, d); else if (r == "feed_forward1.linear1.bias") vec(L.b_ff1a, ff);
-        else if (r == "feed_forward1.linear2.weight") mat(L.W_ff1b, d, ff); else if (r == "feed_forward1.linear2.bias") vec(L.b_ff1b, d);
-        else if (r == "norm_self_att.weight") vec(L.ln_attw, d); else if (r == "norm_self_att.bias") vec(L.ln_attb, d);
-        else if (r == "self_attn.linear_q.weight") part(0, true); else if (r == "self_attn.linear_q.bias") part(0, false);
-        else if (r == "self_attn.linear_k.weight") part(1, true); else if (r == "self_attn.linear_k.bias") part(1, false);
-        else if (r == "self_attn.linear_v.weight") part(2, true); else if (r == "self_attn.linear_v.bias") part(2, false);
-        else if (r == "self_attn.linear_out.weight") mat(L.Wo, d, d); else if (r == "self_attn.linear_out.bias") vec(L.bo, d);
-        else if (r == "self_attn.linear_pos.weight") mat(L.Wpos, d, d);
-        else if (r == "self_attn.pos_bias_u") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); q->upload.put(host, n, L.bias_u, DT_F32, q->st); }
-        else if (r == "self_attn.pos_bias_v") { expect(name, shape, ndim, {D.n_head, d / D.n_head}); q->upload.put(host, n, L.bias_v, DT_F32, q->st); }
-        else if (r == "norm_conv.weight") vec(L.ln_convw, d); else if (r == "norm_conv.bias") vec(L.ln_convb, d);
-        else if (r == "conv.pointwise_conv1.weight") mat(L.Wpw1, 2 * d, d); else if (r == "conv.pointwise_conv1.bias") vec(L.bpw1, 2 * d);
-        else if (r == "conv.depthwise_conv.weight") { expect(name, shape, ndim, {d, K}); q->upload.put(host, n, L.dw_w, DT_F32, q->st); }
-        else if (r == "conv.depthwise_conv.bias") vec(L.dw_b, d);
-        else if (r == "conv.batch_norm.weight") vec(L.bn_w, d); else if (r == "conv.batch_norm.bias") vec(L.bn_b, d);
-        else if (r == "conv.batch_norm.running_mean") vec(L.bn_mean, d); else if (r == "conv.batch_norm.running_var") vec(L.bn_var, d);
-        else if (r == "conv.batch_norm.num_batches_tracked") { /* bookkeeping scalar of nn.BatchNorm1d */ }
-        else if (r == "conv.pointwise_conv2.weight") mat(L.Wpw2, d, d); else if (r == "conv.pointwise_conv2.bias") vec(L.bpw2, d);
-        else if (r == "norm_feed_forward2.weight") vec(L.ln_ff2w, d); else if (r == "norm_feed_forward2.bias") vec(L.ln_ff2b, d);
-        else if (r == "feed_forward2.linear1.weight") mat(L.W_ff2a, ff, d); else if (r == "feed_forward2.linear1.bias") vec(L.b_ff2a, ff);
-        else if (r == "feed_forward2.linear2.weight") mat(L.W_ff2b, d, ff); else if (r == "feed_forward2.linear2.bias") vec(L.b_ff2b, d);
-        else if (r == "norm_out.weight") vec(L.ln_outw, d); else if (r == "norm_out.bias") vec(L.ln_outb, d);
-        else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    }
-    else if (name.rfind("transformer_encoder.layers.", 0) == 0) {
-        const size_t dot = name.find('.', 27);
-        WLK_CHECK(dot != std::string::npos, "unknown tensor %s", name.c_str());
-        const int li = atoi(name.substr(27, dot - 27).c_str());
-        WLK_CHECK(li >= 0 && li < D.tf_n_layer, "layer index out of range in %s", name.c_str());
-        const std::string r = name.substr(dot + 1);
-        SfTLayerW& L = q->TL[li];
-        const size_t es = q->es();
-        auto part = [&](int which, bool w) {
-            if (w) { expect(name, shape, ndim, {t, t}); q->upload.put(host, n, (char*)L.Wqkv + (size_t)which * t * t * es, q->act, q->st); }
-            else { expect(name, shape, ndim, {t}); q->upload.put(host, n, L.bqkv + (size_t)which * t, DT_F32, q->st); }
-        };
-        if (r == "first_sub_layer.query_net.weight") part(0, true); else if (r == "first_sub_layer.query_net.bias") part(0, false);
-        else if (r == "first_sub_layer.key_net.weight") part(1, true); else if (r == "first_sub_layer.key_net.bias") part(1, false);
-        else if (r == "first_sub_layer.value_net.weight") part(2, true); else if (r == "first_sub_layer.value_net.bias") part(2, false);
-        else if (r == "first_sub_layer.out_projection.weight") mat(L.Wo, t, t); else if (r == "first_sub_layer.out_projection.bias") vec(L.bo, t);
-        else if (r == "layer_norm_1.weight") vec(L.ln1w, t); else if (r == "layer_norm_1.bias") vec(L.ln1b, t);
-        else if (r == "second_sub_layer.dense_in.weight") mat(L.W1, D.tf_inner, t); else if (r == "second_sub_layer.dense_in.bias") vec(L.b1, D.tf_inner);
-        else if (r == "second_sub_layer.dense_out.weight") mat(L.W2, t, D.tf_inner); else if (r == "second_sub_layer.dense_out.bias") vec(L.b2, t);
-        else if (r == "layer_norm_2.weight") vec(L.ln2w, t); else if (r == "layer_norm_2.bias") vec(L.ln2b, t);
-        else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    }
-    else if (name == "sortformer_modules.encoder_proj.weight") mat(q->Wproj, t, d);
-    else if (name == "sortformer_modules.encoder_proj.bias") vec(q->bproj, t);
-    else if (name == "sortformer_modules.first_hidden_to_hidden.weight") mat(q->Wh, t, t);
-    else if (name == "sortformer_modules.first_hidden_to_hidden.bias") vec(q->bh, t);
-    else if (name == "sortformer_modules.single_hidden_to_spks.weight") { expect(name, shape, ndim, {D.n_spk, t}); q->upload.put(host, n, q->Wspk, DT_F32, q->st); }
-    else if (name == "sortformer_modules.single_hidden_to_spks.bias") vec(q->bspk, D.n_spk);
-    else WLK_CHECK(false, "unknown tensor %s", name.c_str());
-    q->loaded.insert(name);
-}
-
-std::vector<std::string> required(const wlk_sf_dims& D) {
-    std::vector<std::string> r = {"mel_filters"};
-    const std::string pe = "encoder.pre_encode.";
-    for (const char* s : {"conv.0", "conv.2", "conv.3", "conv.5", "conv.6", "out"}) { r.push_back(pe + s + ".weight"); r.push_back(pe + s + ".bias"); }
-    for (int i = 0; i < D.n_layer; ++i) {
-        const std::string p = "encoder.layers." + std::to_string(i) + ".";
-        for (const char* s : {"norm_feed_forward1", "feed_forward1.linear1", "feed_forward1.linear2", "norm_self_att", "self_attn.linear_q",
-                              "self_attn.linear_k", "self_attn.linear_v", "self_attn.linear_out", "norm_conv", "conv.pointwise_conv1",
-                              "conv.depthwise_conv", "conv.batch_norm", "conv.pointwise_conv2", "norm_feed_forward2", "feed_forward2.linear1",
-                              "feed_forward2.linear2", "norm_out"}) { r.push_back(p + s + ".weight"); r.push_back(p + s + ".bias"); }
-        for (const char* s : {"self_attn.linear_pos.weight", "self_attn.pos_bias_u", "self_attn.pos_bias_v", "conv.batch_norm.running_mean",
-                              "conv.batch_norm.running_var"}) r.push_back(p + s);
-    }
-    for (int i = 0; i < D.tf_n_layer; ++i) {
-        const std::string p = "transformer_encoder.layers." + std::to_string(i) + ".";
-        for (const char* s : {"first_sub_layer.query_net", "first_sub_layer.key_net", "first_sub_layer.value_net", "first_sub_layer.out_projection",
-                              "layer_norm_1", "second_sub_layer.dense_in", "second_sub_layer.dense_out", "layer_norm_2"}) {
-            r.push_back(p + s + ".weight"); r.push_back(p + s + ".bias"); }
-    }
-    for (const char* s : {"sortformer_modules.encoder_proj", "sortformer_modules.first_hidden_to_hidden", "sortformer_modules.single_hidden_to_spks"}) {
-        r.push_back(std::string(s) + ".weight"); r.push_back(std::string(s) + ".bias"); }
-    return r;
-}
 
 void finalize(wlk_sf* q) {
     const wlk_sf_dims& D = q->dims;
-    require_loaded(q->loaded, required(D));
+    q->weights.require_all();
     const int d = D.d_model, P = 2 * SF_MAX_T - 1;
     // RelPositionalEncoding rows for relative positions SF_MAX_T-1 ... -(SF_MAX_T-1); a row depends on its relative
     // position only, so one table serves every sequence length.  linear_pos of it is a constant per layer.
@@ -945,37 +797,94 @@ void create(const wlk_sf_dims* dims, const wlk_config* cfg, wlk_sf** out) {
         q->max_pop = mp; }
     const size_t es = q->es();
     const int C = D.conv_channels, d = D.d_model, t = D.tf_d_model, ff = D.ff_mult * d, K = D.conv_kernel, S = D.n_spk;
-    size_t* aw = &q->bytes_weights;
-    auto fv = [&](size_t n) { return (float*)q->allocs.take(n * 4, aw); };
-    q->window = fv(D.win_length); q->twiddle = (float2*)q->allocs.take((size_t)D.n_fft * 8, aw);
-    q->fbT = fv((size_t)q->n_freq * D.n_mels); q->span = (int2*)q->allocs.take((size_t)D.n_mels * 8, aw);
-    q->c0w = fv((size_t)C * 9); q->c0b = fv(C); q->dw1w = fv((size_t)C * 9); q->dw1b = fv(C); q->dw2w = fv((size_t)C * 9); q->dw2b = fv(C);
-    q->pw1b = fv(C); q->pw2b = fv(C); q->outb = fv(d);
-    q->Wpw1 = q->allocs.take((size_t)C * C * es, aw); q->Wpw2 = q->allocs.take((size_t)C * C * es, aw);
-    q->Wout = q->allocs.take((size_t)d * C * q->F3 * es, aw);
-    q->pe_table = fv((size_t)(2 * SF_MAX_T - 1) * d);
+    WeightTable& T = q->weights;
+    T.rule = WeightTable::LEADING;
+    T.wt = q->act;
+    const int F = q->F3, P = 2 * SF_MAX_T - 1;
+    T.buf(q->window, (size_t)D.win_length * 4);
+    T.buf(q->twiddle, (size_t)D.n_fft * 8);
+    T.buf(q->fbT, (size_t)q->n_freq * D.n_mels * 4);
+    T.buf(q->span, (size_t)D.n_mels * 8);
+    declare_mel_filters(T, q->fbT, q->span, D.n_mels, q->n_freq);    // the Slaney bank of librosa.filters.mel, as NeMo builds it
+    const std::string pe = "encoder.pre_encode.";
+    T.f32(pe + "conv.0.weight", q->c0w, {C, 9});
+    T.f32(pe + "conv.0.bias", q->c0b, {C});
+    T.f32(pe + "conv.2.weight", q->dw1w, {C, 9});
+    T.f32(pe + "conv.2.bias", q->dw1b, {C});
+    T.mat(pe + "conv.3.weight", q->Wpw1, {C, C});
+    T.f32(pe + "conv.3.bias", q->pw1b, {C});
+    T.f32(pe + "conv.5.weight", q->dw2w, {C, 9});
+    T.f32(pe + "conv.5.bias", q->dw2b, {C});
+    T.mat(pe + "conv.6.weight", q->Wpw2, {C, C});
+    T.f32(pe + "conv.6.bias", q->pw2b, {C});
+    // NeMo flattens [C][F] channel-major (x.transpose(1, 2).reshape(b, t, -1))
+    T.mat(pe + "out.weight", q->Wout, {d, (int64_t)C * F}, swap_inner_axes(d, C, F));
+    T.f32(pe + "out.bias", q->outb, {d});
+    T.buf(q->pe_table, (size_t)P * d * 4);
     q->L.resize(D.n_layer);
-    for (auto& L : q->L) {
-        L.W_ff1a = q->allocs.take((size_t)ff * d * es, aw); L.W_ff1b = q->allocs.take((size_t)ff * d * es, aw);
-        L.W_ff2a = q->allocs.take((size_t)ff * d * es, aw); L.W_ff2b = q->allocs.take((size_t)ff * d * es, aw);
-        L.Wqkv = q->allocs.take((size_t)3 * d * d * es, aw); L.Wo = q->allocs.take((size_t)d * d * es, aw); L.Wpos = q->allocs.take((size_t)d * d * es, aw);
-        L.Wpw1 = q->allocs.take((size_t)2 * d * d * es, aw); L.Wpw2 = q->allocs.take((size_t)d * d * es, aw);
-        L.b_ff1a = fv(ff); L.b_ff1b = fv(d); L.b_ff2a = fv(ff); L.b_ff2b = fv(d); L.bqkv = fv(3 * d); L.bo = fv(d); L.bpw1 = fv(2 * d); L.bpw2 = fv(d);
-        L.ln_ff1w = fv(d); L.ln_ff1b = fv(d); L.ln_attw = fv(d); L.ln_attb = fv(d); L.ln_convw = fv(d); L.ln_convb = fv(d);
-        L.ln_ff2w = fv(d); L.ln_ff2b = fv(d); L.ln_outw = fv(d); L.ln_outb = fv(d);
-        L.bias_u = fv(d); L.bias_v = fv(d); L.dw_w = fv((size_t)d * K); L.dw_b = fv(d);
-        L.bn_w = fv(d); L.bn_b = fv(d); L.bn_mean = fv(d); L.bn_var = fv(d); L.bnA = fv(d); L.bnB = fv(d);
-        L.ptab = q->allocs.take((size_t)(2 * SF_MAX_T - 1) * d * es, aw);
+    for (int i = 0; i < D.n_layer; ++i) {
+        const std::string p = "encoder.layers." + std::to_string(i) + ".", a = p + "self_attn.", c = p + "conv.";
+        SfLayerW& L = q->L[i];
+        auto linear = [&](const std::string& n, void*& W, float*& b, int64_t rows, int64_t cols) {
+            T.mat(n + ".weight", W, {rows, cols});
+            T.f32(n + ".bias", b, {rows});
+        };
+        auto norm = [&](const std::string& n, float*& w, float*& b) {
+            T.f32(n + ".weight", w, {d});
+            T.f32(n + ".bias", b, {d});
+        };
+        norm(p + "norm_feed_forward1", L.ln_ff1w, L.ln_ff1b);
+        linear(p + "feed_forward1.linear1", L.W_ff1a, L.b_ff1a, ff, d);
+        linear(p + "feed_forward1.linear2", L.W_ff1b, L.b_ff1b, d, ff);
+        norm(p + "norm_self_att", L.ln_attw, L.ln_attb);
+        T.fused(L.Wqkv, q->act, {{a + "linear_q.weight", d}, {a + "linear_k.weight", d}, {a + "linear_v.weight", d}}, d);
+        T.fused(L.bqkv, DT_F32, {{a + "linear_q.bias", d}, {a + "linear_k.bias", d}, {a + "linear_v.bias", d}}, 0);
+        linear(a + "linear_out", L.Wo, L.bo, d, d);
+        T.mat(a + "linear_pos.weight", L.Wpos, {d, d});
+        T.f32(a + "pos_bias_u", L.bias_u, {D.n_head, d / D.n_head});
+        T.f32(a + "pos_bias_v", L.bias_v, {D.n_head, d / D.n_head});
+        norm(p + "norm_conv", L.ln_convw, L.ln_convb);
+        linear(c + "pointwise_conv1", L.Wpw1, L.bpw1, 2 * d, d);
+        T.f32(c + "depthwise_conv.weight", L.dw_w, {d, K});
+        T.f32(c + "depthwise_conv.bias", L.dw_b, {d});
+        norm(c + "batch_norm", L.bn_w, L.bn_b);
+        T.f32(c + "batch_norm.running_mean", L.bn_mean, {d});
+        T.f32(c + "batch_norm.running_var", L.bn_var, {d});
+        T.add(c + "batch_norm.num_batches_tracked", {}, {}).optional = true;   // bookkeeping scalar of nn.BatchNorm1d
+        linear(c + "pointwise_conv2", L.Wpw2, L.bpw2, d, d);
+        norm(p + "norm_feed_forward2", L.ln_ff2w, L.ln_ff2b);
+        linear(p + "feed_forward2.linear1", L.W_ff2a, L.b_ff2a, ff, d);
+        linear(p + "feed_forward2.linear2", L.W_ff2b, L.b_ff2b, d, ff);
+        norm(p + "norm_out", L.ln_outw, L.ln_outb);
+        T.buf(L.bnA, (size_t)d * 4);
+        T.buf(L.bnB, (size_t)d * 4);
+        T.buf(L.ptab, (size_t)P * d * es);
     }
     q->TL.resize(D.tf_n_layer);
-    for (auto& L : q->TL) {
-        L.Wqkv = q->allocs.take((size_t)3 * t * t * es, aw); L.Wo = q->allocs.take((size_t)t * t * es, aw);
-        L.W1 = q->allocs.take((size_t)D.tf_inner * t * es, aw); L.W2 = q->allocs.take((size_t)D.tf_inner * t * es, aw);
-        L.bqkv = fv(3 * t); L.bo = fv(t); L.b1 = fv(D.tf_inner); L.b2 = fv(t); L.ln1w = fv(t); L.ln1b = fv(t); L.ln2w = fv(t); L.ln2b = fv(t);
+    for (int i = 0; i < D.tf_n_layer; ++i) {
+        const std::string p = "transformer_encoder.layers." + std::to_string(i) + ".", a = p + "first_sub_layer.";
+        SfTLayerW& L = q->TL[i];
+        T.fused(L.Wqkv, q->act, {{a + "query_net.weight", t}, {a + "key_net.weight", t}, {a + "value_net.weight", t}}, t);
+        T.fused(L.bqkv, DT_F32, {{a + "query_net.bias", t}, {a + "key_net.bias", t}, {a + "value_net.bias", t}}, 0);
+        T.mat(a + "out_projection.weight", L.Wo, {t, t});
+        T.f32(a + "out_projection.bias", L.bo, {t});
+        T.f32(p + "layer_norm_1.weight", L.ln1w, {t});
+        T.f32(p + "layer_norm_1.bias", L.ln1b, {t});
+        T.mat(p + "second_sub_layer.dense_in.weight", L.W1, {D.tf_inner, t});
+        T.f32(p + "second_sub_layer.dense_in.bias", L.b1, {D.tf_inner});
+        T.mat(p + "second_sub_layer.dense_out.weight", L.W2, {t, D.tf_inner});
+        T.f32(p + "second_sub_layer.dense_out.bias", L.b2, {t});
+        T.f32(p + "layer_norm_2.weight", L.ln2w, {t});
+        T.f32(p + "layer_norm_2.bias", L.ln2b, {t});
     }
-    q->Wproj = q->allocs.take((size_t)t * d * es, aw); q->bproj = fv(t);
-    q->Wh = q->allocs.take((size_t)t * t * es, aw); q->bh = fv(t);
-    q->Wspk = fv((size_t)S * t); q->bspk = fv(S);
+    const std::string m = "sortformer_modules.";
+    T.mat(m + "encoder_proj.weight", q->Wproj, {t, d});
+    T.f32(m + "encoder_proj.bias", q->bproj, {t});
+    T.mat(m + "first_hidden_to_hidden.weight", q->Wh, {t, t});
+    T.f32(m + "first_hidden_to_hidden.bias", q->bh, {t});
+    T.f32(m + "single_hidden_to_spks.weight", q->Wspk, {S, t});
+    T.f32(m + "single_hidden_to_spks.bias", q->bspk, {S});
+    T.allocate(q->allocs, &q->bytes_weights);
     {   // symmetric Hann window (torch.hann_window(periodic=False), as NeMo builds it) and exp(-2 pi i k / n_fft)
         std::vector<float> win(D.win_length);
         std::vector<float2> tw(D.n_fft);
@@ -1253,7 +1162,7 @@ int wlk_sf_load_tensor(wlk_sf* q, const char* name, const float* host, const int
     WLK_API_BEGIN
     WLK_ENTER(q, q->cfg.device);
     WLK_CHECK(name && host && shape && ndim >= 1, "bad arguments");
-    load_tensor(q, name, host, shape, ndim);
+    q->weights.load(name, host, shape, ndim);
     WLK_API_END
 }
 int wlk_sf_finalize_weights(wlk_sf* q) {
