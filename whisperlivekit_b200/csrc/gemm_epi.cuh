@@ -65,6 +65,150 @@ __device__ __forceinline__ void epilogue_fragment_tile(const Epilogue& epi, cons
     }
 }
 
+// Fused epilogue of a ping-pong consumer's whole 128 x 128 tile.  acc[h] is the m64n128 fragment of tile rows 64h..64h+63,
+// row0 the thread's first row (tile row 16 wq + g), so that it owns rows row0 + 64h + 8r (fragment positions as in ptx.cuh).  It runs while
+// the other consumer's MMAs keep the tensor pipe busy, so it is kept short and straight: every per-tile decision
+// (activation, column scale, residual, output type) is taken once outside the element loops, the arithmetic runs in
+// registers, every residual value is loaded before the first store (C may alias the residual: x += A W^T in place, so a
+// load behind a store would wait for it), and loads and stores are global-space.
+template <bool F32>
+__device__ __forceinline__ void epilogue_store_tile128(const Epilogue& epi, const EpiRow (&row)[4], const float (&acc)[2][64],
+                                                       int n_base, int N, int lane) {
+    constexpr int es = F32 ? 4 : 2;
+    const int t2 = 2 * (lane & 3);
+    // a chunk's column offset is even, so a row whose base is aligned takes a two-element store at every chunk
+    bool vec = n_base + 128 <= N;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        vec = vec && row[i].ptr0 != nullptr && (reinterpret_cast<uintptr_t>(row[i].ptr0) & (2 * es - 1)) == 0;
+        if (epi.mode == EPI_SELF_QKV)
+            vec = vec && row[i].ptr1 != nullptr && (reinterpret_cast<uintptr_t>(row[i].ptr1) & (2 * es - 1)) == 0;
+    }
+    if (vec) {                                               // whole tile, aligned rows: straight-line stores
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            int variant;
+            const int64_t coff = (epi_col(epi, n_base + c * 8, &variant) + t2) * es;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                char* p = (variant ? row[i].ptr1 : row[i].ptr0) + coff;
+                const float v0 = acc[i >> 1][4 * c + 2 * (i & 1)], v1 = acc[i >> 1][4 * c + 2 * (i & 1) + 1];
+                if (F32) ptx::st_global_f32x2(p, v0, v1);
+                else ptx::st_global_b32(p, ptx::pack_bf16x2(v0, v1));
+            }
+        }
+        return;
+    }
+    // tail tiles (rows past M, dropped rows, a partial column block) and unaligned rows
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+        const int n0 = n_base + c * 8;
+        if (n0 >= N) break;
+        int variant;
+        const int64_t coff = (epi_col(epi, n0, &variant) + t2) * es;
+        const int n = n0 + t2;
+        const bool ok0 = n < N, ok1 = n + 1 < N;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            char* p = variant ? row[i].ptr1 : row[i].ptr0;
+            if (p == nullptr || !ok0) continue;
+            p += coff;
+            const float v0 = acc[i >> 1][4 * c + 2 * (i & 1)], v1 = acc[i >> 1][4 * c + 2 * (i & 1) + 1];
+            if (F32) {
+                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 7) == 0) ptx::st_global_f32x2(p, v0, v1);
+                else { ptx::st_global_f32(p, v0); if (ok1) ptx::st_global_f32(p + 4, v1); }
+            } else {
+                if (ok1 && (reinterpret_cast<uintptr_t>(p) & 3) == 0) ptx::st_global_b32(p, ptx::pack_bf16x2(v0, v1));
+                else {
+                    ptx::st_global_b16(p, __bfloat16_as_ushort(__float2bfloat16_rn(v0)));
+                    if (ok1) ptx::st_global_b16(p + 2, __bfloat16_as_ushort(__float2bfloat16_rn(v1)));
+                }
+            }
+        }
+    }
+}
+
+template <typename F>
+__device__ __forceinline__ void epilogue_map_tile128(float (&acc)[2][64], F f) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[h][j] = f(acc[h][j]);
+}
+
+__device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, int M, float (&acc)[2][64], int n_base, int N,
+                                                 int lane) {
+    const int t2 = 2 * (lane & 3);
+    const bool full = n_base + 128 <= N;
+    // 1. bias, activation, column scale: registers only
+    if (epi.bias) {
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            const int n = n_base + 8 * c + t2;
+            const float b0 = n < N ? __ldg(epi.bias + n) : 0.f, b1 = n + 1 < N ? __ldg(epi.bias + n + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                acc[h][4 * c] += b0; acc[h][4 * c + 1] += b1; acc[h][4 * c + 2] += b0; acc[h][4 * c + 3] += b1;
+            }
+        }
+    }
+    switch (epi.gelu) {
+        case 1: epilogue_map_tile128(acc, [](float v) { return gelu_erf_fast(v); }); break;
+        case 2: epilogue_map_tile128(acc, [](float v) { return fmaxf(v, 0.f); }); break;
+        case 3: epilogue_map_tile128(acc, [](float v) { return __fdividef(v, 1.0f + __expf(-v)); }); break;
+        default: break;
+    }
+    if (epi.scale_cols > 0) {
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            const int n0 = n_base + 8 * c;
+            if ((epi.scale_period ? (n0 % epi.scale_period) : n0) >= epi.scale_cols) continue;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[h][4 * c + j] *= epi.col_scale;
+        }
+    }
+    if (epi.residual) {
+        // each pass derives the row pointers it needs: none of them stays live next to the 128 accumulators
+        EpiRow row[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) row[i] = epi_row(epi, row0 + 8 * (i & 1) + 64 * (i >> 1), M);
+        bool vec = full;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) vec = vec && row[i].res != nullptr && (reinterpret_cast<uintptr_t>(row[i].res) & 7) == 0;
+        if (vec) {
+            // the whole tile in one basic block: the scheduler batches the 64 loads as far as registers allow
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int c = 0; c < 16; ++c) {
+                    const float2 v = ptx::ld_global_f32x2(row[i].res + n_base + 8 * c + t2);
+                    acc[i >> 1][4 * c + 2 * (i & 1)] += v.x;
+                    acc[i >> 1][4 * c + 2 * (i & 1) + 1] += v.y;
+                }
+        } else {
+            // tail tiles (rows past M, dropped rows, a partial column block) and unaligned rows
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float* res = row[i].res;
+                if (res == nullptr) continue;
+#pragma unroll
+                for (int c = 0; c < 16; ++c) {
+                    const int n = n_base + 8 * c + t2;
+                    if (n < N) acc[i >> 1][4 * c + 2 * (i & 1)] += ptx::ld_global_f32(res + n);
+                    if (n + 1 < N) acc[i >> 1][4 * c + 2 * (i & 1) + 1] += ptx::ld_global_f32(res + n + 1);
+                }
+            }
+        }
+    }
+    EpiRow row[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) row[i] = epi_row(epi, row0 + 8 * (i & 1) + 64 * (i >> 1), M);
+    if (epi.c_type == DT_F32) epilogue_store_tile128<true>(epi, row, acc, n_base, N, lane);
+    else epilogue_store_tile128<false>(epi, row, acc, n_base, N, lane);
+}
+
 // Tile rasterisation shared by the producer and the consumer warps.  Work item t -> (m block, n block): tiles are walked
 // in bands of `band` m-blocks, n-blocks fastest-but-one inside a band, so the ~num_sms tiles in flight at
 // any time cover one band x a few n-blocks: the band's A rows are fetched from HBM once and then served

@@ -1,6 +1,8 @@
 // wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] * W[N,K]^T), bf16 operands, fp32 accumulate.
 //
-// Persistent, warp-specialised, one CTA per SM:
+// Two kernels.  128 x 128 tiles (the encoder's GEMMs) run on the ping-pong kernel gemm_pp_kernel (below); the 64- and
+// 32-wide tiles of short or narrow problems (the decoder's, with split-K) run on gemm_tc_kernel:
+// persistent, warp-specialised, one CTA per SM:
 //   warps 0..7  MMA + epilogue: two warpgroups, each owning 64 rows of the 128 x BN tile.  Per k-slab four
 //                               wgmma.mma_async (M=64, N=BN, K=16) read both operands from shared memory and
 //                               accumulate in registers, one slab in flight while the next is issued; then the
@@ -254,6 +256,154 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Ping-pong kernel for 128 x 128 tiles (the encoder GEMMs): three warpgroups, persistent, one CTA per SM.
+//   WG0      TMA producer: one thread fills the ring with the k-slabs of the CTA's tiles in walk order; the warpgroup
+//            gives registers back (setmaxnreg.dec).
+//   WG1, WG2 consumers (setmaxnreg.inc): each owns a whole 128 x 128 tile -- two m64n128k16 wgmmas per K16 step,
+//            128 fp32 accumulators per thread -- and they take alternate tiles of the walk.  A named-barrier handoff
+//            orders their mainloops: a consumer issues its tile's MMAs only after the other has issued all of its own,
+//            then runs its epilogue while the other's MMAs keep the tensor pipe busy.
+// The producer fills the ring in the interleaved tile order, so a consumer's j-th tile of the walk starts at k-slab
+// j * num_k of the ring's sequence (every tile has num_k slabs: no split-K here); it skips the other consumer's slabs by
+// recomputing stage and phase from that count.  Each output element is accumulated in the same K order as in
+// gemm_tc_kernel.
+constexpr int PP_THREADS = 3 * 128;
+constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;     // 128 * 40 + 256 * 232 <= 64K registers
+constexpr int PP_BAR_ORDER = 1;                                  // named barriers 1, 2: "consumer c may issue its MMAs"
+// L2 budget for the A rows of one m-band (tile_coords): with two tiles in flight per CTA the band is swept across
+// ~2 x grid tiles at a time, and its A rows should be served from L2 for the whole sweep over n
+constexpr int64_t PP_BAND_BYTES = 20ll << 20;
+
+template <int STAGES, bool X3>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
+               const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmWlo, int M, int N, int K,
+               Epilogue epi) {
+    constexpr int BN = 128;
+    using L = SmemLayout<BN, STAGES, X3>;
+    constexpr uint32_t STAGE_TX = L::PLANES * (L::A_BYTES + L::B_BYTES);
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t sA = smem_base;
+    const uint32_t sB = smem_base + STAGES * L::A_BYTES;
+    const uint32_t sAlo = sB + STAGES * L::B_BYTES;                // X3 only
+    const uint32_t sBlo = sAlo + STAGES * L::A_BYTES;              // X3 only
+    const uint32_t bar_full = smem_base + L::BAR_OFF;              // [STAGES]
+    const uint32_t bar_empty = bar_full + STAGES * 8;              // [STAGES]
+
+    const int wg = threadIdx.x >> 7;
+    const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
+    const int num_tiles = num_m * num_n;
+    const int num_k = (K + BK - 1) / BK;
+    const int band_fit = (int)(PP_BAND_BYTES / ((int64_t)BM * K * 2 * L::PLANES));
+    const int band = max(1, min(2 * (int)gridDim.x, band_fit));
+
+    ptx::griddep_launch();
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tensormap(&tmA);
+        ptx::prefetch_tensormap(&tmW);
+        if (X3) { ptx::prefetch_tensormap(&tmAlo); ptx::prefetch_tensormap(&tmWlo); }
+        for (int i = 0; i < STAGES; ++i) {
+            ptx::mbar_init(bar_full + 8 * i, 1);
+            ptx::mbar_init(bar_empty + 8 * i, 4);                  // lane 0 of each warp of the consuming warpgroup
+        }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        // ===================== TMA producer =====================
+        ptx::setmaxnreg_dec<PP_PRODUCER_REGS>();
+        if (threadIdx.x == 0) {
+            // the first ring-full of weight panels does not depend on the previous kernel: requested before the
+            // grid-dependency wait (see gemm_tc_kernel)
+            int early = 0;
+            if ((int)blockIdx.x < num_tiles) {
+                int m_blk, n_blk;
+                tile_coords(blockIdx.x, num_m, num_n, band, &m_blk, &n_blk);
+                early = min(STAGES, num_k);
+                for (int i = 0; i < early; ++i) {
+                    ptx::mbar_arrive_expect_tx(bar_full + 8 * i, STAGE_TX);
+                    ptx::tma_load_2d(sB + i * L::B_BYTES, &tmW, bar_full + 8 * i, i * BK, n_blk * BN);
+                    if (X3) ptx::tma_load_2d(sBlo + i * L::B_BYTES, &tmWlo, bar_full + 8 * i, i * BK, n_blk * BN);
+                }
+            }
+            ptx::griddep_wait();
+            uint32_t stage = 0, phase = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                int m_blk, n_blk;
+                tile_coords(tile, num_m, num_n, band, &m_blk, &n_blk);
+                for (int kb = 0; kb < num_k; ++kb) {
+                    if (early > 0) {
+                        --early;
+                    } else {
+                        ptx::mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
+                        ptx::mbar_arrive_expect_tx(bar_full + 8 * stage, STAGE_TX);
+                        ptx::tma_load_2d(sB + stage * L::B_BYTES, &tmW, bar_full + 8 * stage, kb * BK, n_blk * BN);
+                        if (X3) ptx::tma_load_2d(sBlo + stage * L::B_BYTES, &tmWlo, bar_full + 8 * stage, kb * BK, n_blk * BN);
+                    }
+                    ptx::tma_load_2d(sA + stage * L::A_BYTES, &tmA, bar_full + 8 * stage, kb * BK, m_blk * BM);
+                    if (X3) ptx::tma_load_2d(sAlo + stage * L::A_BYTES, &tmAlo, bar_full + 8 * stage, kb * BK, m_blk * BM);
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+    } else {
+        // ===================== consumers: MMA + epilogue =====================
+        ptx::setmaxnreg_inc<PP_CONSUMER_REGS>();
+        const int c = wg - 1;
+        const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+        constexpr uint32_t HALF_A = 64 * BK * 2;                   // rows 64..127 of the A tile (+HALF_A >> 4 in a descriptor)
+        ptx::griddep_wait();                                       // residual and C belong to the stream's past
+        for (int tile = blockIdx.x + c * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+            const int j = (tile - (int)blockIdx.x) / (int)gridDim.x;      // position of the tile in the CTA's walk
+            int m_blk, n_blk;
+            tile_coords(tile, num_m, num_n, band, &m_blk, &n_blk);
+            const int row0 = m_blk * BM + wq * 16 + (lane >> 2);
+            const uint32_t slab0 = (uint32_t)j * num_k;
+            uint32_t stage = slab0 % STAGES, phase = (slab0 / STAGES) & 1;
+            float acc[2][64];
+            int prev = -1;                                         // slot whose MMAs are still in flight
+            if (j > 0) ptx::named_bar_sync<256>(PP_BAR_ORDER + c);  // the other consumer has issued its tile
+            for (int kb = 0; kb < num_k; ++kb) {
+                ptx::mbar_wait_mma(bar_full + 8 * stage, phase);
+                const uint64_t da = ptx::wgmma_desc_sw128(sA + stage * L::A_BYTES);
+                const uint64_t db = ptx::wgmma_desc_sw128(sB + stage * L::B_BYTES);
+                const uint64_t dal = ptx::wgmma_desc_sw128(sAlo + stage * L::A_BYTES);
+                const uint64_t dbl = ptx::wgmma_desc_sw128(sBlo + stage * L::B_BYTES);
+                ptx::wgmma_fence_regs(acc[0]);
+                ptx::wgmma_fence_regs(acc[1]);
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint32_t acc_in = (kb > 0 || k > 0) ? 1u : 0u;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint64_t ah = h * (HALF_A >> 4) + 2 * k;
+                        ptx::WgmmaSS<BN>::mma(acc[h], da + ah, db + 2 * k, acc_in);
+                        if (X3) {
+                            ptx::WgmmaSS<BN>::mma(acc[h], dal + ah, db + 2 * k, 1u);
+                            ptx::WgmmaSS<BN>::mma(acc[h], da + ah, dbl + 2 * k, 1u);
+                        }
+                    }
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_wait<1>();                              // the previous slab's MMAs have retired: its slot is free
+                if (prev >= 0 && lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            if (tile + gridDim.x < num_tiles) ptx::named_bar_arrive<256>(PP_BAR_ORDER + (c ^ 1));   // the next tile's turn
+            ptx::wgmma_wait<0>();
+            ptx::wgmma_fence_regs(acc[0]);
+            ptx::wgmma_fence_regs(acc[1]);
+            if (lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
+            epilogue_tile128(epi, row0, M, acc, n_blk * BN, N, lane);
+        }
+    }
+}
+
 // fp32 -> (hi, lo) bf16 planes: hi = bf16(x), lo = bf16(x - hi)
 __global__ void split_f32_kernel(const float* __restrict__ src, bf16* __restrict__ hi, bf16* __restrict__ lo, int64_t n) {
     ptx::griddep_launch();
@@ -315,6 +465,33 @@ void launch(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t 
     else launch_impl<BN, STAGES, false>(g, A_hi, A_lo, st, num_sms, splits);
 }
 
+template <int STAGES, bool X3>
+void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
+    using L = SmemLayout<128, STAGES, X3>;
+    static_assert(L::DYN <= 227 * 1024, "shared memory budget");
+    CUtensorMap tmA, tmW, tmAlo, tmWlo;
+    std::string err;
+    WLK_CHECK(make_tmap_bf16_2d(&tmA, A_hi, g.M, g.K, g.lda, BM, BK, &err), "A tensor map: %s", err.c_str());
+    WLK_CHECK(make_tmap_bf16_2d(&tmW, g.W, g.N, g.K, g.ldw, 128, BK, &err), "W tensor map: %s", err.c_str());
+    if (X3) {
+        WLK_CHECK(make_tmap_bf16_2d(&tmAlo, A_lo, g.M, g.K, g.lda, BM, BK, &err), "A_lo tensor map: %s", err.c_str());
+        WLK_CHECK(make_tmap_bf16_2d(&tmWlo, g.W_lo, g.N, g.K, g.ldw, 128, BK, &err), "W_lo tensor map: %s", err.c_str());
+    } else { tmAlo = tmA; tmWlo = tmW; }
+    static bool seen[64] = {};
+    if (first_on_device(seen))
+        CUDA_CHECK(cudaFuncSetAttribute(gemm_pp_kernel<STAGES, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::DYN));
+    const int num_tiles = ((g.M + BM - 1) / BM) * ((g.N + 127) / 128);
+    const int grid = num_tiles < num_sms ? num_tiles : num_sms;
+    CUDA_CHECK(launch_pdl(gemm_pp_kernel<STAGES, X3>, dim3(grid), dim3(PP_THREADS), L::DYN, st, tmA, tmW, tmAlo, tmWlo,
+                          g.M, g.N, g.K, g.epi));
+}
+
+// 128 x 128 tiles on the ping-pong kernel; ring depth 6 (plain) or 3 (X3: four tiles per slab)
+void launch_pp(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
+    if (g.w_type == DT_BF16X2) launch_pp_impl<3, true>(g, A_hi, A_lo, st, num_sms);
+    else launch_pp_impl<6, false>(g, A_hi, A_lo, st, num_sms);
+}
+
 }  // namespace
 
 void split_f32_planes_async(const float* src, bf16* hi, bf16* lo, int64_t n, cudaStream_t st) {
@@ -357,9 +534,9 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         split_f32_planes_async(reinterpret_cast<const float*>(g.A), hi, lo, n, st);
         A_hi = hi; A_lo = lo;
     }
-    // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = <128,6>, 4 = <32,10>,
+    // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = 128-wide ping-pong, 4 = <32,10>,
     // 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4
-    if (variant == 2) { launch<128, 6, 3>(g, A_hi, A_lo, st, num_sms); return; }
+    if (variant == 2) { launch_pp(g, A_hi, A_lo, st, num_sms); return; }
     if (variant == 1 || (variant >= 4 && variant <= 8)) {
         const int num_k = (g.K + BK - 1) / BK;
         int sp = (variant == 5 || variant == 7) ? 2 : (variant == 6 || variant == 8) ? 4 : 1;
@@ -371,7 +548,7 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         return;
     }
     // 128-wide tiles while they still cover half the SMs, else 64-wide ones
-    if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) launch<128, 6, 3>(g, A_hi, A_lo, st, num_sms);
+    if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) launch_pp(g, A_hi, A_lo, st, num_sms);
     else {
         // Short, narrow problems (the decoder's per-token GEMMs) cannot fill the GPU with output tiles alone and
         // a CTA walking all of K pays one TMA round trip per ring refill.  The K range is split across CTAs

@@ -92,6 +92,42 @@ __device__ __forceinline__ void mbar_wait_mma(uint32_t bar, uint32_t parity) {
     }
 }
 
+// ---- warpgroup register budget and named barriers (warp-specialised kernels) -----------
+// setmaxnreg: every thread of the warpgroup executes it; the producer gives registers back, the consumers take them.
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int THREADS> __device__ __forceinline__ void named_bar_sync(int id) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(THREADS) : "memory");
+}
+template <int THREADS> __device__ __forceinline__ void named_bar_arrive(int id) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(THREADS) : "memory");
+}
+
+// ---- global-space loads and stores (STG / LDG instead of the generic ST / LD the compiler emits for pointers it
+// cannot place in the global window) ----------------------------------------------------------
+__device__ __forceinline__ float ld_global_f32(const float* p) {
+    float v;
+    asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ float2 ld_global_f32x2(const float* p) {
+    float2 v;
+    asm volatile("ld.global.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_global_f32(void* p, float v) {
+    asm volatile("st.global.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+__device__ __forceinline__ void st_global_f32x2(void* p, float a, float b) {
+    asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void st_global_b16(void* p, uint16_t v) {
+    asm volatile("st.global.b16 [%0], %1;" ::"l"(p), "h"(v) : "memory");
+}
+__device__ __forceinline__ void st_global_b32(void* p, uint32_t v) {
+    asm volatile("st.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
 // ---- programmatic dependent launch (see launch_pdl in common.cuh) ----------------------
 // wait: blocks until every grid this one depends on has completed and its writes are visible (no-op when the
 // launch carried no PDL attribute).  launch_dependents: lets the next kernel in the stream start scheduling
