@@ -170,7 +170,7 @@ int wlk_read_align_attn(wlk_engine* e, int32_t sid, float* out, int64_t capacity
 
 /* ---- op-level entry points (kernel tests, roofline benches). Device pointers.
  *      backend: WLK_BACKEND_SIMT, WLK_BACKEND_TCGEN05 (auto tile choice), 3 = force the 64-wide-tile wgmma kernel,
- *      4 = force the 128-wide-tile one.
+ *      4 = force the 128-wide-tile one on lone CTAs, 5 / 6 / 7 = force it in 2x1 / 1x2 / 2x2 clusters (m x n).
  *      a_type/w_type/c_type: 0 = fp32, 1 = bf16.  C[M,N] = act(A[M,K] W[N,K]^T + bias); `gelu` is a flag
  *      word: bit 0 = erf-GELU, bit 1 = accumulate into the fp32 C in place (C += A W^T + bias).           */
 int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t lda,

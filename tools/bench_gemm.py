@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-shape rates of the wgmma GEMM next to cuBLAS (torch.matmul, bf16 out), in one process.
 
-    python tools/bench_gemm.py [--streams 48] [--shapes qkv,fc1,...] [--backend tcgen05|tcgen05_pair|tcgen05_1cta]
+    python tools/bench_gemm.py [--streams 48] [--shapes qkv,fc1,...] [--backend tcgen05,tcgen05_pair,...]
     python tools/bench_gemm.py --mnk M N K           (one custom shape, plain bf16 out)
 
 Default shapes: the large-v3 encoder GEMMs of one tick at --streams streams (M = streams x 1500 rows, or x 3000 for
@@ -9,7 +9,14 @@ conv1), each with the epilogue the engine uses where `op_gemm` exposes it.  The 
 output here (its head-major scatter is an engine-internal mode); the attention-out GEMM is timed as FC2's epilogue
 twin (fp32 residual accumulated in place).  cuBLAS computes the same product without the epilogue.  TFLOP/s come from
 the shapes (2 M N K per call) and CUDA events around many calls.  The card's name, power limit and maximum SM clock
-are printed beside the figures (nvidia-smi, read-only query)."""
+are printed beside the figures (nvidia-smi, read-only query).
+
+--backend takes a comma-separated list; each shape is timed under every backend in turn, on the same operands.
+Backends: tcgen05 (the auto choice), tcgen05_pair (128-wide ping-pong tiles on lone CTAs), tcgen05_pp2x1 /
+tcgen05_pp1x2 / tcgen05_pp2x2 (the same kernel in clusters of m x n CTAs), tcgen05_1cta (64-wide tiles).
+`l2_to_smem_tbs` is the rate at which the 128-wide kernel's TMA loads move its k-slabs out of L2, from the shapes: every
+tile of the cluster-padded grid loads, per 64-deep k-slab, 16 KiB of A shared by the cluster's n CTAs and 16 KiB of W
+shared by its m CTAs."""
 import argparse
 import json
 import os
@@ -35,6 +42,26 @@ SHAPES = {
     "conv2": (1500, D, 3 * D, 2 * D, "gelu", 1),         # stride 2 over conv1's rows
 }
 GELU_BITS = {"plain": 0, "bias": 0, "gelu": 1, "residual": 2}
+BACKENDS = ["tcgen05", "tcgen05_pair", "tcgen05_pp2x1", "tcgen05_pp1x2", "tcgen05_pp2x2", "tcgen05_1cta"]
+# cluster shape (m, n) of the 128-wide backends; the auto choice mirrors gemm_tcgen05 (csrc/gemm_tc.cu)
+CLUSTER = {"tcgen05_pair": (1, 1), "tcgen05_pp2x1": (2, 1), "tcgen05_pp1x2": (1, 2), "tcgen05_pp2x2": (2, 2)}
+
+
+def cluster_of(backend, M, N, K, sms):
+    if backend == "tcgen05":
+        if N < 128 or -(-M // 128) * -(-N // 128) < sms // 2:
+            return None
+        return (2, 2) if K >= 1024 else (1, 1)
+    return CLUSTER.get(backend)
+
+
+def l2_to_smem_bytes(cluster, M, N, K):
+    """Bytes the 128-wide kernel's TMA loads read out of L2 per call (None: another kernel)."""
+    if cluster is None:
+        return None
+    cm, cn = cluster
+    tiles = -(-M // (128 * cm)) * cm * (-(-N // (128 * cn)) * cn)
+    return tiles * -(-K // 64) * (16384 // cn + 16384 // cm)
 
 
 def card_info():
@@ -70,19 +97,23 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=48)
     ap.add_argument("--shapes", default=",".join(SHAPES))
-    ap.add_argument("--backend", default="tcgen05", choices=["tcgen05", "tcgen05_pair", "tcgen05_1cta"])
+    ap.add_argument("--backend", default="tcgen05", help="comma-separated: " + ",".join(BACKENDS))
     ap.add_argument("--mnk", type=int, nargs=3, default=None)
     ap.add_argument("--window-ms", type=float, default=300.0, help="timed work per shape and side")
     ap.add_argument("--no-cublas", action="store_true")
     args = ap.parse_args()
+    backends = args.backend.split(",")
+    for be in backends:
+        assert be in BACKENDS, f"unknown backend {be}"
     assert torch.cuda.is_available(), "tools/bench_gemm.py measures on a GPU"
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
 
     eng = WhisperEngine(DIMS["micro"], None, [(0, 0)], precision="bf16", max_sessions=1, max_batch=1)
     g = torch.Generator(device="cuda").manual_seed(0)
     todo = {"custom": (args.mnk[0], args.mnk[1], args.mnk[2], None, "plain", 1)} if args.mnk else \
         {k: SHAPES[k] for k in args.shapes.split(",")}
     print(json.dumps({"card": card_info(), "backend": args.backend, "streams": args.streams}), flush=True)
-    total = {"engine_ms": 0.0, "cublas_ms": 0.0, "tflop": 0.0}
+    total = {"cublas_ms": 0.0, "tflop": 0.0, **{f"{be}_ms": 0.0 for be in backends}}
     for name, (rows, N, K, lda, epi, layers) in todo.items():
         M = rows if name == "custom" else rows * args.streams
         A, lda_el = operand_a(M, K, lda, g)
@@ -92,16 +123,22 @@ def main():
         c_code = 0 if epi == "residual" else 1
         flop = 2.0 * M * N * K
 
-        def eng_call():
-            eng.op_gemm(args.backend, A.data_ptr(), 1, lda_el, W.data_ptr(), 1, K, b.data_ptr() if b is not None else None,
+        def eng_call(be):
+            eng.op_gemm(be, A.data_ptr(), 1, lda_el, W.data_ptr(), 1, K, b.data_ptr() if b is not None else None,
                         C.data_ptr(), c_code, N, M, N, K, GELU_BITS[epi])
 
-        # rough rate first, then a window of about --window-ms
-        probe = time_ms(eng_call, eng.timer_record, lambda: eng.timer_elapsed_ms(0, 1), 2, warmup=1)
-        iters = max(3, int(args.window_ms / max(probe, 1e-3)))
-        ms = time_ms(eng_call, eng.timer_record, lambda: eng.timer_elapsed_ms(0, 1), iters)
-        line = {"shape": name, "M": M, "N": N, "K": K, "lda": lda_el, "epilogue": epi, "iters": iters,
-                "engine_ms": round(ms, 4), "engine_tflops": round(flop / ms / 1e9, 1)}
+        for be in backends:
+            # rough rate first, then a window of about --window-ms
+            probe = time_ms(lambda: eng_call(be), eng.timer_record, lambda: eng.timer_elapsed_ms(0, 1), 2, warmup=1)
+            iters = max(3, int(args.window_ms / max(probe, 1e-3)))
+            ms = time_ms(lambda: eng_call(be), eng.timer_record, lambda: eng.timer_elapsed_ms(0, 1), iters)
+            line = {"shape": name, "backend": be, "M": M, "N": N, "K": K, "lda": lda_el, "epilogue": epi,
+                    "iters": iters, "engine_ms": round(ms, 4), "engine_tflops": round(flop / ms / 1e9, 1)}
+            l2 = l2_to_smem_bytes(cluster_of(be, M, N, K, sms), M, N, K)
+            if l2 is not None:
+                line["l2_to_smem_tbs"] = round(l2 / ms / 1e9, 2)
+            total[f"{be}_ms"] += layers * ms
+            print(json.dumps(line), flush=True)
         if not args.no_cublas:
             eng.sync()
             Cb = C if C.dtype == torch.bfloat16 else None
@@ -113,19 +150,18 @@ def main():
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
             ms_cb = time_ms(lambda: torch.matmul(A, Wt, out=Cb), lambda i: ev[i].record(),
                             lambda: (torch.cuda.synchronize(), ev[0].elapsed_time(ev[1]))[1], iters)
-            line.update(cublas_ms=round(ms_cb, 4), cublas_tflops=round(flop / ms_cb / 1e9, 1),
-                        engine_over_cublas=round(ms_cb / ms, 3))
+            print(json.dumps({"shape": name, "backend": "cublas", "cublas_ms": round(ms_cb, 4),
+                              "cublas_tflops": round(flop / ms_cb / 1e9, 1)}), flush=True)
             total["cublas_ms"] += layers * ms_cb
             del Cb
-        total["engine_ms"] += layers * ms
         total["tflop"] += layers * flop / 1e12
-        print(json.dumps(line), flush=True)
         del A, W, b
         C = None
         torch.cuda.empty_cache()
     if len(todo) > 1:
         total = {k: round(v, 2) for k, v in total.items()}
-        total["engine_tflops"] = round(total["tflop"] / total["engine_ms"] * 1e3, 1)
+        for be in backends:
+            total[f"{be}_tflops"] = round(total["tflop"] / total[f"{be}_ms"] * 1e3, 1)
         print(json.dumps({"per_tick_layers_weighted": total}), flush=True)
     eng.close()
 

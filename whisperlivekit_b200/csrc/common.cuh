@@ -50,20 +50,35 @@ struct Error {
 // ---------------------------------------------------------------------------------
 bool pdl_enabled();
 
+// The same launch in thread-block clusters of `cluster` CTAs along x (grid.x a multiple of it; 1: no clusters).
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                              Args&&... args) {
+inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                      unsigned cluster, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attr[2];
+    unsigned n = 0;
+    if (pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n++].val.programmaticStreamSerializationAllowed = 1;
+    }
+    if (cluster > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = cluster;
+        attr[n].val.clusterDim.y = 1;
+        attr[n++].val.clusterDim.z = 1;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = n;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                              Args&&... args) {
+    return launch_pdl_cluster(kernel, grid, block, smem, st, 1, static_cast<Args&&>(args)...);
 }
 
 // True the first time it is called for the current device with this flag array: kernel attributes (dynamic shared

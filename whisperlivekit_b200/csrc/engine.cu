@@ -1532,6 +1532,7 @@ int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t l
     if (backend == WLK_BACKEND_TCGEN05) gemm_tcgen05(g, e->st, e->num_sms, 0);
     else if (backend == 3) gemm_tcgen05(g, e->st, e->num_sms, 1);
     else if (backend == 4) gemm_tcgen05(g, e->st, e->num_sms, 2);
+    else if (backend >= 5 && backend <= 7) gemm_tcgen05(g, e->st, e->num_sms, backend + 4);
     else gemm_simt(g, e->st);
     WLK_API_END
 }

@@ -15,6 +15,7 @@
 #include <cudaTypedefs.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <unordered_map>
 
@@ -268,6 +269,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // j * num_k of the ring's sequence (every tile has num_k slabs: no split-K here); it skips the other consumer's slabs by
 // recomputing stage and phase from that count.  Each output element is accumulated in the same K order as in
 // gemm_tc_kernel.
+//
+// Clusters (CM x CN CTAs, CM * CN > 1): the cluster owns a CM x CN block of tiles (a cluster-tile) and walks the
+// cluster-tiles as a lone CTA walks tiles; CTA rank r takes tile (rm, rn) = (r % CM, r / CM) of each.  The CM CTAs of an
+// n column need the same W slab and the CN CTAs of an m row the same A slab, so each loads 1/CM of the W slab and
+// 1/CN of the A slab and multicasts its share to the CTAs that need it: a slab is read from L2 once per cluster instead
+// of once per CTA.  Every CTA's full barrier still expects the whole stage.  A stage is refilled only when the consumers
+// of every CTA of the cluster have released it (each consumer warp arrives on the empty barrier of every CTA), so the
+// CTAs of a cluster run the same slab sequence in lockstep.  A tile past M or N (odd num_m) is loaded (TMA zero-fills
+// it), computed and released like any other; its epilogue stores nothing.  <STAGES, X3, 1, 1> is the lone-CTA kernel.
 constexpr int PP_THREADS = 3 * 128;
 constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;     // 128 * 40 + 256 * 232 <= 64K registers
 constexpr int PP_BAR_ORDER = 1;                                  // named barriers 1, 2: "consumer c may issue its MMAs"
@@ -275,12 +285,14 @@ constexpr int PP_BAR_ORDER = 1;                                  // named barrie
 // ~2 x grid tiles at a time, and its A rows should be served from L2 for the whole sweep over n
 constexpr int64_t PP_BAND_BYTES = 20ll << 20;
 
-template <int STAGES, bool X3>
+template <int STAGES, bool X3, int CM, int CN>
 __global__ void __launch_bounds__(PP_THREADS, 1)
 gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmWlo, int M, int N, int K,
                Epilogue epi) {
     constexpr int BN = 128;
+    constexpr int CS = CM * CN;                                    // CTAs per cluster
+    constexpr int W_ROWS = BN / CM, A_ROWS = BM / CN;              // this CTA's share of a W / A slab (the tensor maps' box)
     using L = SmemLayout<BN, STAGES, X3>;
     constexpr uint32_t STAGE_TX = L::PLANES * (L::A_BYTES + L::B_BYTES);
     extern __shared__ uint8_t smem_raw[];
@@ -293,11 +305,21 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t bar_empty = bar_full + STAGES * 8;              // [STAGES]
 
     const int wg = threadIdx.x >> 7;
+    const int rank = CS > 1 ? (int)ptx::cluster_ctarank() : 0;
+    const int rm = rank % CM, rn = rank / CM;
+    const int cluster = CS > 1 ? (int)ptx::cluster_id_x() : (int)blockIdx.x;
+    const int clusters = CS > 1 ? (int)ptx::num_clusters_x() : (int)gridDim.x;
     const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-    const int num_tiles = num_m * num_n;
+    const int cnum_m = (num_m + CM - 1) / CM, cnum_n = (num_n + CN - 1) / CN;
+    const int num_ct = cnum_m * cnum_n;                            // cluster-tiles
     const int num_k = (K + BK - 1) / BK;
-    const int band_fit = (int)(PP_BAND_BYTES / ((int64_t)BM * K * 2 * L::PLANES));
-    const int band = max(1, min(2 * (int)gridDim.x, band_fit));
+    const int band_fit = (int)(PP_BAND_BYTES / ((int64_t)CM * BM * K * 2 * L::PLANES));
+    const int band = max(1, min(2 * clusters, band_fit));
+    auto coords = [&](int ct, int* m_blk, int* n_blk) {
+        tile_coords(ct, cnum_m, cnum_n, band, m_blk, n_blk);
+        *m_blk = *m_blk * CM + rm;
+        *n_blk = *n_blk * CN + rn;
+    };
 
     ptx::griddep_launch();
     if (threadIdx.x == 0) {
@@ -306,45 +328,62 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (X3) { ptx::prefetch_tensormap(&tmAlo); ptx::prefetch_tensormap(&tmWlo); }
         for (int i = 0; i < STAGES; ++i) {
             ptx::mbar_init(bar_full + 8 * i, 1);
-            ptx::mbar_init(bar_empty + 8 * i, 4);                  // lane 0 of each warp of the consuming warpgroup
+            ptx::mbar_init(bar_empty + 8 * i, 4 * CS);             // lane 0 of each warp of the consuming warpgroups
         }
         ptx::fence_barrier_init();
     }
-    __syncthreads();
+    // the peers' barriers must be initialised before the first multicast lands on them
+    if (CS > 1) ptx::cluster_sync();
+    else __syncthreads();
 
     if (wg == 0) {
         // ===================== TMA producer =====================
         ptx::setmaxnreg_dec<PP_PRODUCER_REGS>();
         if (threadIdx.x == 0) {
+            uint16_t w_mask = 0, a_mask = 0;                       // the CTAs of this one's n column / m row
+            for (int i = 0; i < CM; ++i) w_mask |= 1u << (rn * CM + i);
+            for (int i = 0; i < CN; ++i) a_mask |= 1u << (i * CM + rm);
+            // this CTA's share of a slab: rows [rm * W_ROWS, +W_ROWS) of the W tile, [rn * A_ROWS, +A_ROWS) of the A tile
+            auto load = [&](uint32_t dst, const CUtensorMap* tm, uint32_t bar, int kb, int row, uint16_t mask, bool shared) {
+                if (shared) ptx::tma_load_2d_multicast(dst, tm, bar, kb * BK, row, mask);
+                else ptx::tma_load_2d(dst, tm, bar, kb * BK, row);
+            };
+            auto load_w = [&](uint32_t stage, int kb, int n_blk) {
+                const uint32_t off = stage * L::B_BYTES + rm * W_ROWS * BK * 2, bar = bar_full + 8 * stage;
+                load(sB + off, &tmW, bar, kb, n_blk * BN + rm * W_ROWS, w_mask, CM > 1);
+                if (X3) load(sBlo + off, &tmWlo, bar, kb, n_blk * BN + rm * W_ROWS, w_mask, CM > 1);
+            };
+            auto load_a = [&](uint32_t stage, int kb, int m_blk) {
+                const uint32_t off = stage * L::A_BYTES + rn * A_ROWS * BK * 2, bar = bar_full + 8 * stage;
+                load(sA + off, &tmA, bar, kb, m_blk * BM + rn * A_ROWS, a_mask, CN > 1);
+                if (X3) load(sAlo + off, &tmAlo, bar, kb, m_blk * BM + rn * A_ROWS, a_mask, CN > 1);
+            };
             // the first ring-full of weight panels does not depend on the previous kernel: requested before the
             // grid-dependency wait (see gemm_tc_kernel)
             int early = 0;
-            if ((int)blockIdx.x < num_tiles) {
+            if (cluster < num_ct) {
                 int m_blk, n_blk;
-                tile_coords(blockIdx.x, num_m, num_n, band, &m_blk, &n_blk);
+                coords(cluster, &m_blk, &n_blk);
                 early = min(STAGES, num_k);
                 for (int i = 0; i < early; ++i) {
                     ptx::mbar_arrive_expect_tx(bar_full + 8 * i, STAGE_TX);
-                    ptx::tma_load_2d(sB + i * L::B_BYTES, &tmW, bar_full + 8 * i, i * BK, n_blk * BN);
-                    if (X3) ptx::tma_load_2d(sBlo + i * L::B_BYTES, &tmWlo, bar_full + 8 * i, i * BK, n_blk * BN);
+                    load_w(i, i, n_blk);
                 }
             }
             ptx::griddep_wait();
             uint32_t stage = 0, phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            for (int ct = cluster; ct < num_ct; ct += clusters) {
                 int m_blk, n_blk;
-                tile_coords(tile, num_m, num_n, band, &m_blk, &n_blk);
+                coords(ct, &m_blk, &n_blk);
                 for (int kb = 0; kb < num_k; ++kb) {
                     if (early > 0) {
                         --early;
                     } else {
                         ptx::mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
                         ptx::mbar_arrive_expect_tx(bar_full + 8 * stage, STAGE_TX);
-                        ptx::tma_load_2d(sB + stage * L::B_BYTES, &tmW, bar_full + 8 * stage, kb * BK, n_blk * BN);
-                        if (X3) ptx::tma_load_2d(sBlo + stage * L::B_BYTES, &tmWlo, bar_full + 8 * stage, kb * BK, n_blk * BN);
+                        load_w(stage, kb, n_blk);
                     }
-                    ptx::tma_load_2d(sA + stage * L::A_BYTES, &tmA, bar_full + 8 * stage, kb * BK, m_blk * BM);
-                    if (X3) ptx::tma_load_2d(sAlo + stage * L::A_BYTES, &tmAlo, bar_full + 8 * stage, kb * BK, m_blk * BM);
+                    load_a(stage, kb, m_blk);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -355,11 +394,16 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int c = wg - 1;
         const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
         constexpr uint32_t HALF_A = 64 * BK * 2;                   // rows 64..127 of the A tile (+HALF_A >> 4 in a descriptor)
+        // a stage is free again once this warp is done with it: lane i tells cluster rank i, whose producer may multicast into it
+        auto release = [&](uint32_t stage) {
+            if (CS > 1) { if (lane < CS) ptx::mbar_arrive_cluster(bar_empty + 8 * stage, lane); }
+            else if (lane == 0) ptx::mbar_arrive(bar_empty + 8 * stage);
+        };
         ptx::griddep_wait();                                       // residual and C belong to the stream's past
-        for (int tile = blockIdx.x + c * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
-            const int j = (tile - (int)blockIdx.x) / (int)gridDim.x;      // position of the tile in the CTA's walk
+        for (int ct = cluster + c * clusters; ct < num_ct; ct += 2 * clusters) {
+            const int j = (ct - cluster) / clusters;               // position of the tile in the CTA's walk
             int m_blk, n_blk;
-            tile_coords(tile, num_m, num_n, band, &m_blk, &n_blk);
+            coords(ct, &m_blk, &n_blk);
             const int row0 = m_blk * BM + wq * 16 + (lane >> 2);
             const uint32_t slab0 = (uint32_t)j * num_k;
             uint32_t stage = slab0 % STAGES, phase = (slab0 / STAGES) & 1;
@@ -390,18 +434,20 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
                 ptx::wgmma_commit();
                 ptx::wgmma_wait<1>();                              // the previous slab's MMAs have retired: its slot is free
-                if (prev >= 0 && lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
+                if (prev >= 0) release(prev);
                 prev = stage;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            if (tile + gridDim.x < num_tiles) ptx::named_bar_arrive<256>(PP_BAR_ORDER + (c ^ 1));   // the next tile's turn
+            if (ct + clusters < num_ct) ptx::named_bar_arrive<256>(PP_BAR_ORDER + (c ^ 1));   // the next tile's turn
             ptx::wgmma_wait<0>();
             ptx::wgmma_fence_regs(acc[0]);
             ptx::wgmma_fence_regs(acc[1]);
-            if (lane == 0) ptx::mbar_arrive(bar_empty + 8 * prev);
+            release(prev);
             epilogue_tile128(epi, row0, M, acc, n_blk * BN, N, lane);
         }
     }
+    // no CTA may exit while a peer can still arrive on its barriers
+    if (CS > 1) ptx::cluster_sync();
 }
 
 // fp32 -> (hi, lo) bf16 planes: hi = bf16(x), lo = bf16(x - hi)
@@ -465,31 +511,54 @@ void launch(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t 
     else launch_impl<BN, STAGES, false>(g, A_hi, A_lo, st, num_sms, splits);
 }
 
-template <int STAGES, bool X3>
+template <int STAGES, bool X3, int CM, int CN>
 void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
     using L = SmemLayout<128, STAGES, X3>;
     static_assert(L::DYN <= 227 * 1024, "shared memory budget");
+    constexpr int CS = CM * CN;
+    auto kernel = gemm_pp_kernel<STAGES, X3, CM, CN>;
+    // each CTA loads 1/CN of an A slab and 1/CM of a W slab (the kernel's multicast shares)
     CUtensorMap tmA, tmW, tmAlo, tmWlo;
     std::string err;
-    WLK_CHECK(make_tmap_bf16_2d(&tmA, A_hi, g.M, g.K, g.lda, BM, BK, &err), "A tensor map: %s", err.c_str());
-    WLK_CHECK(make_tmap_bf16_2d(&tmW, g.W, g.N, g.K, g.ldw, 128, BK, &err), "W tensor map: %s", err.c_str());
+    WLK_CHECK(make_tmap_bf16_2d(&tmA, A_hi, g.M, g.K, g.lda, BM / CN, BK, &err), "A tensor map: %s", err.c_str());
+    WLK_CHECK(make_tmap_bf16_2d(&tmW, g.W, g.N, g.K, g.ldw, 128 / CM, BK, &err), "W tensor map: %s", err.c_str());
     if (X3) {
-        WLK_CHECK(make_tmap_bf16_2d(&tmAlo, A_lo, g.M, g.K, g.lda, BM, BK, &err), "A_lo tensor map: %s", err.c_str());
-        WLK_CHECK(make_tmap_bf16_2d(&tmWlo, g.W_lo, g.N, g.K, g.ldw, 128, BK, &err), "W_lo tensor map: %s", err.c_str());
+        WLK_CHECK(make_tmap_bf16_2d(&tmAlo, A_lo, g.M, g.K, g.lda, BM / CN, BK, &err), "A_lo tensor map: %s", err.c_str());
+        WLK_CHECK(make_tmap_bf16_2d(&tmWlo, g.W_lo, g.N, g.K, g.ldw, 128 / CM, BK, &err), "W_lo tensor map: %s", err.c_str());
     } else { tmAlo = tmA; tmWlo = tmW; }
-    static bool seen[64] = {};
-    if (first_on_device(seen))
-        CUDA_CHECK(cudaFuncSetAttribute(gemm_pp_kernel<STAGES, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::DYN));
-    const int num_tiles = ((g.M + BM - 1) / BM) * ((g.N + 127) / 128);
-    const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-    CUDA_CHECK(launch_pdl(gemm_pp_kernel<STAGES, X3>, dim3(grid), dim3(PP_THREADS), L::DYN, st, tmA, tmW, tmAlo, tmWlo,
-                          g.M, g.N, g.K, g.epi));
+    // clusters of this shape the device holds at once (it depends on how the SMs split into GPCs): queried once per device
+    static std::atomic<int> max_clusters[64];
+    const int dev = current_device();
+    int mc = max_clusters[dev].load(std::memory_order_relaxed);
+    if (mc == 0) {
+        CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::DYN));
+        mc = num_sms;
+        if (CS > 1) {
+            cudaLaunchConfig_t cfg = {};
+            cudaLaunchAttribute attr[1];
+            attr[0].id = cudaLaunchAttributeClusterDimension;
+            attr[0].val.clusterDim.x = CS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+            cfg.gridDim = dim3(CS);
+            cfg.blockDim = dim3(PP_THREADS);
+            cfg.dynamicSmemBytes = L::DYN;
+            cfg.attrs = attr;
+            cfg.numAttrs = 1;
+            CUDA_CHECK(cudaOccupancyMaxActiveClusters(&mc, kernel, &cfg));
+            WLK_CHECK(mc > 0, "no %dx%d cluster of the 128-wide GEMM fits on the device", CM, CN);
+        }
+        max_clusters[dev].store(mc, std::memory_order_relaxed);
+    }
+    const int num_ct = ((g.M + BM * CM - 1) / (BM * CM)) * ((g.N + 128 * CN - 1) / (128 * CN));
+    const int clusters = std::max(1, std::min({mc, num_sms / CS, num_ct}));
+    CUDA_CHECK(launch_pdl_cluster(kernel, dim3(clusters * CS), dim3(PP_THREADS), L::DYN, st, CS, tmA, tmW, tmAlo, tmWlo,
+                                  g.M, g.N, g.K, g.epi));
 }
 
-// 128 x 128 tiles on the ping-pong kernel; ring depth 6 (plain) or 3 (X3: four tiles per slab)
+// 128 x 128 tiles on the ping-pong kernel, in clusters of CM x CN CTAs; ring depth 6 (plain) or 3 (X3: four tiles per slab)
+template <int CM, int CN>
 void launch_pp(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
-    if (g.w_type == DT_BF16X2) launch_pp_impl<3, true>(g, A_hi, A_lo, st, num_sms);
-    else launch_pp_impl<6, false>(g, A_hi, A_lo, st, num_sms);
+    if (g.w_type == DT_BF16X2) launch_pp_impl<3, true, 1, 1>(g, A_hi, A_lo, st, num_sms);
+    else launch_pp_impl<6, false, CM, CN>(g, A_hi, A_lo, st, num_sms);
 }
 
 }  // namespace
@@ -534,9 +603,12 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         split_f32_planes_async(reinterpret_cast<const float*>(g.A), hi, lo, n, st);
         A_hi = hi; A_lo = lo;
     }
-    // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = 128-wide ping-pong, 4 = <32,10>,
-    // 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4
-    if (variant == 2) { launch_pp(g, A_hi, A_lo, st, num_sms); return; }
+    // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = 128-wide ping-pong on lone CTAs,
+    // 4 = <32,10>, 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4, 9/10/11 = 128-wide in 2x1 / 1x2 / 2x2 clusters
+    if (variant == 2) { launch_pp<1, 1>(g, A_hi, A_lo, st, num_sms); return; }
+    if (variant == 9) { launch_pp<2, 1>(g, A_hi, A_lo, st, num_sms); return; }
+    if (variant == 10) { launch_pp<1, 2>(g, A_hi, A_lo, st, num_sms); return; }
+    if (variant == 11) { launch_pp<2, 2>(g, A_hi, A_lo, st, num_sms); return; }
     if (variant == 1 || (variant >= 4 && variant <= 8)) {
         const int num_k = (g.K + BK - 1) / BK;
         int sp = (variant == 5 || variant == 7) ? 2 : (variant == 6 || variant == 8) ? 4 : 1;
@@ -547,9 +619,14 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
         else launch<32, 10, 5>(g, A_hi, A_lo, st, num_sms, sp);
         return;
     }
-    // 128-wide tiles while they still cover half the SMs, else 64-wide ones
-    if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) launch_pp(g, A_hi, A_lo, st, num_sms);
-    else {
+    // 128-wide tiles while they still cover half the SMs, else 64-wide ones.  The 128-wide kernel's mainloop is bound by
+    // how fast L2 feeds its k-slabs (6.5-7.4 TB/s at every encoder shape, on lone CTAs), so from K = 1024 it runs in 2x2
+    // clusters, which read each slab from L2 once for two tiles; a shorter K (the conv stem's 384) spends more on the
+    // cluster's lockstep ring fill than it saves.  bf16x3 stays on lone CTAs.
+    if (g.N >= 128 && ((g.M + BM - 1) / BM) * ((g.N + 127) / 128) >= num_sms / 2) {
+        if (g.K >= 1024) launch_pp<2, 2>(g, A_hi, A_lo, st, num_sms);
+        else launch_pp<1, 1>(g, A_hi, A_lo, st, num_sms);
+    } else {
         // Short, narrow problems (the decoder's per-token GEMMs) cannot fill the GPU with output tiles alone and
         // a CTA walking all of K pays one TMA round trip per ring refill.  The K range is split across CTAs
         // (serial fix-up in the epilogue, see gemm_tc_kernel) until the grid covers the SMs.

@@ -92,6 +92,35 @@ __device__ __forceinline__ void mbar_wait_mma(uint32_t bar, uint32_t parity) {
     }
 }
 
+// ---- thread-block clusters ------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ uint32_t num_clusters_x() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+    return r;
+}
+// arrive on the mbarrier at shared-memory offset `bar` of cluster rank `cta` (the calling CTA included).  The release is
+// CTA-scoped: a .cluster-scoped one compiles to MEMBAR.SC.GPU, which waits for all of the thread's outstanding global
+// stores.  Releasing a ring stage needs no more than the retired wgmma reads of it (wgmma.wait_group).
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+// every thread of every CTA of the cluster: the cluster-wide __syncthreads
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+
 // ---- warpgroup register budget and named barriers (warp-specialised kernels) -----------
 // setmaxnreg: every thread of the warpgroup executes it; the producer gives registers back, the consumers take them.
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
@@ -144,6 +173,17 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1)
+        : "memory");
+}
+
+// The same load written to the same shared-memory offset of every CTA of the cluster in cta_mask (bit i: cluster rank i);
+// each destination's mbarrier at offset `bar` receives the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int32_t c0,
+                                                      int32_t c1, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
 

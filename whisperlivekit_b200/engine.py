@@ -255,7 +255,8 @@ class WhisperEngine(L.Engine):
     # -- op-level (device pointers, e.g. torch tensors' data_ptr()) ----------------------
     def op_gemm(self, backend: str, A_ptr, a_type, lda, W_ptr, w_type, ldw, bias_ptr, C_ptr, c_type, ldc,
                 M, N, K, gelu=False):
-        be = {"simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05, "tcgen05_1cta": 3, "tcgen05_pair": 4}[backend]
+        be = {"simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05, "tcgen05_1cta": 3, "tcgen05_pair": 4,
+              "tcgen05_pp2x1": 5, "tcgen05_pp1x2": 6, "tcgen05_pp2x2": 7}[backend]
         L.check(self.lib.wlk_op_gemm(self.h, be, A_ptr, a_type, lda, W_ptr, w_type, ldw, bias_ptr, C_ptr, c_type,
                                      ldc, M, N, K, int(gelu)))
 
