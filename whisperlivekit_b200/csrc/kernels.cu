@@ -1,5 +1,6 @@
 // Non-GEMM kernels of the streaming-Whisper hot path (sm_90a).  Everything here is
 // bandwidth- or latency-bound SIMT code; the tensor-core kernels live in gemm_tc.cu / attn_tc.cu.
+#include "attn_warp.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
 
@@ -559,41 +560,18 @@ void enc_attention_simt(const void* qkv, int type, int batch, int n_head, int d_
     CUDA_CHECK(cudaGetLastError());
 }
 
-template <typename T> struct RowVec;          // 16-byte slice of a 64-wide K/V row held by one lane
-template <> struct RowVec<bf16> {
-    static constexpr int N = 8;
-    typedef uint4 Raw;
-    static __device__ __forceinline__ Raw load(const bf16* p) { return *reinterpret_cast<const uint4*>(p); }
-    static __device__ __forceinline__ void unpack(const Raw& u, float* o) {
-        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { o[2 * i] = __low2float(h[i]); o[2 * i + 1] = __high2float(h[i]); }
-    }
-};
-template <> struct RowVec<float> {
-    static constexpr int N = 4;
-    typedef float4 Raw;
-    static __device__ __forceinline__ Raw load(const float* p) { return *reinterpret_cast<const float4*>(p); }
-    static __device__ __forceinline__ void unpack(const Raw& v, float* o) { o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w; }
-};
-
-
 // =====================================================================================
 // decoder self-attention over the per-session self-KV cache (causal)
 //   (reference whisper/model.py:109-114,130-146,148-173 with the triu(-inf) mask of :278)
 //   grid (H, jobs), 128 threads; queries processed one after the other
 // =====================================================================================
-// One warp per query row (8 queries in flight per CTA), no block-level synchronisation: lanes own keys
-// lane, lane+32, ... for the scores (whole 64-wide K rows per lane, 128-bit loads), softmax by warp shuffles,
-// then lanes own two output dims each and walk the keys with the probabilities broadcast by shuffle.
+// One warp per query row (8 queries in flight per CTA), no block-level synchronisation: attend_row_warp (attn_warp.cuh).
 template <typename T, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 dec_self_attn_kernel(const T* __restrict__ q, const DecJob* __restrict__ jobs, int layer, int n_head, int d_model,
                      int n_text_ctx, T* __restrict__ out) {
     ptx::griddep_launch();                   // programmatic dependent launch: see launch_pdl (common.cuh)
     ptx::griddep_wait();
-    constexpr int MAXK = 14;                 // ceil(448 / 32) keys per lane
-    constexpr int VN = RowVec<T>::N;
     __shared__ float qs[WARPS][64];
     const DecJob job = jobs[blockIdx.y];
     const int h = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -601,65 +579,12 @@ dec_self_attn_kernel(const T* __restrict__ q, const DecJob* __restrict__ jobs, i
     const T* Vc = reinterpret_cast<const T*>(job.self_kv) + (((int64_t)layer * 2 + 1) * n_head + h) * n_text_ctx * 64;
     for (int t = warp; t < job.n_rows; t += WARPS) {
         const int64_t row = job.row_off + t;
-        const int n_keys = job.offset + t + 1;            // causal: keys 0 .. position
         qs[warp][lane] = to_f32(q[row * d_model + h * 64 + lane]);
         qs[warp][lane + 32] = to_f32(q[row * d_model + h * 64 + lane + 32]);
         __syncwarp();
-        float sc[MAXK];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < MAXK; ++i) {
-            const int key = lane + 32 * i;
-            float a = -INFINITY;
-            if (key < n_keys) {
-                a = 0.f;
-                const T* kr = Kc + (int64_t)key * 64;
-#pragma unroll
-                for (int c = 0; c < 64 / VN; ++c) {
-                    float kv[VN];
-                    RowVec<T>::unpack(RowVec<T>::load(kr + c * VN), kv);
-#pragma unroll
-                    for (int j = 0; j < VN; ++j) a = fmaf(qs[warp][c * VN + j], kv[j], a);
-                }
-            }
-            sc[i] = a;
-            mx = fmaxf(mx, a);
-        }
-        mx = warp_max(mx);
-        float sum = 0.f;
-#pragma unroll
-        for (int i = 0; i < MAXK; ++i) {
-            const float p = (lane + 32 * i < n_keys) ? expf(sc[i] - mx) : 0.f;
-            sc[i] = p;
-            sum += p;
-        }
-        sum = warp_sum(sum);
-        float o0 = 0.f, o1 = 0.f;
-#pragma unroll
-        for (int i = 0; i < MAXK; ++i) {
-            if (32 * i >= n_keys) break;                   // warp-uniform
-            const int lim = min(32, n_keys - 32 * i);
-            // 16 V rows are fetched before any is used: a serial walk would expose one global-load latency per key
-            for (int l0 = 0; l0 < lim; l0 += 16) {
-                float v0[16], v1[16];
-#pragma unroll
-                for (int u = 0; u < 16; ++u) {
-                    const int key = 32 * i + min(l0 + u, lim - 1);
-                    const T* vr = Vc + (int64_t)key * 64 + 2 * lane;
-                    v0[u] = to_f32(vr[0]);
-                    v1[u] = to_f32(vr[1]);
-                }
-#pragma unroll
-                for (int u = 0; u < 16; ++u) {
-                    const float p = (l0 + u < lim) ? __shfl_sync(0xffffffffu, sc[i], (l0 + u) & 31) : 0.f;
-                    o0 = fmaf(p, v0[u], o0);
-                    o1 = fmaf(p, v1[u], o1);
-                }
-            }
-        }
-        const float inv = 1.0f / sum;
-        out[row * d_model + h * 64 + 2 * lane] = from_f32<T>(o0 * inv);
-        out[row * d_model + h * 64 + 2 * lane + 1] = from_f32<T>(o1 * inv);
+        // causal: keys 0 .. position; ceil(448 / 32) = 14 keys per lane
+        attend_row_warp<T, 14>(qs[warp], job.offset + t + 1, [&](int key) { return Kc + (int64_t)key * 64; },
+                               [&](int key) { return Vc + (int64_t)key * 64; }, out + row * d_model + h * 64);
         __syncwarp();
     }
 }

@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "../../include/wlk_b200.h"
+#include "attn_warp.cuh"
 #include "host.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -137,13 +138,12 @@ __global__ void qwen_pos_kernel(const int32_t* __restrict__ pos, const float* __
 // Attention of one round (reference causal.py:292-376): a query at position p sees keys at positions
 //   [p - left_ctx + 1, block_max]   (block-bidirectional)   or   [p - left_ctx + 1, p]   (causal),
 // clipped at 0; keys live in the session's ring at slot = position % ring (this round's keys were written by the
-// QKV GEMM).  q arrives pre-scaled by head_dim^-0.5.  One warp per query, grid (head, job); fp32 softmax.
+// QKV GEMM).  q arrives pre-scaled by head_dim^-0.5.  One warp per query (attend_row_warp), grid (head, job).
 // ---------------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(128)
 qwen_attention_kernel(const T* __restrict__ q, const QJob* __restrict__ jobs, int layer, int n_head, int d_model, int ring,
                       int left_ctx, int bidir, T* __restrict__ out) {
-    constexpr int MAXK = 16;                    // keys per lane: ring <= 512
     __shared__ float qs[4][64];
     const QJob job = jobs[blockIdx.y];
     const int h = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -157,47 +157,9 @@ qwen_attention_kernel(const T* __restrict__ q, const QJob* __restrict__ jobs, in
         qs[warp][lane + 32] = to_f32(q[row * d_model + h * 64 + lane + 32]);
         __syncwarp();
         const int lo = max(0, p - left_ctx + 1), hi = bidir ? block_max : p;
-        const int nk = hi - lo + 1;
-        float sc[MAXK];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            const int ki = lane + 32 * j;
-            sc[j] = -INFINITY;
-            if (ki < nk) {
-                const T* kr = kbase + (int64_t)((lo + ki) % ring) * 64;
-                float acc = 0.f;
-#pragma unroll 8
-                for (int e = 0; e < 64; ++e) acc = fmaf(qs[warp][e], to_f32(kr[e]), acc);
-                sc[j] = acc;
-                mx = fmaxf(mx, acc);
-            }
-        }
-        mx = warp_max(mx);
-        float sum = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            const float pexp = (lane + 32 * j < nk) ? expf(sc[j] - mx) : 0.f;
-            sc[j] = pexp;
-            sum += pexp;
-        }
-        sum = warp_sum(sum);
-        float o0 = 0.f, o1 = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            if (32 * j >= nk) break;
-            for (int l = 0; l < 32; ++l) {
-                const int ki = 32 * j + l;
-                if (ki >= nk) break;
-                const float pw = __shfl_sync(0xffffffffu, sc[j], l);
-                const T* vr = vbase + (int64_t)((lo + ki) % ring) * 64;
-                o0 = fmaf(pw, to_f32(vr[2 * lane]), o0);
-                o1 = fmaf(pw, to_f32(vr[2 * lane + 1]), o1);
-            }
-        }
-        const float inv = 1.0f / sum;
-        out[row * d_model + h * 64 + 2 * lane] = from_f32<T>(o0 * inv);
-        out[row * d_model + h * 64 + 2 * lane + 1] = from_f32<T>(o1 * inv);
+        // 16 keys per lane: ring <= 512
+        attend_row_warp<T, 16>(qs[warp], hi - lo + 1, [&](int ki) { return kbase + (int64_t)((lo + ki) % ring) * 64; },
+                               [&](int ki) { return vbase + (int64_t)((lo + ki) % ring) * 64; }, out + row * d_model + h * 64);
         __syncwarp();
     }
 }
@@ -921,10 +883,9 @@ qwin_attn_mma_kernel(const bf16* __restrict__ qkv, const WAttn* __restrict__ ite
     }
 }
 
-// The fp32 parity variant: SIMT, one warp per query row, keys read from global memory, fp32 softmax.
+// The fp32 parity variant: SIMT, one warp per query row (attend_row_warp), keys read from global memory.
 __global__ void __launch_bounds__(128)
 qwin_attn_simt_kernel(const float* __restrict__ qkv, const WAttn* __restrict__ items, int d, float* __restrict__ out) {
-    constexpr int MAXK = QW_KMAX / 32;
     __shared__ float qs[4][64];
     const WAttn it = items[blockIdx.x];
     const int h = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -937,45 +898,9 @@ qwin_attn_simt_kernel(const float* __restrict__ qkv, const WAttn* __restrict__ i
         qs[warp][lane] = qrow[lane];
         qs[warp][lane + 32] = qrow[lane + 32];
         __syncwarp();
-        float sc[MAXK];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            const int ki = lane + 32 * j;
-            sc[j] = -INFINITY;
-            if (ki < nk) {
-                const float* kr = kbase + ki * ld;
-                float acc = 0.f;
-#pragma unroll 8
-                for (int e = 0; e < 64; ++e) acc = fmaf(qs[warp][e], kr[e], acc);
-                sc[j] = acc;
-                mx = fmaxf(mx, acc);
-            }
-        }
-        mx = warp_max(mx);
-        float sum = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            const float p = (lane + 32 * j < nk) ? expf(sc[j] - mx) : 0.f;
-            sc[j] = p;
-            sum += p;
-        }
-        sum = warp_sum(sum);
-        float o0 = 0.f, o1 = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) {
-            if (32 * j >= nk) break;
-            for (int l = 0; l < 32; ++l) {
-                const int ki = 32 * j + l;
-                if (ki >= nk) break;
-                const float pw = __shfl_sync(0xffffffffu, sc[j], l);
-                o0 = fmaf(pw, vbase[ki * ld + 2 * lane], o0);
-                o1 = fmaf(pw, vbase[ki * ld + 2 * lane + 1], o1);
-            }
-        }
-        const float inv = 1.0f / sum;
-        out[(int64_t)(it.row0 + qi) * d + h * 64 + 2 * lane] = o0 * inv;
-        out[(int64_t)(it.row0 + qi) * d + h * 64 + 2 * lane + 1] = o1 * inv;
+        attend_row_warp<float, QW_KMAX / 32>(qs[warp], nk, [&](int ki) { return kbase + ki * ld; },
+                                             [&](int ki) { return vbase + ki * ld; },
+                                             out + (int64_t)(it.row0 + qi) * d + h * 64);
         __syncwarp();
     }
 }
