@@ -393,7 +393,7 @@ void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev) {
                 split_f32_planes_async(reinterpret_cast<const float*>(e->qkv), hi, lo, (int64_t)M * 3 * d, e->st);
                 enc_attention_tcgen05_x3(hi, lo, n, D.n_audio_head, d, reinterpret_cast<float*>(e->att), e->st);
             } else if (e->attn_backend == WLK_BACKEND_TCGEN05)
-                enc_attention_tcgen05(e->qkv, n, D.n_audio_head, d, e->att, e->st);
+                enc_attention_tcgen05(e->qkv, n, D.n_audio_head, d, e->att, e->num_sms, e->st);
             else
                 enc_attention_simt(e->qkv, e->act, n, D.n_audio_head, d, e->att, e->st); }
         {   GemmArgs g;
@@ -1542,7 +1542,7 @@ int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int ty
     ProfScope ps(e, WLK_KC_MISC, 4.0 * batch * e->dims.n_audio_head * (double)N_CTX * N_CTX * 64, 0);
     if (backend == WLK_BACKEND_TCGEN05) {
         WLK_CHECK(type == DT_BF16, "tcgen05 attention needs bf16");
-        enc_attention_tcgen05(qkv, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st);
+        enc_attention_tcgen05(qkv, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->num_sms, e->st);
     } else {
         enc_attention_simt(qkv, type, batch, e->dims.n_audio_head, e->dims.n_audio_state, out, e->st);
     }
