@@ -34,10 +34,7 @@ static const char* kClassNames[WLK_KC_COUNT] = {"mel", "gemm_enc", "attn_enc", "
                                                 "attn_dec_self", "attn_dec_cross", "logits", "align", "misc"};
 
 struct EncLayerW { float *ln1w, *ln1b, *bqkv, *bo, *ln2w, *ln2b, *b1, *b2; void *Wqkv, *Wo, *W1, *W2; };
-struct DecLayerW {
-    float *ln1w, *ln1b, *bqkv, *bo, *lncw, *lncb, *bqc, *boc, *ln2w, *ln2b, *b1, *b2;
-    void *Wqkv, *Wo, *Wqc, *Woc, *W1, *W2;
-};
+struct DecLayerW : EncLayerW { float *lncw, *lncb, *bqc, *boc; void *Wqc, *Woc; };   // + the cross-attention sub-block
 struct Weights {
     float *filtT, *window; float2* twiddle; int2* filt_span;
     void *Wc1, *Wc2; float *bc1, *bc2, *enc_pos;
@@ -272,11 +269,61 @@ Session& get_root_session(wlk_engine* e, int32_t sid, const char* what) {
     WLK_CHECK(s.parent < 0, "session %d is a beam fork of session %d: %s belongs to the parent", sid, s.parent, what);
     return s;
 }
+// a new decoding epoch of one session: no token fed, no alignment row
+void reset_decoder(Session& s) { s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear(); }
+
+// ---------------------------------------------------------------------------------------
+// one pre-LN residual block (model.py:163-170), the same for the encoder's layers and the decoder's
+// ---------------------------------------------------------------------------------------
+// Rows [0, R) of the fp32 residual x (width dm): LN -> fused QKV (bias, 64^-0.25 on q and k) -> attend -> out-projection
+// + residual -> between -> LN -> FC1 + GELU -> FC2 + residual.  qkv_dst(epi) points the QKV epilogue at the path's
+// destination; attend() runs the path's attention into att inside its own ProfScope; between() is the decoder's
+// cross-attention sub-block and nothing in the encoder.  cls profiles the GEMMs, ln_bytes is what each LayerNorm records.
+template <typename QkvDst, typename Attend, typename Between>
+void run_block(wlk_engine* e, const EncLayerW& L, float* x, void* xn, void* att, void* hid, int dm, int R, int cls,
+               double ln_bytes, QkvDst qkv_dst, Attend attend, Between between) {
+    {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
+        layernorm(x, dm, L.ln1w, L.ln1b, xn, e->act, dm, R, dm, nullptr, e->st); }
+    {   GemmArgs g;
+        g.A = xn; g.a_type = e->act; g.lda = dm; g.W = L.Wqkv; g.w_type = e->wt; g.ldw = dm;
+        g.M = R; g.N = 3 * dm; g.K = dm;
+        g.epi.bias = L.bqkv; g.epi.col_scale = powf(64.0f, -0.25f); g.epi.scale_cols = 2 * dm;   // model.py:152
+        g.epi.c_type = e->act;
+        qkv_dst(g.epi);
+        run_gemm(e, g, cls); }
+    attend();
+    {   GemmArgs g;
+        g.A = att; g.a_type = e->act; g.lda = dm; g.W = L.Wo; g.w_type = e->wt; g.ldw = dm;
+        g.M = R; g.N = dm; g.K = dm;
+        g.epi.bias = L.bo; g.epi.residual = x; g.epi.ldr = dm; g.epi.C = x; g.epi.c_type = DT_F32; g.epi.ldc = dm;
+        run_gemm(e, g, cls); }
+    between();
+    {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
+        layernorm(x, dm, L.ln2w, L.ln2b, xn, e->act, dm, R, dm, nullptr, e->st); }
+    {   GemmArgs g;
+        g.A = xn; g.a_type = e->act; g.lda = dm; g.W = L.W1; g.w_type = e->wt; g.ldw = dm;
+        g.M = R; g.N = 4 * dm; g.K = dm;
+        g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = hid; g.epi.c_type = e->act; g.epi.ldc = 4 * dm;
+        run_gemm(e, g, cls); }
+    {   GemmArgs g;
+        g.A = hid; g.a_type = e->act; g.lda = 4 * dm; g.W = L.W2; g.w_type = e->wt; g.ldw = 4 * dm;
+        g.M = R; g.N = dm; g.K = 4 * dm;
+        g.epi.bias = L.b2; g.epi.residual = x; g.epi.ldr = dm; g.epi.C = x; g.epi.c_type = DT_F32; g.epi.ldc = dm;
+        run_gemm(e, g, cls); }
+}
 
 // ---------------------------------------------------------------------------------------
 // encode: log-mel -> conv stem -> L encoder blocks -> ln_post -> cross-K/V for every decoder layer
 // ---------------------------------------------------------------------------------------
-void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev);
+// Checks a batch to encode before any session state is touched
+void check_encode_batch(wlk_engine* e, const int32_t* sids, int n) {
+    WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
+    e->sess.check_batch(sids, n);
+    for (int i = 0; i < n; ++i) {
+        Session& s = get_root_session(e, sids[i], "encode");
+        WLK_CHECK(s.audio_len > 0, "session %d has no audio", sids[i]);
+    }
+}
 
 // One session's log-mel job (shared by the parity and the incremental encode): fills `mj`, moves the reusable raw rows of
 // the incremental log-mel, sets s.content_len.
@@ -317,40 +364,66 @@ void fill_mel_job(wlk_engine* e, Session& s, MelJob& mj, int i, int& max_frames)
     s.content_len = (int)((n_total - N_FRAMES) / 2);            // simul_whisper.py:350 (unclamped: the policy's
 }                                                               // frame_threshold test needs the true value)
 
-void encode_batch(wlk_engine* e, const int32_t* sids, int n, int32_t* content_out) {
-    const wlk_dims& D = e->dims;
-    Weights& W = e->w;
-    const int nm = D.n_mels;
-    const size_t es = e->es();
-    WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
-    // first pass: validation only (no session state is touched until the whole batch is known to be good)
-    e->sess.check_batch(sids, n);
-    for (int i = 0; i < n; ++i) {
-        Session& s = get_root_session(e, sids[i], "encode");
-        WLK_CHECK(s.audio_len > 0, "session %d has no audio", sids[i]);
-    }
-    Stager sg(e->stg);
-    MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(n, &mj_dev);
-    void** xkv_dev; void** xkv = sg.host<void*>(n, &xkv_dev);
+// The log-mel of every stream into e->mel_t: each stream's mel job, then stage(i, s) stages what the encode mode needs
+// of it; then the staging block goes up and mel_forward runs.
+template <typename Stage>
+void run_mel(wlk_engine* e, Stager& sg, const int32_t* sids, int n, MelJob* mj, const MelJob* mj_dev,
+             int32_t* content_out, Stage stage) {
+    const Weights& W = e->w;
+    const int nm = e->dims.n_mels;
     int max_frames = 1;
     for (int i = 0; i < n; ++i) {
         Session& s = e->sess[sids[i]];
         fill_mel_job(e, s, mj[i], i, max_frames);
         content_out[i] = s.content_len;
-        xkv[i] = s.cross_kv;
+        stage(i, s);
     }
     sg.upload(e->st);
-
-    {   ProfScope ps(e, WLK_KC_MEL, 0, (double)n * (480000.0 * 4 + 3000.0 * nm * es));
+    {   ProfScope ps(e, WLK_KC_MEL, 0, (double)n * (480000.0 * 4 + 3000.0 * nm * e->es()));
         mel_forward(mj_dev, n, nm, W.filtT, W.window, W.twiddle, W.filt_span, e->act, max_frames, e->st); }
-    run_encoder(e, sids, n, xkv_dev);
 }
 
-// conv stem -> L encoder blocks -> ln_post -> cross-K/V, from the time-major mel of `n` streams in e->mel_t
+// The L encoder blocks over the R rows of e->x (qkv_dst(epi, layer) and attend(layer) as in run_block), ln_post,
+// write_xa() puts the rows into the streams' xa, then the cross-attention K/V of every decoder layer in one GEMM,
+// scattered head-major into stream i's xkv_dev[i] (row_slot / row_pos place each row; null: N_CTX rows per stream in
+// order), and a new decoding epoch for the streams and their beam forks.
+template <typename QkvDst, typename Attend, typename WriteXa>
+void run_encoder_layers(wlk_engine* e, const int32_t* sids, int n, int R, void** xkv_dev, const int32_t* row_slot,
+                        const int32_t* row_pos, QkvDst qkv_dst, Attend attend, WriteXa write_xa) {
+    const wlk_dims& D = e->dims;
+    Weights& W = e->w;
+    const int d = D.n_audio_state, dt = D.n_text_state;
+    const double ln_bytes = (double)R * d * (4 + e->es());
+    for (int li = 0; li < D.n_audio_layer; ++li)
+        run_block(e, W.enc[li], e->x, e->xn, e->att, e->hid, d, R, WLK_KC_GEMM_ENC, ln_bytes,
+                  [&](Epilogue& epi) { qkv_dst(epi, li); }, [&] { attend(li); }, [] {});
+    {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
+        layernorm(e->x, d, W.lnpw, W.lnpb, e->xn, e->act, d, R, d, nullptr, e->st); }
+    write_xa();
+    {   GemmArgs g;
+        g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = W.Wxkv; g.w_type = e->wt; g.ldw = d;
+        g.M = R; g.N = D.n_text_layer * 2 * dt; g.K = d;
+        g.epi.bias = W.bxkv; g.epi.col_scale = powf(64.0f, -0.25f); g.epi.scale_cols = dt; g.epi.scale_period = 2 * dt;
+        g.epi.mode = EPI_XKV; g.epi.batch_ptrs = xkv_dev; g.epi.rows_per_batch = N_CTX;
+        g.epi.row_slot = row_slot; g.epi.row_pos = row_pos;
+        g.epi.n_head = D.n_text_head; g.epi.d_model = dt; g.epi.kv_len = N_CTX; g.epi.c_type = e->act;
+        run_gemm(e, g, WLK_KC_GEMM_XKV); }
+    for (int i = 0; i < n; ++i) {
+        Session& s = e->sess[sids[i]];
+        s.encoded = true;
+        reset_decoder(s);
+        if (s.n_forks)
+            for (auto& f : e->sess)
+                if (f.open && f.parent == sids[i]) reset_decoder(f);
+    }
+}
+
+// the parity encoder: conv stem -> L encoder blocks -> ln_post -> cross-K/V, from the time-major mel of `n` streams in
+// e->mel_t, every stream's whole window
 void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev) {
     const wlk_dims& D = e->dims;
     Weights& W = e->w;
-    const int d = D.n_audio_state, dt = D.n_text_state, nm = D.n_mels;
+    const int d = D.n_audio_state, nm = D.n_mels;
     const size_t es = e->es();
 
     // conv1 (k=3, pad=1) as a GEMM over overlapping rows of the time-major mel: row t = frames t-1..t+1
@@ -373,19 +446,10 @@ void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev) {
         run_gemm(e, g, WLK_KC_GEMM_ENC); }
 
     const int M = n * N_CTX;
-    const float qk_scale = powf(64.0f, -0.25f);                     // model.py:152
-    for (int li = 0; li < D.n_audio_layer; ++li) {
-        EncLayerW& L = W.enc[li];
-        {   ProfScope ps(e, WLK_KC_LN, 0, (double)M * d * (4 + es));
-            layernorm(e->x, d, L.ln1w, L.ln1b, e->xn, e->act, d, M, d, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = L.Wqkv; g.w_type = e->wt; g.ldw = d;
-            g.M = M; g.N = 3 * d; g.K = d;
-            g.epi.bias = L.bqkv; g.epi.col_scale = qk_scale; g.epi.scale_cols = 2 * d;
-            g.epi.C = e->qkv; g.epi.c_type = e->act; g.epi.ldc = 3 * d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   ProfScope ps(e, WLK_KC_ATTN_ENC, 4.0 * n * D.n_audio_head * (double)N_CTX * N_CTX * 64,
-                         (double)M * 4 * d * es);
+    run_encoder_layers(e, sids, n, M, xkv_dev, nullptr, nullptr,
+        [&](Epilogue& epi, int) { epi.C = e->qkv; epi.ldc = 3 * d; },
+        [&](int) {
+            ProfScope ps(e, WLK_KC_ATTN_ENC, 4.0 * n * D.n_audio_head * (double)N_CTX * N_CTX * 64, (double)M * 4 * d * es);
             if (e->attn_backend == WLK_BACKEND_TCGEN05 && e->wt == DT_BF16X2) {
                 // split the fp32 q|k|v into (hi, lo) planes (the GEMM operand scratch is idle between GEMMs)
                 bf16* hi = reinterpret_cast<bf16*>(e->a_split);
@@ -395,51 +459,26 @@ void run_encoder(wlk_engine* e, const int32_t* sids, int n, void** xkv_dev) {
             } else if (e->attn_backend == WLK_BACKEND_TCGEN05)
                 enc_attention_tcgen05(e->qkv, n, D.n_audio_head, d, e->att, e->num_sms, e->st);
             else
-                enc_attention_simt(e->qkv, e->act, n, D.n_audio_head, d, e->att, e->st); }
-        {   GemmArgs g;
-            g.A = e->att; g.a_type = e->act; g.lda = d; g.W = L.Wo; g.w_type = e->wt; g.ldw = d;
-            g.M = M; g.N = d; g.K = d;
-            g.epi.bias = L.bo; g.epi.residual = e->x; g.epi.ldr = d;
-            g.epi.C = e->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   ProfScope ps(e, WLK_KC_LN, 0, (double)M * d * (4 + es));
-            layernorm(e->x, d, L.ln2w, L.ln2b, e->xn, e->act, d, M, d, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = L.W1; g.w_type = e->wt; g.ldw = d;
-            g.M = M; g.N = 4 * d; g.K = d;
-            g.epi.bias = L.b1; g.epi.gelu = 1;
-            g.epi.C = e->hid; g.epi.c_type = e->act; g.epi.ldc = 4 * d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   GemmArgs g;
-            g.A = e->hid; g.a_type = e->act; g.lda = 4 * d; g.W = L.W2; g.w_type = e->wt; g.ldw = 4 * d;
-            g.M = M; g.N = d; g.K = 4 * d;
-            g.epi.bias = L.b2; g.epi.residual = e->x; g.epi.ldr = d;
-            g.epi.C = e->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-    }
-    {   ProfScope ps(e, WLK_KC_LN, 0, (double)M * d * (4 + es));
-        layernorm(e->x, d, W.lnpw, W.lnpb, e->xn, e->act, d, M, d, nullptr, e->st); }
+                enc_attention_simt(e->qkv, e->act, n, D.n_audio_head, d, e->att, e->st);
+        },
+        [&] {
+            for (int i = 0; i < n; ++i)
+                CUDA_CHECK(cudaMemcpyAsync(e->sess[sids[i]].xa, offs(e->xn, (size_t)i * N_CTX * d, es),
+                                           (size_t)N_CTX * d * es, cudaMemcpyDeviceToDevice, e->st));
+        });
     for (int i = 0; i < n; ++i) {
         Session& s = e->sess[sids[i]];
-        CUDA_CHECK(cudaMemcpyAsync(s.xa, offs(e->xn, (size_t)i * N_CTX * d, es), (size_t)N_CTX * d * es,
-                                   cudaMemcpyDeviceToDevice, e->st));
-    }
-    // cross-attention K/V of every decoder layer in one GEMM, scattered head-major into each session
-    {   GemmArgs g;
-        g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = W.Wxkv; g.w_type = e->wt; g.ldw = d;
-        g.M = M; g.N = D.n_text_layer * 2 * dt; g.K = d;
-        g.epi.bias = W.bxkv; g.epi.col_scale = qk_scale; g.epi.scale_cols = dt; g.epi.scale_period = 2 * dt;
-        g.epi.mode = EPI_XKV; g.epi.batch_ptrs = xkv_dev; g.epi.rows_per_batch = N_CTX;
-        g.epi.n_head = D.n_text_head; g.epi.d_model = dt; g.epi.kv_len = N_CTX; g.epi.c_type = e->act;
-        run_gemm(e, g, WLK_KC_GEMM_XKV); }
-    for (int i = 0; i < n; ++i) {
-        Session& s = e->sess[sids[i]];
-        s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear(); s.encoded = true;
         s.inc_valid = false; s.rot = 0;                  // the parity encode writes every buffer in logical order
-        if (s.n_forks)                                   // a new epoch for the beams of this stream as well
-            for (auto& f : e->sess)
-                if (f.open && f.parent == sids[i]) { f.self_len = 0; f.align_rows = 0; f.iter_row_start.clear(); }
     }
+}
+
+void encode_batch(wlk_engine* e, const int32_t* sids, int n, int32_t* content_out) {
+    check_encode_batch(e, sids, n);
+    Stager sg(e->stg);
+    MelJob* mj_dev; MelJob* mj = sg.host<MelJob>(n, &mj_dev);
+    void** xkv_dev; void** xkv = sg.host<void*>(n, &xkv_dev);
+    run_mel(e, sg, sids, n, mj, mj_dev, content_out, [&](int i, Session& s) { xkv[i] = s.cross_kv; });
+    run_encoder(e, sids, n, xkv_dev);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -488,16 +527,11 @@ void ensure_incremental(wlk_engine* e, Session& s, int sid) {
 void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* content_out, int32_t* block_rows_out) {
     const wlk_dims& D = e->dims;
     Weights& W = e->w;
-    const int d = D.n_audio_state, dt = D.n_text_state, nm = D.n_mels, H = D.n_audio_head;
+    const int d = D.n_audio_state, nm = D.n_mels, H = D.n_audio_head;
     const size_t es = e->es();
     WLK_CHECK(e->act == DT_BF16 && e->wt == DT_BF16 && e->attn_backend == WLK_BACKEND_TCGEN05 && e->gemm_backend == WLK_BACKEND_TCGEN05,
               "the incremental encoder runs in the bf16 wgmma mode only");
-    WLK_CHECK(n >= 1 && n <= e->cfg.max_batch, "encode batch %d outside [1, %d]", n, e->cfg.max_batch);
-    e->sess.check_batch(sids, n);
-    for (int i = 0; i < n; ++i) {
-        Session& s = get_root_session(e, sids[i], "encode");
-        WLK_CHECK(s.audio_len > 0, "session %d has no audio", sids[i]);
-    }
+    check_encode_batch(e, sids, n);
     for (int i = 0; i < n; ++i) ensure_incremental(e, e->sess[sids[i]], sids[i]);
 
     Stager sg(e->stg);
@@ -506,12 +540,9 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
     DecJob* dj_dev; DecJob* dj = sg.host<DecJob>(n, &dj_dev);
     void** ekv_dev; void** ekv = sg.host<void*>(n, &ekv_dev);
     void** xkv_dev; void** xkv = sg.host<void*>(n, &xkv_dev);
-    int max_frames = 1, R = 0, R1 = 0, max_rows = 0;
+    int R = 0, R1 = 0, max_rows = 0;
     std::vector<int> new_rot(n), new_chunks(n);
-    for (int i = 0; i < n; ++i) {
-        Session& s = e->sess[sids[i]];
-        fill_mel_job(e, s, mj[i], i, max_frames);
-        content_out[i] = s.content_len;
+    run_mel(e, sg, sids, n, mj, mj_dev, content_out, [&](int i, Session& s) {
         const int C = std::min(s.content_len, N_CTX);
         int p0 = 0, p1 = N_CTX, rot = 0, chunks = 0;
         const bool whole = !s.inc_valid || s.inc_dropped % 320 != 0 || s.inc_dropped / 320 > s.inc_content ||
@@ -534,10 +565,7 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
         if (block_rows_out) block_rows_out[i] = len;
         R += len; R1 += 2 * len + 1;
         max_rows = std::max(max_rows, len);
-    }
-    sg.upload(e->st);
-    {   ProfScope ps(e, WLK_KC_MEL, 0, (double)n * (480000.0 * 4 + 3000.0 * nm * es));
-        mel_forward(mj_dev, n, nm, W.filtT, W.window, W.twiddle, W.filt_span, e->act, max_frames, e->st); }
+    });
 
     // conv stem over the block: gathered operand rows, two ordinary GEMMs
     void* A1 = e->h1; void* H1 = e->qkv; void* A2 = e->hid;
@@ -558,59 +586,25 @@ void encode_incremental(wlk_engine* e, const int32_t* sids, int n, int32_t* cont
         g.epi.C = e->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
         run_gemm(e, g, WLK_KC_GEMM_ENC); }
 
-    const float qk_scale = powf(64.0f, -0.25f);
-    for (int li = 0; li < D.n_audio_layer; ++li) {
-        EncLayerW& L = W.enc[li];
-        {   ProfScope ps(e, WLK_KC_LN, 0, (double)R * d * (4 + es));
-            layernorm(e->x, d, L.ln1w, L.ln1b, e->xn, e->act, d, R, d, nullptr, e->st); }
-        {   GemmArgs g;                                                   // q -> packed rows, k / v -> the ring slots
-            g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = L.Wqkv; g.w_type = e->wt; g.ldw = d;
-            g.M = R; g.N = 3 * d; g.K = d;
-            g.epi.bias = L.bqkv; g.epi.col_scale = qk_scale; g.epi.scale_cols = 2 * d;
-            g.epi.mode = EPI_SELF_QKV; g.epi.C = e->qkv; g.epi.ldc = d; g.epi.c_type = e->act;
-            g.epi.batch_ptrs = ekv_dev; g.epi.row_slot = e->inc_row_slot; g.epi.row_pos = e->inc_row_pos;
-            g.epi.layer = li; g.epi.n_head = H; g.epi.d_model = d; g.epi.kv_len = N_CTX;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   ProfScope ps(e, WLK_KC_ATTN_ENC, 4.0 * H * (double)R * N_CTX * 64, (double)n * 2 * d * N_CTX * es);
-            dec_cross_attention_tcgen05(e->qkv, R, dj_dev, n, max_rows, li, H, d, e->enc_maps_dev, e->enc_norank_dev, e->att, e->st); }
-        {   GemmArgs g;
-            g.A = e->att; g.a_type = e->act; g.lda = d; g.W = L.Wo; g.w_type = e->wt; g.ldw = d;
-            g.M = R; g.N = d; g.K = d;
-            g.epi.bias = L.bo; g.epi.residual = e->x; g.epi.ldr = d; g.epi.C = e->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   ProfScope ps(e, WLK_KC_LN, 0, (double)R * d * (4 + es));
-            layernorm(e->x, d, L.ln2w, L.ln2b, e->xn, e->act, d, R, d, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = L.W1; g.w_type = e->wt; g.ldw = d;
-            g.M = R; g.N = 4 * d; g.K = d;
-            g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = e->hid; g.epi.c_type = e->act; g.epi.ldc = 4 * d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-        {   GemmArgs g;
-            g.A = e->hid; g.a_type = e->act; g.lda = 4 * d; g.W = L.W2; g.w_type = e->wt; g.ldw = 4 * d;
-            g.M = R; g.N = d; g.K = 4 * d;
-            g.epi.bias = L.b2; g.epi.residual = e->x; g.epi.ldr = d; g.epi.C = e->x; g.epi.c_type = DT_F32; g.epi.ldc = d;
-            run_gemm(e, g, WLK_KC_GEMM_ENC); }
-    }
-    {   ProfScope ps(e, WLK_KC_LN, 0, (double)R * d * (4 + es));
-        layernorm(e->x, d, W.lnpw, W.lnpb, e->xn, e->act, d, R, d, nullptr, e->st); }
-    {   ProfScope ps(e, WLK_KC_MISC);
-        inc_scatter_rows(ij_dev, n, max_rows, d, e->xn, e->act, e->st); }
-    {   GemmArgs g;                                                       // cross-K/V of the block's rows only
-        g.A = e->xn; g.a_type = e->act; g.lda = d; g.W = W.Wxkv; g.w_type = e->wt; g.ldw = d;
-        g.M = R; g.N = D.n_text_layer * 2 * dt; g.K = d;
-        g.epi.bias = W.bxkv; g.epi.col_scale = qk_scale; g.epi.scale_cols = dt; g.epi.scale_period = 2 * dt;
-        g.epi.mode = EPI_XKV; g.epi.batch_ptrs = xkv_dev; g.epi.rows_per_batch = N_CTX;
-        g.epi.row_slot = e->inc_row_slot; g.epi.row_pos = e->inc_row_pos;
-        g.epi.n_head = D.n_text_head; g.epi.d_model = dt; g.epi.kv_len = N_CTX; g.epi.c_type = e->act;
-        run_gemm(e, g, WLK_KC_GEMM_XKV); }
+    // the block's rows only: cross-K/V and xa into their ring slots
+    run_encoder_layers(e, sids, n, R, xkv_dev, e->inc_row_slot, e->inc_row_pos,
+        [&](Epilogue& epi, int li) {                                      // q -> packed rows, k / v -> the ring slots
+            epi.mode = EPI_SELF_QKV; epi.C = e->qkv; epi.ldc = d;
+            epi.batch_ptrs = ekv_dev; epi.row_slot = e->inc_row_slot; epi.row_pos = e->inc_row_pos;
+            epi.layer = li; epi.n_head = H; epi.d_model = d; epi.kv_len = N_CTX;
+        },
+        [&](int li) {
+            ProfScope ps(e, WLK_KC_ATTN_ENC, 4.0 * H * (double)R * N_CTX * 64, (double)n * 2 * d * N_CTX * es);
+            dec_cross_attention_tcgen05(e->qkv, R, dj_dev, n, max_rows, li, H, d, e->enc_maps_dev, e->enc_norank_dev, e->att, e->st);
+        },
+        [&] {
+            ProfScope ps(e, WLK_KC_MISC);
+            inc_scatter_rows(ij_dev, n, max_rows, d, e->xn, e->act, e->st);
+        });
     for (int i = 0; i < n; ++i) {
         Session& s = e->sess[sids[i]];
-        s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear(); s.encoded = true;
         s.inc_valid = true; s.rot = new_rot[i]; s.inc_chunks = new_chunks[i];
         s.inc_content = std::min(s.content_len, N_CTX); s.inc_dropped = 0;
-        if (s.n_forks)
-            for (auto& f : e->sess)
-                if (f.open && f.parent == sids[i]) { f.self_len = 0; f.align_rows = 0; f.iter_row_start.clear(); }
     }
 }
 
@@ -667,60 +661,45 @@ void decode_batch(wlk_engine* e, const int32_t* sids, int n, const int32_t* toke
         embed_tokens(tok_dev, pos_dev, W.emb_f32, W.dec_pos, e->dx, R, dt, e->st); }
     const float qk_scale = powf(64.0f, -0.25f);
     for (int li = 0; li < D.n_text_layer; ++li) {
-        DecLayerW& L = W.dec[li];
-        {   ProfScope ps(e, WLK_KC_LN);
-            layernorm(e->dx, dt, L.ln1w, L.ln1b, e->dxn, e->act, dt, R, dt, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->dxn; g.a_type = e->act; g.lda = dt; g.W = L.Wqkv; g.w_type = e->wt; g.ldw = dt;
-            g.M = R; g.N = 3 * dt; g.K = dt;
-            g.epi.bias = L.bqkv; g.epi.col_scale = qk_scale; g.epi.scale_cols = 2 * dt;
-            g.epi.mode = EPI_SELF_QKV; g.epi.C = e->dq; g.epi.ldc = dt; g.epi.c_type = e->act;
-            g.epi.batch_ptrs = skv_dev; g.epi.row_slot = slot_dev; g.epi.row_pos = pos_dev;
-            g.epi.layer = li; g.epi.n_head = H; g.epi.d_model = dt; g.epi.kv_len = ctx;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
-        {   ProfScope ps(e, WLK_KC_ATTN_DEC_SELF);
-            // prefills on the tensor cores (causal, per-session cache planes through TMA); token steps and the fp32
-            // modes on the SIMT kernel
-            if (e->attn_backend == WLK_BACKEND_TCGEN05 && e->act == DT_BF16 && max_tq >= 16)
-                dec_self_attention_tcgen05(e->dq, R, dj_dev, n, max_tq, li, H, dt, ctx, e->self_maps_dev, e->datt, e->st);
-            else
-                dec_self_attention(e->dq, e->act, dj_dev, n, li, H, dt, ctx, e->datt, max_tq, e->st); }
-        {   GemmArgs g;
-            g.A = e->datt; g.a_type = e->act; g.lda = dt; g.W = L.Wo; g.w_type = e->wt; g.ldw = dt;
-            g.M = R; g.N = dt; g.K = dt;
-            g.epi.bias = L.bo; g.epi.residual = e->dx; g.epi.ldr = dt; g.epi.C = e->dx; g.epi.c_type = DT_F32; g.epi.ldc = dt;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
-        {   ProfScope ps(e, WLK_KC_LN);
-            layernorm(e->dx, dt, L.lncw, L.lncb, e->dxn, e->act, dt, R, dt, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->dxn; g.a_type = e->act; g.lda = dt; g.W = L.Wqc; g.w_type = e->wt; g.ldw = dt;
-            g.M = R; g.N = dt; g.K = dt;
-            g.epi.bias = L.bqc; g.epi.col_scale = qk_scale; g.epi.scale_cols = dt;
-            g.epi.C = e->dq; g.epi.c_type = e->act; g.epi.ldc = dt;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
-        {   ProfScope ps(e, WLK_KC_ATTN_DEC_CROSS, 0, (double)n * 2 * H * N_CTX * 64 * es);
-            const bool tc_prefill = e->attn_backend == WLK_BACKEND_TCGEN05 && e->act == DT_BF16 && max_tq >= 16;
-            if (tc_prefill)     // all non-alignment heads on the tensor cores; alignment heads need the exported rows
-                dec_cross_attention_tcgen05(e->dq, R, dj_dev, n, max_tq, li, H, dt, e->kv_maps_dev, e->align_rank_dev,
-                                            e->datt, e->st);
-            dec_cross_attention(e->dq, e->act, dj_dev, n, li, H, dt, ctx, e->align_rank_dev, e->datt, max_tq, tc_prefill, e->st); }
-        {   GemmArgs g;
-            g.A = e->datt; g.a_type = e->act; g.lda = dt; g.W = L.Woc; g.w_type = e->wt; g.ldw = dt;
-            g.M = R; g.N = dt; g.K = dt;
-            g.epi.bias = L.boc; g.epi.residual = e->dx; g.epi.ldr = dt; g.epi.C = e->dx; g.epi.c_type = DT_F32; g.epi.ldc = dt;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
-        {   ProfScope ps(e, WLK_KC_LN);
-            layernorm(e->dx, dt, L.ln2w, L.ln2b, e->dxn, e->act, dt, R, dt, nullptr, e->st); }
-        {   GemmArgs g;
-            g.A = e->dxn; g.a_type = e->act; g.lda = dt; g.W = L.W1; g.w_type = e->wt; g.ldw = dt;
-            g.M = R; g.N = 4 * dt; g.K = dt;
-            g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = e->dhid; g.epi.c_type = e->act; g.epi.ldc = 4 * dt;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
-        {   GemmArgs g;
-            g.A = e->dhid; g.a_type = e->act; g.lda = 4 * dt; g.W = L.W2; g.w_type = e->wt; g.ldw = 4 * dt;
-            g.M = R; g.N = dt; g.K = 4 * dt;
-            g.epi.bias = L.b2; g.epi.residual = e->dx; g.epi.ldr = dt; g.epi.C = e->dx; g.epi.c_type = DT_F32; g.epi.ldc = dt;
-            run_gemm(e, g, WLK_KC_GEMM_DEC); }
+        const DecLayerW& L = W.dec[li];
+        run_block(e, L, e->dx, e->dxn, e->datt, e->dhid, dt, R, WLK_KC_GEMM_DEC, 0,
+            [&](Epilogue& epi) {
+                epi.mode = EPI_SELF_QKV; epi.C = e->dq; epi.ldc = dt;
+                epi.batch_ptrs = skv_dev; epi.row_slot = slot_dev; epi.row_pos = pos_dev;
+                epi.layer = li; epi.n_head = H; epi.d_model = dt; epi.kv_len = ctx;
+            },
+            [&] {
+                ProfScope ps(e, WLK_KC_ATTN_DEC_SELF);
+                // prefills on the tensor cores (causal, per-session cache planes through TMA); token steps and the fp32
+                // modes on the SIMT kernel
+                if (e->attn_backend == WLK_BACKEND_TCGEN05 && e->act == DT_BF16 && max_tq >= 16)
+                    dec_self_attention_tcgen05(e->dq, R, dj_dev, n, max_tq, li, H, dt, ctx, e->self_maps_dev, e->datt, e->st);
+                else
+                    dec_self_attention(e->dq, e->act, dj_dev, n, li, H, dt, ctx, e->datt, max_tq, e->st);
+            },
+            [&] {   // cross-attention: LN, q, attention over the session's cross-K/V, out-projection + residual
+                {   ProfScope ps(e, WLK_KC_LN);
+                    layernorm(e->dx, dt, L.lncw, L.lncb, e->dxn, e->act, dt, R, dt, nullptr, e->st); }
+                {   GemmArgs g;
+                    g.A = e->dxn; g.a_type = e->act; g.lda = dt; g.W = L.Wqc; g.w_type = e->wt; g.ldw = dt;
+                    g.M = R; g.N = dt; g.K = dt;
+                    g.epi.bias = L.bqc; g.epi.col_scale = qk_scale; g.epi.scale_cols = dt;
+                    g.epi.C = e->dq; g.epi.c_type = e->act; g.epi.ldc = dt;
+                    run_gemm(e, g, WLK_KC_GEMM_DEC); }
+                {   ProfScope ps(e, WLK_KC_ATTN_DEC_CROSS, 0, (double)n * 2 * H * N_CTX * 64 * es);
+                    const bool tc_prefill = e->attn_backend == WLK_BACKEND_TCGEN05 && e->act == DT_BF16 && max_tq >= 16;
+                    if (tc_prefill)     // all non-alignment heads on the tensor cores; alignment heads need the exported rows
+                        dec_cross_attention_tcgen05(e->dq, R, dj_dev, n, max_tq, li, H, dt, e->kv_maps_dev, e->align_rank_dev,
+                                                    e->datt, e->st);
+                    dec_cross_attention(e->dq, e->act, dj_dev, n, li, H, dt, ctx, e->align_rank_dev, e->datt, max_tq,
+                                        tc_prefill, e->st); }
+                {   GemmArgs g;
+                    g.A = e->datt; g.a_type = e->act; g.lda = dt; g.W = L.Woc; g.w_type = e->wt; g.ldw = dt;
+                    g.M = R; g.N = dt; g.K = dt;
+                    g.epi.bias = L.boc; g.epi.residual = e->dx; g.epi.ldr = dt; g.epi.C = e->dx; g.epi.c_type = DT_F32;
+                    g.epi.ldc = dt;
+                    run_gemm(e, g, WLK_KC_GEMM_DEC); }
+            });
     }
     if (all_logits_dev) {
         // word-timestamp pass (find_alignment, timing.py:197-201) reads the logits of EVERY fed position
@@ -1221,8 +1200,7 @@ int wlk_session_audio_len(wlk_engine* e, int32_t sid, int64_t* n) {
 int wlk_session_reset_decoder(wlk_engine* e, int32_t sid) {
     WLK_API_BEGIN
     WLK_ENTER(e, e->cfg.device);
-    Session& s = e->sess.at(sid);
-    s.self_len = 0; s.align_rows = 0; s.iter_row_start.clear();
+    reset_decoder(e->sess.at(sid));
     WLK_API_END
 }
 
