@@ -136,11 +136,9 @@ __device__ __forceinline__ void epilogue_map_tile128(float (&acc)[2][64], F f) {
         for (int j = 0; j < 64; ++j) acc[h][j] = f(acc[h][j]);
 }
 
-__device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, int M, float (&acc)[2][64], int n_base, int N,
-                                                 int lane) {
+// bias, activation, column scale of a ping-pong consumer's 128 x 128 tile: registers only
+__device__ __forceinline__ void epilogue_math_tile128(const Epilogue& epi, float (&acc)[2][64], int n_base, int N, int lane) {
     const int t2 = 2 * (lane & 3);
-    const bool full = n_base + 128 <= N;
-    // 1. bias, activation, column scale: registers only
     if (epi.bias) {
 #pragma unroll
         for (int c = 0; c < 16; ++c) {
@@ -169,6 +167,15 @@ __device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, 
                 for (int j = 0; j < 4; ++j) acc[h][4 * c + j] *= epi.col_scale;
         }
     }
+}
+
+// The register-path epilogue of a whole tile (the scatter modes, and plain outputs whose pitch or base a tensor map
+// cannot address): residual from global memory, stores straight from the fragment.
+__device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, int M, float (&acc)[2][64], int n_base, int N,
+                                                 int lane) {
+    const int t2 = 2 * (lane & 3);
+    const bool full = n_base + 128 <= N;
+    epilogue_math_tile128(epi, acc, n_base, N, lane);
     if (epi.residual) {
         // each pass derives the row pointers it needs: none of them stays live next to the 128 accumulators
         EpiRow row[4];
@@ -207,6 +214,44 @@ __device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, 
     for (int i = 0; i < 4; ++i) row[i] = epi_row(epi, row0 + 8 * (i & 1) + 64 * (i >> 1), M);
     if (epi.c_type == DT_F32) epilogue_store_tile128<true>(epi, row, acc, n_base, N, lane);
     else epilogue_store_tile128<false>(epi, row, acc, n_base, N, lane);
+}
+
+// Staged epilogue of a ping-pong consumer's 128 x 128 tile into a plain row-major C (bias, activation and column scale
+// already applied, no residual).  The tile leaves in NS sub-tiles of 128 rows x 128 bytes (32 fp32 or 64 bf16 columns)
+// through the consumer's two 16 KiB buffers at `buf`, which hold them 128B-swizzled as the tensor map tmC expects:
+// 16-byte unit u of row r sits at unit u ^ (r & 7), so every warp-wide fragment store touches each bank once per 128
+// bytes.  One thread (the warpgroup's first) stores a written buffer by TMA while the warpgroup writes the other; a
+// buffer is rewritten once its previous store has read it.  TMA clips rows past M and columns past N.  The values are
+// those epilogue_tile128 stores.
+template <bool F32>
+__device__ __forceinline__ void epilogue_tma_tile128(const float (&acc)[2][64], const CUtensorMap* tmC, int m_base,
+                                                     int n_base, uint32_t buf, int epi_bar, int wq, int lane) {
+    constexpr int NS = F32 ? 4 : 2;                    // sub-tiles per tile
+    constexpr int CPS = 16 / NS;                       // 8-column chunks per sub-tile
+    const int g = lane >> 2, t = lane & 3;
+    const bool leader = wq == 0 && lane == 0;
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+        const uint32_t b = buf + (s & 1) * (128 * 128);
+        if (leader) ptx::bulk_wait_group_read<1>();    // the store that last read buffer b (two sub-tiles ago) is done
+        ptx::named_bar_sync<128>(epi_bar);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t row = b + (16 * wq + g + 8 * (i & 1) + 64 * (i >> 1)) * 128;   // (row & 7) == g
+#pragma unroll
+            for (int cl = 0; cl < CPS; ++cl) {
+                const int j = 4 * (s * CPS + cl) + 2 * (i & 1);
+                if (F32) ptx::st_shared_f32x2(row + (((2 * cl + (t >> 1)) ^ g) << 4) + 8 * (t & 1), acc[i >> 1][j], acc[i >> 1][j + 1]);
+                else ptx::st_shared_b32(row + ((cl ^ g) << 4) + 4 * t, ptx::pack_bf16x2(acc[i >> 1][j], acc[i >> 1][j + 1]));
+            }
+        }
+        ptx::fence_proxy_async_smem();                 // the writes above, before the async proxy reads the buffer
+        ptx::named_bar_sync<128>(epi_bar);
+        if (leader) {
+            ptx::tma_store_2d(tmC, b, n_base + s * (128 / NS), m_base);
+            ptx::bulk_commit_group();
+        }
+    }
 }
 
 // Tile rasterisation shared by the producer and the consumer warps.  Work item t -> (m block, n block): tiles are walked

@@ -36,15 +36,16 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
     return g_encode;
 }
 
-// 2D bf16 tensor map over a row-major [rows, cols] matrix with row pitch ld (elements); box = [box_rows, 64].
-// A descriptor is a pure function of (address, shape, pitch, box): the engine's workspaces and weights sit at fixed
-// addresses, so the ~2 000 maps a tick needs are encoded once per calling thread and then served from a small
-// thread-local table (no lock; unified addressing makes the pointer unique across devices).
+// 2D bf16 (or fp32) tensor map over a row-major [rows, cols] matrix with row pitch ld (elements); box = [box_rows,
+// box_cols], 128B-swizzled.  A descriptor is a pure function of (address, type, shape, pitch, box): the engine's
+// workspaces and weights sit at fixed addresses, so the ~2 000 maps a tick needs are encoded once per calling thread
+// and then served from a small thread-local table (no lock; unified addressing makes the pointer unique across devices).
 namespace {
 struct TmapKey {
-    const void* ptr; uint64_t rows, cols, ld; uint32_t box_rows, box_cols;
+    const void* ptr; uint64_t rows, cols, ld; uint32_t box_rows, box_cols; int dtype;
     bool operator==(const TmapKey& o) const {
-        return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols;
+        return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows &&
+               box_cols == o.box_cols && dtype == o.dtype;
     }
 };
 struct TmapKeyHash {
@@ -54,22 +55,23 @@ struct TmapKeyHash {
         h ^= (k.cols * 1315423911ull + (h << 6) + (h >> 2));
         h ^= (k.ld * 2654435761ull + (h << 6) + (h >> 2));
         h ^= ((uint64_t)k.box_rows << 32 | k.box_cols) + (h << 6) + (h >> 2);
+        h ^= (uint64_t)k.dtype + (h << 6) + (h >> 2);
         return (size_t)h;
     }
 };
-}  // namespace
 
-bool make_tmap_bf16_2d(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
-                       uint32_t box_rows, uint32_t box_cols, std::string* err) {
+bool make_tmap_2d(CUtensorMap* tm, int dtype, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
+                  uint32_t box_rows, uint32_t box_cols, std::string* err) {
     static thread_local std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
-    const TmapKey key{ptr, rows, cols, ld, box_rows, box_cols};
+    const TmapKey key{ptr, rows, cols, ld, box_rows, box_cols, dtype};
     auto it = cache.find(key);
     if (it != cache.end()) { *tm = it->second; return true; }
     cuuint64_t gdim[2] = {cols, rows};
-    cuuint64_t gstride[1] = {ld * 2};
+    cuuint64_t gstride[1] = {ld * dtype_size(dtype)};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = get_encode()(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box,
+    CUresult r = get_encode()(tm, dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                              const_cast<void*>(ptr), gdim, gstride, box,
                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -79,6 +81,12 @@ bool make_tmap_bf16_2d(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t
     if (cache.size() >= 8192) cache.clear();      // decode prefills of every length each leave a few entries behind
     cache.emplace(key, *tm);
     return true;
+}
+}  // namespace
+
+bool make_tmap_bf16_2d(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
+                       uint32_t box_rows, uint32_t box_cols, std::string* err) {
+    return make_tmap_2d(tm, DT_BF16, ptr, rows, cols, ld, box_rows, box_cols, err);
 }
 
 namespace {
@@ -93,12 +101,16 @@ constexpr int NUM_THREADS = 32 * NUM_MMA_WARPS + 32;    // + the TMA warp (last,
 // four tiles (A_hi, A_lo, W_hi, W_lo) and every K=16 step issues three MMAs into the same fp32 accumulator:
 // A_hi W_hi + A_lo W_hi + A_hi W_lo (the lo*lo term is below 2^-16 relative and dropped) -- ~16 mantissa bits per
 // operand instead of 8, on the same tensor cores.
-template <int BN, int STAGES, bool X3 = false>
+// EPI_BUFS: 16 KiB epilogue staging buffers behind the ring (the ping-pong kernel's TMA-store epilogue: two per
+// consumer).
+template <int BN, int STAGES, bool X3 = false, int EPI_BUFS = 0>
 struct SmemLayout {
     static constexpr uint32_t PLANES = X3 ? 2 : 1;
     static constexpr uint32_t A_BYTES = BM * BK * 2;
     static constexpr uint32_t B_BYTES = BN * BK * 2;
-    static constexpr uint32_t BAR_OFF = STAGES * PLANES * (A_BYTES + B_BYTES);
+    static constexpr uint32_t EPI_BYTES = 128 * 128;
+    static constexpr uint32_t EPI_OFF = STAGES * PLANES * (A_BYTES + B_BYTES);     // 1024-aligned (128B swizzle)
+    static constexpr uint32_t BAR_OFF = EPI_OFF + EPI_BUFS * EPI_BYTES;
     static constexpr uint32_t TOTAL = BAR_OFF + 2 * STAGES * 8 + 16;
     static constexpr uint32_t DYN = TOTAL + 1024;   // slack for manual 1024-byte alignment
 };
@@ -278,22 +290,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // of every CTA of the cluster have released it (each consumer warp arrives on the empty barrier of every CTA), so the
 // CTAs of a cluster run the same slab sequence in lockstep.  A tile past M or N (odd num_m) is loaded (TMA zero-fills
 // it), computed and released like any other; its epilogue stores nothing.  <STAGES, X3, 1, 1> is the lone-CTA kernel.
+//
+// TMA_C: plain row-major outputs without a residual that a tensor map can address (the encoder's conv1, QKV and FC1)
+// leave through epilogue_tma_tile128: each consumer stages its tile in two 16 KiB shared-memory buffers and stores it
+// by TMA (tmC).  The scatter modes and the fp32 residual outputs keep the register-path epilogue (epilogue_tile128) and
+// the deeper ring (see tma_epilogue_fits).
 constexpr int PP_THREADS = 3 * 128;
 constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;     // 128 * 40 + 256 * 232 <= 64K registers
 constexpr int PP_BAR_ORDER = 1;                                  // named barriers 1, 2: "consumer c may issue its MMAs"
+constexpr int PP_BAR_EPI = 3;                                    // named barriers 3, 4: consumer c's staged epilogue
 // L2 budget for the A rows of one m-band (tile_coords): with two tiles in flight per CTA the band is swept across
 // ~2 x grid tiles at a time, and its A rows should be served from L2 for the whole sweep over n
 constexpr int64_t PP_BAND_BYTES = 20ll << 20;
 
-template <int STAGES, bool X3, int CM, int CN>
+template <int STAGES, bool X3, int CM, int CN, bool TMA_C>
 __global__ void __launch_bounds__(PP_THREADS, 1)
 gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-               const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmWlo, int M, int N, int K,
+               const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmWlo,
+               const __grid_constant__ CUtensorMap tmC, int M, int N, int K,
                Epilogue epi) {
     constexpr int BN = 128;
     constexpr int CS = CM * CN;                                    // CTAs per cluster
     constexpr int W_ROWS = BN / CM, A_ROWS = BM / CN;              // this CTA's share of a W / A slab (the tensor maps' box)
-    using L = SmemLayout<BN, STAGES, X3>;
+    using L = SmemLayout<BN, STAGES, X3, TMA_C ? 4 : 0>;
     constexpr uint32_t STAGE_TX = L::PLANES * (L::A_BYTES + L::B_BYTES);
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -313,9 +332,10 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int cnum_m = (num_m + CM - 1) / CM, cnum_n = (num_n + CN - 1) / CN;
     const int num_ct = cnum_m * cnum_n;                            // cluster-tiles
     const int num_k = (K + BK - 1) / BK;
-    const int band_fit = (int)(PP_BAND_BYTES / ((int64_t)CM * BM * K * 2 * L::PLANES));
-    const int band = max(1, min(2 * clusters, band_fit));
     auto coords = [&](int ct, int* m_blk, int* n_blk) {
+        // (recomputed per tile in 32-bit arithmetic rather than held in a register across the consumers' tile loop)
+        const int band_fit = (int)((uint32_t)PP_BAND_BYTES / ((uint32_t)CM * BM * 2 * L::PLANES * (uint32_t)K));
+        const int band = max(1, min(2 * clusters, band_fit));
         tile_coords(ct, cnum_m, cnum_n, band, m_blk, n_blk);
         *m_blk = *m_blk * CM + rm;
         *n_blk = *n_blk * CN + rn;
@@ -330,6 +350,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             ptx::mbar_init(bar_full + 8 * i, 1);
             ptx::mbar_init(bar_empty + 8 * i, 4 * CS);             // lane 0 of each warp of the consuming warpgroups
         }
+        if (TMA_C) ptx::prefetch_tensormap(&tmC);
         ptx::fence_barrier_init();
     }
     // the peers' barriers must be initialised before the first multicast lands on them
@@ -443,8 +464,18 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             ptx::wgmma_fence_regs(acc[0]);
             ptx::wgmma_fence_regs(acc[1]);
             release(prev);
-            epilogue_tile128(epi, row0, M, acc, n_blk * BN, N, lane);
+            if (!TMA_C) {
+                epilogue_tile128(epi, row0, M, acc, n_blk * BN, N, lane);
+            } else if (m_blk * BM < M && n_blk * BN < N) {         // (not a cluster-padding tile)
+                epilogue_math_tile128(epi, acc, n_blk * BN, N, lane);
+                const uint32_t buf = smem_base + L::EPI_OFF + c * 2 * L::EPI_BYTES;   // the consumer's two buffers
+                if (epi.c_type == DT_F32) epilogue_tma_tile128<true>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
+                else epilogue_tma_tile128<false>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
+            }
         }
+        // the tile stores have written global memory before the CTA exits (the next kernel's griddepcontrol.wait and
+        // the cluster's exit barrier rely on it)
+        if (TMA_C && threadIdx.x % 128 == 0) ptx::bulk_wait_group<0>();
     }
     // no CTA may exit while a peer can still arrive on its barriers
     if (CS > 1) ptx::cluster_sync();
@@ -511,12 +542,12 @@ void launch(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t 
     else launch_impl<BN, STAGES, false>(g, A_hi, A_lo, st, num_sms, splits);
 }
 
-template <int STAGES, bool X3, int CM, int CN>
+template <int STAGES, bool X3, int CM, int CN, bool TMA_C>
 void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
-    using L = SmemLayout<128, STAGES, X3>;
+    using L = SmemLayout<128, STAGES, X3, TMA_C ? 4 : 0>;
     static_assert(L::DYN <= 227 * 1024, "shared memory budget");
     constexpr int CS = CM * CN;
-    auto kernel = gemm_pp_kernel<STAGES, X3, CM, CN>;
+    auto kernel = gemm_pp_kernel<STAGES, X3, CM, CN, TMA_C>;
     // each CTA loads 1/CN of an A slab and 1/CM of a W slab (the kernel's multicast shares)
     CUtensorMap tmA, tmW, tmAlo, tmWlo;
     std::string err;
@@ -526,6 +557,11 @@ void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaS
         WLK_CHECK(make_tmap_bf16_2d(&tmAlo, A_lo, g.M, g.K, g.lda, BM / CN, BK, &err), "A_lo tensor map: %s", err.c_str());
         WLK_CHECK(make_tmap_bf16_2d(&tmWlo, g.W_lo, g.N, g.K, g.ldw, 128 / CM, BK, &err), "W_lo tensor map: %s", err.c_str());
     } else { tmAlo = tmA; tmWlo = tmW; }
+    // the staged epilogue's sub-tiles: 128 rows x 128 bytes of C
+    CUtensorMap tmC = tmA;
+    if (TMA_C)
+        WLK_CHECK(make_tmap_2d(&tmC, g.epi.c_type, g.epi.C, g.M, g.N, g.epi.ldc, BM, 128 / dtype_size(g.epi.c_type), &err),
+                  "C tensor map: %s", err.c_str());
     // clusters of this shape the device holds at once (it depends on how the SMs split into GPCs): queried once per device
     static std::atomic<int> max_clusters[64];
     const int dev = current_device();
@@ -551,14 +587,25 @@ void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaS
     const int num_ct = ((g.M + BM * CM - 1) / (BM * CM)) * ((g.N + 128 * CN - 1) / (128 * CN));
     const int clusters = std::max(1, std::min({mc, num_sms / CS, num_ct}));
     CUDA_CHECK(launch_pdl_cluster(kernel, dim3(clusters * CS), dim3(PP_THREADS), L::DYN, st, CS, tmA, tmW, tmAlo, tmWlo,
-                                  g.M, g.N, g.K, g.epi));
+                                  tmC, g.M, g.N, g.K, g.epi));
 }
 
-// 128 x 128 tiles on the ping-pong kernel, in clusters of CM x CN CTAs; ring depth 6 (plain) or 3 (X3: four tiles per slab)
+// Whether the ping-pong kernel's staged epilogue writes C: a plain row-major output at a 16-byte aligned base and pitch
+// (what a tensor map can address), without a residual.  The fp32 residual outputs (attention-out and FC2, x += A W^T in
+// place) stay on the register path and its 6-stage ring: with the residual staged through the same buffers by TMA they
+// measured 3-9 % slower (DESIGN.md section 3).
+bool tma_epilogue_fits(const Epilogue& e) {
+    return e.mode == EPI_PLAIN && e.residual == nullptr && reinterpret_cast<uintptr_t>(e.C) % 16 == 0 &&
+           (e.ldc * (int64_t)dtype_size(e.c_type)) % 16 == 0;
+}
+
+// 128 x 128 tiles on the ping-pong kernel, in clusters of CM x CN CTAs.  Ring depth 3 for X3 (four tiles per slab);
+// otherwise 6, or 5 beside the staged epilogue's 64 KiB of buffers.
 template <int CM, int CN>
 void launch_pp(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
-    if (g.w_type == DT_BF16X2) launch_pp_impl<3, true, 1, 1>(g, A_hi, A_lo, st, num_sms);
-    else launch_pp_impl<6, false, CM, CN>(g, A_hi, A_lo, st, num_sms);
+    if (g.w_type == DT_BF16X2) launch_pp_impl<3, true, 1, 1, false>(g, A_hi, A_lo, st, num_sms);
+    else if (tma_epilogue_fits(g.epi)) launch_pp_impl<5, false, CM, CN, true>(g, A_hi, A_lo, st, num_sms);
+    else launch_pp_impl<6, false, CM, CN, false>(g, A_hi, A_lo, st, num_sms);
 }
 
 }  // namespace

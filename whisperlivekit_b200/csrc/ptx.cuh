@@ -157,6 +157,14 @@ __device__ __forceinline__ void st_global_b32(void* p, uint32_t v) {
     asm volatile("st.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
+// ---- shared-space loads and stores at 32-bit shared addresses ------------------------------
+__device__ __forceinline__ void st_shared_f32x2(uint32_t p, float a, float b) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t p, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(p), "r"(v) : "memory");
+}
+
 // ---- programmatic dependent launch (see launch_pdl in common.cuh) ----------------------
 // wait: blocks until every grid this one depends on has completed and its writes are visible (no-op when the
 // launch carried no PDL attribute).  launch_dependents: lets the next kernel in the stream start scheduling
@@ -185,6 +193,22 @@ __device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const C
         " [%0], [%1, {%3, %4}], [%2], %5;"
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
+}
+
+// Tile store shared -> global: the box at (c0, c1) of the tensor map, clipped at its bounds.  Completion is tracked
+// per thread in bulk groups: commit_group closes the stores issued so far into a group; wait_group_read<N> returns once
+// at most N groups still have to read their shared-memory source, wait_group<N> once at most N groups have not
+// finished writing global memory.  (Both waits are single instructions that block in hardware: no spin loop, no call.)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t smem_src, int32_t c0, int32_t c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N> __device__ __forceinline__ void bulk_wait_group() {
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 // 1D bulk copy global -> shared through the TMA engine (16-byte aligned addresses, size a multiple of 16)
