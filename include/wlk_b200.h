@@ -35,9 +35,12 @@ typedef struct wlk_dims {
 
 enum { WLK_PREC_FP32 = 0,     /* SIMT fp32 kernels end to end: the 1e-3-on-logits parity mode                    */
        WLK_PREC_BF16 = 1,     /* bf16 operands / fp32 accumulate + fp32 residual: the serving mode                */
-       WLK_PREC_BF16X3 = 2 }; /* wgmma with split operands (x = hi + lo, both bf16; A_hi W_hi + A_lo W_hi +    *
+       WLK_PREC_BF16X3 = 2,   /* wgmma with split operands (x = hi + lo, both bf16; A_hi W_hi + A_lo W_hi +    *
                                * A_hi W_lo into one fp32 accumulator): 1e-3 on logits at tensor-core speed / 3;   *
                                * activations, softmax, LayerNorm and K/V caches stay fp32                         */
+       WLK_PREC_FP8 = 3 };    /* WLK_PREC_BF16 with the QKV, FC1 and FC2 GEMMs of every encoder layer in e4m3     *
+                               * (fp32 scale per weight row and per activation row, fp32 accumulate): the conv   *
+                               * stem, attention, attention-out, ln_post, cross-K/V and the decoder stay bf16     */
 enum { WLK_BACKEND_AUTO = 0, WLK_BACKEND_SIMT = 1, WLK_BACKEND_TCGEN05 = 2 };
 
 typedef struct wlk_config {
@@ -177,6 +180,23 @@ int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t l
                 const void* W, int w_type, int64_t ldw, const float* bias,
                 void* C, int c_type, int64_t ldc, int M, int N, int K, int gelu);
 int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int type, int batch, void* out);
+/* ---- FP8 (WLK_PREC_FP8) op-level entry points.  Device pointers; e4m3 data are bytes, every scale is fp32.
+ *      wlk_op_gemm_fp8: C = epilogue((A W^T)[m, n] * a_scale[m] * w_scale[n]), A [M, K] and W [N, K] e4m3 (K-major,
+ *        pitches and K multiples of 16); epilogue as wlk_op_gemm (+ bias, flags bit 0 erf-GELU, columns < scale_cols
+ *        times col_scale, flags bit 1 = fp32 C accumulated in place); c_type 0 fp32, 1 bf16, 3 e4m3 stored as
+ *        e4m3(v / c_scale[m]).  backend: WLK_BACKEND_TCGEN05 (auto), 4 lone CTAs, 5 / 6 / 7 2x1 / 1x2 / 2x2 clusters.
+ *      wlk_op_quantize_rows: src [rows, cols] (src_type 0 fp32, 1 bf16, pitch lds) -> scale[r] = max|row| / 448,
+ *        dst[r, c] = e4m3(src / scale[r]) (nearest even, saturated; an all-zero row: scale 0, bytes 0).
+ *      wlk_op_layernorm_fp8: LayerNorm(x) of `rows` rows of width d -> out e4m3 (pitch ldo bytes) with s_a as
+ *        wlk_op_quantize_rows; s_h (may be NULL) = (||dequantized row|| * w1_norm_max + b1_abs_max) / 448, the row
+ *        scale of the FC1 output it feeds.                                                                      */
+int wlk_op_gemm_fp8(wlk_engine* e, int backend, const void* A, const float* a_scale, int64_t lda,
+                    const void* W, const float* w_scale, int64_t ldw, const float* bias, float col_scale, int scale_cols,
+                    void* C, int c_type, const float* c_scale, int64_t ldc, int M, int N, int K, int flags);
+int wlk_op_quantize_rows(wlk_engine* e, const void* src, int src_type, int64_t lds, int rows, int cols, void* dst,
+                         int64_t ldd, float* scale);
+int wlk_op_layernorm_fp8(wlk_engine* e, const float* x, int64_t ldx, const float* w, const float* b, int rows, int d,
+                         void* out, int64_t ldo, float* s_a, float* s_h, float w1_norm_max, float b1_abs_max);
 
 /* ---- word-timestamp kernels of the LocalAgreement path: native replacements of the reference's Triton
  *      median_kernel / dtw_kernel (whisper/triton_ops.py:13-103) with the semantics of its CPU path

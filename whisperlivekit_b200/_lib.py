@@ -53,9 +53,9 @@ class wlk_config(C.Structure):
         "max_align_heads", "reserved")]
 
 
-PREC_FP32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+PREC_FP32, PREC_BF16, PREC_BF16X3, PREC_FP8 = 0, 1, 2, 3
 BACKEND_AUTO, BACKEND_SIMT, BACKEND_TCGEN05 = 0, 1, 2
-PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "bf16x3": PREC_BF16X3}
+PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "bf16x3": PREC_BF16X3, "fp8": PREC_FP8}
 BACKENDS = {"auto": BACKEND_AUTO, "simt": BACKEND_SIMT, "tcgen05": BACKEND_TCGEN05}
 KERNEL_CLASSES = ["mel", "gemm_enc", "attn_enc", "layernorm", "gemm_xkv", "gemm_dec",
                   "attn_dec_self", "attn_dec_cross", "logits", "align", "misc"]
@@ -180,6 +180,11 @@ SIGNATURES = {
     "wlk_op_gemm": (C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_int64, _vp, C.c_int, C.c_int64, _vp,
                               _vp, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]),
     "wlk_op_encoder_attention": (C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_int, _vp]),
+    "wlk_op_gemm_fp8": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, _vp, C.c_int64, _vp, C.c_float, C.c_int,
+                                  _vp, C.c_int, _vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "wlk_op_quantize_rows": (C.c_int, [_vp, _vp, C.c_int, C.c_int64, C.c_int, C.c_int, _vp, C.c_int64, _vp]),
+    "wlk_op_layernorm_fp8": (C.c_int, [_vp, _vp, C.c_int64, _vp, _vp, C.c_int, C.c_int, _vp, C.c_int64, _vp, _vp,
+                                       C.c_float, C.c_float]),
     "wlk_op_median_filter": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
     "wlk_op_dtw": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _i32p]),
     "wlk_timer_record": (C.c_int, [_vp, C.c_int]),

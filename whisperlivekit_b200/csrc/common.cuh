@@ -96,8 +96,10 @@ inline bool first_on_device(bool (&seen)[64]) {
 inline int current_device() { int d = 0; cudaGetDevice(&d); return d & 63; }
 
 // DT_BF16X2: weights of the WLK_PREC_BF16X3 mode -- two bf16 planes (hi, then lo right behind it), 4 bytes per element
-enum DType { DT_F32 = 0, DT_BF16 = 1, DT_BF16X2 = 2 };
-inline size_t dtype_size(int t) { return t == DT_BF16 ? 2 : 4; }
+// DT_E4M3: FP8 e4m3 bytes (WLK_PREC_FP8), each row or output channel with an fp32 scale beside it
+enum DType { DT_F32 = 0, DT_BF16 = 1, DT_BF16X2 = 2, DT_E4M3 = 3 };
+inline size_t dtype_size(int t) { return t == DT_BF16 ? 2 : t == DT_E4M3 ? 1 : 4; }
+constexpr float E4M3_MAX = 448.f;
 
 // ---------------------------------------------------------------------------------
 // GEMM epilogue description shared by the SIMT and the tensor-core GEMM kernels.
@@ -133,6 +135,11 @@ struct Epilogue {
     int layer = 0;                       // EPI_SELF_QKV
     const int32_t* row_slot = nullptr;   // EPI_SELF_QKV (and EPI_XKV when set): row -> index into batch_ptrs
     const int32_t* row_pos = nullptr;    // EPI_SELF_QKV (and EPI_XKV when set): row -> row of the K/V plane
+    // e4m3 operands (wgmma kernel only): acc is first multiplied by a_scale[m] * w_scale[n]; an e4m3 output (EPI_PLAIN,
+    // no residual) stores e4m3(v / c_scale[m])
+    const float* a_scale = nullptr;
+    const float* w_scale = nullptr;
+    const float* c_scale = nullptr;
 };
 
 struct GemmArgs {
@@ -295,7 +302,7 @@ struct EpiRow {
 __device__ __forceinline__ EpiRow epi_row(const Epilogue& e, int m, int M) {
     EpiRow r{nullptr, nullptr, nullptr};
     if (m >= M) return r;
-    const int es = (e.c_type == DT_F32) ? 4 : 2;
+    const int es = (e.c_type == DT_F32) ? 4 : (e.c_type == DT_E4M3) ? 1 : 2;
     switch (e.mode) {
         default:
         case EPI_PLAIN:

@@ -33,7 +33,11 @@ constexpr int AUDIO_CAP = 2 * 480000;       // samples a session may buffer (ref
 static const char* kClassNames[WLK_KC_COUNT] = {"mel", "gemm_enc", "attn_enc", "layernorm", "gemm_xkv", "gemm_dec",
                                                 "attn_dec_self", "attn_dec_cross", "logits", "align", "misc"};
 
-struct EncLayerW { float *ln1w, *ln1b, *bqkv, *bo, *ln2w, *ln2b, *b1, *b2; void *Wqkv, *Wo, *W1, *W2; };
+struct EncLayerW {
+    float *ln1w, *ln1b, *bqkv, *bo, *ln2w, *ln2b, *b1, *b2; void *Wqkv, *Wo, *W1, *W2;
+    // WLK_PREC_FP8 encoder layers: Wqkv, W1 and W2 are e4m3 with these row scales; fc1_bound = {max_n ||W1_n||, max|b1|}
+    float *sqkv = nullptr, *s1 = nullptr, *s2 = nullptr, *fc1_bound = nullptr;
+};
 struct DecLayerW : EncLayerW { float *lncw, *lncb, *bqc, *boc; void *Wqc, *Woc; };   // + the cross-attention sub-block
 struct Weights {
     float *filtT, *window; float2* twiddle; int2* filt_span;
@@ -82,6 +86,7 @@ using namespace wlk;
 struct wlk_engine : EngineBase {       // act: also the type of every session buffer
     wlk_dims dims{};
     int wt = DT_F32;                  // weight-matrix type: = act, or DT_BF16X2 (hi + lo bf16 planes) in WLK_PREC_BF16X3
+    bool enc_fp8 = false;             // WLK_PREC_FP8: the encoder layers' QKV, FC1 and FC2 in e4m3 (e4m3 weights there)
     void* a_split = nullptr; size_t a_split_elems = 0;   // BF16X3: (hi, lo) planes of a GEMM's fp32 activation operand
     int gemm_backend = WLK_BACKEND_SIMT, attn_backend = WLK_BACKEND_SIMT;
     // token-step CUDA graphs: the ~390 launches of one decoder step depend only on the batch size (every per-session
@@ -109,6 +114,8 @@ struct wlk_engine : EngineBase {       // act: also the type of every session bu
     // encoder workspace (max_batch streams)
     void *mel_t = nullptr, *h1 = nullptr, *xn = nullptr, *qkv = nullptr, *att = nullptr, *hid = nullptr;
     float* x = nullptr;
+    uint8_t* xq = nullptr;                    // WLK_PREC_FP8: e4m3 LayerNorm output (the MLP hidden is e4m3 in `hid`)
+    float *s_a = nullptr, *s_h = nullptr;     // WLK_PREC_FP8: row scales of xq and of the hidden
     int64_t* pad_rows_dev = nullptr;          // rows of h1 to re-zero after the conv1 GEMM
     void** xptrs_dev = nullptr;               // x + b*1500*d
     float* audio_scratch = nullptr;
@@ -191,24 +198,34 @@ void declare_weights(wlk_engine* e) {
     T.mat("encoder.conv2.weight", W.Wc2, {d, d, 3}, swap_inner_axes(d, d, 3));
     T.f32("encoder.conv2.bias", W.bc2, {d});
     T.f32("encoder.positional_embedding", W.enc_pos, {D.n_audio_ctx, d});
-    // the parts every block has: self-attention (q / k / v rows fused; key has no bias) and the MLP around `between`
-    auto block = [&](const std::string& p, int dm, auto& l, auto&& between) {
+    // the parts every block has: self-attention (q / k / v rows fused; key has no bias) and the MLP around `between`.
+    // mt: type of the QKV, FC1 and FC2 matrices (DT_E4M3 adds their row scales and the FC1 bound)
+    auto block = [&](const std::string& p, int dm, auto& l, int mt, auto&& between) {
         T.f32(p + "attn_ln.weight", l.ln1w, {dm});
         T.f32(p + "attn_ln.bias", l.ln1b, {dm});
-        T.fused(l.Wqkv, wt, {{p + "attn.query.weight", dm}, {p + "attn.key.weight", dm}, {p + "attn.value.weight", dm}}, dm);
+        T.fused(l.Wqkv, mt, {{p + "attn.query.weight", dm}, {p + "attn.key.weight", dm}, {p + "attn.value.weight", dm}}, dm,
+                &l.sqkv);
         T.fused(l.bqkv, DT_F32, {{p + "attn.query.bias", dm}, {"", dm}, {p + "attn.value.bias", dm}}, 0);
         T.mat(p + "attn.out.weight", l.Wo, {dm, dm});
         T.f32(p + "attn.out.bias", l.bo, {dm});
         between();
         T.f32(p + "mlp_ln.weight", l.ln2w, {dm});
         T.f32(p + "mlp_ln.bias", l.ln2b, {dm});
-        T.mat(p + "mlp.0.weight", l.W1, {4 * dm, dm});
-        T.f32(p + "mlp.0.bias", l.b1, {4 * dm});
-        T.mat(p + "mlp.2.weight", l.W2, {dm, 4 * dm});
+        if (mt == DT_E4M3) {
+            T.fused(l.W1, mt, {{p + "mlp.0.weight", 4 * dm}}, dm, &l.s1);
+            T.f32(p + "mlp.0.bias", l.b1, {4 * dm});
+            T.fused(l.W2, mt, {{p + "mlp.2.weight", dm}}, 4 * dm, &l.s2);
+            T.buf(l.fc1_bound, 2 * sizeof(float));
+        } else {
+            T.mat(p + "mlp.0.weight", l.W1, {4 * dm, dm});
+            T.f32(p + "mlp.0.bias", l.b1, {4 * dm});
+            T.mat(p + "mlp.2.weight", l.W2, {dm, 4 * dm});
+        }
         T.f32(p + "mlp.2.bias", l.b2, {dm});
     };
     W.enc.resize(D.n_audio_layer);
-    for (int i = 0; i < D.n_audio_layer; ++i) block("encoder.blocks." + std::to_string(i) + ".", d, W.enc[i], [] {});
+    for (int i = 0; i < D.n_audio_layer; ++i)
+        block("encoder.blocks." + std::to_string(i) + ".", d, W.enc[i], e->enc_fp8 ? DT_E4M3 : wt, [] {});
     T.f32("encoder.ln_post.weight", W.lnpw, {d});
     T.f32("encoder.ln_post.bias", W.lnpb, {d});
     // the token embedding in fp32 (the decoder's input rows) and, unless that is the weight type, in the weight type
@@ -223,7 +240,7 @@ void declare_weights(wlk_engine* e) {
     for (int i = 0; i < D.n_text_layer; ++i) {
         const std::string p = "decoder.blocks." + std::to_string(i) + ".";
         DecLayerW& l = W.dec[i];
-        block(p, dt, l, [&] {
+        block(p, dt, l, wt, [&] {
             T.f32(p + "cross_attn_ln.weight", l.lncw, {dt});
             T.f32(p + "cross_attn_ln.bias", l.lncb, {dt});
             T.mat(p + "cross_attn.query.weight", l.Wqc, {dt, dt});
@@ -259,6 +276,7 @@ void run_gemm(wlk_engine* e, GemmArgs& g, int cls) {
         e->gemm.run(g, true, e->st, e->num_sms, "bf16x3");
         return;
     }
+    if (g.a_type == DT_E4M3) { e->gemm.run(g, true, e->st, e->num_sms, "fp8"); return; }
     e->gemm.run(g, e->gemm_backend == WLK_BACKEND_TCGEN05, e->st, e->num_sms);
 }
 
@@ -279,13 +297,23 @@ void reset_decoder(Session& s) { s.self_len = 0; s.align_rows = 0; s.iter_row_st
 // + residual -> between -> LN -> FC1 + GELU -> FC2 + residual.  qkv_dst(epi) points the QKV epilogue at the path's
 // destination; attend() runs the path's attention into att inside its own ProfScope; between() is the decoder's
 // cross-attention sub-block and nothing in the encoder.  cls profiles the GEMMs, ln_bytes is what each LayerNorm records.
+// fp8: both LayerNorms write e4m3 rows (e->xq, scales e->s_a) and QKV, FC1 and FC2 run on e4m3 operands (L's e4m3
+// matrices); FC1 writes the e4m3 hidden with the row scales e->s_h the second LayerNorm derived from L.fc1_bound.
 template <typename QkvDst, typename Attend, typename Between>
 void run_block(wlk_engine* e, const EncLayerW& L, float* x, void* xn, void* att, void* hid, int dm, int R, int cls,
-               double ln_bytes, QkvDst qkv_dst, Attend attend, Between between) {
+               double ln_bytes, bool fp8, QkvDst qkv_dst, Attend attend, Between between) {
+    // the A operand of QKV / FC1: the LayerNorm output in the activation type or in e4m3
+    auto ln_operand = [&](GemmArgs& g) {
+        if (fp8) { g.A = e->xq; g.a_type = DT_E4M3; g.epi.a_scale = e->s_a; }
+        else { g.A = xn; g.a_type = e->act; }
+        g.lda = dm;
+    };
     {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
-        layernorm(x, dm, L.ln1w, L.ln1b, xn, e->act, dm, R, dm, nullptr, e->st); }
+        if (fp8) layernorm_fp8(x, dm, L.ln1w, L.ln1b, e->xq, dm, e->s_a, nullptr, nullptr, R, dm, e->st);
+        else layernorm(x, dm, L.ln1w, L.ln1b, xn, e->act, dm, R, dm, nullptr, e->st); }
     {   GemmArgs g;
-        g.A = xn; g.a_type = e->act; g.lda = dm; g.W = L.Wqkv; g.w_type = e->wt; g.ldw = dm;
+        ln_operand(g);
+        g.W = L.Wqkv; g.w_type = fp8 ? DT_E4M3 : e->wt; g.ldw = dm; g.epi.w_scale = L.sqkv;
         g.M = R; g.N = 3 * dm; g.K = dm;
         g.epi.bias = L.bqkv; g.epi.col_scale = powf(64.0f, -0.25f); g.epi.scale_cols = 2 * dm;   // model.py:152
         g.epi.c_type = e->act;
@@ -299,14 +327,18 @@ void run_block(wlk_engine* e, const EncLayerW& L, float* x, void* xn, void* att,
         run_gemm(e, g, cls); }
     between();
     {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
-        layernorm(x, dm, L.ln2w, L.ln2b, xn, e->act, dm, R, dm, nullptr, e->st); }
+        if (fp8) layernorm_fp8(x, dm, L.ln2w, L.ln2b, e->xq, dm, e->s_a, e->s_h, L.fc1_bound, R, dm, e->st);
+        else layernorm(x, dm, L.ln2w, L.ln2b, xn, e->act, dm, R, dm, nullptr, e->st); }
     {   GemmArgs g;
-        g.A = xn; g.a_type = e->act; g.lda = dm; g.W = L.W1; g.w_type = e->wt; g.ldw = dm;
+        ln_operand(g);
+        g.W = L.W1; g.w_type = fp8 ? DT_E4M3 : e->wt; g.ldw = dm; g.epi.w_scale = L.s1;
         g.M = R; g.N = 4 * dm; g.K = dm;
-        g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = hid; g.epi.c_type = e->act; g.epi.ldc = 4 * dm;
+        g.epi.bias = L.b1; g.epi.gelu = 1; g.epi.C = hid; g.epi.c_type = fp8 ? DT_E4M3 : e->act; g.epi.ldc = 4 * dm;
+        if (fp8) g.epi.c_scale = e->s_h;
         run_gemm(e, g, cls); }
     {   GemmArgs g;
-        g.A = hid; g.a_type = e->act; g.lda = 4 * dm; g.W = L.W2; g.w_type = e->wt; g.ldw = 4 * dm;
+        g.A = hid; g.a_type = fp8 ? DT_E4M3 : e->act; g.lda = 4 * dm; g.W = L.W2; g.w_type = fp8 ? DT_E4M3 : e->wt; g.ldw = 4 * dm;
+        if (fp8) { g.epi.a_scale = e->s_h; g.epi.w_scale = L.s2; }
         g.M = R; g.N = dm; g.K = 4 * dm;
         g.epi.bias = L.b2; g.epi.residual = x; g.epi.ldr = dm; g.epi.C = x; g.epi.c_type = DT_F32; g.epi.ldc = dm;
         run_gemm(e, g, cls); }
@@ -395,7 +427,7 @@ void run_encoder_layers(wlk_engine* e, const int32_t* sids, int n, int R, void**
     const int d = D.n_audio_state, dt = D.n_text_state;
     const double ln_bytes = (double)R * d * (4 + e->es());
     for (int li = 0; li < D.n_audio_layer; ++li)
-        run_block(e, W.enc[li], e->x, e->xn, e->att, e->hid, d, R, WLK_KC_GEMM_ENC, ln_bytes,
+        run_block(e, W.enc[li], e->x, e->xn, e->att, e->hid, d, R, WLK_KC_GEMM_ENC, ln_bytes, e->enc_fp8,
                   [&](Epilogue& epi) { qkv_dst(epi, li); }, [&] { attend(li); }, [] {});
     {   ProfScope ps(e, WLK_KC_LN, 0, ln_bytes);
         layernorm(e->x, d, W.lnpw, W.lnpb, e->xn, e->act, d, R, d, nullptr, e->st); }
@@ -662,7 +694,7 @@ void decode_batch(wlk_engine* e, const int32_t* sids, int n, const int32_t* toke
     const float qk_scale = powf(64.0f, -0.25f);
     for (int li = 0; li < D.n_text_layer; ++li) {
         const DecLayerW& L = W.dec[li];
-        run_block(e, L, e->dx, e->dxn, e->datt, e->dhid, dt, R, WLK_KC_GEMM_DEC, 0,
+        run_block(e, L, e->dx, e->dxn, e->datt, e->dhid, dt, R, WLK_KC_GEMM_DEC, 0, false,
             [&](Epilogue& epi) {
                 epi.mode = EPI_SELF_QKV; epi.C = e->dq; epi.ldc = dt;
                 epi.batch_ptrs = skv_dev; epi.row_slot = slot_dev; epi.row_pos = pos_dev;
@@ -865,13 +897,17 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     WLK_CHECK(dims->n_text_state % 64 == 0 && dims->n_text_state / dims->n_text_head == 64, "text heads must be 64 wide");
     WLK_CHECK(dims->n_mels % 8 == 0 && dims->n_mels <= 128, "n_mels must be 80 or 128");
     WLK_CHECK(cfg->max_sessions >= 1 && cfg->max_batch >= 1, "max_sessions / max_batch must be >= 1");
-    WLK_CHECK(cfg->precision == WLK_PREC_FP32 || cfg->precision == WLK_PREC_BF16 || cfg->precision == WLK_PREC_BF16X3,
-              "unknown precision %d", cfg->precision);
+    WLK_CHECK(cfg->precision == WLK_PREC_FP32 || cfg->precision == WLK_PREC_BF16 || cfg->precision == WLK_PREC_BF16X3 ||
+              cfg->precision == WLK_PREC_FP8, "unknown precision %d", cfg->precision);
+    WLK_CHECK(cfg->precision != WLK_PREC_FP8 || cfg->gemm_backend != WLK_BACKEND_SIMT,
+              "WLK_PREC_FP8 runs its GEMMs on the wgmma kernels: gemm_backend cannot be WLK_BACKEND_SIMT");
 
     auto* e = new wlk_engine();
     e->open(*cfg);
     e->dims = *dims;
-    e->act = cfg->precision == WLK_PREC_BF16 ? DT_BF16 : DT_F32;
+    // FP8: the bf16 serving mode with the encoder layers' QKV, FC1 and FC2 in e4m3
+    e->enc_fp8 = cfg->precision == WLK_PREC_FP8;
+    e->act = cfg->precision == WLK_PREC_BF16 || e->enc_fp8 ? DT_BF16 : DT_F32;
     e->wt = cfg->precision == WLK_PREC_BF16X3 ? DT_BF16X2 : e->act;
     e->gemm_backend = cfg->gemm_backend != WLK_BACKEND_AUTO ? cfg->gemm_backend
                       : (e->act == DT_BF16 ? WLK_BACKEND_TCGEN05 : WLK_BACKEND_SIMT);
@@ -912,6 +948,11 @@ void create_engine(const wlk_dims* dims, const wlk_config* cfg, wlk_engine** out
     e->qkv = e->allocs.take((size_t)B * N_CTX * 3 * d * es, acct);
     e->att = e->allocs.take((size_t)B * N_CTX * d * es, acct);
     e->hid = e->allocs.take((size_t)B * N_CTX * 4 * d * es, acct);
+    if (e->enc_fp8) {
+        e->xq = (uint8_t*)e->allocs.take((size_t)B * N_CTX * d, acct);
+        e->s_a = (float*)e->allocs.take((size_t)B * N_CTX * sizeof(float), acct);
+        e->s_h = (float*)e->allocs.take((size_t)B * N_CTX * sizeof(float), acct);
+    }
     e->audio_scratch = (float*)e->allocs.take(AUDIO_CAP * sizeof(float), acct);
     e->mel_scratch = (float*)e->allocs.take((size_t)MEL_STORE_FRAMES * D.n_mels * sizeof(float), acct);
     if (e->gemm_backend == WLK_BACKEND_TCGEN05) e->gemm.alloc(e->allocs, acct);
@@ -1014,6 +1055,11 @@ int wlk_engine_finalize_weights(wlk_engine* e) {
     WLK_ENTER(e, e->cfg.device);
     e->weights.require_all();
     e->upload.release();
+    if (e->enc_fp8) {
+        const int d = e->dims.n_audio_state;
+        for (auto& l : e->w.enc) fp8_fc1_bound((const uint8_t*)l.W1, l.s1, l.b1, 4 * d, d, l.fc1_bound, e->st);
+        CUDA_CHECK(cudaStreamSynchronize(e->st));
+    }
     e->finalized = true;
     WLK_API_END
 }
@@ -1512,6 +1558,45 @@ int wlk_op_gemm(wlk_engine* e, int backend, const void* A, int a_type, int64_t l
     else if (backend == 4) gemm_tcgen05(g, e->st, e->num_sms, 2);
     else if (backend >= 5 && backend <= 7) gemm_tcgen05(g, e->st, e->num_sms, backend + 4);
     else gemm_simt(g, e->st);
+    WLK_API_END
+}
+int wlk_op_gemm_fp8(wlk_engine* e, int backend, const void* A, const float* a_scale, int64_t lda, const void* Wm,
+                    const float* w_scale, int64_t ldw, const float* bias, float col_scale, int scale_cols, void* C, int c_type,
+                    const float* c_scale, int64_t ldc, int M, int N, int K, int flags) {
+    WLK_API_BEGIN
+    WLK_ENTER(e, e->cfg.device);
+    WLK_CHECK(c_type == DT_F32 || c_type == DT_BF16 || c_type == DT_E4M3, "c_type %d: fp32, bf16 or e4m3", c_type);
+    WLK_CHECK(backend == WLK_BACKEND_TCGEN05 || (backend >= 4 && backend <= 7),
+              "backend %d: e4m3 runs on the 128-wide wgmma kernel only (2 auto, 4 lone CTAs, 5 / 6 / 7 clusters)", backend);
+    GemmArgs g;
+    g.A = A; g.a_type = DT_E4M3; g.lda = lda; g.W = Wm; g.w_type = DT_E4M3; g.ldw = ldw; g.M = M; g.N = N; g.K = K;
+    g.epi.bias = bias; g.epi.gelu = flags & 1; g.epi.col_scale = col_scale; g.epi.scale_cols = scale_cols;
+    g.epi.C = C; g.epi.c_type = c_type; g.epi.ldc = ldc;
+    g.epi.a_scale = a_scale; g.epi.w_scale = w_scale; g.epi.c_scale = c_scale;
+    if (flags & 2) { WLK_CHECK(c_type == DT_F32, "in-place accumulation needs an fp32 output"); g.epi.residual = (const float*)C; g.epi.ldr = ldc; }
+    std::string why;
+    WLK_CHECK(gemm_tcgen05_supported(g, &why), "wlk_op_gemm_fp8: %s", why.c_str());
+    ProfScope ps(e, WLK_KC_MISC, 2.0 * M * (double)N * K, 0);
+    gemm_tcgen05(g, e->st, e->num_sms, backend == WLK_BACKEND_TCGEN05 ? 0 : backend == 4 ? 2 : backend + 4);
+    WLK_API_END
+}
+int wlk_op_quantize_rows(wlk_engine* e, const void* src, int src_type, int64_t lds, int rows, int cols, void* dst,
+                         int64_t ldd, float* scale) {
+    WLK_API_BEGIN
+    WLK_ENTER(e, e->cfg.device);
+    WLK_CHECK(src && dst && scale, "null argument");
+    quantize_rows(src, src_type, lds, rows, cols, (uint8_t*)dst, ldd, scale, e->st);
+    WLK_API_END
+}
+int wlk_op_layernorm_fp8(wlk_engine* e, const float* x, int64_t ldx, const float* w, const float* b, int rows, int d,
+                         void* out, int64_t ldo, float* s_a, float* s_h, float w1_norm_max, float b1_abs_max) {
+    WLK_API_BEGIN
+    WLK_ENTER(e, e->cfg.device);
+    WLK_CHECK(x && w && b && out && s_a, "null argument");
+    OpUpload up{e->st};
+    const float bound_host[2] = {w1_norm_max, b1_abs_max};
+    const float* bound = s_h ? up.put(bound_host, 2) : nullptr;
+    layernorm_fp8(x, ldx, w, b, (uint8_t*)out, ldo, s_a, s_h, bound, rows, d, e->st);
     WLK_API_END
 }
 int wlk_op_encoder_attention(wlk_engine* e, int backend, const void* qkv, int type, int batch, void* out) {

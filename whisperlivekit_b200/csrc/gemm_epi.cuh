@@ -136,9 +136,47 @@ __device__ __forceinline__ void epilogue_map_tile128(float (&acc)[2][64], F f) {
         for (int j = 0; j < 64; ++j) acc[h][j] = f(acc[h][j]);
 }
 
-// bias, activation, column scale of a ping-pong consumer's 128 x 128 tile: registers only
-__device__ __forceinline__ void epilogue_math_tile128(const Epilogue& epi, float (&acc)[2][64], int n_base, int N, int lane) {
+// bias, activation, column scale of a ping-pong consumer's 128 x 128 tile: registers only.  FP8 (e4m3 operands): first
+// acc[m, n] * a_scale[m] * w_scale[n], a row scale at a time and then the column scales by shuffle, so that no more than
+// a few loaded scales are live next to the 128 accumulators.
+template <bool FP8 = false>
+__device__ __forceinline__ void epilogue_math_tile128(const Epilogue& epi, float (&acc)[2][64], int n_base, int N, int lane,
+                                                      int row0 = 0, int M = 0) {
     const int t2 = 2 * (lane & 3);
+    if (FP8) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = row0 + 8 * (i & 1) + 64 * (i >> 1);
+            const float sa = m < M ? __ldg(epi.a_scale + m) : 0.f;
+#pragma unroll
+            for (int c = 0; c < 16; ++c) { acc[i >> 1][4 * c + 2 * (i & 1)] *= sa; acc[i >> 1][4 * c + 2 * (i & 1) + 1] *= sa; }
+        }
+        // column scales: lane l loads columns 4l .. 4l + 3 of the tile once; a chunk's pair comes by shuffle (loading all
+        // 32 of a thread's scales next to the bias would hold 64 loaded values beside the 128 accumulators)
+        float4 wv = make_float4(0.f, 0.f, 0.f, 0.f);
+        {
+            const int n = n_base + 4 * lane;
+            if (n + 3 < N && (reinterpret_cast<uintptr_t>(epi.w_scale + n) & 15) == 0) wv = __ldg(reinterpret_cast<const float4*>(epi.w_scale + n));
+            else {
+                if (n < N) wv.x = __ldg(epi.w_scale + n);
+                if (n + 1 < N) wv.y = __ldg(epi.w_scale + n + 1);
+                if (n + 2 < N) wv.z = __ldg(epi.w_scale + n + 2);
+                if (n + 3 < N) wv.w = __ldg(epi.w_scale + n + 3);
+            }
+        }
+        const bool odd = (lane & 1) != 0;
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            const int src = 2 * c + ((lane & 3) >> 1);       // the lane holding columns 8c + 2t, +1
+            const float x = __shfl_sync(0xffffffffu, wv.x, src), y = __shfl_sync(0xffffffffu, wv.y, src);
+            const float z = __shfl_sync(0xffffffffu, wv.z, src), w = __shfl_sync(0xffffffffu, wv.w, src);
+            const float w0 = odd ? z : x, w1 = odd ? w : y;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                acc[h][4 * c] *= w0; acc[h][4 * c + 1] *= w1; acc[h][4 * c + 2] *= w0; acc[h][4 * c + 3] *= w1;
+            }
+        }
+    }
     if (epi.bias) {
 #pragma unroll
         for (int c = 0; c < 16; ++c) {
@@ -169,13 +207,30 @@ __device__ __forceinline__ void epilogue_math_tile128(const Epilogue& epi, float
     }
 }
 
+// e4m3 output: every row divided by its scale c_scale[m] (a zero scale stores zeros), ready for the saturating convert
+__device__ __forceinline__ void epilogue_out_scale_tile128(const Epilogue& epi, int row0, int M, float (&acc)[2][64]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int m = row0 + 8 * (i & 1) + 64 * (i >> 1);
+        const float s = m < M ? __ldg(epi.c_scale + m) : 0.f;
+        const float inv = s > 0.f ? 1.0f / s : 0.f;
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            acc[i >> 1][4 * c + 2 * (i & 1)] *= inv;
+            acc[i >> 1][4 * c + 2 * (i & 1) + 1] *= inv;
+        }
+    }
+}
+
 // The register-path epilogue of a whole tile (the scatter modes, and plain outputs whose pitch or base a tensor map
-// cannot address): residual from global memory, stores straight from the fragment.
+// cannot address): residual from global memory, stores straight from the fragment.  FP8: e4m3 operands (an e4m3 output
+// always leaves through the staged epilogue: gemm_tcgen05_supported).
+template <bool FP8 = false>
 __device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, int M, float (&acc)[2][64], int n_base, int N,
                                                  int lane) {
     const int t2 = 2 * (lane & 3);
     const bool full = n_base + 128 <= N;
-    epilogue_math_tile128(epi, acc, n_base, N, lane);
+    epilogue_math_tile128<FP8>(epi, acc, n_base, N, lane, row0, M);
     if (epi.residual) {
         // each pass derives the row pointers it needs: none of them stays live next to the 128 accumulators
         EpiRow row[4];
@@ -217,16 +272,17 @@ __device__ __forceinline__ void epilogue_tile128(const Epilogue& epi, int row0, 
 }
 
 // Staged epilogue of a ping-pong consumer's 128 x 128 tile into a plain row-major C (bias, activation and column scale
-// already applied, no residual).  The tile leaves in NS sub-tiles of 128 rows x 128 bytes (32 fp32 or 64 bf16 columns)
-// through the consumer's two 16 KiB buffers at `buf`, which hold them 128B-swizzled as the tensor map tmC expects:
+// already applied, no residual).  The tile leaves in NS sub-tiles of 128 rows x 128 bytes (32 fp32, 64 bf16 or 128 e4m3
+// columns) through the consumer's two 16 KiB buffers at `buf`, which hold them 128B-swizzled as the tensor map tmC expects:
 // 16-byte unit u of row r sits at unit u ^ (r & 7), so every warp-wide fragment store touches each bank once per 128
 // bytes.  One thread (the warpgroup's first) stores a written buffer by TMA while the warpgroup writes the other; a
 // buffer is rewritten once its previous store has read it.  TMA clips rows past M and columns past N.  The values are
-// those epilogue_tile128 stores.
-template <bool F32>
+// those epilogue_tile128 stores.  ES: bytes per element of C.
+template <int ES>
 __device__ __forceinline__ void epilogue_tma_tile128(const float (&acc)[2][64], const CUtensorMap* tmC, int m_base,
                                                      int n_base, uint32_t buf, int epi_bar, int wq, int lane) {
-    constexpr int NS = F32 ? 4 : 2;                    // sub-tiles per tile
+    constexpr bool F32 = ES == 4;
+    constexpr int NS = ES == 4 ? 4 : ES == 2 ? 2 : 1;  // sub-tiles per tile
     constexpr int CPS = 16 / NS;                       // 8-column chunks per sub-tile
     const int g = lane >> 2, t = lane & 3;
     const bool leader = wq == 0 && lane == 0;
@@ -242,6 +298,8 @@ __device__ __forceinline__ void epilogue_tma_tile128(const float (&acc)[2][64], 
             for (int cl = 0; cl < CPS; ++cl) {
                 const int j = 4 * (s * CPS + cl) + 2 * (i & 1);
                 if (F32) ptx::st_shared_f32x2(row + (((2 * cl + (t >> 1)) ^ g) << 4) + 8 * (t & 1), acc[i >> 1][j], acc[i >> 1][j + 1]);
+                else if (ES == 1) ptx::st_shared_b16(row + (((cl >> 1) ^ g) << 4) + 8 * (cl & 1) + 2 * t,
+                                                     ptx::pack_e4m3x2(acc[i >> 1][j], acc[i >> 1][j + 1]));
                 else ptx::st_shared_b32(row + ((cl ^ g) << 4) + 4 * t, ptx::pack_bf16x2(acc[i >> 1][j], acc[i >> 1][j + 1]));
             }
         }

@@ -36,7 +36,7 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
     return g_encode;
 }
 
-// 2D bf16 (or fp32) tensor map over a row-major [rows, cols] matrix with row pitch ld (elements); box = [box_rows,
+// 2D bf16 (or fp32, or e4m3 bytes) tensor map over a row-major [rows, cols] matrix with row pitch ld (elements); box = [box_rows,
 // box_cols], 128B-swizzled.  A descriptor is a pure function of (address, type, shape, pitch, box): the engine's
 // workspaces and weights sit at fixed addresses, so the ~2 000 maps a tick needs are encoded once per calling thread
 // and then served from a small thread-local table (no lock; unified addressing makes the pointer unique across devices).
@@ -70,7 +70,9 @@ bool make_tmap_2d(CUtensorMap* tm, int dtype, const void* ptr, uint64_t rows, ui
     cuuint64_t gstride[1] = {ld * dtype_size(dtype)};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = get_encode()(tm, dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+    const CUtensorMapDataType dt = dtype == DT_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : dtype == DT_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    CUresult r = get_encode()(tm, dt, 2,
                               const_cast<void*>(ptr), gdim, gstride, box,
                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -303,13 +305,14 @@ constexpr int PP_BAR_EPI = 3;                                    // named barrie
 // ~2 x grid tiles at a time, and its A rows should be served from L2 for the whole sweep over n
 constexpr int64_t PP_BAND_BYTES = 20ll << 20;
 
-template <int STAGES, bool X3, int CM, int CN, bool TMA_C>
+template <int STAGES, bool X3, int CM, int CN, bool TMA_C, bool FP8>
 __global__ void __launch_bounds__(PP_THREADS, 1)
 gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmWlo,
                const __grid_constant__ CUtensorMap tmC, int M, int N, int K,
                Epilogue epi) {
     constexpr int BN = 128;
+    constexpr int KE = FP8 ? 2 * BK : BK;                          // K elements per 128-byte slab row
     constexpr int CS = CM * CN;                                    // CTAs per cluster
     constexpr int W_ROWS = BN / CM, A_ROWS = BM / CN;              // this CTA's share of a W / A slab (the tensor maps' box)
     using L = SmemLayout<BN, STAGES, X3, TMA_C ? 4 : 0>;
@@ -331,10 +334,10 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
     const int cnum_m = (num_m + CM - 1) / CM, cnum_n = (num_n + CN - 1) / CN;
     const int num_ct = cnum_m * cnum_n;                            // cluster-tiles
-    const int num_k = (K + BK - 1) / BK;
+    const int num_k = (K + KE - 1) / KE;
     auto coords = [&](int ct, int* m_blk, int* n_blk) {
         // (recomputed per tile in 32-bit arithmetic rather than held in a register across the consumers' tile loop)
-        const int band_fit = (int)((uint32_t)PP_BAND_BYTES / ((uint32_t)CM * BM * 2 * L::PLANES * (uint32_t)K));
+        const int band_fit = (int)((uint32_t)PP_BAND_BYTES / ((uint32_t)CM * BM * (FP8 ? 1 : 2) * L::PLANES * (uint32_t)K));
         const int band = max(1, min(2 * clusters, band_fit));
         tile_coords(ct, cnum_m, cnum_n, band, m_blk, n_blk);
         *m_blk = *m_blk * CM + rm;
@@ -366,8 +369,8 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int i = 0; i < CN; ++i) a_mask |= 1u << (i * CM + rm);
             // this CTA's share of a slab: rows [rm * W_ROWS, +W_ROWS) of the W tile, [rn * A_ROWS, +A_ROWS) of the A tile
             auto load = [&](uint32_t dst, const CUtensorMap* tm, uint32_t bar, int kb, int row, uint16_t mask, bool shared) {
-                if (shared) ptx::tma_load_2d_multicast(dst, tm, bar, kb * BK, row, mask);
-                else ptx::tma_load_2d(dst, tm, bar, kb * BK, row);
+                if (shared) ptx::tma_load_2d_multicast(dst, tm, bar, kb * KE, row, mask);
+                else ptx::tma_load_2d(dst, tm, bar, kb * KE, row);
             };
             auto load_w = [&](uint32_t stage, int kb, int n_blk) {
                 const uint32_t off = stage * L::B_BYTES + rm * W_ROWS * BK * 2, bar = bar_full + 8 * stage;
@@ -446,7 +449,8 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const uint64_t ah = h * (HALF_A >> 4) + 2 * k;
-                        ptx::WgmmaSS<BN>::mma(acc[h], da + ah, db + 2 * k, acc_in);
+                        if (FP8) ptx::wgmma_e4m3_n128(acc[h], da + ah, db + 2 * k, acc_in);   // K = 32 e4m3: 32 bytes too
+                        else ptx::WgmmaSS<BN>::mma(acc[h], da + ah, db + 2 * k, acc_in);
                         if (X3) {
                             ptx::WgmmaSS<BN>::mma(acc[h], dal + ah, db + 2 * k, 1u);
                             ptx::WgmmaSS<BN>::mma(acc[h], da + ah, dbl + 2 * k, 1u);
@@ -465,12 +469,15 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             ptx::wgmma_fence_regs(acc[1]);
             release(prev);
             if (!TMA_C) {
-                epilogue_tile128(epi, row0, M, acc, n_blk * BN, N, lane);
+                epilogue_tile128<FP8>(epi, row0, M, acc, n_blk * BN, N, lane);
             } else if (m_blk * BM < M && n_blk * BN < N) {         // (not a cluster-padding tile)
-                epilogue_math_tile128(epi, acc, n_blk * BN, N, lane);
+                epilogue_math_tile128<FP8>(epi, acc, n_blk * BN, N, lane, row0, M);
                 const uint32_t buf = smem_base + L::EPI_OFF + c * 2 * L::EPI_BYTES;   // the consumer's two buffers
-                if (epi.c_type == DT_F32) epilogue_tma_tile128<true>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
-                else epilogue_tma_tile128<false>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
+                if (epi.c_type == DT_F32) epilogue_tma_tile128<4>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
+                else if (FP8 && epi.c_type == DT_E4M3) {
+                    epilogue_out_scale_tile128(epi, row0, M, acc);
+                    epilogue_tma_tile128<1>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
+                } else epilogue_tma_tile128<2>(acc, &tmC, m_blk * BM, n_blk * BN, buf, PP_BAR_EPI + c, wq, lane);
             }
         }
         // the tile stores have written global memory before the CTA exits (the next kernel's griddepcontrol.wait and
@@ -542,17 +549,19 @@ void launch(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t 
     else launch_impl<BN, STAGES, false>(g, A_hi, A_lo, st, num_sms, splits);
 }
 
-template <int STAGES, bool X3, int CM, int CN, bool TMA_C>
+template <int STAGES, bool X3, int CM, int CN, bool TMA_C, bool FP8 = false>
 void launch_pp_impl(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
     using L = SmemLayout<128, STAGES, X3, TMA_C ? 4 : 0>;
     static_assert(L::DYN <= 227 * 1024, "shared memory budget");
     constexpr int CS = CM * CN;
-    auto kernel = gemm_pp_kernel<STAGES, X3, CM, CN, TMA_C>;
-    // each CTA loads 1/CN of an A slab and 1/CM of a W slab (the kernel's multicast shares)
+    auto kernel = gemm_pp_kernel<STAGES, X3, CM, CN, TMA_C, FP8>;
+    // each CTA loads 1/CN of an A slab and 1/CM of a W slab (the kernel's multicast shares); a slab row is 128 bytes
+    constexpr int OP = FP8 ? DT_E4M3 : DT_BF16;
+    constexpr uint32_t KE = FP8 ? 2 * BK : BK;
     CUtensorMap tmA, tmW, tmAlo, tmWlo;
     std::string err;
-    WLK_CHECK(make_tmap_bf16_2d(&tmA, A_hi, g.M, g.K, g.lda, BM / CN, BK, &err), "A tensor map: %s", err.c_str());
-    WLK_CHECK(make_tmap_bf16_2d(&tmW, g.W, g.N, g.K, g.ldw, 128 / CM, BK, &err), "W tensor map: %s", err.c_str());
+    WLK_CHECK(make_tmap_2d(&tmA, OP, A_hi, g.M, g.K, g.lda, BM / CN, KE, &err), "A tensor map: %s", err.c_str());
+    WLK_CHECK(make_tmap_2d(&tmW, OP, g.W, g.N, g.K, g.ldw, 128 / CM, KE, &err), "W tensor map: %s", err.c_str());
     if (X3) {
         WLK_CHECK(make_tmap_bf16_2d(&tmAlo, A_lo, g.M, g.K, g.lda, BM / CN, BK, &err), "A_lo tensor map: %s", err.c_str());
         WLK_CHECK(make_tmap_bf16_2d(&tmWlo, g.W_lo, g.N, g.K, g.ldw, 128 / CM, BK, &err), "W_lo tensor map: %s", err.c_str());
@@ -600,10 +609,12 @@ bool tma_epilogue_fits(const Epilogue& e) {
 }
 
 // 128 x 128 tiles on the ping-pong kernel, in clusters of CM x CN CTAs.  Ring depth 3 for X3 (four tiles per slab);
-// otherwise 6, or 5 beside the staged epilogue's 64 KiB of buffers.
+// otherwise 6, or 5 beside the staged epilogue's 64 KiB of buffers; e4m3 operands (FP8) use the same ring.
 template <int CM, int CN>
 void launch_pp(const GemmArgs& g, const void* A_hi, const void* A_lo, cudaStream_t st, int num_sms) {
     if (g.w_type == DT_BF16X2) launch_pp_impl<3, true, 1, 1, false>(g, A_hi, A_lo, st, num_sms);
+    else if (g.w_type == DT_E4M3 && tma_epilogue_fits(g.epi)) launch_pp_impl<5, false, CM, CN, true, true>(g, A_hi, A_lo, st, num_sms);
+    else if (g.w_type == DT_E4M3) launch_pp_impl<6, false, CM, CN, false, true>(g, A_hi, A_lo, st, num_sms);
     else if (tma_epilogue_fits(g.epi)) launch_pp_impl<5, false, CM, CN, true>(g, A_hi, A_lo, st, num_sms);
     else launch_pp_impl<6, false, CM, CN, false>(g, A_hi, A_lo, st, num_sms);
 }
@@ -619,6 +630,20 @@ void split_f32_planes_async(const float* src, bf16* hi, bf16* lo, int64_t n, cud
 bool gemm_tcgen05_supported(const GemmArgs& g, std::string* why) {
     auto fail = [&](const char* m) { if (why) *why = m; return false; };
     const bool x3 = g.w_type == DT_BF16X2;
+    if (g.a_type == DT_E4M3 || g.w_type == DT_E4M3) {
+        // e4m3: 128-wide ping-pong kernel only, K-major operands with a 16-byte pitch, the scales present
+        if (g.a_type != DT_E4M3 || g.w_type != DT_E4M3) return fail("e4m3: both operands must be e4m3");
+        if (reinterpret_cast<uintptr_t>(g.A) % 16 || reinterpret_cast<uintptr_t>(g.W) % 16)
+            return fail("operands must be 16-byte aligned");
+        if (g.lda % 16 || g.ldw % 16) return fail("e4m3: row pitch must be a multiple of 16 elements (16 bytes)");
+        if (g.K % 16) return fail("e4m3: K must be a multiple of 16");
+        if (!g.epi.a_scale || !g.epi.w_scale) return fail("e4m3: operand scales missing");
+        if (g.epi.c_type == DT_E4M3 && (!g.epi.c_scale || !tma_epilogue_fits(g.epi)))
+            return fail("e4m3 output: plain rows at a 16-byte aligned base and pitch, no residual, with a row scale");
+        if (g.M <= 0 || g.N <= 0 || g.K <= 0) return fail("empty problem");
+        return true;
+    }
+    if (g.epi.c_type == DT_E4M3) return fail("an e4m3 output needs e4m3 operands");
     if (x3) {
         if (g.a_type != DT_F32) return fail("bf16x3: the activation operand must be fp32 (it is split on the fly)");
         if (!g.W_lo) return fail("bf16x3: missing lo plane of the weights");
@@ -652,6 +677,18 @@ void gemm_tcgen05(const GemmArgs& g, cudaStream_t st, int num_sms, int variant) 
     }
     // forced tile width / split-K (op-level tests, WLK_GEMM_VARIANT): 1 = <64,8>, 2 = 128-wide ping-pong on lone CTAs,
     // 4 = <32,10>, 5/6 = <64,8> split-K 2/4, 7/8 = <32,10> split-K 2/4, 9/10/11 = 128-wide in 2x1 / 1x2 / 2x2 clusters
+    if (g.w_type == DT_E4M3) {
+        // e4m3 runs on the 128-wide kernel only, unsplit (deterministic, batch-invariant): 2x2 clusters from K = 1024 when
+        // the tiles cover half the SMs, lone CTAs otherwise (the conv-free short K, the incremental encoder's blocks)
+        WLK_CHECK(variant == 0 || variant == 2 || (variant >= 9 && variant <= 11),
+                  "gemm_tcgen05: variant %d has no e4m3 kernel (e4m3 runs on the 128-wide ping-pong kernel only)", variant);
+        const int tiles = ((g.M + BM - 1) / BM) * ((g.N + 127) / 128);
+        if (variant == 9) launch_pp<2, 1>(g, A_hi, A_lo, st, num_sms);
+        else if (variant == 10) launch_pp<1, 2>(g, A_hi, A_lo, st, num_sms);
+        else if (variant == 11 || (variant == 0 && g.K >= 1024 && tiles >= num_sms / 2)) launch_pp<2, 2>(g, A_hi, A_lo, st, num_sms);
+        else launch_pp<1, 1>(g, A_hi, A_lo, st, num_sms);
+        return;
+    }
     if (variant == 2) { launch_pp<1, 1>(g, A_hi, A_lo, st, num_sms); return; }
     if (variant == 9) { launch_pp<2, 1>(g, A_hi, A_lo, st, num_sms); return; }
     if (variant == 10) { launch_pp<1, 2>(g, A_hi, A_lo, st, num_sms); return; }

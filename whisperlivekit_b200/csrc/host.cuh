@@ -87,8 +87,9 @@ struct WeightUpload {
     size_t cap = 0;
 
     // n floats -> dst as fp32 (a copy) or as dst_type (a conversion).  DT_BF16X2 puts the hi plane at dst and the lo
-    // plane `plane` elements behind it.  Synchronous: `host` may be reused on return.
-    void put(const float* host, size_t n, void* dst, int dst_type, cudaStream_t st, size_t plane = 0) {
+    // plane `plane` elements behind it; DT_E4M3 quantizes rows of `plane` columns, their scales to `scale`.  Synchronous:
+    // `host` may be reused on return.
+    void put(const float* host, size_t n, void* dst, int dst_type, cudaStream_t st, size_t plane = 0, float* scale = nullptr) {
         if (n > cap) {
             if (buf) { CUDA_CHECK(cudaStreamSynchronize(st)); CUDA_CHECK(cudaFree(buf)); }
             CUDA_CHECK(cudaMalloc(&buf, n * 4));
@@ -97,6 +98,8 @@ struct WeightUpload {
         CUDA_CHECK(cudaMemcpyAsync(buf, host, n * 4, cudaMemcpyHostToDevice, st));
         if (dst_type == DT_F32) CUDA_CHECK(cudaMemcpyAsync(dst, buf, n * 4, cudaMemcpyDeviceToDevice, st));
         else if (dst_type == DT_BF16X2) split_f32_to_planes(buf, (bf16*)dst, (bf16*)dst + plane, (int64_t)n, st);
+        else if (dst_type == DT_E4M3)
+            quantize_rows(buf, DT_F32, (int64_t)plane, (int)(n / plane), (int)plane, (uint8_t*)dst, (int64_t)plane, scale, st);
         else convert_f32_to(buf, dst, dst_type, (int64_t)n, st);
         CUDA_CHECK(cudaStreamSynchronize(st));
     }
@@ -143,8 +146,10 @@ struct WeightTable {
         void** base;
         size_t off = 0;                  // element offset from *base (into the hi plane in DT_BF16X2)
         int type = DT_F32;
-        size_t plane = 0;                // DT_BF16X2: elements from the hi plane to the lo plane (the whole matrix)
+        size_t plane = 0;                // DT_BF16X2: elements from the hi plane to the lo plane (the whole matrix);
+                                         // DT_E4M3: columns of a row
         Perm perm = nullptr;
+        float** scale = nullptr;         // DT_E4M3: the matrix's row scales (row off / plane)
         template <typename T>
         Dst(T*& b, size_t o = 0, int t = DT_F32, size_t p = 0, Perm f = nullptr)
             : base(reinterpret_cast<void**>(&b)), off(o), type(t), plane(p), perm(std::move(f)) {}
@@ -192,18 +197,22 @@ struct WeightTable {
         return add(name, std::move(shape), {Dst(slot, 0, wt, n, std::move(perm))});
     }
     // Tensors one after another in one buffer of `type`: [sum of rows][cols], or a vector when cols is 0.  A part without a
-    // name is left zero.
+    // name is left zero.  DT_E4M3 (a matrix) also places its fp32 row scales at `scale`.
     template <typename T>
-    void fused(T*& slot, int type, const std::vector<std::pair<std::string, int64_t>>& parts, int64_t cols) {
+    void fused(T*& slot, int type, const std::vector<std::pair<std::string, int64_t>>& parts, int64_t cols,
+               float** scale = nullptr) {
         int64_t rows = 0;
         for (auto& p : parts) rows += p.second;
         const size_t n = (size_t)rows * (cols ? cols : 1);
         buf(slot, n * dtype_size(type));
+        if (type == DT_E4M3) buf(*scale, (size_t)rows * 4);
         int64_t r = 0;
         for (auto& p : parts) {
-            if (!p.first.empty())
-                add(p.first, cols ? std::vector<int64_t>{p.second, cols} : std::vector<int64_t>{p.second},
-                    {Dst(slot, (size_t)r * (cols ? cols : 1), type, n)});
+            if (!p.first.empty()) {
+                Dst d(slot, (size_t)r * (cols ? cols : 1), type, type == DT_E4M3 ? (size_t)cols : n);
+                d.scale = scale;
+                add(p.first, cols ? std::vector<int64_t>{p.second, cols} : std::vector<int64_t>{p.second}, {d});
+            }
             r += p.second;
         }
     }
@@ -235,8 +244,9 @@ struct WeightTable {
         for (const Dst& d : e.dst) {
             std::vector<float> tmp;
             if (d.perm) tmp = d.perm(host);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(*d.base) + d.off * (d.type == DT_F32 ? 4 : 2);
-            up.put(d.perm ? tmp.data() : host, d.perm ? tmp.size() : (size_t)n, dst, d.type, st, d.plane);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(*d.base) + d.off * (d.type == DT_F32 ? 4 : d.type == DT_E4M3 ? 1 : 2);
+            float* scale = d.type == DT_E4M3 ? *d.scale + d.off / d.plane : nullptr;
+            up.put(d.perm ? tmp.data() : host, d.perm ? tmp.size() : (size_t)n, dst, d.type, st, d.plane, scale);
         }
         loaded.insert(name);
     }

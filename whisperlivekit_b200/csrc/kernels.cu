@@ -417,6 +417,153 @@ void layernorm(const float* x, int64_t ldx, const float* w, const float* b, void
     else CUDA_CHECK(launch_pdl(layernorm_kernel<bf16>, dim3(grid), dim3(256), 0, st, x, ldx, w, b, (bf16*)out, ldo, rows, d, row_index));
 }
 
+// =====================================================================================
+// FP8 (WLK_PREC_FP8): per-row e4m3 quantization, one warp per row
+// =====================================================================================
+__device__ __forceinline__ float e4m3_to_f32(uint8_t b) {
+    uint32_t h;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((uint16_t)b));
+    return __half2float(__ushort_as_half((uint16_t)(h & 0xffff)));
+}
+
+// scale = amax / 448 (0 for an all-zero row, whose bytes are then 0); byte = e4m3(x / scale), nearest even, saturated.
+// x / scale is the correctly rounded fp32 quotient, so the bytes are those of (x / scale).clamp(+-448).to(e4m3fn).
+template <typename TI>
+__global__ void __launch_bounds__(256)
+quantize_rows_kernel(const TI* __restrict__ src, int64_t lds, int rows, int cols, uint8_t* __restrict__ dst, int64_t ldd,
+                     float* __restrict__ scale) {
+    ptx::griddep_launch();
+    ptx::griddep_wait();
+    const int warp = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= rows) return;
+    const TI* s = src + (int64_t)warp * lds;
+    float amax = 0.f;
+    for (int k = lane; k < cols; k += 32) amax = fmaxf(amax, fabsf(to_f32(s[k])));
+    amax = warp_max(amax);
+    const float sc = amax / E4M3_MAX;
+    uint8_t* d = dst + (int64_t)warp * ldd;
+    for (int k = lane; k < cols; k += 32)
+        d[k] = sc > 0.f ? (uint8_t)(ptx::pack_e4m3x2(__fdiv_rn(to_f32(s[k]), sc), 0.f) & 0xff) : 0;
+    if (lane == 0) scale[warp] = sc;
+}
+void quantize_rows(const void* src, int src_type, int64_t lds, int rows, int cols, uint8_t* dst, int64_t ldd, float* scale,
+                   cudaStream_t st) {
+    if (rows <= 0) return;
+    WLK_CHECK(cols >= 1 && (src_type == DT_F32 || src_type == DT_BF16), "quantize_rows: fp32 or bf16 rows of >= 1 column");
+    const int grid = (rows + 7) / 8;
+    if (src_type == DT_F32)
+        CUDA_CHECK(launch_pdl(quantize_rows_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)src, lds, rows, cols, dst, ldd, scale));
+    else
+        CUDA_CHECK(launch_pdl(quantize_rows_kernel<bf16>, dim3(grid), dim3(256), 0, st, (const bf16*)src, lds, rows, cols, dst, ldd, scale));
+}
+
+// LayerNorm with e4m3 output: y as layernorm_kernel computes it, s_a = max|y| / 448, bytes e4m3(y / s_a).  With `bound`
+// = {max_n ||W1_n||, max_n |b1_n|} (the dequantized FC1 weight rows) also the FC1 output scale of the row,
+// s_h = (||y^|| bound[0] + bound[1]) / 448 with y^ the dequantized row: by Cauchy-Schwarz no |h| and hence no GELU(h)
+// exceeds 448 s_h (up to the accumulation's rounding, which the saturating convert absorbs).
+__global__ void __launch_bounds__(256)
+layernorm_fp8_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, const float* __restrict__ b,
+                     uint8_t* __restrict__ out, int64_t ldo, float* __restrict__ s_a, float* __restrict__ s_h,
+                     const float* __restrict__ bound, int rows, int d) {
+    ptx::griddep_launch();
+    ptx::griddep_wait();
+    constexpr int MAXV = 10;                          // float4 per lane: d <= 1280
+    const int warp = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= rows) return;
+    const float4* xr = reinterpret_cast<const float4*>(x + (int64_t)warp * ldx);
+    const int nvec = d >> 2;
+    float4 v[MAXV];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec) { v[i] = xr[idx]; s += (v[i].x + v[i].y) + (v[i].z + v[i].w); }
+        else v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    const float mean = warp_sum(s) / d;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+        if (lane + 32 * i < nvec) {
+            float a = v[i].x - mean, bb = v[i].y - mean, c = v[i].z - mean, dd = v[i].w - mean;
+            q += (a * a + bb * bb) + (c * c + dd * dd);
+        }
+    }
+    const float rstd = 1.0f / sqrtf(warp_sum(q) / d + 1e-5f);
+    const float4* w4 = reinterpret_cast<const float4*>(w);
+    const float4* b4 = reinterpret_cast<const float4*>(b);
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec) {
+            const float4 ww = w4[idx], bb = b4[idx];
+            v[i] = make_float4((v[i].x - mean) * rstd * ww.x + bb.x, (v[i].y - mean) * rstd * ww.y + bb.y,
+                               (v[i].z - mean) * rstd * ww.z + bb.z, (v[i].w - mean) * rstd * ww.w + bb.w);
+            amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+        }
+    }
+    amax = warp_max(amax);
+    const float sa = amax / E4M3_MAX;
+    uint8_t* o = out + (int64_t)warp * ldo;
+    float sq = 0.f;                                   // sum of the squared e4m3 values: ||y^|| = s_a sqrt(sq)
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec) {
+            uint32_t u = 0;
+            if (sa > 0.f) {
+                const uint16_t lo = ptx::pack_e4m3x2(__fdiv_rn(v[i].x, sa), __fdiv_rn(v[i].y, sa));
+                const uint16_t hi = ptx::pack_e4m3x2(__fdiv_rn(v[i].z, sa), __fdiv_rn(v[i].w, sa));
+                u = (uint32_t)lo | ((uint32_t)hi << 16);
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) { const float f = e4m3_to_f32((uint8_t)(u >> (8 * j))); sq += f * f; }
+            *reinterpret_cast<uint32_t*>(o + 4 * idx) = u;
+        }
+    }
+    sq = warp_sum(sq);
+    if (lane == 0) {
+        s_a[warp] = sa;
+        if (s_h) s_h[warp] = (sa * sqrtf(sq) * bound[0] + bound[1]) / E4M3_MAX;
+    }
+}
+void layernorm_fp8(const float* x, int64_t ldx, const float* w, const float* b, uint8_t* out, int64_t ldo, float* s_a,
+                   float* s_h, const float* bound, int rows, int d, cudaStream_t st) {
+    if (rows <= 0) return;
+    WLK_CHECK(d % 4 == 0 && d <= 1280 && ldx % 4 == 0 && ldo % 4 == 0, "layernorm_fp8: d=%d must be a multiple of 4 and <= 1280", d);
+    WLK_CHECK(!s_h || bound, "layernorm_fp8: the FC1 output scale needs the layer's bound");
+    CUDA_CHECK(launch_pdl(layernorm_fp8_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, x, ldx, w, b, out, ldo, s_a, s_h, bound,
+                          rows, d));
+}
+
+// bound = {max_n s_w[n] ||e4m3 row n||, max_n |bias[n]|} of an e4m3 matrix [N][K] with row scales s_w: one block, a warp
+// per row in a fixed order (deterministic)
+__global__ void __launch_bounds__(1024)
+fp8_fc1_bound_kernel(const uint8_t* __restrict__ wq, const float* __restrict__ s_w, const float* __restrict__ bias, int N, int K,
+                     float* __restrict__ bound) {
+    __shared__ float red[2][32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float nmax = 0.f, bmax = 0.f;
+    for (int n = warp; n < N; n += 32) {
+        float sq = 0.f;
+        for (int k = lane; k < K; k += 32) { const float f = e4m3_to_f32(wq[(int64_t)n * K + k]); sq += f * f; }
+        nmax = fmaxf(nmax, s_w[n] * sqrtf(warp_sum(sq)));
+        bmax = fmaxf(bmax, fabsf(bias[n]));
+    }
+    if (lane == 0) { red[0][warp] = nmax; red[1][warp] = bmax; }
+    __syncthreads();
+    if (warp == 0) {
+        nmax = warp_max(red[0][lane]);
+        bmax = warp_max(red[1][lane]);
+        if (lane == 0) { bound[0] = nmax; bound[1] = bmax; }
+    }
+}
+void fp8_fc1_bound(const uint8_t* wq, const float* s_w, const float* bias, int N, int K, float* bound, cudaStream_t st) {
+    fp8_fc1_bound_kernel<<<1, 1024, 0, st>>>(wq, s_w, bias, N, K, bound);
+    CUDA_CHECK(cudaGetLastError());
+}
+
 __global__ void embed_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ pos,
                              const float* __restrict__ emb, const float* __restrict__ pos_emb, float* __restrict__ x,
                              int rows, int d) {

@@ -68,6 +68,14 @@ void inc_scatter_rows(const IncJob* jobs, int n, int max_rows, int d, const void
 void layernorm(const float* x, int64_t ldx, const float* w, const float* b, void* out, int out_type, int64_t ldo,
                int rows, int d, const int32_t* row_index_dev, cudaStream_t st);
 
+// WLK_PREC_FP8: rows -> e4m3 bytes + one fp32 scale per row (amax / 448); LayerNorm with e4m3 output, its row scales s_a
+// and, given bound = {max_n ||W1_n||, max_n |b1_n|} (device), the FC1 output scales s_h; that bound of an e4m3 matrix
+void quantize_rows(const void* src, int src_type, int64_t lds, int rows, int cols, uint8_t* dst, int64_t ldd, float* scale,
+                   cudaStream_t st);
+void layernorm_fp8(const float* x, int64_t ldx, const float* w, const float* b, uint8_t* out, int64_t ldo, float* s_a,
+                   float* s_h, const float* bound, int rows, int d, cudaStream_t st);
+void fp8_fc1_bound(const uint8_t* wq, const float* s_w, const float* bias, int N, int K, float* bound, cudaStream_t st);
+
 void embed_tokens(const int32_t* tokens_dev, const int32_t* pos_dev, const float* emb, const float* pos_emb, float* x,
                   int rows, int d, cudaStream_t st);
 

@@ -29,7 +29,7 @@ class WhisperEngine(L.Engine):
     CREATE, DESTROY = "wlk_engine_create", "wlk_engine_destroy"
     LOAD_TENSOR, FINALIZE, MEMORY = "wlk_engine_load_tensor", "wlk_engine_finalize_weights", "wlk_engine_memory"
     SESSION_OPEN, SESSION_CLOSE = "wlk_session_open", "wlk_session_close"
-    precisions = ("fp32", "bf16", "bf16x3")
+    precisions = ("fp32", "bf16", "bf16x3", "fp8")
     reset_session = None            # no whole-session reset: reset_decoder / reset_incremental reset its parts
 
     def __init__(self, dims: ModelDimensions, state_dict: Optional[Dict[str, np.ndarray]] = None,
@@ -259,6 +259,23 @@ class WhisperEngine(L.Engine):
               "tcgen05_pp2x1": 5, "tcgen05_pp1x2": 6, "tcgen05_pp2x2": 7}[backend]
         L.check(self.lib.wlk_op_gemm(self.h, be, A_ptr, a_type, lda, W_ptr, w_type, ldw, bias_ptr, C_ptr, c_type,
                                      ldc, M, N, K, int(gelu)))
+
+    def op_gemm_fp8(self, backend: str, A_ptr, a_scale_ptr, lda, W_ptr, w_scale_ptr, ldw, bias_ptr, C_ptr, c_type, ldc,
+                    M, N, K, *, c_scale_ptr=None, gelu=False, accumulate=False, col_scale=1.0, scale_cols=0):
+        """e4m3 GEMM (wlk_op_gemm_fp8); c_type 0 fp32, 1 bf16, 3 e4m3 (with c_scale_ptr)."""
+        be = {"tcgen05": L.BACKEND_TCGEN05, "tcgen05_pair": 4, "tcgen05_pp2x1": 5, "tcgen05_pp1x2": 6,
+              "tcgen05_pp2x2": 7}.get(backend, 3)        # anything else (e.g. the 64-wide kernel) is refused by the library
+        L.check(self.lib.wlk_op_gemm_fp8(self.h, be, A_ptr, a_scale_ptr, lda, W_ptr, w_scale_ptr, ldw, bias_ptr,
+                                         float(col_scale), int(scale_cols), C_ptr, c_type, c_scale_ptr, ldc, M, N, K,
+                                         int(gelu) | (2 if accumulate else 0)))
+
+    def op_quantize_rows(self, src_ptr, src_type, lds, rows, cols, dst_ptr, ldd, scale_ptr):
+        L.check(self.lib.wlk_op_quantize_rows(self.h, src_ptr, src_type, lds, rows, cols, dst_ptr, ldd, scale_ptr))
+
+    def op_layernorm_fp8(self, x_ptr, ldx, w_ptr, b_ptr, rows, d, out_ptr, ldo, s_a_ptr, s_h_ptr=None,
+                         w1_norm_max=0.0, b1_abs_max=0.0):
+        L.check(self.lib.wlk_op_layernorm_fp8(self.h, x_ptr, ldx, w_ptr, b_ptr, rows, d, out_ptr, ldo, s_a_ptr, s_h_ptr,
+                                              float(w1_norm_max), float(b1_abs_max)))
 
     def op_encoder_attention(self, backend: str, qkv_ptr, dtype_code, batch, out_ptr):
         be = {"simt": L.BACKEND_SIMT, "tcgen05": L.BACKEND_TCGEN05}[backend]
